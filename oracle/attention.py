@@ -46,25 +46,30 @@ def ref_torch_attn_impl(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask:
     return out
 
 
-def masked_attention_bhsd(q, k, v, mask_fn, row_chunk: int = 1024):
+def masked_attention_bhsd(q, k, v, mask_fn, row_chunk: int = 1024, sm_scale=None, return_lse: bool = False,
+                          dtype=torch.float32):
     """q,k,v: [BH, S, D]; mask_fn(q_idx[Sq,1], kv_idx[1,S]) -> bool[Sq,S] or None.
-    Row-chunked so it scales to long S without materialising S x S."""
+    Row-chunked so it scales to long S without materialising S x S.  sm_scale defaults to D^-1/2; `dtype` is the
+    compute precision (torch.float64 for LSE checks).  return_lse: also the natural-log log-sum-exp of the scaled,
+    masked scores [BH, S] (-inf for rows without a key)."""
     BH, S, D = q.shape
-    out = torch.empty(BH, S, D, dtype=torch.float32)
-    scale = D ** -0.5
+    out = torch.empty(BH, S, D, dtype=dtype)
+    lse = torch.empty(BH, S, dtype=dtype)
+    scale = D ** -0.5 if sm_scale is None else sm_scale
     kv_idx = torch.arange(S).view(1, S)
     for h in range(BH):
-        kh = k[h].float()
-        vh = v[h].float()
+        kh = k[h].to(dtype)
+        vh = v[h].to(dtype)
         for r0 in range(0, S, row_chunk):
             r1 = min(S, r0 + row_chunk)
-            s = (q[h, r0:r1].float() @ kh.T) * scale
+            s = (q[h, r0:r1].to(dtype) @ kh.T) * scale
             if mask_fn is not None:
                 m = mask_fn(torch.arange(r0, r1).view(-1, 1), kv_idx)
                 s = s.masked_fill(~m, float("-inf"))
             w = torch.nan_to_num(torch.softmax(s, dim=-1), nan=0.0)
             out[h, r0:r1] = w @ vh
-    return out
+            lse[h, r0:r1] = torch.logsumexp(s, dim=-1)
+    return (out, lse) if return_lse else out
 
 
 def gen_mask_block2element(block_mask: np.ndarray, block_size, len_text_prompt: int) -> torch.Tensor:
@@ -85,21 +90,25 @@ def block_mask_to_element_mask(block_mask_map: torch.Tensor, block_row_sz, block
     return torch.repeat_interleave(rows, c, dim=1)
 
 
-def dynamic_block_sparse_fwd(q, k, v, dynamic_map, qc_size, kc_size):
+def dynamic_block_sparse_fwd(q, k, v, dynamic_map, qc_size, kc_size, sm_scale=None, return_lse: bool = False,
+                             dtype=torch.float32):
     """Variable-block sparse attention, [B,H,S,D].  Same result as kmeans_utils.py:902-995 (online
     softmax over selected blocks == masked softmax over the expanded element mask; rows with no
-    reachable key -> 0, :993).  Computed as masked softmax in fp32."""
+    reachable key -> 0, :993).  Computed as masked softmax in fp32 (or `dtype`).  return_lse: also the
+    natural-log log-sum-exp of the scaled, masked scores [B,H,S] (-inf for rows without a key)."""
     B, H, S, D = q.shape
-    out = torch.zeros(B, H, S, D, dtype=torch.float32)
-    scale = D ** -0.5
+    out = torch.zeros(B, H, S, D, dtype=dtype)
+    lse = torch.empty(B, H, S, dtype=dtype)
+    scale = D ** -0.5 if sm_scale is None else sm_scale
     for b in range(B):
         for h in range(H):
             em = block_mask_to_element_mask(dynamic_map[b, h], qc_size[b, h], kc_size[b, h])
-            s = (q[b, h].float() @ k[b, h].float().T) * scale
+            s = (q[b, h].to(dtype) @ k[b, h].to(dtype).T) * scale
             s = s.masked_fill(~em, float("-inf"))
             w = torch.nan_to_num(torch.softmax(s, dim=-1), nan=0.0)
-            out[b, h] = w @ v[b, h].float()
-    return out
+            out[b, h] = w @ v[b, h].to(dtype)
+            lse[b, h] = torch.logsumexp(s, dim=-1)
+    return (out, lse) if return_lse else out
 
 
 # --------------------------------------------------------------------------------------------

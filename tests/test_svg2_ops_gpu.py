@@ -97,6 +97,51 @@ def test_kmeans_run_matches_reference_control_flow(cuda):
     assert torch.equal(c.cpu(), rc) and torch.equal(lab.cpu().long(), rl)
 
 
+@pytest.mark.parametrize("D,dtype", [(128, torch.bfloat16), (64, torch.float16)])
+def test_kmeans_assign_exact_ties(cuda, D, dtype):
+    """Duplicated centroids, as production's randint initialisation (kmeans_utils.py) draws them: every point that
+    copies -- or lies near -- a duplicated centroid is equally far from both copies, and the documented rule
+    (include/svgb200.h: lowest k wins ties) must pick the lower index.  The pairs sit inside one 32-group (3, 17),
+    in two groups of one 128-chunk (5, 40) and in two chunks (7, 200), with K > 256.  Checked with a caller-supplied
+    x_sq (svgb_kmeans_assign) and through one Lloyd iteration (svgb_kmeans_run: |x|^2 from shared memory), whose
+    update leaves the higher copy empty with its old centroid."""
+    from oracle import kmeans as ok
+    from svgb200 import core
+
+    g = torch.Generator().manual_seed(41)
+    BH, N, K = 2, 4000, 300
+    pairs = [(3, 17), (5, 40), (7, 200)]
+    c = (torch.randn(BH, K, D, generator=g) * 2.0).to(dtype)
+    for lo, hi in pairs:
+        c[:, hi] = c[:, lo]
+    x = (torch.gather(c.float(), 1, torch.randint(0, K, (BH, N, 1), generator=g).expand(-1, -1, D))
+         + 0.3 * torch.randn(BH, N, D, generator=g))
+    expect = torch.full((BH, N), -1, dtype=torch.long)
+    n_tie = 0
+    for lo, hi in pairs:
+        for near in (False, True):  # 40 exact copies, then 40 points at distance ~0.05 * sqrt(D)
+            sl = slice(n_tie, n_tie + 40)
+            x[:, sl] = c[:, lo].float()[:, None] + (0.05 * torch.randn(BH, 40, D, generator=g) if near else 0)
+            expect[:, sl] = lo
+            n_tie += 40
+    x = x.to(dtype)
+    tie = expect >= 0
+    # assign with the caller's x_sq
+    x_sq = ok.row_sqnorm(x)
+    lab = core.kmeans_assign(x.to(cuda), c.to(cuda), x_sq.to(cuda)).cpu().long()
+    assert torch.equal(lab[tie], expect[tie]), f"{int((lab[tie] != expect[tie]).sum())} tied points off"
+    ref, margin = ok.euclid_assign(x, c, x_sq)
+    safe = (margin > 1e-2) & ~tie
+    assert torch.equal(lab[safe], ref[safe])
+    # one Lloyd iteration: |x|^2 from the point tile in shared memory, then the update
+    lab1, c1, cnt1, _ = core.kmeans_run(x.to(cuda), c.to(cuda), 1)
+    lab1, c1, cnt1 = lab1.cpu().long(), c1.cpu(), cnt1.cpu()
+    assert torch.equal(lab1[tie], expect[tie])
+    for lo, hi in pairs:
+        assert bool((cnt1[:, hi] == 0).all()) and bool((cnt1[:, lo] >= 80).all())
+        assert torch.equal(c1[:, hi], c[:, hi])  # an empty cluster keeps its old centroid
+
+
 @pytest.mark.parametrize("QC,KC,dtype", [(40, 100, torch.bfloat16), (64, 1000, torch.bfloat16), (33, 257, torch.float16)])
 def test_dynamic_map(cuda, QC, KC, dtype):
     from oracle import kmeans as ok
