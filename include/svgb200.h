@@ -35,6 +35,14 @@ extern "C" {
 #define SVGB_MASK_HY 1  /* hyvideo/utils.py:20-44  m0=F*P, m1=F*P+prompt_len, m2=W              */
 #define SVGB_MASK_WAN 2 /* wan/utils.py:25-41      m0=P (first-frame sink), m2=W  (|q-kv| <= W) */
 #define SVGB_MASK_COG 3 /* cog/utils.py:30-46      m0=first-col limit, m1=prompt_len, m2=W      */
+/* SVG1 online-profiling masks (get_attention_mask), 128-token block band |bq - bk| < thres; m0=F, m1=P.
+ * HY / WAN: m2=thres.  COG: m2=thres | ctx << 12 (thres < 4096).  See attn_common.cuh MaskMode. */
+#define SVGB_MASK_PROF_HY_S 4   /* hyvideo/utils.py:47-93 spatial, text last (text rows / columns attend)   */
+#define SVGB_MASK_PROF_HY_T 5   /* ... temporal (token-major order)                                      */
+#define SVGB_MASK_PROF_WAN_S 6  /* wan/utils.py:63-110 spatial, first-frame sink                          */
+#define SVGB_MASK_PROF_WAN_T 7  /* ... temporal                                                           */
+#define SVGB_MASK_PROF_COG_S 8  /* cog/utils.py:61-88 spatial, text first (text rows / columns attend)    */
+#define SVGB_MASK_PROF_COG_T 9  /* ... temporal, video x video only (text rows / columns see nothing)     */
 
 /* ---- library ---------------------------------------------------------------------------- */
 int svgb_version(void);

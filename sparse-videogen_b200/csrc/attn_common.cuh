@@ -3,6 +3,7 @@
 // lowered to, and the element-mask predicates used on partial tiles.
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 
 namespace svgb {
@@ -101,52 +102,139 @@ __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, in
   }
 }
 
-// Device-side evaluator of the same predicate for 32 consecutive key columns of one query row:
-// row-constant terms are hoisted, the token-major index of the profiling masks is advanced
-// incrementally (one division per 32 columns instead of two per element), and the result is a bitmask.
-struct MaskRow {
-  int mode, q, m0, m1, m2;
-  int qi_blk;     // profiling masks: 128-token block of the (possibly token-major) query index
-  bool q_text;    // profiling masks: query row is a text row
-  __device__ __forceinline__ void init(int mode_, int q_, int m0_, int m1_, int m2_) {
-    mode = mode_; q = q_; m0 = m0_; m1 = m1_; m2 = m2_;
-    qi_blk = 0; q_text = false;
-    if (mode >= MASK_PROF_HY_S && mode <= MASK_PROF_WAN_T) {
-      const int F = m0, P = m1, V = F * P;
-      const bool temporal = (mode == MASK_PROF_HY_T) | (mode == MASK_PROF_WAN_T);
-      q_text = q >= V;
-      const int qq = q_text ? 0 : q;
-      qi_blk = (temporal ? (qq % P) * F + qq / P : qq) >> 7;
+// Element masks inside the attention kernel.  A thread holds the scores of two query rows at positions q[0], q[1]
+// and key columns kvb + 8*jj + v0 (jj < 16, v0 < 2; kvb = chunk start + 2*(lane % 4)), the wgmma accumulator
+// layout.  ElemMask::bits returns them as two 32-bit masks: bit 2*jj + v0 of keep[v1] <=> mask_allowed(mode, q[v1],
+// kvb + 8*jj + v0).
+// The mask family is dispatched once per chunk, never per element.  The band families and the CogVideoX spatial
+// profiling mask inline mask_allowed with the mode as a compile-time constant (comparisons and shifts only).  The
+// banded profiling masks (HY / WAN spatial and temporal, COG temporal) hoist the query's 128-token block to init
+// (once per stream) and, in temporal order, step the key's (frame, token) pair across the columns: one division
+// per chunk instead of two per element.
+struct ElemMask {
+  int mode, m0, m1, m2;
+  // per query row, one register (the kernel is register-bound):
+  //   direct families: the query position
+  //   banded profiling masks: band_lo = qblk - thres + 1, the first key block of the row's band, so that
+  //   |qblk - kblk| < thres <=> (unsigned)(kblk - band_lo) < 2*thres - 1; or kRowOut when the query lies outside
+  //   the banded part (every key then gives Prof::outside_val)
+  int row[2];
+  static constexpr int kRowOut = INT_MIN;  // band_lo >= INT_MIN + 2 for 0 < thres <= INT_MAX, and 0 for thres <= 0
+
+  // parameters of the banded profiling masks, in the form the evaluator uses
+  struct Prof {
+    int F, P, off, lim, thres;  // token index r = position - off; r < 0 or r >= lim is outside the band
+    bool temporal, outside_val, sink;  // sink: WAN first frame (token-major index < P) always attends
+  };
+  __device__ __forceinline__ static bool banded(int mode) {
+    return (mode >= MASK_PROF_HY_S && mode <= MASK_PROF_WAN_T) || mode == MASK_PROF_COG_T;
+  }
+  __device__ __forceinline__ Prof prof() const {
+    Prof p;
+    p.F = m0;
+    p.P = m1;
+    const bool cog = mode == MASK_PROF_COG_T;
+    // HY / WAN: text rows and columns (index >= F*P) give `hy`.  COG temporal: text comes first (index < ctx)
+    // and gives false; there is no upper limit (mask_allowed bands every index >= ctx)
+    p.off = cog ? m2 >> 12 : 0;
+    p.lim = cog ? INT_MAX : m0 * m1;
+    p.thres = cog ? m2 & 0xfff : m2;
+    p.temporal = cog || mode == MASK_PROF_HY_T || mode == MASK_PROF_WAN_T;
+    p.outside_val = mode == MASK_PROF_HY_S || mode == MASK_PROF_HY_T;
+    p.sink = mode == MASK_PROF_WAN_S || mode == MASK_PROF_WAN_T;
+    return p;
+  }
+
+  __device__ __forceinline__ void init(int mode_, const int (&qm)[2], int m0_, int m1_, int m2_) {
+    mode = mode_; m0 = m0_; m1 = m1_; m2 = m2_;
+#pragma unroll
+    for (int v1 = 0; v1 < 2; ++v1) row[v1] = qm[v1];
+    if (!banded(mode)) return;
+    const Prof p = prof();
+#pragma unroll
+    for (int v1 = 0; v1 < 2; ++v1) {
+      const int r = qm[v1] - p.off;
+      if (r < 0 || r >= p.lim) {
+        row[v1] = kRowOut;
+      } else {
+        const int qi = p.temporal ? (r % p.P) * p.F + r / p.P : r;
+        row[v1] = p.thres > 0 ? static_cast<int>(static_cast<uint32_t>(qi >> 7) - static_cast<uint32_t>(p.thres) + 1u) : 0;
+      }
     }
   }
-  // bit i set <=> (q, kv0 + i) allowed
-  __device__ __forceinline__ uint32_t bits32(int kv0) const {
-    uint32_t out = 0;
-    if (mode >= MASK_PROF_HY_S && mode <= MASK_PROF_WAN_T) {
-      const int F = m0, P = m1, V = F * P;
-      const bool hy = mode <= MASK_PROF_HY_T;
-      const bool temporal = (mode == MASK_PROF_HY_T) | (mode == MASK_PROF_WAN_T);
-      const int kvc = kv0 < V ? kv0 : 0;
-      int f = kvc / P, p = kvc - f * P;
+
+  template <int kMode>
+  __device__ __forceinline__ void bits_direct(int kvb, uint32_t (&keep)[2]) const {
+#pragma unroll 1
+    for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int kv = kv0 + i;
-        const int ki = temporal ? p * F + f : kv;
-        int bd = qi_blk - (ki >> 7);
-        bd = bd < 0 ? -bd : bd;
-        const bool text = q_text | (kv >= V);
-        const bool a = text ? hy : ((bd < m2) | (!hy & (ki < P)));
-        out |= (a ? 1u : 0u) << i;
-        ++p;
-        const bool wrap = p == P;
-        p = wrap ? 0 : p;
-        f += wrap ? 1 : 0;
+      for (int v0 = 0; v0 < 2; ++v0) {
+        const int kv = kvb + 8 * jj + v0;
+#pragma unroll
+        for (int v1 = 0; v1 < 2; ++v1)
+          keep[v1] |= (mask_allowed(kMode, row[v1], kv, m0, m1, m2) ? 1u : 0u) << (2 * jj + v0);
       }
-      return out;
+  }
+
+  template <bool kTemporal>
+  __device__ __forceinline__ void bits_banded(int kvb, uint32_t (&keep)[2]) const {
+    const Prof pr = prof();
+    const int F = pr.F, P = pr.P;
+    const uint32_t width = pr.thres > 0 ? 2u * static_cast<uint32_t>(pr.thres) - 1u : 0u;
+    const int r0 = kvb - pr.off;
+    // temporal: (f, p) = floor division of the token index by P, stepped by 1 within a column pair and by 8
+    // (= f8 frames + p8 tokens) from one pair to the next
+    int f = 0, p = 0, f8 = 0, p8 = 0;
+    if (kTemporal) {
+      f = r0 >= 0 ? r0 / P : -((P - 1 - r0) / P);
+      p = r0 - f * P;
+      f8 = 8 / P;
+      p8 = 8 - f8 * P;
     }
+#pragma unroll 1
+    for (int jj = 0; jj < 16; ++jj) {
+      int fc = f, pc = p;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) out |= (mask_allowed(mode, q, kv0 + i, m0, m1, m2) ? 1u : 0u) << i;
-    return out;
+      for (int v0 = 0; v0 < 2; ++v0) {
+        const int r = r0 + 8 * jj + v0;
+        const int ki = kTemporal ? pc * F + fc : r;
+        const bool col_out = r < 0 || r >= pr.lim;
+        const bool sink = pr.sink & (ki < P);
+        const uint32_t kb = static_cast<uint32_t>(ki >> 7);
+#pragma unroll
+        for (int v1 = 0; v1 < 2; ++v1) {
+          const bool out = row[v1] == kRowOut || col_out;
+          const bool a = out ? pr.outside_val : ((kb - static_cast<uint32_t>(row[v1]) < width) | sink);
+          keep[v1] |= (a ? 1u : 0u) << (2 * jj + v0);
+        }
+        if (kTemporal && v0 == 0) {
+          ++pc;
+          if (pc == P) {
+            pc = 0;
+            ++fc;
+          }
+        }
+      }
+      if (kTemporal) {
+        p += p8;
+        f += f8;
+        if (p >= P) {
+          p -= P;
+          ++f;
+        }
+      }
+    }
+  }
+
+  __device__ __forceinline__ void bits(int kvb, uint32_t (&keep)[2]) const {
+    keep[0] = keep[1] = 0;
+    if (mode == MASK_HY) bits_direct<MASK_HY>(kvb, keep);
+    else if (mode == MASK_WAN) bits_direct<MASK_WAN>(kvb, keep);
+    else if (mode == MASK_COG) bits_direct<MASK_COG>(kvb, keep);
+    else if (mode == MASK_PROF_COG_S) bits_direct<MASK_PROF_COG_S>(kvb, keep);
+    else if (mode == MASK_PROF_HY_S || mode == MASK_PROF_WAN_S) bits_banded<false>(kvb, keep);
+    else if (banded(mode)) bits_banded<true>(kvb, keep);
+    else keep[0] = keep[1] = ~0u;  // MASK_NONE (mask_allowed's default)
   }
 };
 

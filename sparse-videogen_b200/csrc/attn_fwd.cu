@@ -544,7 +544,7 @@ int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, vo
   if (svgb_attn_plan_band_bytes(S, &need)) return -1;
   SVGB_REQUIRE(plan_ws && plan, "null pointer");
   SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_COG, "unknown mask mode %d", mask_mode);
+  SVGB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_PROF_COG_T, "unknown mask mode %d", mask_mode);
   const BandSegs sg = band_segments(mask_mode, m0, m1, S);
   const int n_items = band_total_items(sg);
   const int n_items_cap = (S + kItemRows - 1) / kItemRows + 4;

@@ -229,11 +229,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
 
     // per thread: rows r0 = 16*wq + lane/4 and r0 + 8 of this warpgroup's 64; columns 8j + 2*(lane%4) (+1)
     const int rloc = 64 * wg + 16 * wq + (lane >> 2);
-    int qm[2];
+    ElemMask em;
+    if constexpr (!kGather) {  // gather plans carry no element masks
+      int qm[2];
 #pragma unroll
-    for (int v1 = 0; v1 < 2; ++v1) {
-      const int q = q0 + rloc + 8 * v1;
-      qm[v1] = (args.q_index && q < args.S) ? __ldg(&args.q_index[q]) : q;  // position seen by the mask
+      for (int v1 = 0; v1 < 2; ++v1) {
+        const int q = q0 + rloc + 8 * v1;
+        qm[v1] = (args.q_index && q < args.S) ? __ldg(&args.q_index[q]) : q;  // position seen by the mask
+      }
+      em.init(mode, qm, m0, m1, m2);
     }
     float o[D / 2];
 #pragma unroll
@@ -295,6 +299,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         elem = (ch.y & kChunkElem) != 0;
       }
       if (valid < kChunkCols || elem) {
+        // keep[v1] bit 2*jj + v0: column 8*jj + 2*(lane%4) + v0 of row v1 is an allowed key
+        uint32_t keep[2] = {~0u, ~0u};
+        if (elem) em.bits(kv0 + 2 * (lane & 3), keep);
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
@@ -302,7 +309,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
 #pragma unroll
             for (int v0 = 0; v0 < 2; ++v0) {
               const int col = 8 * jj + 2 * (lane & 3) + v0;
-              const bool ok = col < valid && (!elem || mask_allowed(mode, qm[v1], kv0 + col, m0, m1, m2));
+              const bool ok = col < valid && ((keep[v1] >> (2 * jj + v0)) & 1u);
               if (!ok) s[4 * jj + 2 * v1 + v0] = -INFINITY;
             }
       }

@@ -116,10 +116,12 @@ struct SmseLayout {
   int nsplit, n_chunks;
   size_t qg, qidx, counts, items, chunks_plain, chunks_elem, o_part, lse_part, partial, total;
 };
-static SmseLayout smse_layout(int BH, int S, int D) {
+// n_sms: SM count of the current device.  The attention kernel fits one CTA per SM (its shared memory), so
+// BH * nsplit <= n_sms keeps each pass to one wave; one CTA more would run as a second wave and double the pass.
+static SmseLayout smse_layout(int BH, int S, int D, int n_sms) {
   SmseLayout L;
   L.n_chunks = (S + kChunkCols - 1) / kChunkCols;
-  L.nsplit = 148 / BH;  // one wave: BH * nsplit <= number of SMs
+  L.nsplit = n_sms / BH;
   if (L.nsplit > 32) L.nsplit = 32;  // few heads (per-head pipelines): keep the merge cheap
   if (L.nsplit > L.n_chunks) L.nsplit = L.n_chunks;
   if (L.nsplit < 1) L.nsplit = 1;
@@ -143,6 +145,13 @@ static SmseLayout smse_layout(int BH, int S, int D) {
   return L;
 }
 
+static int device_sms(int* n_sms) {
+  int dev = 0;
+  SVGB_CUDA(cudaGetDevice(&dev));
+  SVGB_CUDA(cudaDeviceGetAttribute(n_sms, cudaDevAttrMultiProcessorCount, dev));
+  return 0;
+}
+
 }  // namespace svgb
 
 using namespace svgb;
@@ -152,7 +161,9 @@ extern "C" {
 int svgb_sample_mse_bytes(int BH, int S, int D, int n_rows, size_t* bytes) {
   SVGB_REQUIRE(BH > 0 && S > 0 && (D == 64 || D == 128) && n_rows > 0 && n_rows <= 128 && bytes,
                "bad arguments (n_rows <= 128, D in {64,128})");
-  *bytes = smse_layout(BH, S, D).total;
+  int n_sms = 0;
+  if (device_sms(&n_sms)) return -1;
+  *bytes = smse_layout(BH, S, D, n_sms).total;
   return 0;
 }
 
@@ -167,7 +178,9 @@ int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* 
   SVGB_REQUIRE(S == ctx + F * P, "seq_len %d != ctx %d + F %d * P %d", S, ctx, F, P);
   SVGB_REQUIRE(layout != 1 || ctx == 0, "WAN layout has no text tokens");
   SVGB_REQUIRE(layout != 2 || ctx < (1 << 19), "COG layout: context length %d too large", ctx);
-  const SmseLayout L = smse_layout(BH, S, D);
+  int n_sms = 0;
+  if (device_sms(&n_sms)) return -1;
+  const SmseLayout L = smse_layout(BH, S, D, n_sms);  // the same device, so the same layout as the byte count
   char* w = static_cast<char*>(ws);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int vpr = D * 2 / 16;

@@ -12,6 +12,8 @@ import torch
 from ._lib import Plan, SvgbError, check, lib
 
 MASK_NONE, MASK_HY, MASK_WAN, MASK_COG = 0, 1, 2, 3
+# SVG1 profiling masks (include/svgb200.h SVGB_MASK_PROF_*): the element masks of sample_mse, also accepted by plan_band
+MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_S, MASK_PROF_COG_T = 4, 5, 6, 7, 8, 9
 
 # launches issued through this module since import (bench.py reports it as gpu_launches)
 launch_count = 0
