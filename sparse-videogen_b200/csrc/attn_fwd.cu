@@ -358,7 +358,8 @@ selftest_tile_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_cons
   }
   mbar_wait(smem_u32(bar), 0, 20);
   float s[64];
-  attn_qk<D, DT>(s, sQ + 64 * wg * 128, sK);
+  attn_qk_issue<D, DT>(s, sQ + 64 * wg * 128, sK);
+  attn_wait<0>(s);
   // S -> global, P = 16-bit(S * p_scale), O = P V
   const int row0 = 64 * wg + 16 * wq + (lane >> 2), col0 = 2 * (lane & 3);
 #pragma unroll
@@ -374,7 +375,10 @@ selftest_tile_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_cons
   float o[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
-  attn_pv<D, BF16>(o, s, sV);
+  uint32_t pa[8][4];
+  attn_pack_p<BF16>(pa, s);
+  attn_pv_issue<D, BF16>(o, pa, sV);
+  attn_wait<0>(o);
 #pragma unroll
   for (int jj = 0; jj < D / 8; ++jj)
 #pragma unroll

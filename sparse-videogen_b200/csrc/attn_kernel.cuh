@@ -4,12 +4,16 @@
 // 128-row tile.  A work item is one or two 128-row STREAMS (a two-tile item: rows 0-127 and 128-255 over the same
 // chunk list; a dual item: two independent tails, each with its own chunk list), run one after the other.
 //   Q tile          : TMA (or cp.async row gather), 128-byte swizzle, stays in shared memory for the stream
-//   K(j), V(j)      : double-buffered; chunk j+1 is loaded while chunk j is computed
+//   K(j), V(j)      : three stages; chunk j+3 is requested once chunk j's stage is free
 //   S = Q K^T       : wgmma m64n128 (SS, both operands K-major), fp32 accumulators in registers
 //   softmax         : online, in registers (each row is spread over the 4 lanes of a quad)
 //   O += P V        : wgmma m64nD (RS: P from registers in the accumulator layout of S, V MN-major)
+// The chunk loop is software-pipelined inside each warpgroup: iteration j issues S = Q K(j+1)^T and then
+// O += P(j) V(j) as two wgmma groups, waits for the first only, and runs the mask and softmax of chunk j+1 while
+// P V(j) is still on the tensor cores.  Every row still sees the same operations in the same order as a
+// one-chunk-at-a-time loop (rescale O by alpha(j+1), then accumulate P(j+1) V(j+1)).
 // FP8 (e4m3) inputs: Q K^T runs on e4m3 wgmma (k32); wgmma has no MN-major 8-bit B operand, so each V tile is
-// widened to fp16 in shared memory and P V runs in fp16.
+// widened to fp16 in shared memory (two buffers: V(j+1) is widened while P V(j) reads V(j)) and P V runs in fp16.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -24,6 +28,9 @@ namespace svgb {
 
 // element type of Q/K/V: 0 = bf16, 1 = fp16, 2 = fp8 e4m3 (output bf16)
 constexpr int DT_BF16 = 0, DT_F16 = 1, DT_E4M3 = 2;
+// K/V stages: with P V(j) still running when Q K(j+1)^T is issued, chunk j's stage frees late in iteration j, so
+// the load of chunk j+3 into it gets about two chunks of lead time
+constexpr int kKvStages = 3;
 
 template <int D, int DT = DT_BF16>
 struct AttnCfg {
@@ -36,18 +43,21 @@ struct AttnCfg {
   static constexpr int kPanelBytes = 128 * 128;          // 128 rows x 128 B
   static constexpr int kTileBytes = kPanelBytes * kHalves;
   static constexpr int kKSteps = kRowBytes / 32;         // wgmma K steps of Q K^T (32 bytes each)
-  static constexpr int kVhBytes = DT == DT_E4M3 ? 2 * kPanelBytes : 0;  // fp16 copy of the e4m3 V tile
+  static constexpr int kVhBytes = DT == DT_E4M3 ? 2 * kPanelBytes : 0;  // fp16 copy of one e4m3 V tile
   static constexpr int kMaxRunsSmem = kTileBytes / 8 - 1;
   static constexpr int kBarBytes = 1024;                 // mbarriers + gather row table
   // + 1 KB: the kernel aligns the dynamic window to 1024 bytes itself
-  static constexpr int kSmemBytes = 1024 + kTileBytes + 4 * kTileBytes + kVhBytes + kBarBytes;
+  static constexpr int kSmemBytes = 1024 + kTileBytes + 2 * kKvStages * kTileBytes + 2 * kVhBytes + kBarBytes;
   static constexpr int kThreads = 256;
   static_assert(kSmemBytes <= 227 * 1024, "exceeds the 227 KB per-CTA shared memory of sm_90");
 };
 
+// The wgmma products are issued and committed as one group each; their accumulators (and the P fragments of
+// P V) may not be touched until attn_wait has retired the group.
+
 // S[64 x 128] = Q[64 rows of the tile] K^T for one warpgroup
 template <int D, int DT>
-__device__ __forceinline__ void attn_qk(float (&s)[64], uint32_t sQw, uint32_t sK) {
+__device__ __forceinline__ void attn_qk_issue(float (&s)[64], uint32_t sQw, uint32_t sK) {
   using Cfg = AttnCfg<D, DT>;
 #pragma unroll
   for (int i = 0; i < 64; ++i) s[i] = 0.f;
@@ -60,18 +70,20 @@ __device__ __forceinline__ void attn_qk(float (&s)[64], uint32_t sQw, uint32_t s
     else wgmma_m64n128k16_ss<DT == DT_BF16>(s, a, b, kk > 0);
   }
   wg_commit();
-  wg_wait<0>();
-  wg_fence_regs(s);
 }
 
-// O[64 x D] += P[64 x 128] V[128 x D]; P in the accumulator layout of S, packed to 16 bit (kBF16: bf16, else fp16)
-template <int D, bool kBF16>
-__device__ __forceinline__ void attn_pv(float (&o)[D / 2], const float (&p)[64], uint32_t sV) {
-  uint32_t a[8][4];
+// P[64 x 128] in the accumulator layout of S -> the A fragments of P V, packed to 16 bit (kBF16: bf16, else fp16)
+template <bool kBF16>
+__device__ __forceinline__ void attn_pack_p(uint32_t (&a)[8][4], const float (&p)[64]) {
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk)
 #pragma unroll
     for (int r = 0; r < 4; ++r) a[kk][r] = pack2<kBF16>(p[8 * kk + 2 * r], p[8 * kk + 2 * r + 1]);
+}
+
+// O[64 x D] += P[64 x 128] V[128 x D]
+template <int D, bool kBF16>
+__device__ __forceinline__ void attn_pv_issue(float (&o)[D / 2], const uint32_t (&a)[8][4], uint32_t sV) {
   wg_fence();
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk) {
@@ -80,14 +92,21 @@ __device__ __forceinline__ void attn_pv(float (&o)[D / 2], const float (&p)[64],
     else wgmma_m64n64k16_rs<kBF16>(o, a[kk], b, 1);
   }
   wg_commit();
-  wg_wait<0>();
-  wg_fence_regs(o);
+}
+
+// wait until at most N of this warpgroup's wgmma groups are pending (groups retire in issue order), then let the
+// accumulators `d` of a retired group be read
+template <int N, int M>
+__device__ __forceinline__ void attn_wait(float (&d)[M]) {
+  wg_wait<N>();
+  wg_fence_regs(d);
 }
 
 struct AttnSmemCtl {
   uint64_t q_full;
-  uint64_t kv_full[2];
+  uint64_t kv_full[kKvStages];
   int src[128];  // gather: source row of each of the 128 rows being loaded (-1: zero fill)
+  float pin[8];  // one word per warp, written and never read (see the chunk loop)
 };
 
 // kGather selects the loader: false = TMA boxes over contiguous key ranges (chunk list), true = cp.async
@@ -118,15 +137,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   uint8_t* smem_al = smem_raw + (base - raw_u32);
   const uint32_t sQ = base;
   const uint32_t sK0 = sQ + Cfg::kTileBytes;  // stage s: K at sK0 + 2s*tile, V at sK0 + (2s+1)*tile
-  const uint32_t sVh = sK0 + 4 * Cfg::kTileBytes;
-  AttnSmemCtl* ctl = reinterpret_cast<AttnSmemCtl*>(smem_al + Cfg::kTileBytes * 5 + Cfg::kVhBytes);
+  const uint32_t sVh = sK0 + 2 * kKvStages * Cfg::kTileBytes;  // FP8: buffer b at sVh + b*kVhBytes
+  AttnSmemCtl* ctl =
+      reinterpret_cast<AttnSmemCtl*>(smem_al + Cfg::kTileBytes * (1 + 2 * kKvStages) + 2 * Cfg::kVhBytes);
 
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wt = tid & 127, lane = tid & 31, wq = wt >> 5;
+  const uint32_t sQw = sQ + 64 * wg * 128;  // this warpgroup's 64 rows of the Q tile
   if (tid == 0) {
     mbar_init(smem_u32(&ctl->q_full), 1);
-    mbar_init(smem_u32(&ctl->kv_full[0]), 1);
-    mbar_init(smem_u32(&ctl->kv_full[1]), 1);
+    for (int i = 0; i < kKvStages; ++i) mbar_init(smem_u32(&ctl->kv_full[i]), 1);
     mbar_fence_init();
     if constexpr (!kGather) {
       tma_prefetch_desc(&qmap);
@@ -178,7 +198,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     }
   };
 
-  int g = 0;       // chunks loaded so far (stage = g & 1, mbarrier phase = (g >> 1) & 1)
+  int g = 0;       // chunks of this CTA before the current stream (the stream's chunk j is the CTA's chunk g + j)
   int nq = 0;      // Q tiles loaded so far (q_full phase)
   const int nstreams = (dual || item.y > kTileRows) ? 2 : 1;
   for (int st = 0; st < nstreams; ++st) {
@@ -188,9 +208,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     const int2* __restrict__ chunks = args.chunks + ((second && dual) ? item2.z : item.z);
     const int nch = kGather ? (total_kv + kChunkCols - 1) / kChunkCols : ((second && dual) ? item2.w : item.w);
 
-    // issue the loads of chunk j into stage `stage`
-    auto load_chunk = [&](int j, int stage) {
-      const uint32_t sK = sK0 + 2 * stage * Cfg::kTileBytes, sV = sK + Cfg::kTileBytes;
+    // CTA chunk n lives in K/V stage n % 3 (kv_full phase (n / 3) & 1); FP8: its fp16 V copy in buffer n & 1
+    auto stage_k = [&](int j) { return sK0 + 2 * ((g + j) % kKvStages) * Cfg::kTileBytes; };
+    auto pv_b = [&](int j) { return FP8 ? sVh + ((g + j) & 1) * Cfg::kVhBytes : stage_k(j) + Cfg::kTileBytes; };
+
+    // issue the loads of chunk j
+    auto load_chunk = [&](int j) {
+      const uint32_t sK = stage_k(j), sV = sK + Cfg::kTileBytes;
       if constexpr (kGather) {
         resolve_chunk(j);
         __syncthreads();
@@ -199,7 +223,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         __syncthreads();  // ctl->src is reused by the next resolve
       } else if (tid == 0) {
         const int kv0 = __ldg(&chunks[j].x);
-        const uint32_t fb = smem_u32(&ctl->kv_full[stage]);
+        const uint32_t fb = smem_u32(&ctl->kv_full[(g + j) % kKvStages]);
         mbar_expect_tx(fb, 2 * Cfg::kTileBytes);
         for (int h = 0; h < Cfg::kHalves; ++h) {
           tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, fb, h * Cfg::kPanelElems, kv0, bh);
@@ -207,25 +231,44 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         }
       }
     };
-
-    if (nch > 0) {
-      // ---- Q (rows past nr: zero filled by the gather, other rows' data by TMA -- never stored)
+    // wait until chunk j has landed; gather: `later` chunks were requested after it
+    auto wait_chunk = [&](int j, int later) {
       if constexpr (kGather) {
-        if (tid < 128) {
-          const int* q_rows = args.q_rows ? args.q_rows + static_cast<size_t>(bh) * args.S : nullptr;
-          const int qr = q0 + tid;
-          ctl->src[tid] = tid < nr ? (q_rows ? __ldg(&q_rows[qr]) : qr) : -1;
-        }
+        if (later >= 2) cp_async_wait<2>();
+        else if (later == 1) cp_async_wait<1>();
+        else cp_async_wait<0>();
+        fence_proxy_async_smem();
         __syncthreads();
-        gather_rows(sQ, static_cast<const uint16_t*>(args.q_ptr) + bh * args.in_head_stride, false, nullptr, 0);
-        __syncthreads();
-      } else if (tid == 0) {
-        const uint32_t qb = smem_u32(&ctl->q_full);
-        mbar_expect_tx(qb, Cfg::kTileBytes);
-        for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sQ + h * Cfg::kPanelBytes, &qmap, qb, h * Cfg::kPanelElems, q0, bh);
+      } else {
+        mbar_wait(smem_u32(&ctl->kv_full[(g + j) % kKvStages]), ((g + j) / kKvStages) & 1, 2);
       }
-      load_chunk(0, g & 1);  // gather: Q and chunk 0 share one cp.async group
-    }
+    };
+    // FP8: widen V(j) (e4m3, one 128-byte panel) to fp16 (two panels) in the same swizzled image.  All 256 threads
+    // write; the copy is published by fence.proxy.async plus a block barrier.
+    auto widen_v = [&](int j) {
+      const uint32_t sV = stage_k(j) + Cfg::kTileBytes, dst = pv_b(j);
+#pragma unroll
+      for (int i = tid; i < 128 * 8; i += 256) {
+        const int r = i >> 3, pc = i & 7;
+        const uint4 w = *reinterpret_cast<const uint4*>(smem_al + (sV - base) + r * 128 + ((pc ^ (r & 7)) << 4));
+        const uint32_t in[4] = {w.x, w.y, w.z, w.w};
+        uint32_t out[8];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(in[k] & 0xffffu), __NV_E4M3);
+          const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(in[k] >> 16), __NV_E4M3);
+          out[2 * k] = static_cast<uint32_t>(lo.x) | (static_cast<uint32_t>(lo.y) << 16);
+          out[2 * k + 1] = static_cast<uint32_t>(hi.x) | (static_cast<uint32_t>(hi.y) << 16);
+        }
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int p16 = 2 * pc + hh;  // 16-byte piece of the fp16 row
+          *reinterpret_cast<uint4*>(smem_al + (dst - base) + (p16 >> 3) * Cfg::kPanelBytes + r * 128 +
+                                    (((p16 & 7) ^ (r & 7)) << 4)) =
+              make_uint4(out[4 * hh], out[4 * hh + 1], out[4 * hh + 2], out[4 * hh + 3]);
+        }
+      }
+    };
 
     // per thread: rows r0 = 16*wq + lane/4 and r0 + 8 of this warpgroup's 64; columns 8j + 2*(lane%4) (+1)
     const int rloc = 64 * wg + 16 * wq + (lane >> 2);
@@ -242,51 +285,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     float o[D / 2];
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
-    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, alpha[2];
+    float s[64];        // S of the chunk being scored, then its P
+    uint32_t pa[8][4];  // P of the chunk whose P V is next, packed to 16 bit
 
-    for (int j = 0; j < nch; ++j, ++g) {
-      const int stage = g & 1;
-      if (j + 1 < nch) load_chunk(j + 1, stage ^ 1);
-      if constexpr (kGather) {
-        if (j + 1 < nch) cp_async_wait<1>();
-        else cp_async_wait<0>();
-        fence_proxy_async_smem();
-        __syncthreads();
-      } else {
-        if (j == 0) mbar_wait(smem_u32(&ctl->q_full), nq & 1, 1);
-        mbar_wait(smem_u32(&ctl->kv_full[stage]), (g >> 1) & 1, 2);
-      }
-      const uint32_t sK = sK0 + 2 * stage * Cfg::kTileBytes, sV = sK + Cfg::kTileBytes;
-      if constexpr (FP8) {
-        // widen V (e4m3, one 128-byte panel) to fp16 (two panels) in the same swizzled image
-#pragma unroll
-        for (int i = tid; i < 128 * 8; i += 256) {
-          const int r = i >> 3, pc = i & 7;
-          const uint4 w = *reinterpret_cast<const uint4*>(smem_al + (sV - base) + r * 128 + ((pc ^ (r & 7)) << 4));
-          const uint32_t in[4] = {w.x, w.y, w.z, w.w};
-          uint32_t out[8];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(in[k] & 0xffffu), __NV_E4M3);
-            const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(in[k] >> 16), __NV_E4M3);
-            out[2 * k] = static_cast<uint32_t>(lo.x) | (static_cast<uint32_t>(lo.y) << 16);
-            out[2 * k + 1] = static_cast<uint32_t>(hi.x) | (static_cast<uint32_t>(hi.y) << 16);
-          }
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int p16 = 2 * pc + hh;  // 16-byte piece of the fp16 row
-            *reinterpret_cast<uint4*>(smem_al + (sVh - base) + (p16 >> 3) * Cfg::kPanelBytes + r * 128 +
-                                      (((p16 & 7) ^ (r & 7)) << 4)) =
-                make_uint4(out[4 * hh], out[4 * hh + 1], out[4 * hh + 2], out[4 * hh + 3]);
-          }
-        }
-        fence_proxy_async_smem();
-        __syncthreads();
-      }
-
-      float s[64];
-      attn_qk<D, DT>(s, sQ + 64 * wg * 128, sK);
-
+    // mask and online softmax of chunk j (scores in log2 units: x * c): S -> P, running max and sum, alpha = the
+    // factor O still has to be scaled by before P(j) V(j) is accumulated
+    auto softmax = [&](int j) {
       // ---- mask: partial chunks and element-mask chunks
       int kv0 = 0, valid = kChunkCols;
       bool elem = false;
@@ -313,8 +318,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
               if (!ok) s[4 * jj + 2 * v1 + v0] = -INFINITY;
             }
       }
-
-      // ---- online softmax (scores in log2 units: x * c)
 #pragma unroll
       for (int v1 = 0; v1 < 2; ++v1) {
         float mx = -INFINITY;
@@ -324,7 +327,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
         const float m_new = fmaxf(m_run[v1], mx);
         const float mc = m_new == -INFINITY ? 0.f : m_new * c;
-        const float alpha = ex2_approx(m_run[v1] == -INFINITY ? -INFINITY : m_run[v1] * c - mc);
+        alpha[v1] = ex2_approx(m_run[v1] == -INFINITY ? -INFINITY : m_run[v1] * c - mc);
         m_run[v1] = m_new;
         float ls = 0.f;
 #pragma unroll
@@ -335,17 +338,75 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
             s[4 * jj + 2 * v1 + v0] = p;
             ls += p;
           }
-        l_run[v1] = l_run[v1] * alpha + ls;
+        l_run[v1] = l_run[v1] * alpha[v1] + ls;
+      }
+    };
+    // O *= alpha and P -> fragments: only once P V of the previous chunk has retired
+    auto rescale_pack = [&]() {
+#pragma unroll
+      for (int v1 = 0; v1 < 2; ++v1)
 #pragma unroll
         for (int jj = 0; jj < D / 8; ++jj) {
-          o[4 * jj + 2 * v1] *= alpha;
-          o[4 * jj + 2 * v1 + 1] *= alpha;
+          o[4 * jj + 2 * v1] *= alpha[v1];
+          o[4 * jj + 2 * v1 + 1] *= alpha[v1];
         }
+      attn_pack_p<kPBF16>(pa, s);
+    };
+
+    if (nch > 0) {
+      // ---- Q (rows past nr: zero filled by the gather, other rows' data by TMA -- never stored)
+      if constexpr (kGather) {
+        if (tid < 128) {
+          const int* q_rows = args.q_rows ? args.q_rows + static_cast<size_t>(bh) * args.S : nullptr;
+          const int qr = q0 + tid;
+          ctl->src[tid] = tid < nr ? (q_rows ? __ldg(&q_rows[qr]) : qr) : -1;
+        }
+        __syncthreads();
+        gather_rows(sQ, static_cast<const uint16_t*>(args.q_ptr) + bh * args.in_head_stride, false, nullptr, 0);
+        __syncthreads();
+      } else if (tid == 0) {
+        const uint32_t qb = smem_u32(&ctl->q_full);
+        mbar_expect_tx(qb, Cfg::kTileBytes);
+        for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sQ + h * Cfg::kPanelBytes, &qmap, qb, h * Cfg::kPanelElems, q0, bh);
       }
-      attn_pv<D, kPBF16>(o, s, FP8 ? sVh : sV);
-      __syncthreads();  // stage `stage` (and the fp16 V copy) may be overwritten from here on
+      const int npre = min(nch, kKvStages);
+      for (int j = 0; j < npre; ++j) load_chunk(j);  // gather: Q and chunk 0 share one cp.async group
+      if constexpr (!kGather) mbar_wait(smem_u32(&ctl->q_full), nq & 1, 1);
+      wait_chunk(0, npre - 1);
+      if constexpr (FP8) {
+        widen_v(0);
+        fence_proxy_async_smem();
+        __syncthreads();
+      }
+      attn_qk_issue<D, DT>(s, sQw, stage_k(0));
+      attn_wait<0>(s);
+      softmax(0);
+      rescale_pack();
+
+      for (int j = 0; j + 1 < nch; ++j) {
+        wait_chunk(j + 1, j + 2 < nch ? 1 : 0);
+        attn_qk_issue<D, DT>(s, sQw, stage_k(j + 1));  // group A
+        attn_pv_issue<D, kPBF16>(o, pa, pv_b(j));       // group B: O and pa stay in flight
+        attn_wait<1>(s);                                // A has retired, B may still be running
+        if constexpr (FP8) widen_v(j + 1);              // buffer (g+j+1) & 1 was last read by P V(j-1)
+        softmax(j + 1);                                 // runs under P V(j)
+        // ptxas schedules wgmma.wait_group ahead of register math that does not depend on it, which would move
+        // the exps below the wait and out from under P V(j).  Shared-memory stores stay ahead of the wait, so
+        // storing the running sums (they depend on every exp of the chunk) keeps the softmax in front of it.
+        if (lane == 0) ctl->pin[tid >> 5] = l_run[0] + l_run[1];
+        attn_wait<0>(o);
+        wg_fence_regs(s);  // P(j+1) is packed into pa only after P V(j) has read it
+        if constexpr (FP8) fence_proxy_async_smem();
+        __syncthreads();   // chunk j's stage is free in both warpgroups; the fp16 copy of V(j+1) is complete
+        if (j + 3 < nch) load_chunk(j + 3);
+        rescale_pack();
+      }
+      attn_pv_issue<D, kPBF16>(o, pa, pv_b(nch - 1));
+      attn_wait<0>(o);
+      __syncthreads();  // the next stream's loads overwrite Q and the stages
+      g += nch;
+      ++nq;
     }
-    if (nch > 0) ++nq;
 
     // ---------------- epilogue: O / l -> global (optionally scattered rows), LSE
 #pragma unroll
