@@ -27,7 +27,7 @@ extern "C" {
 
 #define SVGB_BF16 0
 #define SVGB_F16 1
-#define SVGB_E4M3 2 /* fp8 e4m3 inputs (svgb_attn_fwd_fp8 only) */
+#define SVGB_E4M3 2 /* fp8 e4m3 inputs (svgb_attn_fwd_fp8 / svgb_attn_fwd_fp8_gather only) */
 #define SVGB_F32 3  /* fp32 storage (transformer-block glue ops only) */
 
 /* element-mask families for the SVG1 band plan (reference generate_temporal_head_mask_mod) */
@@ -122,14 +122,23 @@ int svgb_attn_fwd_gather(const void* q, const void* k, const void* v, void* o, f
 /* FP8 attention (BASELINE config 5; the reference has no FP8 sparse attention, README.md:117).  q8,k8,v8 are
  * e4m3 bytes [BH,S,D] (D = 128) with per-head dequantisation scales (x ~= x8 * scale[h]); QK^T runs as e4m3
  * wgmma, each V tile is widened to fp16 in shared memory and PV runs in fp16 (P in fp16), the output is
- * bf16.  Any plan kind except the row-gather one.  svgb_quantize_e4m3 produces the inputs: per-head absmax
- * scaling (scale = absmax / 448), round-to-nearest, saturating. */
+ * bf16.  Any plan kind (a row-gather plan runs with identity rows).  svgb_quantize_e4m3 produces the inputs:
+ * per-head absmax scaling (scale = absmax / 448), round-to-nearest, saturating. */
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
 int svgb_attn_fwd_fp8(const void* q8, const void* k8, const void* v8, const float* q_scale, const float* k_scale,
                       const float* v_scale, void* o, float* lse, const int32_t* o_rows, int BH, int S, int D,
                       long long row_stride, long long head_stride, long long o_row_stride,
                       long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                       void* stream);
+/* FP8 form of svgb_attn_fwd_gather (plan from svgb_attn_plan_varblock_gather, required): e4m3 rows are gathered
+ * through q_rows / kv_rows exactly as there, so SVG2 runs in FP8 on the un-permuted quantised tensors.  Per-head
+ * absmax scales do not change under a row permutation, so the scales of the un-permuted tensors apply. */
+int svgb_attn_fwd_fp8_gather(const void* q8, const void* k8, const void* v8, const float* q_scale,
+                             const float* k_scale, const float* v_scale, void* o, float* lse, const int32_t* q_rows,
+                             const int32_t* kv_rows, const int32_t* o_rows, int BH, int S, int D,
+                             long long row_stride, long long head_stride, long long o_row_stride,
+                             long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
+                             void* stream);
 
 /* density of a variable-block map (density_calculation, svg/kmeans_utils.py:13-31) -> float [BH] */
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

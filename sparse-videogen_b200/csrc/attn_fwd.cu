@@ -391,14 +391,12 @@ template <int D, int DT>
 static int launch_attn(const CUtensorMap& qm, const CUtensorMap& km, const CUtensorMap& vm,
                        const AttnArgs& args, dim3 grid, cudaStream_t stream) {
   using Cfg = AttnCfg<D, DT>;
-  if constexpr (DT != DT_E4M3) {
-    if (args.gather) {
-      auto kern = attn_fwd_kernel<D, DT, true>;
-      SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-      kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args);
-      SVGB_LAUNCH_OK();
-      return 0;
-    }
+  if (args.gather) {
+    auto kern = attn_fwd_kernel<D, DT, true>;
+    SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args);
+    SVGB_LAUNCH_OK();
+    return 0;
   }
   auto kern = attn_fwd_kernel<D, DT, false>;
   SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
@@ -430,7 +428,7 @@ int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const v
   if (encode_tmap_hsd(&vm, v, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
   dim3 grid(grid_x, BH);
   if (dtype == SVGB_E4M3) {
-    SVGB_REQUIRE(D == 128 && !a.gather, "the e4m3 path needs head_dim 128 and a non-gather plan");
+    SVGB_REQUIRE(D == 128, "the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle", D);
     return launch_attn<128, DT_E4M3>(qm, km, vm, a, grid, st);
   }
   if (D == 128) {
@@ -655,6 +653,18 @@ int svgb_attn_fwd_gather(const void* q, const void* k, const void* v, void* o, f
                          void* stream) {
   return attn_fwd_entry(q, k, v, nullptr, nullptr, nullptr, o, lse, q_rows, kv_rows, o_rows, dtype, BH, S, D,
                         row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan, plan_ws, stream);
+}
+
+int svgb_attn_fwd_fp8_gather(const void* q8, const void* k8, const void* v8, const float* q_scale,
+                             const float* k_scale, const float* v_scale, void* o, float* lse, const int32_t* q_rows,
+                             const int32_t* kv_rows, const int32_t* o_rows, int BH, int S, int D,
+                             long long row_stride, long long head_stride, long long o_row_stride,
+                             long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
+                             void* stream) {
+  SVGB_REQUIRE(q_scale && k_scale && v_scale, "fp8 attention needs the three per-head scale vectors");
+  SVGB_REQUIRE(plan && plan->kind == 3, "svgb_attn_fwd_fp8_gather needs a plan from svgb_attn_plan_varblock_gather");
+  return attn_fwd_entry(q8, k8, v8, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, SVGB_E4M3, BH, S,
+                        D, row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

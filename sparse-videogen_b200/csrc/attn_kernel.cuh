@@ -14,11 +14,15 @@
 // one-chunk-at-a-time loop (rescale O by alpha(j+1), then accumulate P(j+1) V(j+1)).
 // FP8 (e4m3) inputs: Q K^T runs on e4m3 wgmma (k32); wgmma has no MN-major 8-bit B operand, so each V tile is
 // widened to fp16 in shared memory (two buffers: V(j+1) is widened while P V(j) reads V(j)) and P V runs in fp16.
+// Both loaders serve e4m3: the row gather copies 128-byte e4m3 rows into the same swizzled image TMA writes, and
+// the widening step that follows is shared.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
+
+#include <type_traits>
 
 #include "attn_common.cuh"
 #include "ptx.cuh"
@@ -119,7 +123,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   constexpr bool BF16 = DT != DT_F16;  // output format (fp8 inputs produce bf16 output)
   constexpr bool FP8 = DT == DT_E4M3;
   constexpr bool kPBF16 = DT == DT_BF16;  // format of P and V in the P V product (fp8: fp16)
-  static_assert(!(FP8 && kGather), "row-gather loads are 16-bit only");
+  using Elem = typename std::conditional<FP8, uint8_t, uint16_t>::type;  // storage element of Q / K / V
   const int bh = blockIdx.y;
   const int n_items = args.item_count[bh * args.counts_stride];
   if (static_cast<int>(blockIdx.x) >= n_items) return;
@@ -159,21 +163,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   const float c = args.scale_log2 * (args.q_scale ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[bh]) : 1.f);
   const float vs = args.v_scale ? __ldg(&args.v_scale[bh]) : 1.f;
   const int mode = args.mask_mode, m0 = args.m0, m1 = args.m1, m2 = args.m2;
-  const uint16_t* kp = static_cast<const uint16_t*>(args.k_ptr) + bh * args.in_head_stride;
-  const uint16_t* vp = static_cast<const uint16_t*>(args.v_ptr) + bh * args.in_head_stride;
+  const Elem* kp = static_cast<const Elem*>(args.k_ptr) + bh * args.in_head_stride;
+  const Elem* vp = static_cast<const Elem*>(args.v_ptr) + bh * args.in_head_stride;
   const int* kv_rows = (kGather && args.kv_rows) ? args.kv_rows + static_cast<size_t>(bh) * args.S : nullptr;
   const int2* __restrict__ runs = args.chunks + item.z;
   const int nruns = item.w;
 
-  // gather: piece p (16 B) of row r -> panel p/8, byte r*128 + ((p%8) ^ (r%8))*16
-  auto gather_rows = [&](uint32_t dst, const uint16_t* src_base, bool two, const uint16_t* src2, uint32_t dst2) {
-    constexpr int kPieces = D / 8;
+  // gather: piece p (16 B) of row r -> panel p/8, byte r*128 + ((p%8) ^ (r%8))*16; a row is kRowBytes bytes
+  // (e4m3 at D = 128: 8 pieces, one panel)
+  auto gather_rows = [&](uint32_t dst, const Elem* src_base, bool two, const Elem* src2, uint32_t dst2) {
+    constexpr int kPieces = Cfg::kRowBytes / 16;
+    constexpr int kPieceElems = 16 / Cfg::kElemBytes;
 #pragma unroll 4
     for (int i = tid; i < 128 * kPieces; i += 256) {
       const int r = i / kPieces, pc = i % kPieces;
       const int src = ctl->src[r];
       const uint32_t off = (pc >> 3) * Cfg::kPanelBytes + r * 128 + (((pc & 7) ^ (r & 7)) << 4);
-      const long long so = static_cast<long long>(src < 0 ? 0 : src) * args.in_row_stride + pc * 8;
+      const long long so = static_cast<long long>(src < 0 ? 0 : src) * args.in_row_stride + pc * kPieceElems;
       cp_async16(dst + off, src_base + so, src >= 0 ? 16u : 0u);
       if (two) cp_async16(dst2 + off, src2 + so, src >= 0 ? 16u : 0u);
     }
@@ -362,7 +368,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
           ctl->src[tid] = tid < nr ? (q_rows ? __ldg(&q_rows[qr]) : qr) : -1;
         }
         __syncthreads();
-        gather_rows(sQ, static_cast<const uint16_t*>(args.q_ptr) + bh * args.in_head_stride, false, nullptr, 0);
+        gather_rows(sQ, static_cast<const Elem*>(args.q_ptr) + bh * args.in_head_stride, false, nullptr, 0);
         __syncthreads();
       } else if (tid == 0) {
         const uint32_t qb = smem_u32(&ctl->q_full);

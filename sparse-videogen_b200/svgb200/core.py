@@ -180,8 +180,11 @@ def quantize_e4m3(x: torch.Tensor):
 
 
 def attn_fwd_fp8(q8, k8, v8, q_scale, k_scale, v_scale, plan: AttnPlan, *, o_rows: Optional[torch.Tensor] = None,
+                 q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
                  return_lse: bool = False, sm_scale: Optional[float] = None):
-    """FP8 (e4m3) block-sparse attention: q8,k8,v8 uint8 [B,H,S,128] + per-head scales -> bf16 [B,H,S,128]."""
+    """FP8 (e4m3) block-sparse attention: q8,k8,v8 uint8 [B,H,S,128] + per-head scales -> bf16 [B,H,S,128].
+    With a gather plan (plan_varblock(..., gather=True)), q_rows / kv_rows read the rows through index vectors, as in
+    attn_fwd."""
     _need_cuda(q8, k8, v8, q_scale, k_scale, v_scale)
     if not (q8.dtype == k8.dtype == v8.dtype == torch.uint8) or not (q8.shape == k8.shape == v8.shape):
         raise SvgbError("q8, k8, v8 must be uint8 tensors of one shape")
@@ -196,10 +199,23 @@ def attn_fwd_fp8(q8, k8, v8, q_scale, k_scale, v_scale, plan: AttnPlan, *, o_row
     # by the allocator for the next one and alias two operands)
     q8c, k8c, v8c = q8.contiguous(), k8.contiguous(), v8.contiguous()
     sqc, skc, svc = (t.to(torch.float32).contiguous() for t in (q_scale, k_scale, v_scale))
-    check(lib().svgb_attn_fwd_fp8(q8c.data_ptr(), k8c.data_ptr(), v8c.data_ptr(), sqc.data_ptr(), skc.data_ptr(),
-                                  svc.data_ptr(), o.data_ptr(), _p(lse), _p(o_rows), BH, S, D,
-                                  D, S * D, D, S * D, scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q8)),
-          "svgb_attn_fwd_fp8")
+    if plan.desc.kind == 3:
+        if q_rows is not None:
+            q_rows = q_rows.reshape(BH, S).to(torch.int32).contiguous()
+        if kv_rows is not None:
+            kv_rows = kv_rows.reshape(BH, S).to(torch.int32).contiguous()
+        check(lib().svgb_attn_fwd_fp8_gather(q8c.data_ptr(), k8c.data_ptr(), v8c.data_ptr(), sqc.data_ptr(),
+                                             skc.data_ptr(), svc.data_ptr(), o.data_ptr(), _p(lse), _p(q_rows),
+                                             _p(kv_rows), _p(o_rows), BH, S, D, D, S * D, D, S * D, scale,
+                                             C.byref(plan.desc), plan.ws.data_ptr(), _stream(q8)),
+              "svgb_attn_fwd_fp8_gather")
+    else:
+        if q_rows is not None or kv_rows is not None:
+            raise SvgbError("q_rows / kv_rows need a gather plan (plan_varblock(..., gather=True))")
+        check(lib().svgb_attn_fwd_fp8(q8c.data_ptr(), k8c.data_ptr(), v8c.data_ptr(), sqc.data_ptr(), skc.data_ptr(),
+                                      svc.data_ptr(), o.data_ptr(), _p(lse), _p(o_rows), BH, S, D,
+                                      D, S * D, D, S * D, scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q8)),
+              "svgb_attn_fwd_fp8")
     _bump()
     return (o, lse) if return_lse else o
 

@@ -102,3 +102,24 @@ def dynamic_block_sparse_fwd_flashinfer(q, k, v, block_mask_map, block_row_sz, b
 def dynamic_block_sparse_fwd_triton(q, k, v, dynamic_map, qc_size, kc_size):
     """svg/kmeans_utils.py:1205-1316 (same semantics, same kernel here)."""
     return dynamic_block_sparse_fwd_flashinfer(q, k, v, dynamic_map, qc_size, kc_size, is_cpu=False)
+
+
+def dynamic_block_sparse_fwd_flashinfer_fp8(q, k, v, block_mask_map, block_row_sz, block_col_sz, is_cpu=True):
+    """dynamic_block_sparse_fwd_flashinfer in FP8: q, k, v (already in cluster order) quantised to e4m3 per head and
+    run on the e4m3 kernel; head_dim 128 only; the result comes back in q.dtype."""
+    from .models.common import check_fp8_head_dim, quantize_qkv
+
+    B, H, S, D = q.shape
+    check_fp8_head_dim(D)
+    QC, KC = block_row_sz.shape[-1], block_col_sz.shape[-1]
+    assert block_mask_map.shape == (B, H, QC, KC)
+    dev = q.device
+    plan = core.plan_varblock(block_mask_map.to(dev).reshape(B * H, QC, KC), block_row_sz.to(dev).reshape(B * H, QC),
+                              block_col_sz.to(dev).reshape(B * H, KC), S)
+    (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(q, k, v)
+    return core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, plan).to(q.dtype)
+
+
+def dynamic_block_sparse_fwd_triton_fp8(q, k, v, dynamic_map, qc_size, kc_size):
+    """dynamic_block_sparse_fwd_triton in FP8 (see dynamic_block_sparse_fwd_flashinfer_fp8)."""
+    return dynamic_block_sparse_fwd_flashinfer_fp8(q, k, v, dynamic_map, qc_size, kc_size, is_cpu=False)

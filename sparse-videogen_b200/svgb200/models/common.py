@@ -39,6 +39,25 @@ def sparse_flex_attention(query, key, value, block_mask: BandMask):
     return core.attn_fwd(query, key, value, block_mask.plan)
 
 
+def check_fp8_head_dim(D):
+    if D != 128:
+        raise core.SvgbError(f"fp8 attention needs head_dim 128 (got {D}): the e4m3 kernel is built for 128-byte rows")
+
+
+def quantize_qkv(query, key, value):
+    """Per-head e4m3 quantisation of Q, K, V -> ((q8, s_q), (k8, s_k), (v8, s_v))."""
+    return tuple(core.quantize_e4m3(t) for t in (query, key, value))
+
+
+def sparse_flex_attention_fp8(query, key, value, block_mask: BandMask):
+    """sparse_flex_attention in FP8: Q, K, V quantised to e4m3 per head, the band plan run on the e4m3 kernel.  The
+    kernel writes bf16; the result comes back in query.dtype."""
+    check_fp8_head_dim(query.shape[-1])
+    (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(query, key, value)
+    o = core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, block_mask.plan)
+    return o.to(query.dtype)
+
+
 def dense_attention(query, key, value, seg_lens=None):
     """Dense fall-back (b11).  seg_lens: optional list of segment lengths that only attend inside
     themselves (HunyuanVideo's padded-prompt varlen split, hyvideo/attention.py:308-316,807-875)."""
@@ -82,16 +101,20 @@ class SVG1Core:
     """Sparse VideoGen v1 attention core: online profiling -> head placement -> one band mask -> inverse
     placement (svg/models/hyvideo/attention.py:473-524; wan :284-328; cosmos :200-238; cog :164-196).
 
-    Subclasses fix the text layout (`text_first`, `smse_layout`) and build `block_mask`."""
+    Subclasses fix the text layout (`text_first`, `smse_layout`) and build `block_mask`.
+
+    fp8=True runs the band attention on e4m3 Q, K, V (sparse_flex_attention_fp8, head_dim 128 only); sample_mse, the
+    placements and the dense branch stay 16-bit, so the head choice is the 16-bit core's."""
 
     text_first = False
     smse_layout = 0  # svgb_sample_mse layout id (0 = HY text-last band 1.5*P, 1 = WAN sink band 2*P)
 
     def __init__(self, context_length, num_frame, frame_size, num_sampled_rows=64, sample_mse_max_row=10000,
-                 first_layers_fp=0, first_times_fp=0, layer_idx=0):
+                 first_layers_fp=0, first_times_fp=0, layer_idx=0, fp8=False):
         self.context_length, self.num_frame, self.frame_size = context_length, num_frame, frame_size
         self.num_sampled_rows, self.sample_mse_max_row = num_sampled_rows, sample_mse_max_row
         self.first_layers_fp, self.first_times_fp, self.layer_idx = first_layers_fp, first_times_fp, layer_idx
+        self.fp8 = fp8
         self.block_mask: Optional[BandMask] = None
 
     # -- reference method names ---------------------------------------------------------------------
@@ -108,6 +131,8 @@ class SVG1Core:
         return mse.view(2, cfg, H).to(query.dtype)
 
     def sparse_flex_attention(self, query, key, value, block_mask):
+        if self.fp8:
+            return sparse_flex_attention_fp8(query, key, value, block_mask)
         return sparse_flex_attention(query, key, value, block_mask)
 
     def fast_sparse_head_placement(self, query, key, value, query_out, key_out, value_out, best_mask_idx,
@@ -282,12 +307,17 @@ class SAPCore:
 
     k-means on Q and K -> centroid top-p dynamic map -> permute Q,K,V by cluster -> variable-block sparse
     attention -> inverse permutation.  Here the inverse permutation is fused into the attention epilogue
-    (o_rows) and the text tokens ride the same gather (no write-back copies)."""
+    (o_rows) and the text tokens ride the same gather (no write-back copies).
+
+    fp8=True runs the sparse attention on e4m3 Q, K, V (head_dim 128 only): the un-permuted tensors are quantised per
+    head and the row-gather kernel reads them through the cluster permutations, so no permuted copy is made.
+    k-means, the dynamic map and the dense branch stay 16-bit, so the maps and permutations are the 16-bit core's."""
 
     def __init__(self, context_length, num_frame, frame_size, num_q_centroids, num_k_centroids, top_p_kmeans,
                  min_kc_ratio, kmeans_iter_init, kmeans_iter_step, prompt_length=0, zero_step_kmeans_init=False,
                  first_layers_fp=0, first_times_fp=0, layer_idx=0, state: Optional[KMeansState] = None,
-                 logging_file: Optional[str] = None):
+                 logging_file: Optional[str] = None, fp8=False):
+        self.fp8 = fp8
         self.context_length, self.num_frame, self.frame_size = context_length, num_frame, frame_size
         self.prompt_length = prompt_length
         self.logging_file = logging_file  # density JSONL (hyvideo/attention.py:786-802); None = off
@@ -339,6 +369,8 @@ class SAPCore:
 
         cfg, H, S, D = query.shape
         assert cfg == 1, "Batch size must be 1 for kmeans block sparse attention"
+        if self.fp8:
+            check_fp8_head_dim(D)
         layer_idx = self.layer_idx if layer_idx is None else layer_idx
         ctx, V = self.context_length, self.num_frame * self.frame_size
         dev = query.device
@@ -364,13 +396,21 @@ class SAPCore:
             dyn[:, -1, -1] = True
             row_sz = torch.cat([row_sz, extra], dim=1)
             col_sz = torch.cat([col_sz, extra], dim=1)
-        with time_logging_decorator("Level 3 - semantic aware permutation"):
-            qp = core.permute_gather(query, q_perm)
-            kp = core.permute_gather(key, k_perm)
-            vp = core.permute_gather(value, k_perm)
-        with time_logging_decorator("Level 3 - sparse flashinfer attention"):
-            plan = core.plan_varblock(dyn, row_sz, col_sz, S)
-            out = core.attn_fwd(qp, kp, vp, plan, o_rows=q_perm)  # inverse permutation fused into the store
+        if self.fp8:
+            with time_logging_decorator("Level 3 - fp8 quantization"):
+                (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(query, key, value)
+            with time_logging_decorator("Level 3 - sparse flashinfer attention"):
+                plan = core.plan_varblock(dyn, row_sz, col_sz, S, gather=True)
+                out = core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, plan, q_rows=q_perm, kv_rows=k_perm,
+                                        o_rows=q_perm).to(query.dtype)
+        else:
+            with time_logging_decorator("Level 3 - semantic aware permutation"):
+                qp = core.permute_gather(query, q_perm)
+                kp = core.permute_gather(key, k_perm)
+                vp = core.permute_gather(value, k_perm)
+            with time_logging_decorator("Level 3 - sparse flashinfer attention"):
+                plan = core.plan_varblock(dyn, row_sz, col_sz, S)
+                out = core.attn_fwd(qp, kp, vp, plan, o_rows=q_perm)  # inverse permutation fused into the store
         self.last = {"dynamic_map": dyn, "q_sizes": row_sz, "k_sizes": col_sz, "q_sorted_indices": q_perm,
                      "k_sorted_indices": k_perm}
         if self.logging_file is not None:

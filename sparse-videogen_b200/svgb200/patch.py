@@ -48,6 +48,18 @@ def flex_attention(query, key, value, block_mask=None, **kw):
     return sparse_flex_attention(query, key, value, block_mask)
 
 
+def flex_attention_fp8(query, key, value, block_mask=None, **kw):
+    """flex_attention with the band attention on e4m3 Q, K, V (models.common.sparse_flex_attention_fp8)."""
+    from .models.common import BandMask, sparse_flex_attention_fp8
+
+    if not isinstance(block_mask, BandMask):
+        raise TypeError("svgb200.patch.flex_attention_fp8 needs the BandMask returned by the patched "
+                        f"prepare_flexattention (got {type(block_mask).__name__}); rebuild block_mask after patch.install()")
+    if kw:
+        raise TypeError(f"unsupported flex_attention arguments: {sorted(kw)}")
+    return sparse_flex_attention_fp8(query, key, value, block_mask)
+
+
 def flashinfer_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv):
     """hyvideo/attention.py:807-875: dense attention inside each cu_seqlens segment, q,k,v [B,H,S,D]."""
     from .models.common import dense_attention
@@ -81,18 +93,29 @@ def _model_of(module):
     return None
 
 
-def install(module, sample_mse: bool = True) -> list:
+_NAMES_FP8 = {
+    "dynamic_block_sparse_fwd_flashinfer": _ku.dynamic_block_sparse_fwd_flashinfer_fp8,
+    "dynamic_block_sparse_fwd_triton": _ku.dynamic_block_sparse_fwd_triton_fp8,
+}
+
+
+def install(module, sample_mse: bool = True, fp8: bool = False) -> list:
     """Replace every operator name the module already defines (the reference resolves them as module globals,
     svg/models/hyvideo/attention.py:12-28).  Besides the kernels this covers the module-level attention entry points
     `flex_attention`, `prepare_flexattention`, `flashinfer_varlen_func`, `flash_attn_varlen_func`, and — with
     sample_mse=True — the processors' `sample_mse` method (the reference version needs the materialised
-    [10000, S] profiling masks in `attention_masks`; ours evaluates them analytically).  Returns the names replaced."""
+    [10000, S] profiling masks in `attention_masks`; ours evaluates them analytically).  fp8=True installs FP8 (e4m3,
+    head_dim 128) versions of the sparse attention calls, `flex_attention` and `dynamic_block_sparse_fwd_flashinfer` /
+    `_triton`; profiling, k-means, the maps, the permutations and the dense calls stay 16-bit.  Returns the names
+    replaced."""
     done = []
-    for name, fn in _NAMES.items():
+    names = {**_NAMES, **_NAMES_FP8} if fp8 else _NAMES
+    for name, fn in names.items():
         if hasattr(module, name):
             setattr(module, name, fn)
             done.append(name)
-    for name, fn in (("flex_attention", flex_attention), ("flashinfer_varlen_func", flashinfer_varlen_func),
+    for name, fn in (("flex_attention", flex_attention_fp8 if fp8 else flex_attention),
+                     ("flashinfer_varlen_func", flashinfer_varlen_func),
                      ("flash_attn_varlen_func", flash_attn_varlen_func)):
         if hasattr(module, name):
             setattr(module, name, fn)
