@@ -13,7 +13,7 @@
  *   - no function allocates device memory or synchronises the device: the caller provides the
  *     workspace (sizes from the *_bytes queries) and the cudaStream_t (passed as void*).
  *   - integer outputs (labels, permutations, plans, maps) are bit-exact, deterministic.
- *   - dtype: SVGB_BF16 or SVGB_F16 for q/k/v/o.
+ *   - dtype: SVGB_BF16 or SVGB_F16 for q/k/v/o (svgb_attn_fwd also takes SVGB_E4M3 inputs).
  */
 #ifndef SVGB200_H_
 #define SVGB200_H_
@@ -27,7 +27,7 @@ extern "C" {
 
 #define SVGB_BF16 0
 #define SVGB_F16 1
-#define SVGB_E4M3 2 /* fp8 e4m3 inputs (svgb_attn_fwd_fp8 / svgb_attn_fwd_fp8_gather only) */
+#define SVGB_E4M3 2 /* fp8 e4m3 q/k/v of svgb_attn_fwd (with per-head scales) */
 #define SVGB_F32 3  /* fp32 storage (transformer-block glue ops only) */
 
 /* element-mask families for the SVG1 band plan (reference generate_temporal_head_mask_mod) */
@@ -53,8 +53,11 @@ int svgb_device_check(int* sm_major, int* sm_minor, int* num_sms);
 /* ---- attention plans -------------------------------------------------------------------- */
 /* Host-side descriptor of a device-resident plan (filled by the plan functions, read by
  * svgb_attn_fwd).  Plain data; copyable. */
+#define SVGB_PLAN_VARBLOCK 1 /* variable-block map, TMA chunks (svgb_attn_plan_varblock) */
+#define SVGB_PLAN_BAND 2     /* element-exact band mask (svgb_attn_plan_band) */
+#define SVGB_PLAN_GATHER 3   /* variable-block map, row gather (svgb_attn_plan_varblock_gather) */
 typedef struct svgb_plan {
-  int32_t kind;          /* 1 = variable-block (TMA chunks), 2 = band, 3 = variable-block (row gather) */
+  int32_t kind;          /* SVGB_PLAN_* */
   int32_t BH, S;
   int32_t max_items;     /* grid.x of the attention launch */
   int32_t items_stride;  /* 0 when one plan serves every head */
@@ -78,7 +81,7 @@ int svgb_attn_plan_varblock(const uint8_t* map, const int32_t* row_sz, const int
 
 /* Same map, lowered for the row-gather kernel path: the selected key ranges are kept as runs and the
  * kernel gathers exactly-full 128-key chunks across run boundaries with cp.async (no padded tail chunk per
- * run), optionally through row-index vectors (svgb_attn_fwd_gather) so the cluster permutation of Q, K, V
+ * run), optionally through row-index vectors (q_rows / kv_rows of svgb_attn_fwd) so the cluster permutation of Q, K, V
  * (permute_tensor_by_labels_triton x3, svg/models/hyvideo/attention.py:651-653) never materialises. */
 int svgb_attn_plan_varblock_gather(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH,
                                    int S, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
@@ -99,46 +102,28 @@ int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, vo
  *           s*row_stride + d.  [B,H,S,D] contiguous: row_stride=D, head_stride=S*D.
  *           [S,H,D]: row_stride=H*D, head_stride=D.   D in {64,128}; base pointers 16-B aligned,
  *           strides multiples of 8 elements.
- *   o     : same addressing with its own strides.
+ *   o     : same addressing with its own strides; 16-byte aligned, strides multiples of 8 elements.
  *   o_rows: optional int32 [BH,S]; when non-NULL output row for query row s is o_rows[h,s]
  *           (fuses apply_inverse_permutation_triton, svg/kernels/triton/permute.py:131-170).
  *   lse   : optional float [BH,S], natural-log log-sum-exp of the scaled scores.
- *   plan  : host pointer. */
-int svgb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
+ *   plan  : host pointer, any SVGB_PLAN_* kind.
+ * Row gathers (SVGB_PLAN_GATHER only; NULL = identity): row r of the plan's (cluster-sorted) query order is read
+ *   from q[h, q_rows[h,r]], key/value row r from k/v[h, kv_rows[h,r]], and written to o[h, o_rows[h,r]] — pass
+ *   the argsort of the q-labels as q_rows AND o_rows and the argsort of the k-labels as kv_rows to run SVG2
+ *   attention directly on the un-permuted tensors.  q_rows / kv_rows with another plan kind are an error.
+ * FP8 (dtype SVGB_E4M3; BASELINE config 5, the reference has no FP8 sparse attention, README.md:117): q,k,v are
+ *   e4m3 bytes (D = 128) with per-head dequantisation scales q_scale, k_scale, v_scale float [BH] (x ~= x8 *
+ *   scale[h]), all three required; QK^T runs as e4m3 wgmma, each V tile is widened to fp16 in shared memory and
+ *   PV runs in fp16 (P in fp16); o is bf16.  Per-head absmax scales do not change under a row permutation, so
+ *   the scales of the un-permuted tensors serve row gathers too.  16-bit dtypes take no scales (pass NULL; o has
+ *   the input dtype).  svgb_quantize_e4m3 produces the inputs: per-head absmax scaling (scale = absmax / 448),
+ *   round-to-nearest, saturating. */
+int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
+                  const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
-                  long long head_stride, long long o_row_stride, long long o_head_stride,
-                  float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream);
-
-/* Gather form (plan from svgb_attn_plan_varblock_gather).  Row r of the plan's (cluster-sorted) query order
- * is read from q[h, q_rows[h,r]] (q_rows NULL: identity), key/value row r from k/v[h, kv_rows[h,r]], and the
- * output row is written to o[h, o_rows[h,r]] — pass the argsort of the q-labels as q_rows AND o_rows and the
- * argsort of the k-labels as kv_rows to run SVG2 attention directly on the un-permuted tensors. */
-int svgb_attn_fwd_gather(const void* q, const void* k, const void* v, void* o, float* lse,
-                         const int32_t* q_rows, const int32_t* kv_rows, const int32_t* o_rows, int dtype,
-                         int BH, int S, int D, long long row_stride, long long head_stride,
-                         long long o_row_stride, long long o_head_stride, float sm_scale,
-                         const svgb_plan* plan, const void* plan_ws, void* stream);
-
-/* FP8 attention (BASELINE config 5; the reference has no FP8 sparse attention, README.md:117).  q8,k8,v8 are
- * e4m3 bytes [BH,S,D] (D = 128) with per-head dequantisation scales (x ~= x8 * scale[h]); QK^T runs as e4m3
- * wgmma, each V tile is widened to fp16 in shared memory and PV runs in fp16 (P in fp16), the output is
- * bf16.  Any plan kind (a row-gather plan runs with identity rows).  svgb_quantize_e4m3 produces the inputs:
- * per-head absmax scaling (scale = absmax / 448), round-to-nearest, saturating. */
+                  long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
+                  const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
-int svgb_attn_fwd_fp8(const void* q8, const void* k8, const void* v8, const float* q_scale, const float* k_scale,
-                      const float* v_scale, void* o, float* lse, const int32_t* o_rows, int BH, int S, int D,
-                      long long row_stride, long long head_stride, long long o_row_stride,
-                      long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
-                      void* stream);
-/* FP8 form of svgb_attn_fwd_gather (plan from svgb_attn_plan_varblock_gather, required): e4m3 rows are gathered
- * through q_rows / kv_rows exactly as there, so SVG2 runs in FP8 on the un-permuted quantised tensors.  Per-head
- * absmax scales do not change under a row permutation, so the scales of the un-permuted tensors apply. */
-int svgb_attn_fwd_fp8_gather(const void* q8, const void* k8, const void* v8, const float* q_scale,
-                             const float* k_scale, const float* v_scale, void* o, float* lse, const int32_t* q_rows,
-                             const int32_t* kv_rows, const int32_t* o_rows, int BH, int S, int D,
-                             long long row_stride, long long head_stride, long long o_row_stride,
-                             long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
-                             void* stream);
 
 /* density of a variable-block map (density_calculation, svg/kmeans_utils.py:13-31) -> float [BH] */
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

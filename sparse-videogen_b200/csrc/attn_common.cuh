@@ -239,41 +239,41 @@ struct ElemMask {
 };
 
 struct AttnArgs {
-  const int4* items;
+  const int4* items = nullptr;
   // variable-block plans: optional second stream per work item.  items2[i].y > 0 makes item i a DUAL item: two
   // single-tile streams (<= 128 rows each, usually the tails of two different q-blocks) share one CTA -- T0 runs
   // items[i], T1 runs items2[i], each with its own chunk list and its own K/V tiles through the common ring.
-  const int4* items2;
-  const int* item_count;
-  const int2* chunks;
-  int items_stride;   // 0: one plan shared by all heads (band masks); else items per head
-  int counts_stride;  // 0 or 1
-  void* o;
-  long long o_row_stride;   // elements
-  long long o_head_stride;  // elements
-  const int* o_rows;        // optional [BH, S]: output row for query row q (fused inverse permutation)
-  float* lse;               // optional [BH, S] (natural log), indexed like o rows
-  float scale_log2;         // softmax scale * log2(e)
-  int S;                    // query rows per head (indexing of o_rows / lse / q_index)
-  int mask_mode, m0, m1, m2;
-  const int* q_index;       // optional [S]: query position used by the element mask (sampled rows)
-  int out_f32;              // 1: o is fp32 (used for split-KV partials)
+  const int4* items2 = nullptr;
+  const int* item_count = nullptr;
+  const int2* chunks = nullptr;
+  int items_stride = 0;   // 0: one plan shared by all heads (band masks); else items per head
+  int counts_stride = 0;  // 0 or 1
+  void* o = nullptr;
+  long long o_row_stride = 0;   // elements
+  long long o_head_stride = 0;  // elements
+  const int* o_rows = nullptr;  // optional [BH, S]: output row for query row q (fused inverse permutation)
+  float* lse = nullptr;         // optional [BH, S] (natural log), indexed like o rows
+  float scale_log2 = 0;         // softmax scale * log2(e)
+  int S = 0;                    // query rows per head (indexing of o_rows / lse / q_index)
+  int mask_mode = 0, m0 = 0, m1 = 0, m2 = 0;
+  const int* q_index = nullptr;  // optional [S]: query position used by the element mask (sampled rows)
+  int out_f32 = 0;               // 1: o is fp32 (used for split-KV partials)
   // FP8 (e4m3) inputs: per-head dequantisation scales [BH]; s_q * s_k multiplies the logits, s_v the
   // output.  NULL for 16-bit inputs.
-  const float* q_scale;
-  const float* k_scale;
-  const float* v_scale;
-  // ---- gather mode (SVG2): `chunks` holds RUNS {src_start, cum_before} (+ a sentinel {0, total}) of the
-  // selected key ranges; K/V rows are gathered with cp.async into exactly-full 128-token chunks, optionally
-  // through row-index vectors so the cluster permutation of Q, K, V never materialises in HBM.
-  int gather;
-  const int* item_total;    // [BH * items_stride | items]: selected keys per item
-  const int* q_rows;        // optional [BH, S]: source row of (permuted) query row
-  const int* kv_rows;       // optional [BH, S]: source row of (permuted) key/value row
-  const void* q_ptr;        // raw tensors for the gather path ([BH,S,D] with the strides below)
-  const void* k_ptr;
-  const void* v_ptr;
-  long long in_row_stride, in_head_stride;  // elements
+  const float* q_scale = nullptr;
+  const float* k_scale = nullptr;
+  const float* v_scale = nullptr;
+  // ---- gather mode (SVG2; attn_fwd_kernel<..., kGather = true>): `chunks` holds RUNS {src_start, cum_before}
+  // (+ a sentinel {0, total}) of the selected key ranges; K/V rows are gathered with cp.async into exactly-full
+  // 128-token chunks, optionally through row-index vectors so the cluster permutation of Q, K, V never
+  // materialises in HBM.
+  const int* item_total = nullptr;  // [BH * items_stride | items]: selected keys per item; non-NULL = gather mode
+  const int* q_rows = nullptr;      // optional [BH, S]: source row of (permuted) query row
+  const int* kv_rows = nullptr;     // optional [BH, S]: source row of (permuted) key/value row
+  const void* q_ptr = nullptr;      // raw tensors for the gather path ([BH,S,D] with the strides below)
+  const void* k_ptr = nullptr;
+  const void* v_ptr = nullptr;
+  long long in_row_stride = 0, in_head_stride = 0;  // elements
 };
 
 }  // namespace svgb

@@ -1,7 +1,5 @@
 // Attention plans (device-built work lists), the attention launcher, density, and the tile
 // self-test.  See attn_kernel.cuh for the kernel itself.
-#include <stdlib.h>
-
 #include "../../include/svgb200.h"
 #include "attn_kernel.cuh"
 #include "host_common.h"
@@ -108,7 +106,7 @@ plan_lists_kernel(const uint8_t* __restrict__ map, const int* __restrict__ row_s
 
 __global__ void plan_items_kernel(const int* __restrict__ row_sz, const int* __restrict__ nch_all,
                                   const int* __restrict__ tot_all, int QC, int max_items, int chunk_cap,
-                                  int pair_tails, int* __restrict__ counts,
+                                  int* __restrict__ counts,
                                   int4* __restrict__ items, int4* __restrict__ items2, int* __restrict__ item_total) {
   // TMA form (items2 != nullptr): a q-block of r rows becomes r/256 two-tile items (+ one more when r % 256 > 128,
   // its second tile partial) and, when 0 < r % 256 <= 128, a single-tile TAIL.  Tails are where k-means clusters
@@ -125,7 +123,7 @@ __global__ void plan_items_kernel(const int* __restrict__ row_sz, const int* __r
   __shared__ int s_total2, s_nlong;
   const int bh = blockIdx.x;
   row_sz += static_cast<size_t>(bh) * QC;
-  const bool pair = !gather && pair_tails;
+  const bool pair = !gather;
   for (int i = threadIdx.x; i < QC; i += blockDim.x) {
     nch_of[i] = nch_all[static_cast<size_t>(bh) * QC + i];
     rowoff[i] = row_sz[i];  // staged: the serial pass below turns the sizes into offsets in place
@@ -391,14 +389,7 @@ template <int D, int DT>
 static int launch_attn(const CUtensorMap& qm, const CUtensorMap& km, const CUtensorMap& vm,
                        const AttnArgs& args, dim3 grid, cudaStream_t stream) {
   using Cfg = AttnCfg<D, DT>;
-  if (args.gather) {
-    auto kern = attn_fwd_kernel<D, DT, true>;
-    SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args);
-    SVGB_LAUNCH_OK();
-    return 0;
-  }
-  auto kern = attn_fwd_kernel<D, DT, false>;
+  auto kern = args.item_total ? attn_fwd_kernel<D, DT, true> : attn_fwd_kernel<D, DT, false>;
   SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args);
   SVGB_LAUNCH_OK();
@@ -484,7 +475,7 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
                "plan too large for 32-bit chunk offsets");
   const int max_items = varblock_max_items(S, QC);
   const int cap = varblock_chunk_cap(S, KC);
-  plan->kind = gather ? 3 : 1;
+  plan->kind = gather ? SVGB_PLAN_GATHER : SVGB_PLAN_VARBLOCK;
   plan->BH = BH;
   plan->S = S;
   plan->max_items = max_items;
@@ -492,7 +483,7 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   plan->counts_stride = 1;
   plan->mask_mode = MASK_NONE;
   plan->m0 = gather ? (KC + 1) / 2 + 1 : 0;  // gather: upper bound of runs per q-block (kernel smem table)
-  plan->m1 = S / KC;                          // average key-cluster size (selects the softmax thread mapping)
+  plan->m1 = 0;
   plan->m2 = 0;
   plan->counts_off = 0;
   plan->items_off = align_up(sizeof(int) * BH, 256);
@@ -506,14 +497,12 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   const size_t smem1 = sizeof(int) * (KC + 1);
   const size_t smem2 = sizeof(int) * (2 * (QC + 1) + 2 * QC);
   SVGB_REQUIRE(smem1 <= 48 * 1024 && smem2 <= 48 * 1024, "QC/KC too large for the plan kernels (%zu / %zu B smem)", smem1, smem2);
-  // SVGB_ATTN_PAIR=0 keeps every tail a single-tile item (A/B switch for bring-up)
-  static const int pair_tails = [] { const char* e = getenv("SVGB_ATTN_PAIR"); return (e && e[0] == '0') ? 0 : 1; }();
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   plan_lists_kernel<<<dim3((QC + kPlanWarps - 1) / kPlanWarps, BH), kPlanWarps * 32, smem1, st>>>(map, row_sz, col_sz, QC, KC, cap, gather ? 1 : 0,
                                                                  reinterpret_cast<int2*>(ws + plan->chunks_off), nch_of, tot_of);
   SVGB_LAUNCH_OK();
   plan_items_kernel<<<BH, 256, smem2, st>>>(
-      row_sz, nch_of, tot_of, QC, max_items, cap, pair_tails, reinterpret_cast<int*>(ws + plan->counts_off),
+      row_sz, nch_of, tot_of, QC, max_items, cap, reinterpret_cast<int*>(ws + plan->counts_off),
       reinterpret_cast<int4*>(ws + plan->items_off), gather ? nullptr : reinterpret_cast<int4*>(ws + plan->aux_off),
       gather ? reinterpret_cast<int*>(ws + plan->aux_off) : nullptr);
   SVGB_LAUNCH_OK();
@@ -553,7 +542,7 @@ int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, vo
   const int n_chunks = (S + kChunkCols - 1) / kChunkCols;
   SVGB_REQUIRE(n_items <= n_items_cap, "internal: item count");
   SVGB_REQUIRE(static_cast<size_t>(n_items_cap) * n_chunks < (1ull << 31), "plan too large");
-  plan->kind = 2;
+  plan->kind = SVGB_PLAN_BAND;
   plan->BH = BH;
   plan->S = S;
   plan->max_items = n_items;
@@ -576,27 +565,31 @@ int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, vo
   return 0;
 }
 
-static int attn_fwd_entry(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
-                          const float* v_scale, void* o, float* lse,
-                          const int32_t* q_rows, const int32_t* kv_rows, const int32_t* o_rows, int dtype, int BH,
-                          int S, int D, long long row_stride, long long head_stride, long long o_row_stride,
-                          long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
-                          void* stream) {
+int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
+                  const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
+                  const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
+                  long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
+                  const svgb_plan* plan, const void* plan_ws, void* stream) {
   SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
-  SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16 || dtype == SVGB_E4M3, "dtype %d unsupported", dtype);
+  SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
+               "fp8 attention needs the three per-head scale vectors");
+  SVGB_REQUIRE(dtype == SVGB_E4M3 || (!q_scale && !k_scale && !v_scale),
+               "per-head scale vectors are for e4m3 inputs only (dtype %d)", dtype);
+  const bool gather = plan->kind == SVGB_PLAN_GATHER;
+  SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
+               "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");
   SVGB_REQUIRE(plan->S == S && (plan->items_stride == 0 || plan->BH == BH),
                "plan was built for BH=%d S=%d, called with BH=%d S=%d", plan->BH, plan->S, BH, S);
   SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && o_row_stride % 8 == 0 && o_head_stride % 8 == 0,
                "output must be 16-byte aligned with strides multiple of 8 elements");
-  SVGB_REQUIRE(plan->kind == 3 || (!q_rows && !kv_rows), "row gathers need a plan from svgb_attn_plan_varblock_gather");
-  SVGB_REQUIRE(plan->kind != 3 || plan->m0 <= AttnCfg<64>::kMaxRunsSmem, "gather plan has too many runs per q-block (%d)", plan->m0);
+  SVGB_REQUIRE(!gather || plan->m0 <= AttnCfg<64>::kMaxRunsSmem, "gather plan has too many runs per q-block (%d)", plan->m0);
   const char* ws = static_cast<const char*>(plan_ws);
   AttnArgs a;
   a.items = reinterpret_cast<const int4*>(ws + plan->items_off);
   a.item_count = reinterpret_cast<const int*>(ws + plan->counts_off);
   a.chunks = reinterpret_cast<const int2*>(ws + plan->chunks_off);
-  a.items2 = plan->kind == 1 ? reinterpret_cast<const int4*>(ws + plan->aux_off) : nullptr;
+  if (plan->kind == SVGB_PLAN_VARBLOCK) a.items2 = reinterpret_cast<const int4*>(ws + plan->aux_off);
+  if (gather) a.item_total = reinterpret_cast<const int*>(ws + plan->aux_off);
   a.items_stride = plan->items_stride;
   a.counts_stride = plan->counts_stride;
   a.o = o;
@@ -610,13 +603,9 @@ static int attn_fwd_entry(const void* q, const void* k, const void* v, const flo
   a.m0 = plan->m0;
   a.m1 = plan->m1;
   a.m2 = plan->m2;
-  a.q_index = nullptr;
-  a.out_f32 = 0;
   a.q_scale = q_scale;
   a.k_scale = k_scale;
   a.v_scale = v_scale;
-  a.gather = plan->kind == 3 ? 1 : 0;
-  a.item_total = plan->kind == 3 ? reinterpret_cast<const int*>(ws + plan->aux_off) : nullptr;
   a.q_rows = q_rows;
   a.kv_rows = kv_rows;
   a.q_ptr = q;
@@ -626,45 +615,6 @@ static int attn_fwd_entry(const void* q, const void* k, const void* v, const flo
   a.in_head_stride = head_stride;
   return attn_fwd_impl(q, S, row_stride, head_stride, k, v, S, row_stride, head_stride, dtype, BH, D, a,
                        plan->max_items, static_cast<cudaStream_t>(stream));
-}
-
-int svgb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
-                  const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
-                  long long head_stride, long long o_row_stride, long long o_head_stride,
-                  float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
-  return attn_fwd_entry(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, o_rows, dtype, BH, S, D,
-                        row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan, plan_ws, stream);
-}
-
-int svgb_attn_fwd_fp8(const void* q8, const void* k8, const void* v8, const float* q_scale, const float* k_scale,
-                      const float* v_scale, void* o, float* lse, const int32_t* o_rows, int BH, int S, int D,
-                      long long row_stride, long long head_stride, long long o_row_stride,
-                      long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
-                      void* stream) {
-  SVGB_REQUIRE(q_scale && k_scale && v_scale, "fp8 attention needs the three per-head scale vectors");
-  return attn_fwd_entry(q8, k8, v8, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, o_rows, SVGB_E4M3, BH, S,
-                        D, row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan, plan_ws, stream);
-}
-
-int svgb_attn_fwd_gather(const void* q, const void* k, const void* v, void* o, float* lse, const int32_t* q_rows,
-                         const int32_t* kv_rows, const int32_t* o_rows, int dtype, int BH, int S, int D,
-                         long long row_stride, long long head_stride, long long o_row_stride,
-                         long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
-                         void* stream) {
-  return attn_fwd_entry(q, k, v, nullptr, nullptr, nullptr, o, lse, q_rows, kv_rows, o_rows, dtype, BH, S, D,
-                        row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan, plan_ws, stream);
-}
-
-int svgb_attn_fwd_fp8_gather(const void* q8, const void* k8, const void* v8, const float* q_scale,
-                             const float* k_scale, const float* v_scale, void* o, float* lse, const int32_t* q_rows,
-                             const int32_t* kv_rows, const int32_t* o_rows, int BH, int S, int D,
-                             long long row_stride, long long head_stride, long long o_row_stride,
-                             long long o_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
-                             void* stream) {
-  SVGB_REQUIRE(q_scale && k_scale && v_scale, "fp8 attention needs the three per-head scale vectors");
-  SVGB_REQUIRE(plan && plan->kind == 3, "svgb_attn_fwd_fp8_gather needs a plan from svgb_attn_plan_varblock_gather");
-  return attn_fwd_entry(q8, k8, v8, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, SVGB_E4M3, BH, S,
-                        D, row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

@@ -50,7 +50,7 @@ int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S
 
 struct AttnArgs;
 // attention launch with independent query / key-value geometry (attn_fwd.cu); used by svgb_attn_fwd
-// and by sample_mse's split-KV passes.
+// and by sample_mse's split-KV passes.  Checks D and dtype; a.item_total != NULL selects the row-gather kernel.
 int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const void* k, const void* v, int Skv,
                   long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, int grid_x,
                   cudaStream_t st);

@@ -202,15 +202,11 @@ int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* 
   for (int var = 0; var < 3; ++var) {
     AttnArgs a;
     a.items = reinterpret_cast<const int4*>(w + L.items);
-    a.items2 = nullptr;
     a.item_count = reinterpret_cast<const int*>(w + L.counts);
     a.chunks = reinterpret_cast<const int2*>(w + (var == 0 ? L.chunks_plain : L.chunks_elem));
-    a.items_stride = 0;
-    a.counts_stride = 0;
     a.o = w + L.o_part + 4ull * var * BH * rows_per_head * D;
     a.o_row_stride = D;
     a.o_head_stride = static_cast<long long>(rows_per_head) * D;
-    a.o_rows = nullptr;
     a.lse = reinterpret_cast<float*>(w + L.lse_part) + static_cast<size_t>(var) * BH * rows_per_head;
     a.scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(D));
     a.S = rows_per_head;
@@ -220,12 +216,6 @@ int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* 
     a.m2 = layout == 2 ? (thres | (ctx << 12)) : thres;
     a.q_index = reinterpret_cast<const int*>(w + L.qidx);
     a.out_f32 = 1;
-    a.q_scale = a.k_scale = a.v_scale = nullptr;
-    a.gather = 0;
-    a.item_total = nullptr;
-    a.q_rows = a.kv_rows = nullptr;
-    a.q_ptr = a.k_ptr = a.v_ptr = nullptr;
-    a.in_row_stride = a.in_head_stride = 0;
     if (attn_fwd_impl(w + L.qg, rows_per_head, D, static_cast<long long>(rows_per_head) * D, k, v, S, D,
                       static_cast<long long>(S) * D, dtype, BH, D, a, L.nsplit, st))
       return -1;

@@ -14,6 +14,9 @@ from ._lib import Plan, SvgbError, check, lib
 MASK_NONE, MASK_HY, MASK_WAN, MASK_COG = 0, 1, 2, 3
 # SVG1 profiling masks (include/svgb200.h SVGB_MASK_PROF_*): the element masks of sample_mse, also accepted by plan_band
 MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_S, MASK_PROF_COG_T = 4, 5, 6, 7, 8, 9
+# svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
+PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER = 1, 2, 3
+_E4M3 = 2  # SVGB_E4M3 (the 16-bit dtype ids come from _dt)
 
 # launches issued through this module since import (bench.py reports it as gpu_launches)
 launch_count = 0
@@ -80,15 +83,13 @@ class AttnPlan:
 
 
 def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.Tensor, S: int,
-                  ws: Optional[torch.Tensor] = None, gather: bool = False, shared_scratch: bool = False) -> AttnPlan:
+                  gather: bool = False) -> AttnPlan:
     """block_map [BH,QC,KC] bool/uint8, row_sz [BH,QC], col_sz [BH,KC] (any int dtype) on GPU.
     gather=True lowers the map for the row-gather kernel path (exactly-full chunks, optional fused
     permutation through attn_fwd(..., q_rows=, kv_rows=)).
 
-    Workspace ownership: by default every plan gets its OWN device work list (torch's caching allocator makes the
-    per-call allocation free of cudaMalloc / syncs), so two plans of one shape can be held and executed in any
-    order or on different streams.  shared_scratch=True reuses one shape-keyed scratch buffer instead: only for
-    callers that execute the plan immediately, on the same stream, before building the next one of that shape."""
+    Every plan owns its device work list (torch's caching allocator makes the per-call allocation free of
+    cudaMalloc / syncs), so plans of one shape can be held and executed in any order or on different streams."""
     _need_cuda(block_map, row_sz, col_sz)
     BH, QC, KC = block_map.shape
     m = block_map.contiguous()
@@ -97,9 +98,7 @@ def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.T
     c = col_sz.reshape(BH, KC).to(torch.int32).contiguous()
     nbytes = C.c_size_t()
     check(lib().svgb_attn_plan_varblock_bytes(BH, S, QC, KC, C.byref(nbytes)), "plan_varblock_bytes")
-    if ws is None:
-        ws = (workspace(("vb", BH, S, QC, KC), nbytes.value, m.device) if shared_scratch
-              else torch.empty(nbytes.value, dtype=torch.uint8, device=m.device))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=m.device)
     desc = Plan()
     fn = lib().svgb_attn_plan_varblock_gather if gather else lib().svgb_attn_plan_varblock
     check(fn(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, S, QC, KC, ws.data_ptr(), ws.numel(), C.byref(desc),
@@ -123,10 +122,24 @@ def plan_band(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device
 # ----------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------
+def _attn(q, k, v, scales, o, dtype, plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows, return_lse, sm_scale):
+    """One svgb_attn_fwd launch; q, k, v and o share the row / head strides rs, hs (elements)."""
+    rows = [None if r is None else r.reshape(BH, S).to(torch.int32).contiguous() for r in (q_rows, kv_rows, o_rows)]
+    lse = torch.empty(BH, S, dtype=torch.float32, device=q.device) if return_lse else None
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    check(lib().svgb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), *map(_p, scales), o.data_ptr(), _p(lse),
+                              *map(_p, rows), dtype, BH, S, D, rs, hs, rs, hs, scale, C.byref(plan.desc),
+                              plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd")
+    _bump()
+    return (o, lse) if return_lse else o
+
+
 def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[torch.Tensor] = None,
              q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
              return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
-    """layout 'bhsd': q,k,v [B,H,S,D] contiguous;  'shd': [S,H,D] contiguous (ops API)."""
+    """layout 'bhsd': q,k,v [B,H,S,D] contiguous;  'shd': [S,H,D] contiguous (ops API).
+    o_rows scatters the output rows; q_rows / kv_rows gather the input rows and need a gather plan
+    (plan_varblock(..., gather=True)); all three are int [BH,S] (include/svgb200.h, svgb_attn_fwd)."""
     _need_cuda(q, k, v)
     if not (q.is_contiguous() and k.is_contiguous() and v.is_contiguous()):
         raise SvgbError("q, k, v must be contiguous")
@@ -141,27 +154,8 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     else:
         raise SvgbError(f"unknown layout {layout}")
     o = torch.empty_like(q) if out is None else out
-    lse = torch.empty(BH, S, dtype=torch.float32, device=q.device) if return_lse else None
-    if o_rows is not None:
-        o_rows = o_rows.reshape(BH, S).to(torch.int32).contiguous()
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    if plan.desc.kind == 3:
-        if q_rows is not None:
-            q_rows = q_rows.reshape(BH, S).to(torch.int32).contiguous()
-        if kv_rows is not None:
-            kv_rows = kv_rows.reshape(BH, S).to(torch.int32).contiguous()
-        check(lib().svgb_attn_fwd_gather(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse),
-                                         _p(q_rows), _p(kv_rows), _p(o_rows), _dt(q), BH, S, D, rs, hs, rs, hs,
-                                         scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
-              "svgb_attn_fwd_gather")
-    else:
-        if q_rows is not None or kv_rows is not None:
-            raise SvgbError("q_rows / kv_rows need a gather plan (plan_varblock(..., gather=True))")
-        check(lib().svgb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), _p(o_rows),
-                                  _dt(q), BH, S, D, rs, hs, rs, hs, scale, C.byref(plan.desc),
-                                  plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd")
-    _bump()
-    return (o, lse) if return_lse else o
+    return _attn(q, k, v, (None, None, None), o, _dt(q), plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows,
+                 return_lse, sm_scale)
 
 
 def quantize_e4m3(x: torch.Tensor):
@@ -189,35 +183,13 @@ def attn_fwd_fp8(q8, k8, v8, q_scale, k_scale, v_scale, plan: AttnPlan, *, o_row
     if not (q8.dtype == k8.dtype == v8.dtype == torch.uint8) or not (q8.shape == k8.shape == v8.shape):
         raise SvgbError("q8, k8, v8 must be uint8 tensors of one shape")
     B, H, S, D = q8.shape
-    BH = B * H
     o = torch.empty(B, H, S, D, dtype=torch.bfloat16, device=q8.device)
-    lse = torch.empty(BH, S, dtype=torch.float32, device=q8.device) if return_lse else None
-    if o_rows is not None:
-        o_rows = o_rows.reshape(BH, S).to(torch.int32).contiguous()
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
     # temporaries are bound to locals that outlive the launch call (a dropped .contiguous() copy could be recycled
     # by the allocator for the next one and alias two operands)
     q8c, k8c, v8c = q8.contiguous(), k8.contiguous(), v8.contiguous()
-    sqc, skc, svc = (t.to(torch.float32).contiguous() for t in (q_scale, k_scale, v_scale))
-    if plan.desc.kind == 3:
-        if q_rows is not None:
-            q_rows = q_rows.reshape(BH, S).to(torch.int32).contiguous()
-        if kv_rows is not None:
-            kv_rows = kv_rows.reshape(BH, S).to(torch.int32).contiguous()
-        check(lib().svgb_attn_fwd_fp8_gather(q8c.data_ptr(), k8c.data_ptr(), v8c.data_ptr(), sqc.data_ptr(),
-                                             skc.data_ptr(), svc.data_ptr(), o.data_ptr(), _p(lse), _p(q_rows),
-                                             _p(kv_rows), _p(o_rows), BH, S, D, D, S * D, D, S * D, scale,
-                                             C.byref(plan.desc), plan.ws.data_ptr(), _stream(q8)),
-              "svgb_attn_fwd_fp8_gather")
-    else:
-        if q_rows is not None or kv_rows is not None:
-            raise SvgbError("q_rows / kv_rows need a gather plan (plan_varblock(..., gather=True))")
-        check(lib().svgb_attn_fwd_fp8(q8c.data_ptr(), k8c.data_ptr(), v8c.data_ptr(), sqc.data_ptr(), skc.data_ptr(),
-                                      svc.data_ptr(), o.data_ptr(), _p(lse), _p(o_rows), BH, S, D,
-                                      D, S * D, D, S * D, scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q8)),
-              "svgb_attn_fwd_fp8")
-    _bump()
-    return (o, lse) if return_lse else o
+    scales = tuple(t.to(torch.float32).contiguous() for t in (q_scale, k_scale, v_scale))
+    return _attn(q8c, k8c, v8c, scales, o, _E4M3, plan, B * H, S, D, D, S * D, o_rows, q_rows, kv_rows, return_lse,
+                 sm_scale)
 
 
 def density(block_map, row_sz, col_sz):

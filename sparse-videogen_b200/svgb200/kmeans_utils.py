@@ -87,15 +87,19 @@ def identify_dynamic_map(query_centroids, key_centroids, q_cluster_sizes, k_clus
     return m.view(B, H, QC, KC)
 
 
-def dynamic_block_sparse_fwd_flashinfer(q, k, v, block_mask_map, block_row_sz, block_col_sz, is_cpu=True):
-    """svg/kmeans_utils.py:1319-1392.  q,k,v [B,H,S,D]; map bool [B,H,QC,KC]; sizes [B,H,QC]/[B,H,KC]
-    (on CPU when is_cpu, like the reference's default; moved to the GPU here)."""
+def _flashinfer_plan(q, block_mask_map, block_row_sz, block_col_sz):
     B, H, S, D = q.shape
     QC, KC = block_row_sz.shape[-1], block_col_sz.shape[-1]
     assert block_mask_map.shape == (B, H, QC, KC)
     dev = q.device
-    plan = core.plan_varblock(block_mask_map.to(dev).reshape(B * H, QC, KC), block_row_sz.to(dev).reshape(B * H, QC),
+    return core.plan_varblock(block_mask_map.to(dev).reshape(B * H, QC, KC), block_row_sz.to(dev).reshape(B * H, QC),
                               block_col_sz.to(dev).reshape(B * H, KC), S)
+
+
+def dynamic_block_sparse_fwd_flashinfer(q, k, v, block_mask_map, block_row_sz, block_col_sz, is_cpu=True):
+    """svg/kmeans_utils.py:1319-1392.  q,k,v [B,H,S,D]; map bool [B,H,QC,KC]; sizes [B,H,QC]/[B,H,KC]
+    (on CPU when is_cpu, like the reference's default; moved to the GPU here)."""
+    plan = _flashinfer_plan(q, block_mask_map, block_row_sz, block_col_sz)
     return core.attn_fwd(q.contiguous(), k.contiguous(), v.contiguous(), plan)
 
 
@@ -107,17 +111,9 @@ def dynamic_block_sparse_fwd_triton(q, k, v, dynamic_map, qc_size, kc_size):
 def dynamic_block_sparse_fwd_flashinfer_fp8(q, k, v, block_mask_map, block_row_sz, block_col_sz, is_cpu=True):
     """dynamic_block_sparse_fwd_flashinfer in FP8: q, k, v (already in cluster order) quantised to e4m3 per head and
     run on the e4m3 kernel; head_dim 128 only; the result comes back in q.dtype."""
-    from .models.common import check_fp8_head_dim, quantize_qkv
+    from .models.common import fp8_attention
 
-    B, H, S, D = q.shape
-    check_fp8_head_dim(D)
-    QC, KC = block_row_sz.shape[-1], block_col_sz.shape[-1]
-    assert block_mask_map.shape == (B, H, QC, KC)
-    dev = q.device
-    plan = core.plan_varblock(block_mask_map.to(dev).reshape(B * H, QC, KC), block_row_sz.to(dev).reshape(B * H, QC),
-                              block_col_sz.to(dev).reshape(B * H, KC), S)
-    (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(q, k, v)
-    return core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, plan).to(q.dtype)
+    return fp8_attention(q, k, v, _flashinfer_plan(q, block_mask_map, block_row_sz, block_col_sz))
 
 
 def dynamic_block_sparse_fwd_triton_fp8(q, k, v, dynamic_map, qc_size, kc_size):

@@ -49,13 +49,19 @@ def quantize_qkv(query, key, value):
     return tuple(core.quantize_e4m3(t) for t in (query, key, value))
 
 
-def sparse_flex_attention_fp8(query, key, value, block_mask: BandMask):
-    """sparse_flex_attention in FP8: Q, K, V quantised to e4m3 per head, the band plan run on the e4m3 kernel.  The
-    kernel writes bf16; the result comes back in query.dtype."""
+def fp8_attention(query, key, value, plan: core.AttnPlan, **rows):
+    """Attention under `plan` in FP8: Q, K, V [B,H,S,128] quantised to e4m3 per head and run on the e4m3 kernel
+    (rows: q_rows / kv_rows / o_rows of core.attn_fwd_fp8).  The kernel writes bf16; the result comes back in
+    query.dtype."""
     check_fp8_head_dim(query.shape[-1])
     (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(query, key, value)
-    o = core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, block_mask.plan)
-    return o.to(query.dtype)
+    return core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, plan, **rows).to(query.dtype)
+
+
+def sparse_flex_attention_fp8(query, key, value, block_mask: BandMask):
+    """sparse_flex_attention in FP8 (fp8_attention under the band plan)."""
+    check_fp8_head_dim(query.shape[-1])  # before block_mask is read: a head_dim-64 model fails on its cause
+    return fp8_attention(query, key, value, block_mask.plan)
 
 
 def dense_attention(query, key, value, seg_lens=None):

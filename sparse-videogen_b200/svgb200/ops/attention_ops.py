@@ -87,11 +87,7 @@ def bsr_to_plan(indptr, indices, block_size, video_len, text_len, device) -> cor
         bm[0, :, 0] = True   # video rows see the text columns (o_image_r, :180-186)
         row[0, 0] = text_len
         col[0, 0] = text_len
-    S = video_len + text_len
-    nbytes = core.C.c_size_t()
-    core.check(core.lib().svgb_attn_plan_varblock_bytes(1, S, MB + t, NB + t, core.C.byref(nbytes)), "plan bytes")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # long-lived, owned by the plan
-    plan = core.plan_varblock(bm, row, col, S, ws=ws)
+    plan = core.plan_varblock(bm, row, col, video_len + text_len)  # owns its workspace: safe to cache
     plan.desc.items_stride = 0   # one map for every head: share the plan (svgb200.h, svgb_plan)
     plan.desc.counts_stride = 0
     _plan_cache[key] = (weakref.ref(indptr), weakref.ref(indices), plan)

@@ -34,30 +34,31 @@ _NAMES = {
 }
 
 
+def _flex_attention(name, attend, query, key, value, block_mask, kw):
+    from .models.common import BandMask
+
+    if not isinstance(block_mask, BandMask):
+        raise TypeError(f"svgb200.patch.{name} needs the BandMask returned by the patched prepare_flexattention "
+                        f"(got {type(block_mask).__name__}); rebuild block_mask after patch.install()")
+    if kw:
+        raise TypeError(f"unsupported flex_attention arguments: {sorted(kw)}")
+    return attend(query, key, value, block_mask)
+
+
 def flex_attention(query, key, value, block_mask=None, **kw):
     """Stand-in for torch.nn.attention.flex_attention.flex_attention as the reference processors call it
     (`flex_attention(q, k, v, block_mask=cls.block_mask)`, hyvideo/attention.py:401-403): block_mask must be the
     BandMask built by the patched prepare_flexattention."""
-    from .models.common import BandMask, sparse_flex_attention
+    from .models.common import sparse_flex_attention
 
-    if not isinstance(block_mask, BandMask):
-        raise TypeError("svgb200.patch.flex_attention needs the BandMask returned by the patched prepare_flexattention "
-                        f"(got {type(block_mask).__name__}); rebuild block_mask after patch.install()")
-    if kw:
-        raise TypeError(f"unsupported flex_attention arguments: {sorted(kw)}")
-    return sparse_flex_attention(query, key, value, block_mask)
+    return _flex_attention("flex_attention", sparse_flex_attention, query, key, value, block_mask, kw)
 
 
 def flex_attention_fp8(query, key, value, block_mask=None, **kw):
     """flex_attention with the band attention on e4m3 Q, K, V (models.common.sparse_flex_attention_fp8)."""
-    from .models.common import BandMask, sparse_flex_attention_fp8
+    from .models.common import sparse_flex_attention_fp8
 
-    if not isinstance(block_mask, BandMask):
-        raise TypeError("svgb200.patch.flex_attention_fp8 needs the BandMask returned by the patched "
-                        f"prepare_flexattention (got {type(block_mask).__name__}); rebuild block_mask after patch.install()")
-    if kw:
-        raise TypeError(f"unsupported flex_attention arguments: {sorted(kw)}")
-    return sparse_flex_attention_fp8(query, key, value, block_mask)
+    return _flex_attention("flex_attention_fp8", sparse_flex_attention_fp8, query, key, value, block_mask, kw)
 
 
 def flashinfer_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv):

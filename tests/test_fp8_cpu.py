@@ -1,5 +1,5 @@
-"""FP8 mode without a GPU: argument errors of svgb_attn_fwd_fp8_gather, the head-dim check of the cores, and which
-operators patch.install(..., fp8=) puts in place."""
+"""FP8 mode without a GPU: argument errors of svgb_attn_fwd for e4m3 inputs and row gathers, the head-dim check of the
+cores, and which operators patch.install(..., fp8=) puts in place."""
 import ctypes as C
 import types
 from pathlib import Path
@@ -22,23 +22,37 @@ def lib():
     return _lib.lib()
 
 
-def _call(lib, plan, scales=True):
+SVGB_BF16, SVGB_E4M3 = 0, 2
+
+
+def _call(lib, plan, scales=True, rows=False, dtype=SVGB_E4M3):
     p = C.c_void_p(4096)  # never dereferenced: the arguments are rejected first
     s = p if scales else None
-    return lib.svgb_attn_fwd_fp8_gather(p, p, p, s, s, s, p, None, None, None, None, 1, 1024, 128, 128, 1024 * 128,
-                                        128, 1024 * 128, 0.088, C.byref(plan), p, None)
+    r = p if rows else None
+    return lib.svgb_attn_fwd(p, p, p, s, s, s, p, None, r, r, None, dtype, 1, 1024, 128, 128, 1024 * 128,
+                             128, 1024 * 128, 0.088, C.byref(plan), p, None)
 
 
-def test_fp8_gather_argument_errors(lib):
+def test_attn_fwd_e4m3_argument_errors(lib):
     from svgb200._lib import Plan
+    from svgb200.core import PLAN_BAND, PLAN_GATHER, PLAN_VARBLOCK
 
-    plan = Plan(kind=3, BH=1, S=1024, max_items=4, items_stride=4, counts_stride=1)
-    assert _call(lib, plan, scales=False) < 0
+    plan = Plan(kind=PLAN_GATHER, BH=1, S=1024, max_items=4, items_stride=4, counts_stride=1)
+    assert _call(lib, plan, scales=False, rows=True) < 0
     assert b"scale" in lib.svgb_last_error()
-    for kind in (1, 2):
+    for kind in (PLAN_VARBLOCK, PLAN_BAND):
         plan.kind = kind
-        assert _call(lib, plan) < 0
+        assert _call(lib, plan, rows=True) < 0
         assert b"svgb_attn_plan_varblock_gather" in lib.svgb_last_error()
+
+
+def test_scales_are_rejected_with_16bit_inputs(lib):
+    from svgb200._lib import Plan
+    from svgb200.core import PLAN_VARBLOCK
+
+    plan = Plan(kind=PLAN_VARBLOCK, BH=1, S=1024, max_items=4, items_stride=4, counts_stride=1)
+    assert _call(lib, plan, dtype=SVGB_BF16) < 0
+    assert b"scale" in lib.svgb_last_error()
 
 
 def test_cores_reject_head_dim_64_in_fp8():

@@ -1,4 +1,4 @@
-"""FP8 (e4m3) through every layer: the row-gather kernel path (svgb_attn_fwd_fp8_gather / core.attn_fwd_fp8 with
+"""FP8 (e4m3) through every layer: the row-gather kernel path (svgb_attn_fwd on a gather plan / core.attn_fwd_fp8 with
 q_rows / kv_rows), the SVG1 and SVG2 cores with fp8=True, and patch.install(..., fp8=True).
 
 Kernel results are compared with the fp64 oracle on the de-quantised inputs at the FP8 tolerances of

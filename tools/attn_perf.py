@@ -71,7 +71,7 @@ for QC, KC, rho, heads in [(465, 931, 0.3, 24), (400, 1000, 0.3, 24), (400, 1000
         qq, kk, vv = qq.contiguous(), kk.contiguous(), vv.contiguous()
     ms = t(lambda: core.attn_fwd(qq, kk, vv, pl))
     emit(case=f"varblock_QC{QC}_KC{KC}_rho{rho}_h{heads}", ms=ms, tflops=fl / ms / 1e9)
-    plg = core.plan_varblock(bm.to(dev), row.to(dev), col.to(dev), S, ws=torch.empty_like(pl.ws), gather=True)
+    plg = core.plan_varblock(bm.to(dev), row.to(dev), col.to(dev), S, gather=True)
     ms = t(lambda: core.attn_fwd(qq, kk, vv, plg))
     emit(case=f"varblock_GATHER_QC{QC}_KC{KC}_rho{rho}_h{heads}", ms=ms, tflops=fl / ms / 1e9)
 
