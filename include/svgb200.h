@@ -191,7 +191,9 @@ int svgb_kmeans_run_sorted(const void* x, long long x_head_stride, const void* i
 /* ---- mask selection --------------------------------------------------------------------- */
 /* identify_dynamic_map (svg/kmeans_utils.py:864-896): qc [BH,QC,D], kc [BH,KC,D] 16-bit,
  * k_sizes int32 [BH,KC] -> map uint8 [BH,QC,KC].  Ties in the descending sort resolve to the
- * lower column index (stable). */
+ * lower column index (stable).  The running sum is torch's CUDA block scan of BH*QC rows, bit for bit;
+ * for a single row (BH*QC == 1) torch.cumsum runs cub::DeviceScan instead, and the map may differ from
+ * torch's there. */
 int svgb_dynamic_map(const void* qc, const void* kc, const int32_t* k_sizes, int BH, int QC, int KC,
                      int D, int dtype, float top_p, int preserve, uint8_t* map, void* stream);
 /* sample_mse (hyvideo/attention.py:375-399): MSE between full attention and attention under the two

@@ -122,7 +122,9 @@ def cumsum_like_torch_cuda(x: torch.Tensor, num_rows: int | None = None) -> torc
     whose every `+` is a bf16 add (std::plus<BFloat16>), carrying the block total into element 0 of the next block.
     Near the top-p threshold (0.9, bf16 spacing 2^-8) single small probabilities are absorbed, so the GPU keeps
     systematically MORE clusters than an fp32-accumulated cumsum would (recorded reference maps: +5 of 1000 on
-    average, up to +38).  nx = 2^cuda_scan_log_threads(rows, row_size) — 16 for every shape on this path."""
+    average, up to +38).  nx = 2^cuda_scan_log_threads(rows, row_size): 16 at 24 heads x 400 q-centroids x 1000
+    columns, up to 512 for a few short rows (2 rows x 1024 columns).  One row (numel == row_size) is not this scan:
+    torch hands it to cub::DeviceScan, which associates the 16-bit adds differently."""
     dt = x.dtype
     shape = x.shape
     row = shape[-1]
@@ -144,6 +146,31 @@ def cumsum_like_torch_cuda(x: torch.Tensor, num_rows: int | None = None) -> torc
             seg[:, ti] = seg[:, ti] + seg[:, si]  # 16-bit add: rounds to the tensor dtype
         total = seg[:, blk - 1].clone()
     return buf[:, :row].reshape(shape)
+
+
+def onehot_dynmap_inputs(BH, QC, KC, D, dtype, gen):
+    """Inputs on which every step of identify_dynamic_map is exact, so any two implementations must agree bit for bit.
+    Key centroid j is 64 * e_c(j), q centroid i is 64 * e_g(i) or zero: scores are 4096 / sqrt(D) ("live", c(j) = g(i))
+    or 0 in every summation order and in both 16-bit types; dead columns sit >= 4096 / 16 = 256 below the row maximum,
+    where fp32 exp underflows to exactly 0, live ones give exp(0) = 1; the live sizes sum exactly in fp32 (< 2^24), so
+    prob_j = round16(fl32(w_j / W_i)).  What follows (sort, 16-bit scan, cut, scatter) is fixed by documented roundings.
+    Direction 0 holds ~30 % of the keys, all of size 7 (a long run of equal probabilities across the top-p cut), 1 keys of
+    size 0 (W = 0: the 1e-12 denominator keeps every column), 2 exactly one key, 3 none (a row that hits no key: all
+    columns live); ~15 % of the q rows are zero (all columns live).  Returns qc [BH,QC,D], kc [BH,KC,D], k_sizes int32."""
+    assert D >= 8
+    r = torch.rand(BH, KC, generator=gen)
+    c = torch.where(r < 0.30, 0, torch.where(r < 0.35, 1, torch.randint(4, D, (BH, KC), generator=gen)))
+    sizes = torch.randint(0, 300, (BH, KC), generator=gen, dtype=torch.int32)
+    sizes = torch.where(c == 0, 7, torch.where(c == 1, 0, sizes)).to(torch.int32)
+    c[:, KC // 2] = 2
+    sizes[:, KC // 2] = 100
+    g = torch.randint(0, D, (BH, QC), generator=gen)
+    lead = torch.tensor([-1, 0, 1, 2, 3])[:QC]  # zero row, then one row per special direction
+    g = torch.where(torch.rand(BH, QC, generator=gen) < 0.15, -1, g)
+    g[:, : lead.numel()] = lead
+    kc = torch.zeros(BH, KC, D).scatter_(2, c[..., None], 64.0)
+    qc = torch.zeros(BH, QC, D).scatter_(2, g.clamp(min=0)[..., None], 64.0) * (g >= 0)[..., None]
+    return qc.to(dtype), kc.to(dtype), sizes
 
 
 def identify_dynamic_map(qc, kc, q_sizes, k_sizes, p, min_kc_ratio=0.0, cumsum="cuda"):

@@ -8,10 +8,13 @@
 //   cums   = torch.cumsum of the sorted 16-bit tensor AS THE CUDA BACKEND COMPUTES IT (the reference runs on the
 //            GPU): blocks of 2*nx elements scanned by a Sklansky network in which every add rounds to 16 bit, block
 //            totals carried into element 0 of the next block (ATen/native/cuda/ScanUtils.cuh:
-//            tensor_kernel_scan_innermost_dim; nx from get_log_num_threads_x_inner_scan(rows, KC), 16 on this path).
+//            tensor_kernel_scan_innermost_dim; nx from get_log_num_threads_x_inner_scan(rows = BH*QC, KC): 16 at
+//            24 x 400 x 1000, up to 512 for a few long rows).
 //            This is NOT an fp32 running sum: near p = 0.9 (bf16 spacing 2^-8) small probabilities are absorbed and
-//            the GPU keeps more clusters.  Reproduced bit for bit: maps recorded from the reference on a GPU
-//            (tests/golden/kmeans_golden.npz, 800 x 1000) match exactly.
+//            the GPU keeps more clusters.  Reproduced bit for bit at every nx (tests/test_dynmap_exact_gpu.py) and on
+//            maps recorded from the reference on a GPU (tests/golden/kmeans_golden.npz, 800 x 1000).
+//            Not covered: a single row (BH*QC == 1), where torch.cumsum runs cub::DeviceScan instead, whose 16-bit adds
+//            associate differently -- the kernel keeps the block scan, so its map can differ from torch's there.
 //   keep[t] = t == 0 || !(cums[t-1] > round16(p)) || t < preserve   (:884-890; scalar compared in 16 bit)
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -291,7 +294,7 @@ extern "C" int svgb_dynamic_map(const void* qc, const void* kc, const int32_t* k
   int KCpad = 2;
   while (KCpad < KC) KCpad <<= 1;
   // block size of torch's CUDA scan for a [BH*QC, KC] tensor: get_log_num_threads_x_inner_scan (ScanUtils.cuh:19-41,
-  // uint32 arithmetic) -- 4 (32-element blocks) for every shape on this path
+  // uint32 arithmetic) -- 4 (32-element blocks) at 24 x 400 rows of 1000, up to 9 (1024-element blocks) for a few rows
   uint32_t lx = 0, ly = 0;
   while ((1u << lx) < static_cast<uint32_t>(KC)) ++lx;
   while ((1ull << ly) < static_cast<unsigned long long>(BH) * QC) ++ly;
