@@ -1,19 +1,23 @@
 // Block-sparse flash attention forward for sm_90a (Hopper wgmma).
 //
-// One CTA per work item, 256 threads = two consumer warpgroups; warpgroup w owns query rows 64w .. 64w+63 of a
-// 128-row tile.  A work item is one or two 128-row STREAMS (a two-tile item: rows 0-127 and 128-255 over the same
-// chunk list; a dual item: two independent tails, each with its own chunk list), run one after the other.
+// One CTA per work item, 384 threads in three warpgroups.  Warpgroup 0 is the PRODUCER: it does every load.
+// Warpgroups 1 and 2 are the CONSUMERS: consumer c owns query rows 64c .. 64c+63 of a 128-row tile.  A work item is
+// one or two 128-row STREAMS (a two-tile item: rows 0-127 and 128-255 over the same chunk list; a dual item: two
+// independent tails, each with its own chunk list), run one after the other.
 //   Q tile          : TMA (or cp.async row gather), 128-byte swizzle, stays in shared memory for the stream
-//   K(j), V(j)      : three stages; chunk j+3 is requested once chunk j's stage is free
+//   K(j), V(j)      : three stages, each half with its own full and empty mbarrier
 //   S = Q K^T       : wgmma m64n128 (SS, both operands K-major), fp32 accumulators in registers
 //   softmax         : online, in registers (each row is spread over the 4 lanes of a quad)
 //   O += P V        : wgmma m64nD (RS: P from registers in the accumulator layout of S, V MN-major)
-// The chunk loop is software-pipelined inside each warpgroup: iteration j issues S = Q K(j+1)^T and then
-// O += P(j) V(j) as two wgmma groups, waits for the first only, and runs the mask and softmax of chunk j+1 while
-// P V(j) is still on the tensor cores.  Every row still sees the same operations in the same order as a
-// one-chunk-at-a-time loop (rescale O by alpha(j+1), then accumulate P(j+1) V(j+1)).
-// FP8 (e4m3) inputs: Q K^T runs on e4m3 wgmma (k32); wgmma has no MN-major 8-bit B operand, so each V tile is
-// widened to fp16 in shared memory (two buffers: V(j+1) is widened while P V(j) reads V(j)) and P V runs in fp16.
+// The producer and the consumers meet only at mbarriers (the protocol table is in DESIGN.md §1); after the role
+// split there is no block-wide barrier.  The chunk loop is software-pipelined inside each consumer: iteration j
+// issues S = Q K(j+1)^T and then O += P(j) V(j) as two wgmma groups, waits for the first only, and runs the mask
+// and softmax of chunk j+1 while P V(j) is still on the tensor cores.  The two consumers take turns issuing their
+// groups (two named barriers), so one consumer's softmax also runs under the other's MMAs.  Every row still sees
+// the same operations in the same order as a one-chunk-at-a-time loop (rescale O by alpha(j+1), then accumulate
+// P(j+1) V(j+1)).
+// FP8 (e4m3) inputs: Q K^T runs on e4m3 wgmma (k32); wgmma has no MN-major 8-bit B operand, so the producer widens
+// each V tile to fp16 in shared memory (two buffers, with their own full and empty barriers) and P V runs in fp16.
 // Both loaders serve e4m3: the row gather copies 128-byte e4m3 rows into the same swizzled image TMA writes, and
 // the widening step that follows is shared.
 #pragma once
@@ -32,8 +36,8 @@ namespace svgb {
 
 // element type of Q/K/V: 0 = bf16, 1 = fp16, 2 = fp8 e4m3 (output bf16)
 constexpr int DT_BF16 = 0, DT_F16 = 1, DT_E4M3 = 2;
-// K/V stages: with P V(j) still running when Q K(j+1)^T is issued, chunk j's stage frees late in iteration j, so
-// the load of chunk j+3 into it gets about two chunks of lead time
+// K/V stages: with P V(j) still running when Q K(j+1)^T is issued, V(j) frees late in iteration j, so the load of
+// chunk j+3 into its stage gets about two chunks of lead time
 constexpr int kKvStages = 3;
 
 template <int D, int DT = DT_BF16>
@@ -52,7 +56,7 @@ struct AttnCfg {
   static constexpr int kBarBytes = 1024;                 // mbarriers + gather row table
   // + 1 KB: the kernel aligns the dynamic window to 1024 bytes itself
   static constexpr int kSmemBytes = 1024 + kTileBytes + 2 * kKvStages * kTileBytes + 2 * kVhBytes + kBarBytes;
-  static constexpr int kThreads = 256;
+  static constexpr int kThreads = 384;  // producer warpgroup + two consumer warpgroups
   static_assert(kSmemBytes <= 227 * 1024, "exceeds the 227 KB per-CTA shared memory of sm_90");
 };
 
@@ -106,17 +110,28 @@ __device__ __forceinline__ void attn_wait(float (&d)[M]) {
   wg_fence_regs(d);
 }
 
+// mbarriers of the producer / consumer protocol.  A full barrier completes once its data has landed: one arrival
+// with the transaction bytes from the TMA-issuing thread, or (row gather) one cp.async arrival from each of the
+// producer's 128 threads.  An empty barrier completes once both consumers are done with the buffer: one arrival
+// from thread 0 of each consumer warpgroup.  vh_full: one arrival from each producer thread after widening.
 struct AttnSmemCtl {
-  uint64_t q_full;
-  uint64_t kv_full[kKvStages];
+  uint64_t q_full, q_empty;
+  uint64_t k_full[kKvStages], k_empty[kKvStages];
+  uint64_t v_full[kKvStages], v_empty[kKvStages];
+  uint64_t vh_full[2], vh_empty[2];  // FP8: the two fp16 copies of V
   int src[128];  // gather: source row of each of the 128 rows being loaded (-1: zero fill)
-  float pin[8];  // one word per warp, written and never read (see the chunk loop)
+  float pin[8];  // one word per consumer warp, written and never read (see the chunk loop)
 };
+
+// named barriers (0 is __syncthreads): the producer's own 128 threads, and the two consumers' turns
+constexpr int kBarProducer = 1, kBarTurn = 2;  // consumer c waits for its turn on kBarTurn + c
+// register split of the 64 K registers: 128 x 24 (producer) + 256 x 240 (consumers) = 64,512
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;
 
 // kGather selects the loader: false = TMA boxes over contiguous key ranges (chunk list), true = cp.async
 // row gathers over a run list.
 template <int D, int DT, bool kGather>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant__ CUtensorMap kmap,
                 const __grid_constant__ CUtensorMap vmap, const AttnArgs args) {
   using Cfg = AttnCfg<D, DT>;
@@ -146,11 +161,24 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       reinterpret_cast<AttnSmemCtl*>(smem_al + Cfg::kTileBytes * (1 + 2 * kKvStages) + 2 * Cfg::kVhBytes);
 
   const int tid = threadIdx.x;
-  const int wg = tid >> 7, wt = tid & 127, lane = tid & 31, wq = wt >> 5;
-  const uint32_t sQw = sQ + 64 * wg * 128;  // this warpgroup's 64 rows of the Q tile
+  // the warpgroup index through a shuffle, so that ptxas sees it is warp-uniform and splits the register allocation
+  // at the setmaxnreg of each role
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+  const int wt = tid & 127, lane = tid & 31, wq = wt >> 5;
   if (tid == 0) {
-    mbar_init(smem_u32(&ctl->q_full), 1);
-    for (int i = 0; i < kKvStages; ++i) mbar_init(smem_u32(&ctl->kv_full[i]), 1);
+    const uint32_t full_count = kGather ? 128 : 1;
+    mbar_init(smem_u32(&ctl->q_full), full_count);
+    mbar_init(smem_u32(&ctl->q_empty), 2);
+    for (int i = 0; i < kKvStages; ++i) {
+      mbar_init(smem_u32(&ctl->k_full[i]), full_count);
+      mbar_init(smem_u32(&ctl->k_empty[i]), 2);
+      mbar_init(smem_u32(&ctl->v_full[i]), full_count);
+      mbar_init(smem_u32(&ctl->v_empty[i]), 2);
+    }
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(smem_u32(&ctl->vh_full[b]), 128);
+      mbar_init(smem_u32(&ctl->vh_empty[b]), 2);
+    }
     mbar_fence_init();
     if constexpr (!kGather) {
       tma_prefetch_desc(&qmap);
@@ -158,36 +186,55 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       tma_prefetch_desc(&vmap);
     }
   }
-  __syncthreads();
+  __syncthreads();  // the barriers are initialised; the last block-wide barrier of the kernel
 
-  const float c = args.scale_log2 * (args.q_scale ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[bh]) : 1.f);
-  const float vs = args.v_scale ? __ldg(&args.v_scale[bh]) : 1.f;
-  const int mode = args.mask_mode, m0 = args.m0, m1 = args.m1, m2 = args.m2;
-  const Elem* kp = static_cast<const Elem*>(args.k_ptr) + bh * args.in_head_stride;
-  const Elem* vp = static_cast<const Elem*>(args.v_ptr) + bh * args.in_head_stride;
-  const int* kv_rows = (kGather && args.kv_rows) ? args.kv_rows + static_cast<size_t>(bh) * args.S : nullptr;
-  const int2* __restrict__ runs = args.chunks + item.z;
-  const int nruns = item.w;
-
-  // gather: piece p (16 B) of row r -> panel p/8, byte r*128 + ((p%8) ^ (r%8))*16; a row is kRowBytes bytes
-  // (e4m3 at D = 128: 8 pieces, one panel)
-  auto gather_rows = [&](uint32_t dst, const Elem* src_base, bool two, const Elem* src2, uint32_t dst2) {
-    constexpr int kPieces = Cfg::kRowBytes / 16;
-    constexpr int kPieceElems = 16 / Cfg::kElemBytes;
-#pragma unroll 4
-    for (int i = tid; i < 128 * kPieces; i += 256) {
-      const int r = i / kPieces, pc = i % kPieces;
-      const int src = ctl->src[r];
-      const uint32_t off = (pc >> 3) * Cfg::kPanelBytes + r * 128 + (((pc & 7) ^ (r & 7)) << 4);
-      const long long so = static_cast<long long>(src < 0 ? 0 : src) * args.in_row_stride + pc * kPieceElems;
-      cp_async16(dst + off, src_base + so, src >= 0 ? 16u : 0u);
-      if (two) cp_async16(dst2 + off, src2 + so, src >= 0 ? 16u : 0u);
-    }
+  const int nstreams = (dual || item.y > kTileRows) ? 2 : 1;
+  // stream st of the item: first query row, rows, chunk list and chunk count
+  struct Stream {
+    int q0, nr, nch;
+    const int2* chunks;
   };
-  // gather: source rows of keys j*128 .. j*128+127 of this item -> ctl->src (threads 0..127)
-  auto resolve_chunk = [&](int j) {
-    if (tid < 128) {
-      const int pos = j * kChunkCols + tid;
+  auto stream = [&](int st) {
+    const bool second = st == 1;
+    Stream sm;
+    sm.q0 = second ? (dual ? item2.x : item.x + kTileRows) : item.x;
+    sm.nr = second ? (dual ? item2.y : item.y - kTileRows) : (dual ? item.y : min(item.y, kTileRows));
+    sm.chunks = args.chunks + ((second && dual) ? item2.z : item.z);
+    sm.nch = kGather ? (total_kv + kChunkCols - 1) / kChunkCols : ((second && dual) ? item2.w : item.w);
+    return sm;
+  };
+  // Both roles count chunks over the whole CTA: chunk n (the stream's chunk j is n = g + j, g = chunks of the earlier
+  // streams) lives in K/V stage n % 3, phase (n / 3) & 1 of that stage's barriers; FP8: its fp16 V copy in buffer
+  // n & 1, phase (n / 2) & 1.  An empty barrier's wait for round r is on parity (r & 1) ^ 1: round 0 passes at once.
+  auto stage_k = [&](int n) { return sK0 + 2 * (n % kKvStages) * Cfg::kTileBytes; };
+  auto vh_buf = [&](int n) { return sVh + (n & 1) * Cfg::kVhBytes; };
+
+  if (wg == 0) {
+    // ======================= producer: every load, and the FP8 widening of V
+    setmaxnreg_dec<kProducerRegs>();
+    const Elem* kp = static_cast<const Elem*>(args.k_ptr) + bh * args.in_head_stride;
+    const Elem* vp = static_cast<const Elem*>(args.v_ptr) + bh * args.in_head_stride;
+    const int* kv_rows = (kGather && args.kv_rows) ? args.kv_rows + static_cast<size_t>(bh) * args.S : nullptr;
+    const int2* __restrict__ runs = args.chunks + item.z;
+    const int nruns = item.w;
+
+    // gather: piece p (16 B) of row r -> panel p/8, byte r*128 + ((p%8) ^ (r%8))*16; a row is kRowBytes bytes
+    // (e4m3 at D = 128: 8 pieces, one panel)
+    auto gather_rows = [&](uint32_t dst, const Elem* src_base) {
+      constexpr int kPieces = Cfg::kRowBytes / 16;
+      constexpr int kPieceElems = 16 / Cfg::kElemBytes;
+#pragma unroll 4
+      for (int i = wt; i < 128 * kPieces; i += 128) {
+        const int r = i / kPieces, pc = i % kPieces;
+        const int src = ctl->src[r];
+        const uint32_t off = (pc >> 3) * Cfg::kPanelBytes + r * 128 + (((pc & 7) ^ (r & 7)) << 4);
+        const long long so = static_cast<long long>(src < 0 ? 0 : src) * args.in_row_stride + pc * kPieceElems;
+        cp_async16(dst + off, src_base + so, src >= 0 ? 16u : 0u);
+      }
+    };
+    // gather: source rows of keys j*128 .. j*128+127 of this item -> ctl->src
+    auto resolve_chunk = [&](int j) {
+      const int pos = j * kChunkCols + wt;
       int src = -1;
       if (pos < total_kv) {
         int lo = 0, hi = nruns - 1;  // largest run with keys_before <= pos
@@ -200,61 +247,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         const int prow = rr.x + (pos - rr.y);
         src = kv_rows ? __ldg(&kv_rows[prow]) : prow;
       }
-      ctl->src[tid] = src;
-    }
-  };
-
-  int g = 0;       // chunks of this CTA before the current stream (the stream's chunk j is the CTA's chunk g + j)
-  int nq = 0;      // Q tiles loaded so far (q_full phase)
-  const int nstreams = (dual || item.y > kTileRows) ? 2 : 1;
-  for (int st = 0; st < nstreams; ++st) {
-    const bool second = st == 1;
-    const int q0 = second ? (dual ? item2.x : item.x + kTileRows) : item.x;
-    const int nr = second ? (dual ? item2.y : item.y - kTileRows) : (dual ? item.y : min(item.y, kTileRows));
-    const int2* __restrict__ chunks = args.chunks + ((second && dual) ? item2.z : item.z);
-    const int nch = kGather ? (total_kv + kChunkCols - 1) / kChunkCols : ((second && dual) ? item2.w : item.w);
-
-    // CTA chunk n lives in K/V stage n % 3 (kv_full phase (n / 3) & 1); FP8: its fp16 V copy in buffer n & 1
-    auto stage_k = [&](int j) { return sK0 + 2 * ((g + j) % kKvStages) * Cfg::kTileBytes; };
-    auto pv_b = [&](int j) { return FP8 ? sVh + ((g + j) & 1) * Cfg::kVhBytes : stage_k(j) + Cfg::kTileBytes; };
-
-    // issue the loads of chunk j
-    auto load_chunk = [&](int j) {
-      const uint32_t sK = stage_k(j), sV = sK + Cfg::kTileBytes;
-      if constexpr (kGather) {
-        resolve_chunk(j);
-        __syncthreads();
-        gather_rows(sK, kp, true, vp, sV);
-        cp_async_commit();
-        __syncthreads();  // ctl->src is reused by the next resolve
-      } else if (tid == 0) {
-        const int kv0 = __ldg(&chunks[j].x);
-        const uint32_t fb = smem_u32(&ctl->kv_full[(g + j) % kKvStages]);
-        mbar_expect_tx(fb, 2 * Cfg::kTileBytes);
-        for (int h = 0; h < Cfg::kHalves; ++h) {
-          tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, fb, h * Cfg::kPanelElems, kv0, bh);
-          tma_load_3d(sV + h * Cfg::kPanelBytes, &vmap, fb, h * Cfg::kPanelElems, kv0, bh);
-        }
-      }
+      ctl->src[wt] = src;
     };
-    // wait until chunk j has landed; gather: `later` chunks were requested after it
-    auto wait_chunk = [&](int j, int later) {
-      if constexpr (kGather) {
-        if (later >= 2) cp_async_wait<2>();
-        else if (later == 1) cp_async_wait<1>();
-        else cp_async_wait<0>();
-        fence_proxy_async_smem();
-        __syncthreads();
-      } else {
-        mbar_wait(smem_u32(&ctl->kv_full[(g + j) % kKvStages]), ((g + j) / kKvStages) & 1, 2);
-      }
-    };
-    // FP8: widen V(j) (e4m3, one 128-byte panel) to fp16 (two panels) in the same swizzled image.  All 256 threads
-    // write; the copy is published by fence.proxy.async plus a block barrier.
-    auto widen_v = [&](int j) {
-      const uint32_t sV = stage_k(j) + Cfg::kTileBytes, dst = pv_b(j);
-#pragma unroll
-      for (int i = tid; i < 128 * 8; i += 256) {
+    // FP8: widen V (e4m3, one 128-byte panel) of chunk n to fp16 (two panels) in the same swizzled image.  The
+    // copy is written through the generic proxy and read by wgmma (async proxy): each writer fences before its
+    // arrival on vh_full, and the consumers' acquire of vh_full orders their wgmma after it.
+    auto widen_v = [&](int n) {
+      mbar_wait(smem_u32(&ctl->v_full[n % kKvStages]), (n / kKvStages) & 1, 9);
+      mbar_wait(smem_u32(&ctl->vh_empty[n & 1]), ((n >> 1) & 1) ^ 1, 8);
+      const uint32_t sV = stage_k(n) + Cfg::kTileBytes, dst = vh_buf(n);
+#pragma unroll 1
+      for (int i = wt; i < 128 * 8; i += 128) {
         const int r = i >> 3, pc = i & 7;
         const uint4 w = *reinterpret_cast<const uint4*>(smem_al + (sV - base) + r * 128 + ((pc ^ (r & 7)) << 4));
         const uint32_t in[4] = {w.x, w.y, w.z, w.w};
@@ -274,10 +277,109 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
               make_uint4(out[4 * hh], out[4 * hh + 1], out[4 * hh + 2], out[4 * hh + 3]);
         }
       }
+      fence_proxy_async_smem();
+      mbar_arrive(smem_u32(&ctl->vh_full[n & 1]));
     };
 
+    // TMA: thread 0 issues every box.  Gather: all 128 threads resolve and copy rows; each one's cp.async arrival
+    // (.noinc: counted by the barrier's 128) fires once its own copies have landed.  Those copies are generic-proxy
+    // writes that wgmma reads through the async proxy; the writer cannot fence after an asynchronous copy, so each
+    // consumer thread fences (fence.proxy.async) after its full-barrier wait, before its warpgroup's wgmma.
+    const bool leader = wt == 0;
+    int g = 0, nq = 0;  // chunks and Q tiles of the earlier streams
+    for (int st = 0; st < nstreams; ++st) {
+      const Stream sm = stream(st);
+      if (sm.nch == 0) continue;
+      // Q (rows past nr: zero filled by the gather, other rows' data by TMA -- never stored); the previous stream's
+      // Q is free once both consumers have retired its last Q K^T
+      if constexpr (kGather) {
+        const int* q_rows = args.q_rows ? args.q_rows + static_cast<size_t>(bh) * args.S : nullptr;
+        ctl->src[wt] = wt < sm.nr ? (q_rows ? __ldg(&q_rows[sm.q0 + wt]) : sm.q0 + wt) : -1;
+        mbar_wait(smem_u32(&ctl->q_empty), (nq & 1) ^ 1, 5);
+        named_bar_sync(kBarProducer, 128);
+        gather_rows(sQ, static_cast<const Elem*>(args.q_ptr) + bh * args.in_head_stride);
+        cp_async_arrive_noinc(smem_u32(&ctl->q_full));
+        named_bar_sync(kBarProducer, 128);  // ctl->src is reused by the next resolve
+      } else if (leader) {
+        const uint32_t qb = smem_u32(&ctl->q_full);
+        mbar_wait(smem_u32(&ctl->q_empty), (nq & 1) ^ 1, 5);
+        mbar_expect_tx(qb, Cfg::kTileBytes);
+        for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sQ + h * Cfg::kPanelBytes, &qmap, qb, h * Cfg::kPanelElems, sm.q0, bh);
+      }
+      for (int j = 0; j < sm.nch; ++j) {
+        const int n = g + j, s = n % kKvStages, par = ((n / kKvStages) & 1) ^ 1;
+        const uint32_t sK = stage_k(n), sV = sK + Cfg::kTileBytes;
+        const uint32_t kf = smem_u32(&ctl->k_full[s]), vf = smem_u32(&ctl->v_full[s]);
+        if constexpr (kGather) {
+          resolve_chunk(j);
+          mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
+          named_bar_sync(kBarProducer, 128);
+          gather_rows(sK, kp);
+          cp_async_arrive_noinc(kf);
+          mbar_wait(smem_u32(&ctl->v_empty[s]), par, 7);
+          gather_rows(sV, vp);
+          cp_async_arrive_noinc(vf);
+          named_bar_sync(kBarProducer, 128);  // ctl->src is reused by the next resolve
+        } else if (leader) {
+          const int kv0 = __ldg(&sm.chunks[j].x);
+          mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
+          mbar_expect_tx(kf, Cfg::kTileBytes);
+          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, kf, h * Cfg::kPanelElems, kv0, bh);
+          mbar_wait(smem_u32(&ctl->v_empty[s]), par, 7);
+          mbar_expect_tx(vf, Cfg::kTileBytes);
+          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sV + h * Cfg::kPanelBytes, &vmap, vf, h * Cfg::kPanelElems, kv0, bh);
+        }
+        // FP8: widen the previous chunk's V, requested one chunk earlier, rather than wait here for V(j) to land
+        if constexpr (FP8) {
+          if (j > 0) widen_v(n - 1);
+        }
+      }
+      if constexpr (FP8) widen_v(g + sm.nch - 1);
+      g += sm.nch;
+      ++nq;
+    }
+    return;
+  }
+
+  // ======================= consumers
+  setmaxnreg_inc<kConsumerRegs>();
+  const int cw = wg - 1;                    // this consumer's 64 rows of the tile: 64cw .. 64cw+63
+  const uint32_t sQw = sQ + 64 * cw * 128;
+  const float c = args.scale_log2 * (args.q_scale ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[bh]) : 1.f);
+  const float vs = args.v_scale ? __ldg(&args.v_scale[bh]) : 1.f;
+  const int mode = args.mask_mode, m0 = args.m0, m1 = args.m1, m2 = args.m2;
+
+  // Turns on the tensor cores: each consumer issues its wgmma groups between turn_wait and turn_pass, so the two
+  // consumers' groups alternate and one's softmax runs under the other's MMAs.  Consumer 0 takes the first turn.
+  auto turn_wait = [&]() { named_bar_sync(kBarTurn + cw, 256); };
+  auto turn_pass = [&]() { named_bar_arrive(kBarTurn + (cw ^ 1), 256); };
+  // thread 0 of the warpgroup arrives for it, after the warpgroup's wgmma reading the buffer has retired
+  auto release = [&](uint64_t& bar) {
+    if (wt == 0) mbar_arrive(smem_u32(&bar));
+  };
+  if (cw == 1) turn_pass();
+
+  int g = 0;   // chunks of this CTA before the current stream (the stream's chunk j is the CTA's chunk g + j)
+  int nq = 0;  // Q tiles loaded so far (q_full phase)
+  for (int st = 0; st < nstreams; ++st) {
+    const Stream sm = stream(st);
+    const int q0 = sm.q0, nr = sm.nr, nch = sm.nch;
+    const int2* __restrict__ chunks = sm.chunks;
+
+    auto wait_k = [&](int n) { mbar_wait(smem_u32(&ctl->k_full[n % kKvStages]), (n / kKvStages) & 1, 2); };
+    auto wait_v = [&](int n) {
+      if constexpr (FP8) mbar_wait(smem_u32(&ctl->vh_full[n & 1]), (n >> 1) & 1, 4);
+      else mbar_wait(smem_u32(&ctl->v_full[n % kKvStages]), (n / kKvStages) & 1, 3);
+    };
+    // FP8: the e4m3 V stage was read by the producer's widening, which the wait on vh_full ordered before P V
+    auto release_v = [&](int n) {
+      release(ctl->v_empty[n % kKvStages]);
+      if constexpr (FP8) release(ctl->vh_empty[n & 1]);
+    };
+    auto pv_b = [&](int n) { return FP8 ? vh_buf(n) : stage_k(n) + Cfg::kTileBytes; };
+
     // per thread: rows r0 = 16*wq + lane/4 and r0 + 8 of this warpgroup's 64; columns 8j + 2*(lane%4) (+1)
-    const int rloc = 64 * wg + 16 * wq + (lane >> 2);
+    const int rloc = 64 * cw + 16 * wq + (lane >> 2);
     ElemMask em;
     if constexpr (!kGather) {  // gather plans carry no element masks
       int qm[2];
@@ -360,56 +462,47 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     };
 
     if (nch > 0) {
-      // ---- Q (rows past nr: zero filled by the gather, other rows' data by TMA -- never stored)
-      if constexpr (kGather) {
-        if (tid < 128) {
-          const int* q_rows = args.q_rows ? args.q_rows + static_cast<size_t>(bh) * args.S : nullptr;
-          const int qr = q0 + tid;
-          ctl->src[tid] = tid < nr ? (q_rows ? __ldg(&q_rows[qr]) : qr) : -1;
-        }
-        __syncthreads();
-        gather_rows(sQ, static_cast<const Elem*>(args.q_ptr) + bh * args.in_head_stride, false, nullptr, 0);
-        __syncthreads();
-      } else if (tid == 0) {
-        const uint32_t qb = smem_u32(&ctl->q_full);
-        mbar_expect_tx(qb, Cfg::kTileBytes);
-        for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sQ + h * Cfg::kPanelBytes, &qmap, qb, h * Cfg::kPanelElems, q0, bh);
-      }
-      const int npre = min(nch, kKvStages);
-      for (int j = 0; j < npre; ++j) load_chunk(j);  // gather: Q and chunk 0 share one cp.async group
-      if constexpr (!kGather) mbar_wait(smem_u32(&ctl->q_full), nq & 1, 1);
-      wait_chunk(0, npre - 1);
-      if constexpr (FP8) {
-        widen_v(0);
-        fence_proxy_async_smem();
-        __syncthreads();
-      }
-      attn_qk_issue<D, DT>(s, sQw, stage_k(0));
+      mbar_wait(smem_u32(&ctl->q_full), nq & 1, 1);
+      wait_k(g);
+      if constexpr (kGather) fence_proxy_async_smem();  // cp.async rows -> wgmma (see the producer)
+      turn_wait();
+      attn_qk_issue<D, DT>(s, sQw, stage_k(g));
+      turn_pass();
       attn_wait<0>(s);
+      release(ctl->k_empty[g % kKvStages]);
+      if (nch == 1) release(ctl->q_empty);
       softmax(0);
       rescale_pack();
 
       for (int j = 0; j + 1 < nch; ++j) {
-        wait_chunk(j + 1, j + 2 < nch ? 1 : 0);
-        attn_qk_issue<D, DT>(s, sQw, stage_k(j + 1));  // group A
-        attn_pv_issue<D, kPBF16>(o, pa, pv_b(j));       // group B: O and pa stay in flight
-        attn_wait<1>(s);                                // A has retired, B may still be running
-        if constexpr (FP8) widen_v(j + 1);              // buffer (g+j+1) & 1 was last read by P V(j-1)
-        softmax(j + 1);                                 // runs under P V(j)
+        const int n = g + j;
+        wait_k(n + 1);
+        wait_v(n);
+        if constexpr (kGather) fence_proxy_async_smem();
+        turn_wait();
+        attn_qk_issue<D, DT>(s, sQw, stage_k(n + 1));  // group A
+        attn_pv_issue<D, kPBF16>(o, pa, pv_b(n));      // group B: O and pa stay in flight
+        turn_pass();
+        attn_wait<1>(s);                               // A has retired, B may still be running
+        release(ctl->k_empty[(n + 1) % kKvStages]);
+        if (j + 2 == nch) release(ctl->q_empty);       // the stream's last Q K^T has retired
+        softmax(j + 1);                                // runs under P V(j)
         // ptxas schedules wgmma.wait_group ahead of register math that does not depend on it, which would move
         // the exps below the wait and out from under P V(j).  Shared-memory stores stay ahead of the wait, so
         // storing the running sums (they depend on every exp of the chunk) keeps the softmax in front of it.
-        if (lane == 0) ctl->pin[tid >> 5] = l_run[0] + l_run[1];
+        if (lane == 0) ctl->pin[4 * cw + wq] = l_run[0] + l_run[1];
         attn_wait<0>(o);
         wg_fence_regs(s);  // P(j+1) is packed into pa only after P V(j) has read it
-        if constexpr (FP8) fence_proxy_async_smem();
-        __syncthreads();   // chunk j's stage is free in both warpgroups; the fp16 copy of V(j+1) is complete
-        if (j + 3 < nch) load_chunk(j + 3);
+        release_v(n);
         rescale_pack();
       }
-      attn_pv_issue<D, kPBF16>(o, pa, pv_b(nch - 1));
+      wait_v(g + nch - 1);
+      if constexpr (kGather) fence_proxy_async_smem();
+      turn_wait();
+      attn_pv_issue<D, kPBF16>(o, pa, pv_b(g + nch - 1));
+      turn_pass();
       attn_wait<0>(o);
-      __syncthreads();  // the next stream's loads overwrite Q and the stages
+      release_v(g + nch - 1);
       g += nch;
       ++nq;
     }
@@ -447,6 +540,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       }
     }
   }
+  if (cw == 0) turn_wait();  // consumer 1's hand-over after its last turn, so no named barrier is left pending
 }
 
 }  // namespace svgb

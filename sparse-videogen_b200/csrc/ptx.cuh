@@ -51,6 +51,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 // Device-visible watchdog word: a kernel that spins > ~4e9 cycles on one barrier records which
 // barrier it was and traps, so a protocol bug surfaces as a CUDA error instead of a hung box.
 static __device__ unsigned int g_svgb_watchdog[4];
+// Out of line: a trap inlined into a kernel that splits its registers with setmaxnreg keeps ptxas from giving the
+// region after the split more registers than the launch count, and the kernel spills.
+static __device__ __noinline__ void svgb_trap() { __trap(); }
 
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag = 0) {
   if (mbar_try_wait(bar, parity)) return;
@@ -62,9 +65,27 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag
       g_svgb_watchdog[2] = blockIdx.y;
       g_svgb_watchdog[3] = threadIdx.x;
       __threadfence_system();
-      __trap();
+      svgb_trap();
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// named barriers (id 0 is __syncthreads) and per-warpgroup register reallocation
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -95,11 +116,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, uint
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 // the mbarrier receives one arrival from this thread once all of the thread's earlier cp.async copies have
 // landed (.noinc: the arrival is part of the barrier's expected count)
