@@ -61,14 +61,12 @@ typedef struct svgb_plan {
   int32_t BH, S;
   int32_t max_items;     /* grid.x of the attention launch */
   int32_t items_stride;  /* 0 when one plan serves every head */
-  int32_t counts_stride;
   int32_t mask_mode, m0, m1, m2;
   int64_t counts_off, items_off, chunks_off; /* byte offsets inside the plan workspace */
   int64_t bytes;
-  int64_t aux_off;       /* kind 3: per-item selected-key totals */
 } svgb_plan;
 /* A plan built with BH == 1 may serve every head of a launch (one map for all heads, e.g. BSR masks):
- * set items_stride = counts_stride = 0 in the host struct. */
+ * set items_stride = 0 in the host struct. */
 
 /* SVG2 / BSR / dense: q-block i of head h attends k-block j iff map[h,i,j] != 0.
  * Stands behind dynamic_block_sparse_fwd_flashinfer's wrapper.plan (svg/kmeans_utils.py:1355-1385).

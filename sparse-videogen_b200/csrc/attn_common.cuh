@@ -8,11 +8,16 @@
 
 namespace svgb {
 
-// One work item = one CTA: up to 256 consecutive query rows of one head (two 128-row MMA tiles that
-// share every K/V tile) and a list of KV chunks.
-//   item  = {q_row0, nrows (1..256), chunk_off, nchunks}
-//   chunk = {kv_start, meta}; meta bits [0,8) = valid columns - 1 (0..127), bit 8 = ELEM (evaluate
-//           the element mask predicate on this chunk), bit 9 = reserved.
+// One work item = one CTA = two STREAM descriptors, items[2 * item + st] (st = 0, 1), run one after the other:
+//   stream = {q_row0, nrows (0..128; 0 = no stream), list_off, list_len}
+// A stream is up to 128 consecutive query rows of one head (one MMA tile) over the list at chunks + list_off.
+// Stream 0 always has rows; stream 1 has nrows == 0 when the CTA runs one stream.  The planners cut query rows into
+// items of up to kItemRows rows (put_item); a variable-block TMA plan also pairs two tails of different q-blocks,
+// each with its own list.  The list is
+//   TMA plans   : list_len chunks {kv_start, meta}; meta bits [0,8) = valid columns - 1 (0..127), bit 8 = ELEM
+//                 (evaluate the element mask predicate on this chunk), bit 9 = reserved.
+//   gather plans: list_len runs {src_start, keys before the run} of the selected key ranges and a sentinel
+//                 {0, total}; the kernel gathers exactly-full 128-key chunks across run boundaries.
 constexpr int kItemRows = 256;
 constexpr int kTileRows = 128;
 constexpr int kChunkCols = 128;
@@ -22,6 +27,12 @@ __host__ __device__ inline int chunk_meta(int valid, bool elem) {
   return ((valid - 1) & 0xff) | (elem ? kChunkElem : 0);
 }
 __host__ __device__ inline int chunk_valid(int meta) { return (meta & 0xff) + 1; }
+
+// the two streams of an item of nrows (1..kItemRows) consecutive query rows from q0, both over one list
+__device__ inline void put_item(int4* item, int q0, int nrows, int list_off, int list_len) {
+  item[0] = make_int4(q0, min(nrows, kTileRows), list_off, list_len);
+  item[1] = make_int4(q0 + kTileRows, max(nrows - kTileRows, 0), list_off, list_len);
+}
 
 // Element mask families (SURVEY §8 a5): parameters m0,m1,m2.
 enum MaskMode : int {
@@ -239,15 +250,10 @@ struct ElemMask {
 };
 
 struct AttnArgs {
-  const int4* items = nullptr;
-  // variable-block plans: optional second stream per work item.  items2[i].y > 0 makes item i a DUAL item: two
-  // single-tile streams (<= 128 rows each, usually the tails of two different q-blocks) share one CTA -- T0 runs
-  // items[i], T1 runs items2[i], each with its own chunk list and its own K/V tiles through the common ring.
-  const int4* items2 = nullptr;
-  const int* item_count = nullptr;
-  const int2* chunks = nullptr;
-  int items_stride = 0;   // 0: one plan shared by all heads (band masks); else items per head
-  int counts_stride = 0;  // 0 or 1
+  const int4* items = nullptr;      // two stream descriptors per item
+  const int* item_count = nullptr;  // [BH] when items_stride != 0, else [1]
+  const int2* chunks = nullptr;     // chunk or run lists
+  int items_stride = 0;             // 0: one plan shared by all heads (band masks); else items per head
   void* o = nullptr;
   long long o_row_stride = 0;   // elements
   long long o_head_stride = 0;  // elements
@@ -263,11 +269,8 @@ struct AttnArgs {
   const float* q_scale = nullptr;
   const float* k_scale = nullptr;
   const float* v_scale = nullptr;
-  // ---- gather mode (SVG2; attn_fwd_kernel<..., kGather = true>): `chunks` holds RUNS {src_start, cum_before}
-  // (+ a sentinel {0, total}) of the selected key ranges; K/V rows are gathered with cp.async into exactly-full
-  // 128-token chunks, optionally through row-index vectors so the cluster permutation of Q, K, V never
-  // materialises in HBM.
-  const int* item_total = nullptr;  // [BH * items_stride | items]: selected keys per item; non-NULL = gather mode
+  // ---- gather mode (SVG2; attn_fwd_kernel<..., kGather = true>, run lists): K/V rows are gathered with cp.async,
+  // optionally through row-index vectors so the cluster permutation of Q, K, V never materialises in HBM.
   const int* q_rows = nullptr;      // optional [BH, S]: source row of (permuted) query row
   const int* kv_rows = nullptr;     // optional [BH, S]: source row of (permuted) key/value row
   const void* q_ptr = nullptr;      // raw tensors for the gather path ([BH,S,D] with the strides below)

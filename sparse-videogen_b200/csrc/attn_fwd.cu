@@ -19,8 +19,7 @@ namespace svgb {
 constexpr int kPlanWarps = 8;
 __global__ void __launch_bounds__(kPlanWarps * 32)
 plan_lists_kernel(const uint8_t* __restrict__ map, const int* __restrict__ row_sz, const int* __restrict__ col_sz,
-                  int QC, int KC, int chunk_cap, int gather, int2* __restrict__ chunks, int* __restrict__ nch_of,
-                  int* __restrict__ tot_of) {
+                  int QC, int KC, int chunk_cap, int gather, int2* __restrict__ chunks, int* __restrict__ nch_of) {
   // gather form: the list holds RUNS {start, keys before this run} plus a sentinel {0, total}; the kernel then
   // gathers exactly-full 128-key chunks across run boundaries.
   extern __shared__ int sm[];
@@ -98,27 +97,22 @@ plan_lists_kernel(const uint8_t* __restrict__ map, const int* __restrict__ row_s
     if (run_s >= 0) flush();
     if (gather && lane == 0) out[n] = make_int2(0, total);  // sentinel: ends the last run
   }
-  if (lane == 0) {
-    nch_of[static_cast<size_t>(bh) * QC + qb] = n;
-    tot_of[static_cast<size_t>(bh) * QC + qb] = total;
-  }
+  if (lane == 0) nch_of[static_cast<size_t>(bh) * QC + qb] = n;
 }
 
-__global__ void plan_items_kernel(const int* __restrict__ row_sz, const int* __restrict__ nch_all,
-                                  const int* __restrict__ tot_all, int QC, int max_items, int chunk_cap,
-                                  int* __restrict__ counts,
-                                  int4* __restrict__ items, int4* __restrict__ items2, int* __restrict__ item_total) {
-  // TMA form (items2 != nullptr): a q-block of r rows becomes r/256 two-tile items (+ one more when r % 256 > 128,
-  // its second tile partial) and, when 0 < r % 256 <= 128, a single-tile TAIL.  Tails are where k-means clusters
-  // lose tensor-core rows (a 297-row cluster = 256 + 41) and a lone single-tile CTA leaves half of the softmax
-  // warps idle, so the tails of a head are sorted by chunk count and packed two per CTA as DUAL items
-  // (items[i] = stream of T0, items2[i] = stream of T1; see AttnArgs::items2).  Launch order: two-tile items in
-  // q-block order, then the dual items from long to short.
-  const bool gather = item_total != nullptr;
+__global__ void plan_items_kernel(const int* __restrict__ row_sz, const int* __restrict__ nch_all, int QC,
+                                  int max_items, int chunk_cap, int gather, int* __restrict__ counts,
+                                  int4* __restrict__ items) {
+  // TMA form: a q-block of r rows becomes r/256 two-tile items (+ one more when r % 256 > 128, its second tile
+  // partial) and, when 0 < r % 256 <= 128, a single-tile TAIL.  Tails are where k-means clusters lose tensor-core
+  // rows (a 297-row cluster = 256 + 41) and a lone single-tile CTA leaves half of the softmax warps idle, so the
+  // tails of a head are sorted by chunk count and packed two per CTA, one per stream, each with its own list.
+  // Launch order: two-tile items in q-block order, then the paired tails from long to short.  Gather form: every
+  // q-block is cut into items of up to 256 rows; tails are not paired.
   extern __shared__ int sm[];
   int* rowoff = sm;                 // QC + 1
   int* itembase = rowoff + QC + 1;  // QC + 1 : first two-tile item of the q-block (gather: first item)
-  int* long_of = itembase + QC + 1; // QC     : rows of the q-block's tail (1..128; 0 = none) -> dual item
+  int* long_of = itembase + QC + 1; // QC     : rows of the q-block's tail (1..128; 0 = none) -> paired
   int* nch_of = long_of + QC;       // QC
   __shared__ int s_total2, s_nlong;
   const int bh = blockIdx.x;
@@ -164,19 +158,15 @@ __global__ void plan_items_kernel(const int* __restrict__ row_sz, const int* __r
     const int nit = itembase[qb + 1] - itembase[qb];
     for (int t = 0; t < nit; ++t) {
       const int idx = itembase[qb] + t;
-      if (idx < max_items) {
-        items[static_cast<size_t>(bh) * max_items + idx] =
-            make_int4(rowoff[qb] + t * kItemRows, min(kItemRows, r - t * kItemRows), static_cast<int>(list), n);
-        if (items2) items2[static_cast<size_t>(bh) * max_items + idx] = make_int4(0, 0, 0, 0);
-        if (gather) item_total[static_cast<size_t>(bh) * max_items + idx] = tot_all[static_cast<size_t>(bh) * QC + qb];
-      }
+      if (idx < max_items)
+        put_item(items + 2 * (static_cast<size_t>(bh) * max_items + idx), rowoff[qb] + t * kItemRows,
+                 min(kItemRows, r - t * kItemRows), static_cast<int>(list), n);
     }
   }
   if (!pair) return;
-  // tails: rank by (chunk count descending, q-block ascending); ranks 2i and 2i+1 share CTA i
+  // tails: rank by (chunk count descending, q-block ascending); ranks 2i and 2i+1 are streams 0 and 1 of CTA i
   const int base = s_total2;
-  int4* a = items + static_cast<size_t>(bh) * max_items + base;
-  int4* b = items2 + static_cast<size_t>(bh) * max_items + base;
+  int4* pairs = items + 2 * (static_cast<size_t>(bh) * max_items + base);
   const int cap = max_items - base;
   for (int qb = threadIdx.x; qb < QC; qb += blockDim.x) {
     const int rows = long_of[qb];
@@ -188,14 +178,9 @@ __global__ void plan_items_kernel(const int* __restrict__ row_sz, const int* __r
     const int r = rowoff[qb + 1] - rowoff[qb];
     const int4 it = make_int4(rowoff[qb] + (r / kItemRows) * kItemRows, rows,
                               static_cast<int>((static_cast<size_t>(bh) * QC + qb) * chunk_cap), mine);
-    const int idx = rank >> 1;
-    if (idx < cap) {
-      if ((rank & 1) == 0) {
-        a[idx] = it;
-        if (rank == s_nlong - 1) b[idx] = make_int4(0, 0, 0, 0);  // odd one out
-      } else {
-        b[idx] = it;
-      }
+    if ((rank >> 1) < cap) {
+      pairs[rank] = it;
+      if (rank == s_nlong - 1 && (rank & 1) == 0) pairs[rank + 1] = make_int4(0, 0, 0, 0);  // odd one out
     }
   }
 }
@@ -246,7 +231,7 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
     }
   }
   if (threadIdx.x == 0) {
-    items[item] = make_int4(q_row0, nrows, static_cast<int>(static_cast<size_t>(item) * n_chunks_total), n);
+    put_item(items + 2 * item, q_row0, nrows, static_cast<int>(static_cast<size_t>(item) * n_chunks_total), n);
     if (item == 0) counts[0] = gridDim.x;
   }
 }
@@ -387,9 +372,9 @@ selftest_tile_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_cons
 
 template <int D, int DT>
 static int launch_attn(const CUtensorMap& qm, const CUtensorMap& km, const CUtensorMap& vm,
-                       const AttnArgs& args, dim3 grid, cudaStream_t stream) {
+                       const AttnArgs& args, bool gather, dim3 grid, cudaStream_t stream) {
   using Cfg = AttnCfg<D, DT>;
-  auto kern = args.item_total ? attn_fwd_kernel<D, DT, true> : attn_fwd_kernel<D, DT, false>;
+  auto kern = gather ? attn_fwd_kernel<D, DT, true> : attn_fwd_kernel<D, DT, false>;
   SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args);
   SVGB_LAUNCH_OK();
@@ -409,8 +394,8 @@ static int launch_selftest(const CUtensorMap& qm, const CUtensorMap& km, const C
 }
 
 int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const void* k, const void* v, int Skv,
-                  long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, int grid_x,
-                  cudaStream_t st) {
+                  long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, bool gather,
+                  int grid_x, cudaStream_t st) {
   SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16 || dtype == SVGB_E4M3, "dtype %d unsupported", dtype);
   CUtensorMap qm, km, vm;
@@ -420,30 +405,17 @@ int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const v
   dim3 grid(grid_x, BH);
   if (dtype == SVGB_E4M3) {
     SVGB_REQUIRE(D == 128, "the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle", D);
-    return launch_attn<128, DT_E4M3>(qm, km, vm, a, grid, st);
+    return launch_attn<128, DT_E4M3>(qm, km, vm, a, gather, grid, st);
   }
   if (D == 128) {
-    return dtype == SVGB_BF16 ? launch_attn<128, DT_BF16>(qm, km, vm, a, grid, st)
-                              : launch_attn<128, DT_F16>(qm, km, vm, a, grid, st);
+    return dtype == SVGB_BF16 ? launch_attn<128, DT_BF16>(qm, km, vm, a, gather, grid, st)
+                              : launch_attn<128, DT_F16>(qm, km, vm, a, gather, grid, st);
   }
-  return dtype == SVGB_BF16 ? launch_attn<64, DT_BF16>(qm, km, vm, a, grid, st)
-                            : launch_attn<64, DT_F16>(qm, km, vm, a, grid, st);
+  return dtype == SVGB_BF16 ? launch_attn<64, DT_BF16>(qm, km, vm, a, gather, grid, st)
+                            : launch_attn<64, DT_F16>(qm, km, vm, a, gather, grid, st);
 }
 
 static int varblock_chunk_cap(int S, int KC) { return S / kChunkCols + (KC + 1) / 2 + 2; }
-
-// per-q-block scratch (list length, key total) that follows the aux region of a variable-block plan workspace
-struct VarScratch {
-  size_t nch_off, tot_off;
-};
-static VarScratch var_scratch(long long aux_off, int BH, int max_items, int QC) {
-  VarScratch L;
-  const size_t aux_bytes = align_up(sizeof(int4) * BH * max_items, 256);
-  const size_t len_bytes = align_up(sizeof(int) * static_cast<size_t>(BH) * QC, 256);
-  L.nch_off = aux_off + aux_bytes;
-  L.tot_off = L.nch_off + len_bytes;
-  return L;
-}
 static int varblock_max_items(int S, int QC) { return S / kItemRows + QC + 1; }
 
 }  // namespace svgb
@@ -455,12 +427,10 @@ extern "C" {
 int svgb_attn_plan_varblock_bytes(int BH, int S, int QC, int KC, size_t* bytes) {
   SVGB_REQUIRE(BH > 0 && S > 0 && QC > 0 && KC > 0 && bytes, "bad arguments");
   const size_t counts = align_up(sizeof(int) * BH, 256);
-  const size_t items = align_up(sizeof(int4) * BH * varblock_max_items(S, QC), 256);
+  const size_t items = align_up(2 * sizeof(int4) * BH * varblock_max_items(S, QC), 256);
   const size_t chunks = align_up(sizeof(int2) * static_cast<size_t>(BH) * QC * varblock_chunk_cap(S, KC), 256);
-  // aux: TMA plans = second stream of dual items (int4 per item); gather plans = selected keys per item (int)
-  const size_t aux = align_up(sizeof(int4) * BH * varblock_max_items(S, QC), 256);
-  const size_t lens = 2 * align_up(sizeof(int) * static_cast<size_t>(BH) * QC, 256);  // per q-block list length / key total
-  *bytes = counts + items + chunks + aux + lens;
+  const size_t lens = align_up(sizeof(int) * static_cast<size_t>(BH) * QC, 256);  // per q-block list length
+  *bytes = counts + items + chunks + lens;
   return 0;
 }
 
@@ -480,31 +450,28 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   plan->S = S;
   plan->max_items = max_items;
   plan->items_stride = max_items;
-  plan->counts_stride = 1;
   plan->mask_mode = MASK_NONE;
-  plan->m0 = gather ? (KC + 1) / 2 + 1 : 0;  // gather: upper bound of runs per q-block (kernel smem table)
+  plan->m0 = 0;
   plan->m1 = 0;
   plan->m2 = 0;
   plan->counts_off = 0;
   plan->items_off = align_up(sizeof(int) * BH, 256);
-  plan->chunks_off = plan->items_off + align_up(sizeof(int4) * BH * max_items, 256);
-  plan->aux_off = plan->chunks_off + align_up(sizeof(int2) * static_cast<size_t>(BH) * QC * cap, 256);
+  plan->chunks_off = plan->items_off + align_up(2 * sizeof(int4) * BH * max_items, 256);
   plan->bytes = need;
   char* ws = static_cast<char*>(plan_ws);
-  const VarScratch tl = var_scratch(plan->aux_off, BH, max_items, QC);
-  int* nch_of = reinterpret_cast<int*>(ws + tl.nch_off);
-  int* tot_of = reinterpret_cast<int*>(ws + tl.tot_off);
+  // per q-block list lengths: scratch of the two plan kernels, after the lists
+  const size_t lens_off = plan->chunks_off + align_up(sizeof(int2) * static_cast<size_t>(BH) * QC * cap, 256);
+  int* nch_of = reinterpret_cast<int*>(ws + lens_off);
   const size_t smem1 = sizeof(int) * (KC + 1);
   const size_t smem2 = sizeof(int) * (2 * (QC + 1) + 2 * QC);
   SVGB_REQUIRE(smem1 <= 48 * 1024 && smem2 <= 48 * 1024, "QC/KC too large for the plan kernels (%zu / %zu B smem)", smem1, smem2);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   plan_lists_kernel<<<dim3((QC + kPlanWarps - 1) / kPlanWarps, BH), kPlanWarps * 32, smem1, st>>>(map, row_sz, col_sz, QC, KC, cap, gather ? 1 : 0,
-                                                                 reinterpret_cast<int2*>(ws + plan->chunks_off), nch_of, tot_of);
+                                                                 reinterpret_cast<int2*>(ws + plan->chunks_off), nch_of);
   SVGB_LAUNCH_OK();
-  plan_items_kernel<<<BH, 256, smem2, st>>>(
-      row_sz, nch_of, tot_of, QC, max_items, cap, reinterpret_cast<int*>(ws + plan->counts_off),
-      reinterpret_cast<int4*>(ws + plan->items_off), gather ? nullptr : reinterpret_cast<int4*>(ws + plan->aux_off),
-      gather ? reinterpret_cast<int*>(ws + plan->aux_off) : nullptr);
+  plan_items_kernel<<<BH, 256, smem2, st>>>(row_sz, nch_of, QC, max_items, cap, gather ? 1 : 0,
+                                            reinterpret_cast<int*>(ws + plan->counts_off),
+                                            reinterpret_cast<int4*>(ws + plan->items_off));
   SVGB_LAUNCH_OK();
   return 0;
 }
@@ -525,7 +492,7 @@ int svgb_attn_plan_band_bytes(int S, size_t* bytes) {
   SVGB_REQUIRE(S > 0 && bytes, "bad arguments");
   const size_t n_items = (S + kItemRows - 1) / kItemRows + 4;  // + one partial item per extra row segment
   const size_t n_chunks = (S + kChunkCols - 1) / kChunkCols;
-  *bytes = 256 + align_up(sizeof(int4) * n_items, 256) + align_up(sizeof(int2) * n_items * n_chunks, 256);
+  *bytes = 256 + align_up(2 * sizeof(int4) * n_items, 256) + align_up(sizeof(int2) * n_items * n_chunks, 256);
   return 0;
 }
 
@@ -547,15 +514,13 @@ int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, vo
   plan->S = S;
   plan->max_items = n_items;
   plan->items_stride = 0;
-  plan->counts_stride = 0;
   plan->mask_mode = mask_mode;
   plan->m0 = m0;
   plan->m1 = m1;
   plan->m2 = m2;
   plan->counts_off = 0;
   plan->items_off = 256;
-  plan->chunks_off = 256 + align_up(sizeof(int4) * n_items_cap, 256);
-  plan->aux_off = 0;
+  plan->chunks_off = 256 + align_up(2 * sizeof(int4) * n_items_cap, 256);
   plan->bytes = need;
   char* ws = static_cast<char*>(plan_ws);
   plan_band_kernel<<<n_items, kItemRows, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -582,16 +547,12 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                "plan was built for BH=%d S=%d, called with BH=%d S=%d", plan->BH, plan->S, BH, S);
   SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && o_row_stride % 8 == 0 && o_head_stride % 8 == 0,
                "output must be 16-byte aligned with strides multiple of 8 elements");
-  SVGB_REQUIRE(!gather || plan->m0 <= AttnCfg<64>::kMaxRunsSmem, "gather plan has too many runs per q-block (%d)", plan->m0);
   const char* ws = static_cast<const char*>(plan_ws);
   AttnArgs a;
   a.items = reinterpret_cast<const int4*>(ws + plan->items_off);
   a.item_count = reinterpret_cast<const int*>(ws + plan->counts_off);
   a.chunks = reinterpret_cast<const int2*>(ws + plan->chunks_off);
-  if (plan->kind == SVGB_PLAN_VARBLOCK) a.items2 = reinterpret_cast<const int4*>(ws + plan->aux_off);
-  if (gather) a.item_total = reinterpret_cast<const int*>(ws + plan->aux_off);
   a.items_stride = plan->items_stride;
-  a.counts_stride = plan->counts_stride;
   a.o = o;
   a.o_row_stride = o_row_stride;
   a.o_head_stride = o_head_stride;
@@ -613,7 +574,7 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
   a.v_ptr = v;
   a.in_row_stride = row_stride;
   a.in_head_stride = head_stride;
-  return attn_fwd_impl(q, S, row_stride, head_stride, k, v, S, row_stride, head_stride, dtype, BH, D, a,
+  return attn_fwd_impl(q, S, row_stride, head_stride, k, v, S, row_stride, head_stride, dtype, BH, D, a, gather,
                        plan->max_items, static_cast<cudaStream_t>(stream));
 }
 

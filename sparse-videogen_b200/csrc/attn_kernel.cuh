@@ -2,8 +2,8 @@
 //
 // One CTA per work item, 384 threads in three warpgroups.  Warpgroup 0 is the PRODUCER: it does every load.
 // Warpgroups 1 and 2 are the CONSUMERS: consumer c owns query rows 64c .. 64c+63 of a 128-row tile.  A work item is
-// one or two 128-row STREAMS (a two-tile item: rows 0-127 and 128-255 over the same chunk list; a dual item: two
-// independent tails, each with its own chunk list), run one after the other.
+// one or two 128-row STREAMS, each a descriptor {q_row0, nrows, list_off, list_len} (attn_common.cuh), run one after
+// the other.
 //   Q tile          : TMA (or cp.async row gather), 128-byte swizzle, stays in shared memory for the stream
 //   K(j), V(j)      : three stages, each half with its own full and empty mbarrier
 //   S = Q K^T       : wgmma m64n128 (SS, both operands K-major), fp32 accumulators in registers
@@ -52,7 +52,6 @@ struct AttnCfg {
   static constexpr int kTileBytes = kPanelBytes * kHalves;
   static constexpr int kKSteps = kRowBytes / 32;         // wgmma K steps of Q K^T (32 bytes each)
   static constexpr int kVhBytes = DT == DT_E4M3 ? 2 * kPanelBytes : 0;  // fp16 copy of one e4m3 V tile
-  static constexpr int kMaxRunsSmem = kTileBytes / 8 - 1;
   static constexpr int kBarBytes = 1024;                 // mbarriers + gather row table
   // + 1 KB: the kernel aligns the dynamic window to 1024 bytes itself
   static constexpr int kSmemBytes = 1024 + kTileBytes + 2 * kKvStages * kTileBytes + 2 * kVhBytes + kBarBytes;
@@ -140,15 +139,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   constexpr bool kPBF16 = DT == DT_BF16;  // format of P and V in the P V product (fp8: fp16)
   using Elem = typename std::conditional<FP8, uint8_t, uint16_t>::type;  // storage element of Q / K / V
   const int bh = blockIdx.y;
-  const int n_items = args.item_count[bh * args.counts_stride];
+  const int n_items = args.item_count[args.items_stride ? bh : 0];
   if (static_cast<int>(blockIdx.x) >= n_items) return;
-  const size_t item_idx = static_cast<size_t>(bh) * args.items_stride + blockIdx.x;
-  const int4 item = args.items[item_idx];
-  int4 item2 = make_int4(0, 0, 0, 0);
-  if (!kGather && args.items2) item2 = args.items2[item_idx];
-  const bool dual = item2.y > 0;
-  // gather mode: item.w = number of runs, chunks are implicit (128 selected keys each, last one partial)
-  const int total_kv = kGather ? args.item_total[item_idx] : 0;
+  const int4* desc = args.items + 2 * (static_cast<size_t>(bh) * args.items_stride + blockIdx.x);
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_u32 = smem_u32(smem_raw);
@@ -188,19 +181,22 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   }
   __syncthreads();  // the barriers are initialised; the last block-wide barrier of the kernel
 
-  const int nstreams = (dual || item.y > kTileRows) ? 2 : 1;
-  // stream st of the item: first query row, rows, chunk list and chunk count
+  const int nstreams = __ldg(&desc[1].y) > 0 ? 2 : 1;
+  // stream st of the item: first query row, rows, list, list length, chunk count and (gather) selected keys.  A
+  // gather stream's chunks are implicit: 128 selected keys each, the last one partial.
   struct Stream {
-    int q0, nr, nch;
-    const int2* chunks;
+    int q0, nr, nlist, nch, total;
+    const int2* list;
   };
   auto stream = [&](int st) {
-    const bool second = st == 1;
+    const int4 d = __ldg(&desc[st]);
     Stream sm;
-    sm.q0 = second ? (dual ? item2.x : item.x + kTileRows) : item.x;
-    sm.nr = second ? (dual ? item2.y : item.y - kTileRows) : (dual ? item.y : min(item.y, kTileRows));
-    sm.chunks = args.chunks + ((second && dual) ? item2.z : item.z);
-    sm.nch = kGather ? (total_kv + kChunkCols - 1) / kChunkCols : ((second && dual) ? item2.w : item.w);
+    sm.q0 = d.x;
+    sm.nr = d.y;
+    sm.list = args.chunks + d.z;
+    sm.nlist = d.w;
+    sm.total = kGather ? __ldg(&sm.list[d.w].y) : 0;  // the run list's sentinel
+    sm.nch = kGather ? (sm.total + kChunkCols - 1) / kChunkCols : d.w;
     return sm;
   };
   // Both roles count chunks over the whole CTA: chunk n (the stream's chunk j is n = g + j, g = chunks of the earlier
@@ -215,8 +211,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     const Elem* kp = static_cast<const Elem*>(args.k_ptr) + bh * args.in_head_stride;
     const Elem* vp = static_cast<const Elem*>(args.v_ptr) + bh * args.in_head_stride;
     const int* kv_rows = (kGather && args.kv_rows) ? args.kv_rows + static_cast<size_t>(bh) * args.S : nullptr;
-    const int2* __restrict__ runs = args.chunks + item.z;
-    const int nruns = item.w;
 
     // gather: piece p (16 B) of row r -> panel p/8, byte r*128 + ((p%8) ^ (r%8))*16; a row is kRowBytes bytes
     // (e4m3 at D = 128: 8 pieces, one panel)
@@ -232,12 +226,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         cp_async16(dst + off, src_base + so, src >= 0 ? 16u : 0u);
       }
     };
-    // gather: source rows of keys j*128 .. j*128+127 of this item -> ctl->src
-    auto resolve_chunk = [&](int j) {
+    // gather: source rows of keys j*128 .. j*128+127 of stream sm -> ctl->src
+    auto resolve_chunk = [&](const Stream& sm, int j) {
+      const int2* __restrict__ runs = sm.list;
       const int pos = j * kChunkCols + wt;
       int src = -1;
-      if (pos < total_kv) {
-        int lo = 0, hi = nruns - 1;  // largest run with keys_before <= pos
+      if (pos < sm.total) {
+        int lo = 0, hi = sm.nlist - 1;  // largest run with keys_before <= pos
         while (lo < hi) {
           const int mid = (lo + hi + 1) >> 1;
           if (__ldg(&runs[mid].y) <= pos) lo = mid;
@@ -311,7 +306,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         const uint32_t sK = stage_k(n), sV = sK + Cfg::kTileBytes;
         const uint32_t kf = smem_u32(&ctl->k_full[s]), vf = smem_u32(&ctl->v_full[s]);
         if constexpr (kGather) {
-          resolve_chunk(j);
+          resolve_chunk(sm, j);
           mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
           named_bar_sync(kBarProducer, 128);
           gather_rows(sK, kp);
@@ -321,7 +316,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
           cp_async_arrive_noinc(vf);
           named_bar_sync(kBarProducer, 128);  // ctl->src is reused by the next resolve
         } else if (leader) {
-          const int kv0 = __ldg(&sm.chunks[j].x);
+          const int kv0 = __ldg(&sm.list[j].x);
           mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
           mbar_expect_tx(kf, Cfg::kTileBytes);
           for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, kf, h * Cfg::kPanelElems, kv0, bh);
@@ -363,8 +358,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   int nq = 0;  // Q tiles loaded so far (q_full phase)
   for (int st = 0; st < nstreams; ++st) {
     const Stream sm = stream(st);
-    const int q0 = sm.q0, nr = sm.nr, nch = sm.nch;
-    const int2* __restrict__ chunks = sm.chunks;
+    const int q0 = sm.q0, nr = sm.nr, nch = sm.nch, total = sm.total;
+    const int2* __restrict__ chunks = sm.list;
 
     auto wait_k = [&](int n) { mbar_wait(smem_u32(&ctl->k_full[n % kKvStages]), (n / kKvStages) & 1, 2); };
     auto wait_v = [&](int n) {
@@ -404,7 +399,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       int kv0 = 0, valid = kChunkCols;
       bool elem = false;
       if constexpr (kGather) {
-        valid = min(kChunkCols, total_kv - j * kChunkCols);
+        valid = min(kChunkCols, total - j * kChunkCols);
       } else {
         const int2 ch = __ldg(&chunks[j]);
         kv0 = ch.x;

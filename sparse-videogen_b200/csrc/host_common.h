@@ -50,10 +50,10 @@ int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S
 
 struct AttnArgs;
 // attention launch with independent query / key-value geometry (attn_fwd.cu); used by svgb_attn_fwd
-// and by sample_mse's split-KV passes.  Checks D and dtype; a.item_total != NULL selects the row-gather kernel.
+// and by sample_mse's split-KV passes.  Checks D and dtype; gather selects the row-gather kernel (run lists).
 int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const void* k, const void* v, int Skv,
-                  long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, int grid_x,
-                  cudaStream_t st);
+                  long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, bool gather,
+                  int grid_x, cudaStream_t st);
 
 // stable counting-sort argsort (layout_ops.cu); `offs` (optional) receives the exclusive prefix of
 // counts per head; `skip_flag` (optional, device) turns the three kernels into no-ops when non-zero.

@@ -41,7 +41,7 @@ __global__ void smse_plan_kernel(int S, int nsplit, int n_chunks, int* counts, i
   }
   for (int s = threadIdx.x; s < nsplit; s += blockDim.x) {
     const int c0 = min(n_chunks, s * cps), c1 = min(n_chunks, c0 + cps);
-    items[s] = make_int4(s * 128, 128, c0, c1 - c0);
+    put_item(items + 2 * s, s * 128, 128, c0, c1 - c0);
   }
   if (threadIdx.x == 0) counts[0] = nsplit;
 }
@@ -135,7 +135,7 @@ static SmseLayout smse_layout(int BH, int S, int D, int n_sms) {
   L.qg = take(2ull * BH * rows * D);
   L.qidx = take(4 * rows);
   L.counts = take(256);
-  L.items = take(sizeof(int4) * L.nsplit);
+  L.items = take(2 * sizeof(int4) * L.nsplit);
   L.chunks_plain = take(sizeof(int2) * L.n_chunks);
   L.chunks_elem = take(sizeof(int2) * L.n_chunks);
   L.o_part = take(4ull * 3 * BH * rows * D);
@@ -217,7 +217,7 @@ int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* 
     a.q_index = reinterpret_cast<const int*>(w + L.qidx);
     a.out_f32 = 1;
     if (attn_fwd_impl(w + L.qg, rows_per_head, D, static_cast<long long>(rows_per_head) * D, k, v, S, D,
-                      static_cast<long long>(S) * D, dtype, BH, D, a, L.nsplit, st))
+                      static_cast<long long>(S) * D, dtype, BH, D, a, false, L.nsplit, st))
       return -1;
   }
   smse_combine_kernel<<<dim3(BH, kCombineParts), 256, 0, st>>>(

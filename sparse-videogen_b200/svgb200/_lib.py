@@ -21,10 +21,10 @@ class Plan(C.Structure):
     """mirror of `struct svgb_plan`"""
     _fields_ = [
         ("kind", C.c_int32), ("BH", C.c_int32), ("S", C.c_int32), ("max_items", C.c_int32),
-        ("items_stride", C.c_int32), ("counts_stride", C.c_int32),
+        ("items_stride", C.c_int32),
         ("mask_mode", C.c_int32), ("m0", C.c_int32), ("m1", C.c_int32), ("m2", C.c_int32),
         ("counts_off", C.c_int64), ("items_off", C.c_int64), ("chunks_off", C.c_int64),
-        ("bytes", C.c_int64), ("aux_off", C.c_int64),
+        ("bytes", C.c_int64),
     ]
 
 

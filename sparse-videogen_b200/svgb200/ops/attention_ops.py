@@ -89,7 +89,6 @@ def bsr_to_plan(indptr, indices, block_size, video_len, text_len, device) -> cor
         col[0, 0] = text_len
     plan = core.plan_varblock(bm, row, col, video_len + text_len)  # owns its workspace: safe to cache
     plan.desc.items_stride = 0   # one map for every head: share the plan (svgb200.h, svgb_plan)
-    plan.desc.counts_stride = 0
     _plan_cache[key] = (weakref.ref(indptr), weakref.ref(indices), plan)
     return plan
 

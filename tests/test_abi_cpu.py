@@ -48,10 +48,18 @@ def test_argument_errors_are_reported(lib):
     assert lib.svgb_sample_mse_bytes(2, 1000, 96, 64, C.byref(n)) < 0
 
 
-def test_plan_struct_layout_matches_header():
+def test_plan_struct_mirrors_header():
+    """_lib.Plan declares the fields of `struct svgb_plan` in include/svgb200.h, in order and with their types."""
     from svgb200._lib import Plan
 
-    assert C.sizeof(Plan) == 10 * 4 + 5 * 8
+    header = (ROOT / "include" / "svgb200.h").read_text()
+    body = re.search(r"typedef struct svgb_plan \{(.*?)\} svgb_plan;", header, re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    ctype = {"int32_t": C.c_int32, "int64_t": C.c_int64}
+    fields = [(name.strip(), ctype[t]) for t, names in re.findall(r"(int32_t|int64_t)\s+([^;]+);", body)
+              for name in names.split(",")]
+    assert fields == list(Plan._fields_)
+    assert C.sizeof(Plan) == 9 * 4 + 4 + 4 * 8  # 4 bytes of padding align the first int64
     assert Plan.counts_off.offset == 40
 
 

@@ -279,29 +279,38 @@ def test_census_wan_sap_last(cuda):
                  o_rows=last["q_sorted_indices"].cpu(), key_ids=last["k_sorted_indices"].cpu(), what="WanSAPCore.last")
 
 
-@pytest.mark.parametrize("D", [64, 128])
-def test_census_gather_plan(cuda, D):
-    """Row-gather plan with q_rows / kv_rows / o_rows (cluster argsorts), empty clusters and a query cluster that
-    selects nothing."""
+@pytest.mark.parametrize("D,KC", [(64, 101), (128, 101), (64, 4096), (128, 4096)],
+                         ids=["64", "128", "64-kc4096", "128-kc4096"])
+def test_census_gather_plan(cuda, D, KC):
+    """Row-gather plan with q_rows / kv_rows / o_rows (cluster argsorts).  KC = 101: empty clusters and a query
+    cluster that selects nothing.  KC = 4096 (the k-means limit): two keys per key cluster and every other cluster
+    selected, so every q-block reads 2048 runs."""
     from svgb200 import core
 
     g = torch.Generator().manual_seed(23)
-    H, S, QC, KC = 3, 6000, 37, 101
-    ql = torch.randint(0, QC, (H, S), generator=g)
-    kl = torch.randint(0, KC, (H, S), generator=g)
-    ql[0][ql[0] == 5] = 6   # an empty query cluster
-    kl[1][kl[1] == 3] = 4   # an empty key cluster
-    bm = torch.rand(H, QC, KC, generator=g) < 0.4
-    bm[2, 7, :] = False     # a query cluster that sees nothing
-    bm[2, 8, :] = True      # and one that sees everything
+    if KC == 4096:
+        H, S, QC = 2, 8192, 23
+        ql = torch.randint(0, QC, (H, S), generator=g)
+        kl = torch.stack([torch.randperm(S, generator=g) // 2 for _ in range(H)])
+        bm = torch.zeros(H, QC, KC, dtype=torch.bool)
+        bm[:, :, 0::2] = True
+    else:
+        H, S, QC = 3, 6000, 37
+        ql = torch.randint(0, QC, (H, S), generator=g)
+        kl = torch.randint(0, KC, (H, S), generator=g)
+        ql[0][ql[0] == 5] = 6   # an empty query cluster
+        kl[1][kl[1] == 3] = 4   # an empty key cluster
+        bm = torch.rand(H, QC, KC, generator=g) < 0.4
+        bm[2, 7, :] = False     # a query cluster that sees nothing
+        bm[2, 8, :] = True      # and one that sees everything
     qperm, qcnt = core.argsort_labels(ql.to(cuda), QC)
     kperm, kcnt = core.argsort_labels(kl.to(cuda), KC)
     run_varblock(cuda, bm, qcnt.cpu(), kcnt.cpu(), S, D, o_rows=qperm.cpu(), key_ids=kperm.cpu(), q_rows=qperm.cpu(),
-                 gather=True, what=f"gather plan D={D}")
+                 gather=True, what=f"gather plan D={D} KC={KC}")
 
 
 def test_census_bsr_shared_plan(cuda):
-    """One BSR plan serving every head (items_stride = counts_stride = 0, svgb200.ops.attention_ops.bsr_to_plan):
+    """One BSR plan serving every head (items_stride = 0, svgb200.ops.attention_ops.bsr_to_plan):
     the reference's temporal BSR blocks over the video plus an all-to-all text prefix."""
     from oracle import attention as oa
     from svgb200.ops import attention_ops

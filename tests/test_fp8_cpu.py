@@ -37,7 +37,7 @@ def test_attn_fwd_e4m3_argument_errors(lib):
     from svgb200._lib import Plan
     from svgb200.core import PLAN_BAND, PLAN_GATHER, PLAN_VARBLOCK
 
-    plan = Plan(kind=PLAN_GATHER, BH=1, S=1024, max_items=4, items_stride=4, counts_stride=1)
+    plan = Plan(kind=PLAN_GATHER, BH=1, S=1024, max_items=4, items_stride=4)
     assert _call(lib, plan, scales=False, rows=True) < 0
     assert b"scale" in lib.svgb_last_error()
     for kind in (PLAN_VARBLOCK, PLAN_BAND):
@@ -50,7 +50,7 @@ def test_scales_are_rejected_with_16bit_inputs(lib):
     from svgb200._lib import Plan
     from svgb200.core import PLAN_VARBLOCK
 
-    plan = Plan(kind=PLAN_VARBLOCK, BH=1, S=1024, max_items=4, items_stride=4, counts_stride=1)
+    plan = Plan(kind=PLAN_VARBLOCK, BH=1, S=1024, max_items=4, items_stride=4)
     assert _call(lib, plan, dtype=SVGB_BF16) < 0
     assert b"scale" in lib.svgb_last_error()
 
