@@ -140,6 +140,74 @@ def distinguishable_limit(n_max: int, out_dtype, c_max: int = 4096) -> int:
     return c_max
 
 
+# --------------------------------------------------------------------------------------------
+# plan shapes that hit the edges of the plan builders (shared by the census and the softmax census)
+# --------------------------------------------------------------------------------------------
+def band_args(kind, F, P, ctx, plen, mul, attn_sink=False):
+    """((mask_mode, m0, m1, m2) of svgb200.core.plan_band, oracle mask predicate) of an SVG1 band mask:
+    "hy" HunyuanVideo (text last), "wan" (first-frame sink), otherwise CogVideoX (text first, optional sink)."""
+    from oracle import attention as oa
+
+    if kind == "hy":
+        return (1, F * P, F * P + plen, oa.hy_band_width(mul, P)), oa.hy_mask_mod(ctx, plen, F, P, mul)
+    if kind == "wan":
+        return (2, P, 0, oa.wan_band_width(mul, P)), oa.wan_mask_mod(F, P, mul)
+    first = plen + P if attn_sink else plen
+    return (3, first, plen, oa.hy_band_width(mul, P)), oa.cog_mask_mod(plen, F, P, mul, attn_sink)
+
+
+def partition(total, n, gen):
+    """n positive sizes summing to total (random cuts)"""
+    cuts = torch.sort(torch.randperm(total - 1, generator=gen)[: n - 1] + 1)[0]
+    return torch.diff(torch.cat([torch.tensor([0]), cuts, torch.tensor([total])]))
+
+
+def _tails(sizes):
+    return sum(1 for r in sizes.tolist() if 0 < r % 256 <= 128)
+
+
+def q_sizes(total, n, gen, extra=()):
+    """q-block sizes that hit every class of r % 256 (0, 1..128, 129..255), empty q-blocks, and an odd number of
+    tails (one dual item then runs a single tail) counting the `extra` blocks appended after them"""
+    special = torch.tensor([0, 0, 1, 17, 128, 129, 200, 255, 256, 257, 384, 385, 511, 512, 513, 640, 767, 768])
+    for _ in range(64):
+        s = torch.cat([special, partition(total - int(special.sum()), n - special.numel(), gen)])
+        s = torch.cat([s[torch.randperm(n, generator=gen)], torch.tensor(extra, dtype=s.dtype)])
+        if _tails(s) % 2 == 1:
+            return s
+    raise AssertionError("no odd tail count")
+
+
+def varblock_head(kind, QC, KC, total, gen):
+    """(map [QC, KC], col sizes [KC]) built to hit one edge of the plan builder"""
+    if kind == "alternating":
+        # every other key block selected: the most runs per row; selected blocks of 129 keys end in a 1-column
+        # chunk, so the chunk count approaches the list capacity S/128 + (KC+1)/2 + 2
+        col = torch.empty(KC, dtype=torch.long)
+        col[0::2] = 129
+        col[1::2] = partition(total - 129 * ((KC + 1) // 2), KC // 2, gen)
+        bm = torch.zeros(QC, KC, dtype=torch.bool)
+        bm[:, 0::2] = True
+        return bm, col
+    if kind == "joined":
+        # every third key block is empty: selected blocks on both sides of an empty one form one run
+        col = torch.zeros(KC, dtype=torch.long)
+        live = torch.arange(KC) % 3 != 1
+        col[live] = partition(total, int(live.sum()), gen)
+        bm = torch.rand(QC, KC, generator=gen) < 0.6
+        bm[:, ::3] = True
+        bm[3, :] = True    # all selected
+        bm[4, :] = False   # none selected
+        return bm, col
+    # random map, density 0.3, some empty key clusters
+    col = partition(total, KC, gen)
+    empty = torch.randperm(KC, generator=gen)[: KC // 20]
+    col[empty[1:]] = 0
+    col[empty[0]] += total - int(col.sum())
+    bm = torch.rand(QC, KC, generator=gen) < 0.3
+    return bm, col
+
+
 def lse_count_error(n_max: int) -> float:
     """Worst |exp(lse) - n| over n <= n_max when the kernel's lse = fp32(fp32(log2 n) * fp32(ln 2)) and its log2 is
     off by one ulp either way (fp64 exp).  Below 0.5, the lse identifies n exactly."""

@@ -10,6 +10,11 @@ maps, never from the engine.  The distinguishability of every table is proven on
 import pytest
 import torch
 
+from oracle.census import band_args as _band_args
+from oracle.census import partition as _partition
+from oracle.census import q_sizes as _q_sizes
+from oracle.census import varblock_head as _varblock_head
+
 pytestmark = pytest.mark.gpu
 
 # the HunyuanVideo 720p and Wan 2.1 720p shapes of BASELINE.json, and a CogVideoX-like one
@@ -61,18 +66,6 @@ def run_band(cuda, mode, m0, m1, m2, mod, H, S, D):
         v = oc.identity_values(S, D, enc, H, torch.float16, cuda)
         o, lse = core.attn_fwd(q, k, v, plan, return_lse=True)
         check_census(o[0], lse, [cnt] * H, [n] * H, enc, f"band mode {mode} m=({m0},{m1},{m2}) S={S} D={D}")
-
-
-def _band_args(kind, F, P, ctx, plen, mul, attn_sink=False):
-    from oracle import attention as oa
-    from svgb200 import core
-
-    if kind == "hy":
-        return (core.MASK_HY, F * P, F * P + plen, oa.hy_band_width(mul, P)), oa.hy_mask_mod(ctx, plen, F, P, mul)
-    if kind == "wan":
-        return (core.MASK_WAN, P, 0, oa.wan_band_width(mul, P)), oa.wan_mask_mod(F, P, mul)
-    first = plen + P if attn_sink else plen
-    return (core.MASK_COG, first, plen, oa.hy_band_width(mul, P)), oa.cog_mask_mod(plen, F, P, mul, attn_sink)
 
 
 @pytest.mark.parametrize("kind,density", [("hy", 0.1), ("hy", 0.3), ("hy", "dense"), ("wan", 0.2), ("wan", 0.45),
@@ -135,58 +128,6 @@ def test_census_band_small(cuda, case, D):
 # --------------------------------------------------------------------------------------------
 # variable-block plans
 # --------------------------------------------------------------------------------------------
-def _partition(total, n, gen):
-    """n positive sizes summing to total (random cuts)"""
-    cuts = torch.sort(torch.randperm(total - 1, generator=gen)[: n - 1] + 1)[0]
-    return torch.diff(torch.cat([torch.tensor([0]), cuts, torch.tensor([total])]))
-
-
-def _tails(sizes):
-    return sum(1 for r in sizes.tolist() if 0 < r % 256 <= 128)
-
-
-def _q_sizes(total, n, gen, extra=()):
-    """q-block sizes that hit every class of r % 256 (0, 1..128, 129..255), empty q-blocks, and an odd number of
-    tails (one dual item then runs a single tail) counting the `extra` blocks appended after them"""
-    special = torch.tensor([0, 0, 1, 17, 128, 129, 200, 255, 256, 257, 384, 385, 511, 512, 513, 640, 767, 768])
-    for _ in range(64):
-        s = torch.cat([special, _partition(total - int(special.sum()), n - special.numel(), gen)])
-        s = torch.cat([s[torch.randperm(n, generator=gen)], torch.tensor(extra, dtype=s.dtype)])
-        if _tails(s) % 2 == 1:
-            return s
-    raise AssertionError("no odd tail count")
-
-
-def _varblock_head(kind, QC, KC, total, gen):
-    """(map [QC, KC], col sizes [KC]) built to hit one edge of the plan builder"""
-    if kind == "alternating":
-        # every other key block selected: the most runs per row; selected blocks of 129 keys end in a 1-column
-        # chunk, so the chunk count approaches the list capacity S/128 + (KC+1)/2 + 2
-        col = torch.empty(KC, dtype=torch.long)
-        col[0::2] = 129
-        col[1::2] = _partition(total - 129 * ((KC + 1) // 2), KC // 2, gen)
-        bm = torch.zeros(QC, KC, dtype=torch.bool)
-        bm[:, 0::2] = True
-        return bm, col
-    if kind == "joined":
-        # every third key block is empty: selected blocks on both sides of an empty one form one run
-        col = torch.zeros(KC, dtype=torch.long)
-        live = torch.arange(KC) % 3 != 1
-        col[live] = _partition(total, int(live.sum()), gen)
-        bm = torch.rand(QC, KC, generator=gen) < 0.6
-        bm[:, ::3] = True
-        bm[3, :] = True    # all selected
-        bm[4, :] = False   # none selected
-        return bm, col
-    # random map, density 0.3, some empty key clusters
-    col = _partition(total, KC, gen)
-    empty = torch.randperm(KC, generator=gen)[: KC // 20]
-    col[empty[1:]] = 0
-    col[empty[0]] += total - int(col.sum())
-    bm = torch.rand(QC, KC, generator=gen) < 0.3
-    return bm, col
-
-
 def run_varblock(cuda, bms, rows, cols, S, D, o_rows=None, key_ids=None, q_rows=None, gather=False, what="",
                  plan=None):
     """bms [H, QC, KC], rows [H, QC], cols [H, KC]; o_rows / key_ids / q_rows [H, S] or None.  `plan`: a prebuilt
