@@ -56,6 +56,7 @@ int svgb_device_check(int* sm_major, int* sm_minor, int* num_sms);
 #define SVGB_PLAN_VARBLOCK 1 /* variable-block map, TMA chunks (svgb_attn_plan_varblock) */
 #define SVGB_PLAN_BAND 2     /* element-exact band mask (svgb_attn_plan_band) */
 #define SVGB_PLAN_GATHER 3   /* variable-block map, row gather (svgb_attn_plan_varblock_gather) */
+#define SVGB_PLAN_BAND_T 4   /* key-major band plan of the backward pass (svgb_attn_plan_band_t) */
 typedef struct svgb_plan {
   int32_t kind;          /* SVGB_PLAN_* */
   int32_t BH, S;
@@ -91,6 +92,13 @@ int svgb_attn_plan_band_bytes(int S, size_t* bytes);
 int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
                         size_t ws_bytes, svgb_plan* plan, void* stream);
 
+/* Key-major form of the same band mask, for svgb_attn_bwd: its items are key ranges and its chunk lists the query ranges
+ * that reach them, voted with mask_allowed(mode, query, key) exactly as the query-major plan votes.  Same parameters and
+ * workspace size as svgb_attn_plan_band; plan->kind = SVGB_PLAN_BAND_T. */
+int svgb_attn_plan_band_t_bytes(int S, size_t* bytes);
+int svgb_attn_plan_band_t(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
+                          size_t ws_bytes, svgb_plan* plan, void* stream);
+
 /* ---- attention -------------------------------------------------------------------------- */
 /* o = softmax(q k^T * sm_scale  [masked by plan]) v, per head.  Stands behind
  * dynamic_block_sparse_fwd_flashinfer (svg/kmeans_utils.py:1319-1392), flex_attention under the
@@ -122,6 +130,22 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
+
+/* Backward of svgb_attn_fwd: dq, dk, dv from q, k, v, the forward's o and natural-log lse, and the output gradient dO.
+ *   q,k,v,o,dO,dq,dk,dv : [BH, S, D] 16-bit (SVGB_BF16 / SVGB_F16), D in {64,128}, all addressed with the one
+ *           row_stride / head_stride pair (elements; 16-byte aligned bases, strides multiples of 8 elements).
+ *   lse   : float [BH,S] written by svgb_attn_fwd under the same plan and sm_scale.
+ *   plan  : the forward (query-major) plan, SVGB_PLAN_VARBLOCK or SVGB_PLAN_BAND with mask SVGB_MASK_NONE / HY / WAN /
+ *           COG.  plan_t: its key-major companion -- svgb_attn_plan_band_t with the same mask for a band plan,
+ *           svgb_attn_plan_varblock(map^T, col_sz, row_sz) for a variable-block plan.
+ *   ws    : device scratch of svgb_attn_bwd_bytes (per-row delta = rowsum(dO * O)).
+ * Every row of dq, dk, dv is written (rows without an allowed key: dq = 0; keys no row reaches: dk = dv = 0); the
+ * result is deterministic (no atomics).  Gather plans, row gathers and e4m3 inputs have no backward. */
+int svgb_attn_bwd_bytes(int BH, int S, size_t* bytes);
+int svgb_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                  void* dq, void* dk, void* dv, int dtype, int BH, int S, int D, long long row_stride,
+                  long long head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
+                  const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream);
 
 /* density of a variable-block map (density_calculation, svg/kmeans_utils.py:13-31) -> float [BH] */
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

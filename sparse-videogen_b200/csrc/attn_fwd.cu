@@ -199,8 +199,10 @@ struct BandSegs {
   int item_cnt[6];
 };
 
+// transposed = 1 builds the KEY-MAJOR plan of the backward pass: rows are keys, chunks are query ranges, and the vote
+// evaluates mask_allowed(mode, query = column, key = row).
 __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_chunks_total, BandSegs segs,
-                                 int* __restrict__ counts, int4* __restrict__ items,
+                                 int transposed, int* __restrict__ counts, int4* __restrict__ items,
                                  int2* __restrict__ chunks) {
   const int item = blockIdx.x;
   int seg = 0;
@@ -218,7 +220,7 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
     bool any = false, all = true;
     if (row_live) {
       for (int i = 0; i < valid; ++i) {
-        const bool a = mask_allowed(mode, q, kv0 + i, m0, m1, m2);
+        const bool a = transposed ? mask_allowed(mode, kv0 + i, q, m0, m1, m2) : mask_allowed(mode, q, kv0 + i, m0, m1, m2);
         any |= a;
         all &= a;
       }
@@ -236,8 +238,10 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
   }
 }
 
-// row-region boundaries of each mask family, and the launch order of the segments
-static BandSegs band_segments(int mode, int m0, int m1, int S) {
+// row-region boundaries of each mask family, and the launch order of the segments.  Key-major (transposed): the
+// HunyuanVideo regions are the same; the Wan sink keys (kv < P) and the CogVideoX first columns (kv < m0) are seen by
+// every query and form the heavy first segment.
+static BandSegs band_segments(int mode, int m0, int m1, int S, bool transposed = false) {
   int cuts[4], nc = 0;
   auto add = [&](int c) {
     if (c > 0 && c < S && (nc == 0 || cuts[nc - 1] < c)) cuts[nc++] = c;
@@ -246,7 +250,9 @@ static BandSegs band_segments(int mode, int m0, int m1, int S) {
     add(m0);  // end of video
     add(m1);  // end of real prompt
   } else if (mode == MASK_COG) {
-    add(m1);  // end of text prefix
+    add(transposed ? m0 : m1);  // end of the first columns (key-major) / of the text prefix
+  } else if (mode == MASK_WAN && transposed) {
+    add(m0);  // end of the first-frame sink keys
   }
   BandSegs sg{};
   sg.n = nc + 1;
@@ -496,20 +502,20 @@ int svgb_attn_plan_band_bytes(int S, size_t* bytes) {
   return 0;
 }
 
-int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
-                        size_t ws_bytes, svgb_plan* plan, void* stream) {
+static int plan_band_impl(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws, size_t ws_bytes,
+                          svgb_plan* plan, void* stream, bool transposed) {
   size_t need = 0;
   if (svgb_attn_plan_band_bytes(S, &need)) return -1;
   SVGB_REQUIRE(plan_ws && plan, "null pointer");
   SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
   SVGB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_PROF_COG_T, "unknown mask mode %d", mask_mode);
-  const BandSegs sg = band_segments(mask_mode, m0, m1, S);
+  const BandSegs sg = band_segments(mask_mode, m0, m1, S, transposed);
   const int n_items = band_total_items(sg);
   const int n_items_cap = (S + kItemRows - 1) / kItemRows + 4;
   const int n_chunks = (S + kChunkCols - 1) / kChunkCols;
   SVGB_REQUIRE(n_items <= n_items_cap, "internal: item count");
   SVGB_REQUIRE(static_cast<size_t>(n_items_cap) * n_chunks < (1ull << 31), "plan too large");
-  plan->kind = SVGB_PLAN_BAND;
+  plan->kind = transposed ? SVGB_PLAN_BAND_T : SVGB_PLAN_BAND;
   plan->BH = BH;
   plan->S = S;
   plan->max_items = n_items;
@@ -524,10 +530,22 @@ int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, vo
   plan->bytes = need;
   char* ws = static_cast<char*>(plan_ws);
   plan_band_kernel<<<n_items, kItemRows, 0, static_cast<cudaStream_t>(stream)>>>(
-      mask_mode, m0, m1, m2, S, n_chunks, sg, reinterpret_cast<int*>(ws + plan->counts_off),
+      mask_mode, m0, m1, m2, S, n_chunks, sg, transposed ? 1 : 0, reinterpret_cast<int*>(ws + plan->counts_off),
       reinterpret_cast<int4*>(ws + plan->items_off), reinterpret_cast<int2*>(ws + plan->chunks_off));
   SVGB_LAUNCH_OK();
   return 0;
+}
+
+int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
+                        size_t ws_bytes, svgb_plan* plan, void* stream) {
+  return plan_band_impl(mask_mode, m0, m1, m2, BH, S, plan_ws, ws_bytes, plan, stream, false);
+}
+
+int svgb_attn_plan_band_t_bytes(int S, size_t* bytes) { return svgb_attn_plan_band_bytes(S, bytes); }
+
+int svgb_attn_plan_band_t(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws, size_t ws_bytes,
+                          svgb_plan* plan, void* stream) {
+  return plan_band_impl(mask_mode, m0, m1, m2, BH, S, plan_ws, ws_bytes, plan, stream, true);
 }
 
 int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
@@ -540,6 +558,8 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                "fp8 attention needs the three per-head scale vectors");
   SVGB_REQUIRE(dtype == SVGB_E4M3 || (!q_scale && !k_scale && !v_scale),
                "per-head scale vectors are for e4m3 inputs only (dtype %d)", dtype);
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND_T,
+               "a key-major band plan (svgb_attn_plan_band_t) is for svgb_attn_bwd; the forward takes svgb_attn_plan_band");
   const bool gather = plan->kind == SVGB_PLAN_GATHER;
   SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
                "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");

@@ -15,7 +15,7 @@ MASK_NONE, MASK_HY, MASK_WAN, MASK_COG = 0, 1, 2, 3
 # SVG1 profiling masks (include/svgb200.h SVGB_MASK_PROF_*): the element masks of sample_mse, also accepted by plan_band
 MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_S, MASK_PROF_COG_T = 4, 5, 6, 7, 8, 9
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
-PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER = 1, 2, 3
+PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T = 1, 2, 3, 4
 _E4M3 = 2  # SVGB_E4M3 (the 16-bit dtype ids come from _dt)
 
 # launches issued through this module since import (bench.py reports it as gpu_launches)
@@ -73,13 +73,45 @@ def device_check():
 # ----------------------------------------------------------------------------------------------
 @dataclass
 class AttnPlan:
-    """Device-resident work list + its host descriptor."""
+    """Device-resident work list + its host descriptor.  `source` keeps what a variable-block plan was built from
+    (map, row sizes, column sizes, and their torch version counters at build time) so that key_major() can plan the
+    transpose; `_key_major` caches that plan."""
     desc: Plan
     ws: torch.Tensor
+    source: Optional[tuple] = None
+    _key_major: Optional["AttnPlan"] = None
 
     @property
     def S(self):
         return self.desc.S
+
+    def key_major(self) -> "AttnPlan":
+        """The plan the backward's dK / dV kernel walks (one work list per key range), built on first use: the band
+        mask's transposed plan, or the variable-block planner on the transposed map with row and column sizes swapped.
+        Gather plans and the profiling masks have no backward."""
+        if self._key_major is None:
+            d = self.desc
+            if d.kind == PLAN_BAND:
+                if d.mask_mode > MASK_COG:
+                    raise SvgbError(f"attention backward: the profiling mask mode {d.mask_mode} has no backward "
+                                    "(executed masks NONE / HY / WAN / COG only)")
+                self._key_major = plan_band_t(d.mask_mode, d.m0, d.m1, d.m2, d.BH, d.S, self.ws.device)
+            elif d.kind == PLAN_VARBLOCK and self.source is not None:
+                *ts, versions = self.source
+                if tuple(t._version for t in ts) != versions:
+                    # the key-major plan must describe the mask this plan was built from (the one the forward ran)
+                    raise SvgbError("attention backward: the block map or block sizes of this plan were modified in "
+                                    "place after the plan was built; rebuild the plan")
+                m, r, c = ts
+                kt = plan_varblock(m.transpose(1, 2), c, r, d.S)
+                if d.items_stride == 0:  # one map shared by every head (svgb200.h, svgb_plan): so is its transpose
+                    kt.desc.items_stride = 0
+                self._key_major = kt
+            elif d.kind == PLAN_GATHER:
+                raise SvgbError("attention backward: gather plans (row-gather path, q_rows / kv_rows) have no backward")
+            else:
+                raise SvgbError(f"attention backward: plan kind {d.kind} has no key-major form")
+        return self._key_major
 
 
 def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.Tensor, S: int,
@@ -104,7 +136,7 @@ def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.T
     check(fn(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, S, QC, KC, ws.data_ptr(), ws.numel(), C.byref(desc),
              _stream(m)), "svgb_attn_plan_varblock")
     _bump()
-    return AttnPlan(desc, ws)
+    return AttnPlan(desc, ws, None if gather else (m, r, c, (m._version, r._version, c._version)))
 
 
 def plan_band(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device) -> AttnPlan:
@@ -115,6 +147,18 @@ def plan_band(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device
     check(lib().svgb_attn_plan_band(mask_mode, m0, m1, m2, BH, S, ws.data_ptr(), ws.numel(),
                                     C.byref(desc), torch.cuda.current_stream(device).cuda_stream),
           "svgb_attn_plan_band")
+    _bump()
+    return AttnPlan(desc, ws)
+
+
+def plan_band_t(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device) -> AttnPlan:
+    """Key-major form of plan_band's mask (include/svgb200.h svgb_attn_plan_band_t), for attn_bwd."""
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_plan_band_t_bytes(S, C.byref(nbytes)), "plan_band_t_bytes")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
+    desc = Plan()
+    check(lib().svgb_attn_plan_band_t(mask_mode, m0, m1, m2, BH, S, ws.data_ptr(), ws.numel(), C.byref(desc),
+                                      torch.cuda.current_stream(device).cuda_stream), "svgb_attn_plan_band_t")
     _bump()
     return AttnPlan(desc, ws)
 
@@ -156,6 +200,70 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     o = torch.empty_like(q) if out is None else out
     return _attn(q, k, v, (None, None, None), o, _dt(q), plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows,
                  return_lse, sm_scale)
+
+
+def _geometry(q, layout):
+    if layout == "bhsd":
+        B, H, S, D = q.shape
+        return B * H, S, D, D, S * D
+    if layout == "shd":
+        S, H, D = q.shape
+        return H, S, D, H * D, D
+    raise SvgbError(f"unknown layout {layout}")
+
+
+def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None):
+    """Gradients (dq, dk, dv) of o = attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale) for the output gradient
+    do; lse is the forward's return_lse output.  Variable-block and band plans (mask NONE / HY / WAN / COG); the plan's
+    key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits."""
+    _need_cuda(q, k, v, o, do, lse)
+    ts = (q, k, v, o, do)
+    if not all(t.is_contiguous() for t in ts):
+        raise SvgbError("q, k, v, o, do must be contiguous")
+    if not all(t.dtype == q.dtype and t.shape == q.shape for t in ts):
+        raise SvgbError("q, k, v, o, do must share dtype and shape")
+    BH, S, D, rs, hs = _geometry(q, layout)
+    plan_t = plan.key_major()
+    lse = lse.to(torch.float32).contiguous()
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_bwd_bytes(BH, S, C.byref(nbytes)), "svgb_attn_bwd_bytes")
+    ws = workspace(("attn_bwd", BH, S), nbytes.value, q.device)
+    dq, dk, dv = (torch.empty_like(q) for _ in range(3))
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    check(lib().svgb_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
+                              dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, S, D, rs, hs, scale,
+                              C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc), plan_t.ws.data_ptr(),
+                              ws.data_ptr(), ws.numel(), _stream(q)), "svgb_attn_bwd")
+    _bump(3)
+    return dq, dk, dv
+
+
+class _Attention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, v, plan, layout, sm_scale):
+        o, lse = attn_fwd(q, k, v, plan, layout=layout, return_lse=True, sm_scale=sm_scale)
+        ctx.save_for_backward(q, k, v, o, lse)
+        ctx.plan, ctx.layout, ctx.sm_scale = plan, layout, sm_scale
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        q, k, v, o, lse = ctx.saved_tensors
+        dq, dk, dv = attn_bwd(q, k, v, o, do.contiguous(), lse, ctx.plan, layout=ctx.layout, sm_scale=ctx.sm_scale)
+        return dq, dk, dv, None, None, None
+
+
+def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None):
+    """attn_fwd as a differentiable op: the forward keeps its LSE and the backward runs attn_bwd.  Plans without a
+    backward (gather plans, the profiling masks) are rejected here, before the forward runs."""
+    if plan.desc.kind == PLAN_GATHER or (plan.desc.kind == PLAN_BAND and plan.desc.mask_mode > MASK_COG):
+        plan.key_major()  # raises, naming what has no backward
+    return _Attention.apply(q, k, v, plan, layout, sm_scale)
+
+
+def needs_grad(*ts) -> bool:
+    """True when autograd would record an op on these tensors: the attention entry points then take attention()."""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
 
 
 def quantize_e4m3(x: torch.Tensor):

@@ -35,8 +35,18 @@ class BandMask:
 
 
 def sparse_flex_attention(query, key, value, block_mask: BandMask):
-    """hyvideo/attention.py:401-403: flex_attention(q, k, v, block_mask=...)  [cfg,H,S,D]."""
+    """hyvideo/attention.py:401-403: flex_attention(q, k, v, block_mask=...)  [cfg,H,S,D].  Differentiable when an input
+    requires grad (core.attention)."""
+    if core.needs_grad(query, key, value):
+        return core.attention(query, key, value, block_mask.plan)
     return core.attn_fwd(query, key, value, block_mask.plan)
+
+
+def check_no_grad(what, *ts):
+    """Attention paths without a backward raise rather than return a result detached from the graph."""
+    if core.needs_grad(*ts):
+        raise core.SvgbError(f"{what} has no backward: call it on tensors that do not require grad "
+                             "(or under torch.no_grad())")
 
 
 def check_fp8_head_dim(D):
@@ -52,7 +62,8 @@ def quantize_qkv(query, key, value):
 def fp8_attention(query, key, value, plan: core.AttnPlan, **rows):
     """Attention under `plan` in FP8: Q, K, V [B,H,S,128] quantised to e4m3 per head and run on the e4m3 kernel
     (rows: q_rows / kv_rows / o_rows of core.attn_fwd_fp8).  The kernel writes bf16; the result comes back in
-    query.dtype."""
+    query.dtype.  FP8 attention has no backward: an input that requires grad raises."""
+    check_no_grad("fp8 attention", query, key, value)
     check_fp8_head_dim(query.shape[-1])
     (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(query, key, value)
     return core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, plan, **rows).to(query.dtype)
@@ -60,6 +71,7 @@ def fp8_attention(query, key, value, plan: core.AttnPlan, **rows):
 
 def sparse_flex_attention_fp8(query, key, value, block_mask: BandMask):
     """sparse_flex_attention in FP8 (fp8_attention under the band plan)."""
+    check_no_grad("fp8 attention", query, key, value)
     check_fp8_head_dim(query.shape[-1])  # before block_mask is read: a head_dim-64 model fails on its cause
     return fp8_attention(query, key, value, block_mask.plan)
 
@@ -74,6 +86,8 @@ def dense_attention(query, key, value, seg_lens=None):
     bm = torch.eye(n, dtype=torch.bool, device=dev).expand(cfg * H, n, n).contiguous()
     sz = torch.tensor(segs, dtype=torch.int32, device=dev).expand(cfg * H, n).contiguous()
     plan = core.plan_varblock(bm, sz, sz, S)
+    if core.needs_grad(query, key, value):
+        return core.attention(query, key, value, plan)
     return core.attn_fwd(query, key, value, plan)
 
 
@@ -375,6 +389,8 @@ class SAPCore:
 
         cfg, H, S, D = query.shape
         assert cfg == 1, "Batch size must be 1 for kmeans block sparse attention"
+        # the permutations and the fused inverse-permutation store have no backward
+        check_no_grad("the SVG2 sparse core (clustered permutation, o_rows)", query, key, value)
         if self.fp8:
             check_fp8_head_dim(D)
         layer_idx = self.layer_idx if layer_idx is None else layer_idx

@@ -83,6 +83,8 @@ def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, m
     bm = torch.eye(n, dtype=torch.bool, device=dev).expand(BH, n, n).contiguous()
     sz = torch.tensor(seg, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
     plan = core.plan_varblock(bm, sz, sz, S)
+    if core.needs_grad(q, k, v):
+        return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
     return core.attn_fwd(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
 
 
