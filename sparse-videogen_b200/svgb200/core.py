@@ -212,23 +212,28 @@ def _geometry(q, layout):
     raise SvgbError(f"unknown layout {layout}")
 
 
-def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None):
+def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
+             out: Optional[tuple] = None):
     """Gradients (dq, dk, dv) of o = attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale) for the output gradient
     do; lse is the forward's return_lse output.  Variable-block and band plans (mask NONE / HY / WAN / COG); the plan's
-    key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits."""
+    key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits.
+    out: optional (dq, dk, dv) tensors of q's dtype and shape, contiguous, written and returned instead of new ones."""
     _need_cuda(q, k, v, o, do, lse)
-    ts = (q, k, v, o, do)
+    ts = (q, k, v, o, do) + (tuple(out) if out is not None else ())
+    if out is not None and len(out) != 3:
+        raise SvgbError("out must be a (dq, dk, dv) tuple")
     if not all(t.is_contiguous() for t in ts):
-        raise SvgbError("q, k, v, o, do must be contiguous")
+        raise SvgbError("q, k, v, o, do (and out) must be contiguous")
     if not all(t.dtype == q.dtype and t.shape == q.shape for t in ts):
-        raise SvgbError("q, k, v, o, do must share dtype and shape")
+        raise SvgbError("q, k, v, o, do (and out) must share dtype and shape")
     BH, S, D, rs, hs = _geometry(q, layout)
     plan_t = plan.key_major()
     lse = lse.to(torch.float32).contiguous()
     nbytes = C.c_size_t()
     check(lib().svgb_attn_bwd_bytes(BH, S, C.byref(nbytes)), "svgb_attn_bwd_bytes")
     ws = workspace(("attn_bwd", BH, S), nbytes.value, q.device)
-    dq, dk, dv = (torch.empty_like(q) for _ in range(3))
+    dq, dk, dv = (torch.empty_like(q) for _ in range(3)) if out is None else out
+    _need_cuda(dq, dk, dv)
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
     check(lib().svgb_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
                               dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, S, D, rs, hs, scale,

@@ -109,7 +109,11 @@ def check_grads(got, ref, dtype):
         assert err <= TOL[dtype] * float(r.abs().max()) + 1e-6, f"{name}: max error {err} vs max |ref| {float(r.abs().max())}"
 
 
-CASES = ["hy", "wan", "cog", "vb0.2", "vb0.7", "vb0.9", "dense", "varlen"]
+# "<kind>/B2": batch 2 (four heads, each with its own variable-block map; 'shd' holds them as four heads);
+# "<kind>/scale": an explicit sm_scale through core.attention, which the backward must take from the forward
+CASES = ["hy", "wan", "cog", "vb0.2", "vb0.7", "vb0.9", "dense", "varlen", "wan/B2", "vb0.5/B2", "cog/scale",
+         "vb0.7/scale"]
+SCALE = 0.3
 
 
 @pytest.mark.parametrize("layout", ["bhsd", "shd"])
@@ -120,42 +124,23 @@ def test_gradients_vs_oracle(cuda, kind, dtype, D, layout):
     """dQ, dK, dV of core.attention under band and variable-block plans vs fp64 autograd of the masked softmax."""
     from svgb200 import core
 
-    H = 2
+    base, _, extra = kind.partition("/")
+    B = 2 if extra == "B2" else 1
+    sm_scale = SCALE if extra == "scale" else None
+    H = 2 * B
     gen = torch.Generator().manual_seed(CASES.index(kind) * 7 + D)
-    S = BANDS[kind][4] if kind in BANDS else 1000
-    plan, masks = make_plan(kind, H, S, cuda, gen)
+    S = BANDS[base][4] if base in BANDS else 1000
+    plan, masks = make_plan(base, H, S, cuda, gen)
     q, k, v, do = inputs(H, S, D, dtype, gen)
-    x = [to_layout(t, layout).to(cuda).requires_grad_() for t in (q, k, v)]
-    o = core.attention(*x, plan, layout=layout)
-    o.backward(to_layout(do, layout).to(cuda))
-    got = [from_layout(t.grad, layout) for t in x]
-    check_grads(got, oracle_grads(q, k, v, do, masks), dtype)
 
+    def lay(t):
+        return to_layout(t, layout) if layout == "shd" else t.view(B, H // B, S, D).contiguous()
 
-@pytest.mark.parametrize("kind", ["hy", "wan", "cog", "none", "vb0.5"])
-def test_backward_key_census(cuda, kind):
-    """q = 0 makes P uniform, 1 / n_i, over each row's allowed keys; with dO[i] the one-hot of i mod D,
-    dV[j, d] = sum over the rows i = d (mod D) that reach key j of 1 / n_i.  One row wrongly kept or dropped for a key
-    moves dV[j, d] by 1 / n_i, far above the fp16 rounding: every key's row set is checked against the brute-force
-    transpose of the mask predicate."""
-    from svgb200 import core
-
-    H, D, dtype = 2, 128, torch.float16
-    gen = torch.Generator().manual_seed(7)
-    S = BANDS[kind][4] if kind in BANDS else 1000
-    plan, masks = make_plan(kind, H, S, cuda, gen)
-    q = torch.zeros(1, H, S, D, dtype=dtype, device=cuda)
-    k, v = (torch.randn(1, H, S, D, generator=gen).to(dtype).to(cuda) for _ in range(2))
-    do = torch.nn.functional.one_hot(torch.arange(S) % D, D).to(dtype).expand(H, S, D)[None].contiguous()
-    o, lse = core.attn_fwd(q, k, v, plan, return_lse=True)
-    _, _, dv = core.attn_bwd(q, k, v, o, do.to(cuda), lse, plan)
-    dv = dv[0].double().cpu()
-    for h, m in enumerate(masks):
-        n = m.sum(1).double()
-        w = torch.where(n > 0, 1.0 / n.clamp(min=1), torch.zeros_like(n))
-        exp = m.double().T @ (w[:, None] * do[0, h].double())
-        bad = (dv[h] - exp).abs() > 0.4 / float(n.max())
-        assert not bool(bad.any()), f"{kind}: head {h}, first wrong key {int(bad.any(1).nonzero()[0])}"
+    x = [lay(t).to(cuda).requires_grad_() for t in (q, k, v)]
+    o = core.attention(*x, plan, layout=layout, sm_scale=sm_scale)
+    o.backward(lay(do).to(cuda))
+    got = [from_layout(t.grad, layout) if layout == "shd" else t.grad.reshape(H, S, D) for t in x]
+    check_grads(got, oracle_grads(q, k, v, do, masks, sm_scale=sm_scale), dtype)
 
 
 def test_edge_rows_and_keys(cuda):
