@@ -267,8 +267,55 @@ def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Option
 
 
 def needs_grad(*ts) -> bool:
-    """True when autograd would record an op on these tensors: the attention entry points then take attention()."""
+    """True when autograd would record an op on these tensors: the attention entry points then take attention(), the
+    layout ops _HeadPlacement / _Permute."""
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
+
+
+class _HeadPlacement(torch.autograd.Function):
+    """head_placement under autograd.  The outputs are the caller's tensors written in place (ctx.mark_dirty, so the
+    caller's own objects carry the history; no copy).  Every row of every output is written, so their old contents get
+    no gradient.  A placement only moves rows, so its backward is the same kernel in the opposite direction (inverse
+    flipped, same text_first), one launch for all incoming gradients.  best_mask_idx is an integer selection and gets
+    no gradient (the head choice of sample_mse is a constant, as the BlockMask is to flex_attention)."""
+
+    @staticmethod
+    def forward(ctx, args, n, *ts):
+        outs = ts[n:]
+        _place(ts[:n], outs, *args)
+        ctx.mark_dirty(*outs)
+        ctx.set_materialize_grads(False)
+        ctx.args, ctx.n = args, n
+        return outs
+
+    @staticmethod
+    def backward(ctx, *gs):
+        idx, BH, S, D, context, F, P, text_first, inverse = ctx.args
+        want = [i for i in range(ctx.n) if ctx.needs_input_grad[2 + i] and gs[i] is not None]
+        grads = [None] * ctx.n
+        if want:
+            src = [gs[i].contiguous() for i in want]
+            dst = [torch.empty_like(g) for g in src]
+            head_placement(src, dst, idx, context, F, P, text_first=text_first, inverse=not inverse)
+            for i, g in zip(want, dst):
+                grads[i] = g
+        return (None, None, *grads, *([None] * ctx.n))
+
+
+class _Permute(torch.autograd.Function):
+    """permute_gather / permute_scatter under autograd: the backward of each is the other under the same permutation.
+    The permutation (sorted indices from the labels) is an integer selection and gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, x, perm, scatter):
+        ctx.save_for_backward(perm)
+        ctx.scatter = scatter
+        return _permute(x, perm, scatter)
+
+    @staticmethod
+    def backward(ctx, g):
+        perm, = ctx.saved_tensors
+        return (permute_gather if ctx.scatter else permute_scatter)(g, perm), None, None
 
 
 def quantize_e4m3(x: torch.Tensor):
@@ -354,29 +401,50 @@ def _rows_op(fn, name, x, perm):
     return out.view(shape)
 
 
-def permute_gather(x, perm):
+def _permute(x, perm, scatter):
+    if scatter:
+        return _rows_op(lib().svgb_permute_scatter, "svgb_permute_scatter", x, perm)
     return _rows_op(lib().svgb_permute_gather, "svgb_permute_gather", x, perm)
 
 
+def permute_gather(x, perm):
+    """out[bh, s] = x[bh, perm[bh, s]].  Differentiable in x when it requires grad (_Permute)."""
+    if needs_grad(x):
+        return _Permute.apply(x, perm, False)
+    return _permute(x, perm, False)
+
+
 def permute_scatter(x, perm):
-    return _rows_op(lib().svgb_permute_scatter, "svgb_permute_scatter", x, perm)
+    """out[bh, perm[bh, s]] = x[bh, s].  Differentiable in x when it requires grad (_Permute)."""
+    if needs_grad(x):
+        return _Permute.apply(x, perm, True)
+    return _permute(x, perm, True)
+
+
+def _place(ins, outs, idx, BH, S, D, ctx, F, P, text_first, inverse):
+    n = len(ins)
+    a_in = (C.c_void_p * n)(*[t.data_ptr() for t in ins])
+    a_out = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
+    check(lib().svgb_head_placement(a_in, a_out, n, idx.data_ptr(), BH, S, D, ctx, F, P,
+                                    1 if text_first else 0, 1 if inverse else 0, _stream(ins[0])),
+          "svgb_head_placement")
+    _bump()
 
 
 def head_placement(ins, outs, best_mask_idx, ctx, F, P, *, text_first=False, inverse=False):
-    """ins / outs: lists (1..3) of [cfg,H,S,D] contiguous 16-bit tensors; writes outs in place."""
+    """ins / outs: lists (1..3) of [cfg,H,S,D] contiguous 16-bit tensors; writes outs in place.  When an input
+    requires grad the outs (the same objects) carry the history (_HeadPlacement)."""
     _need_cuda(*ins, *outs, best_mask_idx)
-    n = len(ins)
     cfg, H, S, D = ins[0].shape
     for t in list(ins) + list(outs):
         if not t.is_contiguous() or t.shape != ins[0].shape or t.element_size() != 2:
             raise SvgbError("placement tensors must be contiguous 16-bit [cfg,H,S,D] of one shape")
     idx = best_mask_idx.reshape(cfg * H).to(torch.int32).contiguous()
-    a_in = (C.c_void_p * n)(*[t.data_ptr() for t in ins])
-    a_out = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
-    check(lib().svgb_head_placement(a_in, a_out, n, idx.data_ptr(), cfg * H, S, D, ctx, F, P,
-                                    1 if text_first else 0, 1 if inverse else 0, _stream(ins[0])),
-          "svgb_head_placement")
-    _bump()
+    args = (idx, cfg * H, S, D, ctx, F, P, text_first, inverse)
+    if needs_grad(*ins, *outs):
+        _HeadPlacement.apply(args, len(ins), *ins, *outs)
+    else:
+        _place(ins, outs, *args)
     return outs
 
 

@@ -124,7 +124,11 @@ class SVG1Core:
     Subclasses fix the text layout (`text_first`, `smse_layout`) and build `block_mask`.
 
     fp8=True runs the band attention on e4m3 Q, K, V (sparse_flex_attention_fp8, head_dim 128 only); sample_mse, the
-    placements and the dense branch stay 16-bit, so the head choice is the 16-bit core's."""
+    placements and the dense branch stay 16-bit, so the head choice is the 16-bit core's.
+
+    Gradients: sparse_core (16-bit) is differentiable in Q, K and V through the placements (core._HeadPlacement) and
+    the band attention (core.attention); the head choice of sample_mse is a constant.  The FP8 core,
+    sparse_core_head_parallel and sparse_core_from_host have no backward and raise under grad."""
 
     text_first = False
     smse_layout = 0  # svgb_sample_mse layout id (0 = HY text-last band 1.5*P, 1 = WAN sink band 2*P)
@@ -168,6 +172,8 @@ class SVG1Core:
 
     # -- the sparse branch ---------------------------------------------------------------------------
     def sparse_core(self, query, key, value, sampled_rows=None, attn_events=None):
+        if self.fp8:
+            check_no_grad("the SVG1 core with fp8 attention", query, key, value)
         # stage labels = the reference's TIME_BENCH table (hyvideo/attention.py:375,401,405,439)
         with time_logging_decorator("Level 3 - sample mse"):
             sampled_mses = self.sample_mse(query, key, value, sampled_rows)
@@ -196,6 +202,8 @@ class SVG1Core:
         head issued on a side stream as soon as that head's attention + inverse placement finished, so the
         NVLink transfer of head i overlaps the attention of head i+1 (svgb200.parallel.HeadParallel).
         Returns the full [1, H_local * world, S, D] output (heads interleaved: global h = i*world + rank)."""
+        # the output is assembled by all-gathers into a plain buffer, outside the autograd graph
+        check_no_grad("the head-parallel SVG1 core (sparse_core_head_parallel)", query, key, value)
         cfg, Hl, S, D = query.shape
         assert cfg == 1
         if trace is not None:
@@ -231,6 +239,8 @@ class SVG1Core:
         Head-parallel (hp = svgb200.parallel.HeadParallel, world > 1): hq/hk/hv/ho hold this rank's heads; each
         group's output is additionally all-gathered into `gathered` [1, H_local*world, S, D] on the device (the
         downstream projection needs every head) on hp's communication stream, overlapping the next group."""
+        # heads travel through staging copies, outside the autograd graph
+        check_no_grad("the host-pipelined SVG1 core (sparse_core_from_host)", hq, hk, hv)
         cfg, H, S, D = hq.shape
         assert cfg == 1
         dev = self.block_mask.plan.ws.device

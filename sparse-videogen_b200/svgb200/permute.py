@@ -1,4 +1,7 @@
-"""Mirror of svg/kernels/triton/permute.py (:82-170)."""
+"""Mirror of svg/kernels/triton/permute.py (:82-170).
+
+Differentiable in the permuted tensor when it requires grad: the backward of the gather is the scatter under the same
+indices and vice versa (core._Permute); labels and sorted indices are constants."""
 from __future__ import annotations
 
 from typing import Optional

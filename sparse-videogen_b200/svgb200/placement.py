@@ -3,6 +3,9 @@
 hunyuan_sparse_head_placement(q,k,v,q_out,k_out,v_out,best_mask_idx,ctx,F,P) writes the outs in place
 (placement.py:124-153); *_hidden_states_placement(h, h_out, best_mask_idx, ctx, F, P) is the inverse on O
 (placement.py:360-387).  wan / cosmos share the text-last kernel (ctx = 0); cog is text-first.
+
+Differentiable when an input requires grad: the caller's outs carry the history and the backward is the placement in
+the opposite direction (core._HeadPlacement); best_mask_idx is a constant.
 """
 from __future__ import annotations
 
