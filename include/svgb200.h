@@ -266,6 +266,34 @@ int svgb_qkv_prep(const void* q_in, const void* k_in, const void* v_in, long lon
                   int rope, const float* cos_t, const float* sin_t, int rope_lo, int rope_n, int dtype,
                   void* stream);
 
+/* Backwards of the chain (DESIGN.md §5).  Deterministic: no atomics; dgamma / dbeta are fp32 sums of per-CTA partials
+ * taken in a fixed order (ws holds the partials; two launches), so two calls give the same bits.
+ * svgb_rms_norm_bwd / svgb_layer_norm_bwd: x [m, n] the norm's 16-bit input, dy the gradient at its output ->
+ *   dx [m, n] (rounded once), dgamma (dbeta) float [n].  eps and n as the forward. */
+int svgb_row_norm_bwd_bytes(long long m, int n, size_t* bytes);
+int svgb_rms_norm_bwd(const void* x, const void* dy, const void* gamma, void* dx, float* dgamma, long long m, int n,
+                      float eps, int dtype, void* ws, size_t ws_bytes, void* stream);
+int svgb_layer_norm_bwd(const void* x, const void* dy, const void* gamma, void* dx, float* dgamma, float* dbeta,
+                        long long m, int n, int dtype, void* ws, size_t ws_bytes, void* stream);
+/* svgb_qk_rope's transpose, out of place: dq [B,Hq,S,D], dk [B,Hk,S,D] -> dq_out, dk_out (same shapes, contiguous);
+ * the rotated rows get the transpose of the rotation, the text rows are copied.  Same modes and tables. */
+int svgb_qk_rope_bwd(const void* dq, const void* dk, void* dq_out, void* dk_out, const float* cos_t,
+                     const float* sin_t, int B, int Hq, int Hk, int S, int D, int len_text, int mode, int dtype,
+                     void* stream);
+/* svgb_qkv_prep's backward: reads rows [out_row0, out_row0+S_in) of dq, dk, dv [B, H, S_out, D] (no other rows) and
+ * the forward's q_in, k_in through their strides (needed when norm != NONE) -> dq_in, dk_in, dv_in contiguous
+ * [B, S_in, H*D], and float dgamma_q / dgamma_k ([D], or [H*D] for SVGB_NORM_RMS_HIDDEN), dbeta_q / dbeta_k for
+ * SVGB_NORM_LAYER.  Arguments as the forward; the RoPE transpose is rounded to the 16-bit dtype before the norm
+ * backward (the forward's rounding point), so it equals svgb_qk_rope_bwd followed by svgb_*_norm_bwd bit for bit. */
+int svgb_qkv_prep_bwd_bytes(int B, int S_in, int H, int D, int norm, size_t* bytes);
+int svgb_qkv_prep_bwd(const void* dq, const void* dk, const void* dv, long long out_head_stride,
+                      long long out_batch_stride, const void* q_in, const void* k_in, long long in_token_stride,
+                      long long in_batch_stride, void* dq_in, void* dk_in, void* dv_in, int B, int S_in, int H, int D,
+                      int out_row0, int norm, const void* gamma_q, const void* gamma_k, float eps, int rope,
+                      const float* cos_t, const float* sin_t, int rope_lo, int rope_n, float* dgamma_q,
+                      float* dgamma_k, float* dbeta_q, float* dbeta_k, int dtype, void* ws, size_t ws_bytes,
+                      void* stream);
+
 /* ---- Wan transformer-block glue (SURVEY 8f-3; svg/kernels/triton/{layernorm,modulate,rmsnorm}.py) ---- */
 /* rows of N elements (N % 8 == 0, N <= 8192), contiguous; x/y/w dtypes: SVGB_BF16 | SVGB_F16 | SVGB_F32;
  * scale/shift/gate are float [nb, N], row r uses vector r / rows_per_batch (rows_per_batch = 0: one vector). */

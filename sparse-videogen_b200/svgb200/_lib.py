@@ -69,6 +69,13 @@ _PROTOS = {
     "svgb_qk_rope": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "svgb_qkv_prep": [_vp, _vp, _vp, _ll, _ll, _vp, _vp, _vp, _ll, _ll, _i, _i, _i, _i, _i, _i,
                       _vp, _vp, _vp, _vp, _f, _i, _vp, _vp, _i, _i, _i, _vp],
+    "svgb_row_norm_bwd_bytes": [_ll, _i, _psz],
+    "svgb_rms_norm_bwd": [_vp, _vp, _vp, _vp, _vp, _ll, _i, _f, _i, _vp, _sz, _vp],
+    "svgb_layer_norm_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _vp, _sz, _vp],
+    "svgb_qk_rope_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "svgb_qkv_prep_bwd_bytes": [_i, _i, _i, _i, _i, _psz],
+    "svgb_qkv_prep_bwd": [_vp, _vp, _vp, _ll, _ll, _vp, _vp, _ll, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i,
+                          _vp, _vp, _f, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _sz, _vp],
     "svgb_layernorm_modulate": [_vp, _i, _vp, _vp, _i, _f, _vp, _vp, _ll, _vp, _i, _ll, _i, _vp],
     "svgb_rmsnorm_hidden": [_vp, _i, _vp, _i, _f, _vp, _i, _ll, _i, _vp],
     "svgb_modulate_shift": [_vp, _i, _vp, _vp, _ll, _vp, _i, _ll, _i, _vp],

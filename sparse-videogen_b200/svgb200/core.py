@@ -268,7 +268,7 @@ def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Option
 
 def needs_grad(*ts) -> bool:
     """True when autograd would record an op on these tensors: the attention entry points then take attention(), the
-    layout ops _HeadPlacement / _Permute."""
+    layout ops _HeadPlacement / _Permute, the pre-attention chain _RowNorm / _QkRope / _QkvPrep."""
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
 
 
@@ -590,33 +590,114 @@ def _contig(*ts):
             raise SvgbError("tensor must be contiguous")
 
 
+def _no_backward(what, *ts):
+    """Ops without a backward raise under grad rather than return a result detached from the graph (the message of
+    models.common.check_no_grad)."""
+    if needs_grad(*ts):
+        raise SvgbError(f"{what} has no backward: call it on tensors that do not require grad "
+                        "(or under torch.no_grad())")
+
+
+def _tables_no_grad(cos, sin):
+    if needs_grad(cos, sin):
+        raise SvgbError("the RoPE tables cos / sin get no gradient: pass tables that do not require grad (.detach())")
+
+
+def _row_norm(x, gamma, beta, eps):
+    n = x.shape[-1]
+    if beta is None:
+        check(lib().svgb_rms_norm(x.data_ptr(), gamma.data_ptr(), x.numel() // n, n, float(eps), _dt(x), _stream(x)),
+              "svgb_rms_norm")
+    else:
+        check(lib().svgb_layer_norm(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), x.numel() // n, n, _dt(x),
+                                    _stream(x)), "svgb_layer_norm")
+    _bump()
+
+
+def _row_norm_bwd(x, dy, gamma, eps, layer):
+    _need_cuda(x, dy, gamma)
+    _contig(x, dy, gamma)
+    if dy.shape != x.shape or dy.dtype != x.dtype:
+        raise SvgbError("dy must have the shape and dtype of x")
+    n = x.shape[-1]
+    m = x.numel() // n
+    nbytes = C.c_size_t()
+    check(lib().svgb_row_norm_bwd_bytes(m, n, C.byref(nbytes)), "svgb_row_norm_bwd_bytes")
+    ws = workspace("row_norm_bwd", nbytes.value, x.device)
+    dx = torch.empty_like(x)
+    dg = torch.empty(n, dtype=torch.float32, device=x.device)
+    if layer:
+        db = torch.empty(n, dtype=torch.float32, device=x.device)
+        check(lib().svgb_layer_norm_bwd(x.data_ptr(), dy.data_ptr(), gamma.data_ptr(), dx.data_ptr(), dg.data_ptr(),
+                                        db.data_ptr(), m, n, _dt(x), ws.data_ptr(), ws.numel(), _stream(x)),
+              "svgb_layer_norm_bwd")
+    else:
+        db = None
+        check(lib().svgb_rms_norm_bwd(x.data_ptr(), dy.data_ptr(), gamma.data_ptr(), dx.data_ptr(), dg.data_ptr(), m, n,
+                                      float(eps), _dt(x), ws.data_ptr(), ws.numel(), _stream(x)), "svgb_rms_norm_bwd")
+    _bump(2)
+    return dx, dg.to(gamma.dtype), None if db is None else db.to(gamma.dtype)
+
+
+def rms_norm_bwd(x, dy, gamma, eps: float = 1e-5):
+    """Gradients (dx, dgamma) of rms_norm_ at its input x (the values before the in-place norm) for the output gradient
+    dy.  dgamma is summed in fp32 in a fixed order and rounded once to gamma's dtype."""
+    dx, dg, _ = _row_norm_bwd(x, dy, gamma, eps, False)
+    return dx, dg
+
+
+def layer_norm_bwd(x, dy, gamma):
+    """Gradients (dx, dgamma, dbeta) of layer_norm_ at its input x for the output gradient dy."""
+    return _row_norm_bwd(x, dy, gamma, 0.0, True)
+
+
+class _RowNorm(torch.autograd.Function):
+    """rms_norm_ / layer_norm_ under autograd.  The norm still runs in place: the caller's tensor (often a .view(-1, D)
+    of a non-leaf) is marked dirty and carries the history.  A copy of x taken before the kernel is the one extra
+    buffer.  eps gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, eps):
+        ctx.save_for_backward(x.clone(), gamma)
+        ctx.eps, ctx.layer = eps, beta is not None
+        _row_norm(x, gamma, beta, eps)
+        ctx.mark_dirty(x)
+        return x
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma = ctx.saved_tensors
+        dx, dg, db = _row_norm_bwd(x, dy.contiguous(), gamma, ctx.eps, ctx.layer)
+        return dx, dg if ctx.needs_input_grad[1] else None, db if ctx.needs_input_grad[2] else None, None
+
+
 def rms_norm_(x: torch.Tensor, gamma: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
-    """In place on x [m, n] (any leading shape; last dim n in {32,64,128,256})."""
+    """In place on x [m, n] (any leading shape; last dim n in {32,64,128,256}).  Differentiable in x and gamma when
+    either requires grad (_RowNorm)."""
     _need_cuda(x, gamma)
     _contig(x, gamma)
     if gamma.dim() != 1 or gamma.shape[0] != x.shape[-1] or gamma.dtype != x.dtype:
         raise SvgbError("gamma must be [n] with the dtype of x")
-    n = x.shape[-1]
-    check(lib().svgb_rms_norm(x.data_ptr(), gamma.data_ptr(), x.numel() // n, n, float(eps), _dt(x), _stream(x)),
-          "svgb_rms_norm")
-    _bump()
+    if needs_grad(x, gamma):
+        return _RowNorm.apply(x, gamma, None, float(eps))
+    _row_norm(x, gamma, None, eps)
     return x
 
 
 def layer_norm_(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor) -> torch.Tensor:
+    """In place on x [m, n], eps 1e-5.  Differentiable in x, gamma and beta (_RowNorm)."""
     _need_cuda(x, gamma, beta)
     _contig(x, gamma, beta)
     n = x.shape[-1]
     if gamma.shape != (n,) or beta.shape != (n,) or gamma.dtype != x.dtype or beta.dtype != x.dtype:
         raise SvgbError("gamma / beta must be [n] with the dtype of x")
-    check(lib().svgb_layer_norm(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), x.numel() // n, n, _dt(x),
-                                _stream(x)), "svgb_layer_norm")
-    _bump()
+    if needs_grad(x, gamma, beta):
+        return _RowNorm.apply(x, gamma, beta, 0.0)
+    _row_norm(x, gamma, beta, 0.0)
     return x
 
 
-def qk_rope_(q: torch.Tensor, k: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, len_text: int, mode: int):
-    """In place on q [B,Hq,S,D], k [B,Hk,S,D]; cos/sin float32 [S-len_text, D] (or [.., D/2] for the complex mode)."""
+def _rope_check(q, k, cos, sin, len_text, mode):
     _need_cuda(q, k, cos, sin)
     _contig(q, k, cos, sin)
     if q.dim() != 4 or k.dim() != 4 or cos.dim() != 2 or sin.dim() != 2:
@@ -630,17 +711,194 @@ def qk_rope_(q: torch.Tensor, k: torch.Tensor, cos: torch.Tensor, sin: torch.Ten
     width = D // 2 if mode == ROPE_COMPLEX_TXT_FIRST else D
     if tuple(cos.shape) != (valid, width) or tuple(sin.shape) != (valid, width):
         raise SvgbError(f"cos / sin must be [{valid}, {width}], got {tuple(cos.shape)} / {tuple(sin.shape)}")
+
+
+def _rope(q, k, cos, sin, len_text, mode):
+    B, Hq, S, D = q.shape
     check(lib().svgb_qk_rope(q.data_ptr(), k.data_ptr(), cos.data_ptr(), sin.data_ptr(), B, Hq, k.shape[1], S, D,
                              int(len_text), int(mode), _dt(q), _stream(q)), "svgb_qk_rope")
     _bump()
+
+
+def qk_rope_bwd(dq, dk, cos, sin, len_text: int, mode: int):
+    """Gradients (dq_in, dk_in) of qk_rope_ for the output gradients dq [B,Hq,S,D], dk [B,Hk,S,D]: the transpose of
+    each rotation on the rotated rows (exact for tables whose pairs differ), the text rows passed through."""
+    _rope_check(dq, dk, cos, sin, len_text, mode)
+    gq, gk = torch.empty_like(dq), torch.empty_like(dk)
+    B, Hq, S, D = dq.shape
+    check(lib().svgb_qk_rope_bwd(dq.data_ptr(), dk.data_ptr(), gq.data_ptr(), gk.data_ptr(), cos.data_ptr(),
+                                 sin.data_ptr(), B, Hq, dk.shape[1], S, D, int(len_text), int(mode), _dt(dq),
+                                 _stream(dq)), "svgb_qk_rope_bwd")
+    _bump()
+    return gq, gk
+
+
+class _QkRope(torch.autograd.Function):
+    """qk_rope_ under autograd: in place, q and k marked dirty; the backward is qk_rope_bwd (out of place)."""
+
+    @staticmethod
+    def forward(ctx, q, k, cos, sin, len_text, mode):
+        _rope(q, k, cos, sin, len_text, mode)
+        ctx.save_for_backward(cos, sin)
+        ctx.len_text, ctx.mode = len_text, mode
+        ctx.mark_dirty(q, k)
+        return q, k
+
+    @staticmethod
+    def backward(ctx, gq, gk):
+        cos, sin = ctx.saved_tensors
+        dq, dk = qk_rope_bwd(gq.contiguous(), gk.contiguous(), cos, sin, ctx.len_text, ctx.mode)
+        return (dq if ctx.needs_input_grad[0] else None, dk if ctx.needs_input_grad[1] else None,
+                None, None, None, None)
+
+
+def qk_rope_(q: torch.Tensor, k: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, len_text: int, mode: int):
+    """In place on q [B,Hq,S,D], k [B,Hk,S,D]; cos/sin float32 [S-len_text, D] (or [.., D/2] for the complex mode).
+    Differentiable in q and k (_QkRope); tables that require grad raise."""
+    _tables_no_grad(cos, sin)
+    _rope_check(q, k, cos, sin, len_text, mode)
+    if needs_grad(q, k):
+        return _QkRope.apply(q, k, cos, sin, int(len_text), int(mode))
+    _rope(q, k, cos, sin, len_text, mode)
     return q, k
+
+
+def qkv_prep_bwd(dq, dk, dv, heads: int, S_in: int, *, q_in=None, k_in=None, out_row0: int = 0,
+                 norm: int = NORM_NONE, gamma_q=None, gamma_k=None, eps: float = 1e-6, rope: int = 0, cos=None,
+                 sin=None, rope_lo: int = 0, rope_n: Optional[int] = None):
+    """Gradients of one qkv_prep call for the output gradients dq, dk, dv [B, H, S_out, D] (only rows
+    [out_row0, out_row0 + S_in) are read).  q_in, k_in: the forward's inputs (any strides qkv_prep takes), needed when
+    norm != NORM_NONE.  Returns (dq_in, dk_in, dv_in) contiguous [B, S_in, H*D] and (dgamma_q, dgamma_k, dbeta_q,
+    dbeta_k) in gamma's dtype (None where the norm has none)."""
+    _need_cuda(dq, dk, dv, q_in, k_in, gamma_q, gamma_k, cos, sin)
+    B, H, S_out, D = dq.shape
+    for t in (dq, dk, dv):
+        if t.shape != dq.shape or t.dtype != dq.dtype or not t.is_contiguous():
+            raise SvgbError("dq, dk, dv must be contiguous [B, H, S_out, D] of one dtype")
+    if H != heads or out_row0 < 0 or out_row0 + S_in > S_out:
+        raise SvgbError("the gradients must be [B, heads, S_out, D] with out_row0 + S_in <= S_out")
+    ts, bs = 0, 0
+    if norm != NORM_NONE:
+        if q_in is None or k_in is None or gamma_q is None or gamma_k is None:
+            raise SvgbError("a norm backward needs q_in, k_in, gamma_q and gamma_k")
+        for t in (q_in, k_in):
+            if tuple(t.shape) != (B, S_in, H * D) or t.dtype != dq.dtype or t.stride(2) != 1 or t.stride() != q_in.stride():
+                raise SvgbError("q_in, k_in must be [B, S_in, H*D] of the gradients' dtype with one set of strides")
+        ts, bs = q_in.stride(1), q_in.stride(0)
+        want = H * D if norm == NORM_RMS_HIDDEN else D
+        for g in (gamma_q, gamma_k):
+            if g.dtype != dq.dtype or g.numel() != want or not g.is_contiguous():
+                raise SvgbError(f"gamma_q / gamma_k must be contiguous [{want}] of the input dtype")
+    if rope:
+        if cos is None or sin is None or cos.dtype != torch.float32 or sin.dtype != torch.float32:
+            raise SvgbError("rope needs float32 cos / sin tables")
+        _contig(cos, sin)
+        if rope_n is None:
+            rope_n = cos.shape[0]
+        width = D // 2 if rope == 2 else D
+        if tuple(cos.shape) != (rope_n, width) or tuple(sin.shape) != (rope_n, width):
+            raise SvgbError(f"cos / sin must be [{rope_n}, {width}]")
+    else:
+        rope_n = 0
+    nbytes = C.c_size_t()
+    check(lib().svgb_qkv_prep_bwd_bytes(B, S_in, H, D, int(norm), C.byref(nbytes)), "svgb_qkv_prep_bwd_bytes")
+    ws = workspace("qkv_prep_bwd", nbytes.value, dq.device)
+    dx = tuple(torch.empty(B, S_in, H * D, dtype=dq.dtype, device=dq.device) for _ in range(3))
+    gw = H * D if norm == NORM_RMS_HIDDEN else D
+    f32 = lambda: torch.empty(gw, dtype=torch.float32, device=dq.device)  # noqa: E731
+    dg = (f32(), f32()) if norm != NORM_NONE else (None, None)
+    db = (f32(), f32()) if norm == NORM_LAYER else (None, None)
+    check(lib().svgb_qkv_prep_bwd(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), S_out * D, H * S_out * D, _p(q_in),
+                                  _p(k_in), ts, bs, dx[0].data_ptr(), dx[1].data_ptr(), dx[2].data_ptr(), B, S_in, H, D,
+                                  int(out_row0), int(norm), _p(gamma_q), _p(gamma_k), float(eps), int(rope), _p(cos),
+                                  _p(sin), int(rope_lo), int(rope_n), _p(dg[0]), _p(dg[1]), _p(db[0]), _p(db[1]),
+                                  _dt(dq), ws.data_ptr(), ws.numel(), _stream(dq)), "svgb_qkv_prep_bwd")
+    _bump({NORM_NONE: 1, NORM_RMS_HIDDEN: 3}.get(norm, 2))
+    cast = [None if g is None else g.to(dq.dtype) for g in (*dg, *db)]
+    return (*dx, *cast)
+
+
+class _QkvPrep(torch.autograd.Function):
+    """One or more qkv_prep calls into one shared output (a single block: one call; the double block: its video and
+    prompt streams) under autograd.  Inputs per call: q_in, k_in, v_in, gamma_q, gamma_k, beta_q, beta_k; `calls` holds
+    each call's other arguments (row range, norm, eps, RoPE tables and range), which get no gradient.  The backward
+    makes one qkv_prep_bwd per call, each reading its own rows of the incoming gradient, with no copies."""
+
+    @staticmethod
+    def forward(ctx, heads, S_out, calls, *ts):
+        B, _, HD = ts[0].shape
+        out = tuple(torch.empty(B, heads, S_out, HD // heads, dtype=ts[0].dtype, device=ts[0].device)
+                    for _ in range(3))
+        saved = []
+        for i, call in enumerate(calls):
+            q_in, k_in, v_in, gq, gk, bq, bk = ts[7 * i:7 * i + 7]
+            _qkv_prep(q_in, k_in, v_in, heads, out=out, gamma_q=gq, gamma_k=gk, beta_q=bq, beta_k=bk, **call)
+            keep = call["norm"] != NORM_NONE  # the norm backward reads x; a transpose or a rotation does not
+            saved += [q_in if keep else None, k_in if keep else None, gq, gk]
+        ctx.save_for_backward(*saved)
+        ctx.heads, ctx.calls, ctx.rows = heads, calls, [t.shape[1] for t in ts[::7]]
+        return out
+
+    @staticmethod
+    def backward(ctx, dq, dk, dv):
+        dq, dk, dv = (g.contiguous() for g in (dq, dk, dv))
+        saved = ctx.saved_tensors
+        grads = []
+        for i, call in enumerate(ctx.calls):
+            q_in, k_in, gq, gk = saved[4 * i:4 * i + 4]
+            dqi, dki, dvi, dgq, dgk, dbq, dbk = qkv_prep_bwd(dq, dk, dv, ctx.heads, ctx.rows[i], q_in=q_in, k_in=k_in,
+                                                             gamma_q=gq, gamma_k=gk, **call)
+            grads += [dqi, dki, dvi, dgq, dgk, dbq, dbk]
+        return (None, None, None, *grads)
+
+
+def qkv_prep_streams(streams, heads: int, S_out: int):
+    """Several qkv_prep calls into one new (q, k, v) [B, H, S_out, D]: streams is a list of ((q_in, k_in, v_in),
+    kwargs) with qkv_prep's keyword arguments (out_row0 places each).  Under grad one _QkvPrep records them all;
+    otherwise they are the plain calls."""
+    ts, calls = [], []
+    for ins, kw in streams:
+        kw = dict(kw)
+        ts += [*ins, *(kw.pop(n, None) for n in ("gamma_q", "gamma_k", "beta_q", "beta_k"))]
+        calls.append(kw)
+    if needs_grad(*ts, *(kw.get(n) for kw in calls for n in ("cos", "sin"))):
+        for kw in calls:
+            _tables_no_grad(kw.get("cos"), kw.get("sin"))
+            kw.setdefault("norm", NORM_NONE)
+        return _QkvPrep.apply(heads, S_out, calls, *ts)
+    q0 = ts[0]
+    B, _, HD = q0.shape
+    out = tuple(torch.empty(B, heads, S_out, HD // heads, dtype=q0.dtype, device=q0.device) for _ in range(3))
+    for i, kw in enumerate(calls):
+        q_in, k_in, v_in, gq, gk, bq, bk = ts[7 * i:7 * i + 7]
+        _qkv_prep(q_in, k_in, v_in, heads, out=out, gamma_q=gq, gamma_k=gk, beta_q=bq, beta_k=bk, **kw)
+    return out
 
 
 def qkv_prep(q_in, k_in, v_in, heads: int, *, out=None, out_row0: int = 0, out_rows: Optional[int] = None,
              norm: int = NORM_NONE, gamma_q=None, gamma_k=None, beta_q=None, beta_k=None, eps: float = 1e-6,
              rope: int = 0, cos=None, sin=None, rope_lo: int = 0, rope_n: Optional[int] = None):
     """[B, S_in, H*D] x3 -> (q, k, v) [B, H, S_out, D] rows [out_row0, out_row0+S_in) in one pass (transpose + QK norm
-    + RoPE).  q_in/k_in/v_in may be views of one packed projection (last dim contiguous)."""
+    + RoPE).  q_in/k_in/v_in may be views of one packed projection (last dim contiguous).  Differentiable in the
+    inputs and the norm weights when one requires grad (_QkvPrep); then out= is refused (a partly written buffer has
+    no clean in-place history) and so are RoPE tables that require grad."""
+    if needs_grad(q_in, k_in, v_in, gamma_q, gamma_k, beta_q, beta_k, cos, sin):
+        _tables_no_grad(cos, sin)
+        if out is not None:
+            raise SvgbError("qkv_prep(out=...) has no backward: under grad let it allocate its outputs")
+        _need_cuda(q_in, k_in, v_in, gamma_q, gamma_k, beta_q, beta_k, cos, sin)
+        kw = dict(out_row0=out_row0, norm=norm, gamma_q=gamma_q, gamma_k=gamma_k, beta_q=beta_q, beta_k=beta_k,
+                  eps=eps, rope=rope, cos=cos, sin=sin, rope_lo=rope_lo, rope_n=rope_n)
+        S_out = out_rows if out_rows is not None else q_in.shape[1]
+        return qkv_prep_streams([((q_in, k_in, v_in), kw)], heads, S_out)
+    return _qkv_prep(q_in, k_in, v_in, heads, out=out, out_row0=out_row0, out_rows=out_rows, norm=norm,
+                     gamma_q=gamma_q, gamma_k=gamma_k, beta_q=beta_q, beta_k=beta_k, eps=eps, rope=rope, cos=cos,
+                     sin=sin, rope_lo=rope_lo, rope_n=rope_n)
+
+
+def _qkv_prep(q_in, k_in, v_in, heads: int, *, out=None, out_row0: int = 0, out_rows: Optional[int] = None,
+              norm: int = NORM_NONE, gamma_q=None, gamma_k=None, beta_q=None, beta_k=None, eps: float = 1e-6,
+              rope: int = 0, cos=None, sin=None, rope_lo: int = 0, rope_n: Optional[int] = None):
     _need_cuda(q_in, k_in, v_in, gamma_q, gamma_k, beta_q, beta_k, cos, sin)
     B, S_in, HD = q_in.shape
     D = HD // heads
@@ -681,6 +939,7 @@ def qkv_prep(q_in, k_in, v_in, heads: int, *, out=None, out_row0: int = 0, out_r
 
 
 # ---- Wan transformer-block glue (svgb_layernorm_modulate / svgb_rmsnorm_hidden / svgb_modulate_shift / svgb_gate_residual)
+# No backward: under grad these raise at entry (_no_backward) instead of returning a detached result.
 _TORCH_DT = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 3}
 
 
@@ -702,6 +961,7 @@ def _rows_per_batch(rows, nb):
 
 
 def layernorm_modulate(x, weight=None, bias=None, eps=1e-6, scale=None, shift=None, out_dtype=None):
+    _no_backward("layernorm_modulate", x, weight, bias, scale, shift)
     _need_cuda(x, weight, bias, scale, shift)
     _contig(x, weight, bias)
     N = x.shape[-1]
@@ -723,6 +983,7 @@ def layernorm_modulate(x, weight=None, bias=None, eps=1e-6, scale=None, shift=No
 
 
 def rmsnorm_hidden(x, weight, eps, out_dtype=None):
+    _no_backward("rmsnorm_hidden", x, weight)
     _need_cuda(x, weight)
     _contig(x, weight)
     N = x.shape[-1]
@@ -734,6 +995,7 @@ def rmsnorm_hidden(x, weight, eps, out_dtype=None):
 
 
 def modulate_shift(x, scale, shift, out_dtype=torch.float32):
+    _no_backward("modulate_shift", x, scale, shift)
     _need_cuda(x, scale, shift)
     _contig(x)
     N = x.shape[-1]
@@ -748,6 +1010,7 @@ def modulate_shift(x, scale, shift, out_dtype=torch.float32):
 
 
 def gate_residual(residual, x, gate, out_dtype=torch.float32):
+    _no_backward("gate_residual", residual, x, gate)
     _need_cuda(residual, x, gate)
     _contig(residual, x)
     if residual.shape != x.shape:

@@ -2,12 +2,10 @@
     get_transpose_qkv -> get_qk_norm -> get_rotary_emb (-> get_encoder_condition_and_concat)
 (svg/models/hyvideo/attention.py:253-301, svg/models/wan/attention.py:100-135, svg/models/cog/attention.py:20-35)
 as single passes over the projection outputs.  Each helper returns (q, k, v) in the [B, H, S, D] layout the
-attention core consumes.
+attention core consumes.  Under grad each helper is differentiable in its projection outputs and norm weights
+(core._QkvPrep; the double block records both streams in one node).
 """
 from __future__ import annotations
-
-
-import torch
 
 from . import core
 
@@ -25,16 +23,13 @@ def hunyuan_double_block_qkv(query, key, value, enc_query, enc_key, enc_value, h
     """Dual-stream block: the video stream is normed + rotated, the prompt stream has its own norms and no RoPE,
     then torch.cat([video, prompt], dim=2) (hyvideo/attention.py:283-301) — here both streams are written
     straight into one [B, H, S_video + S_text, D] tensor."""
-    B, Sv, HD = query.shape
-    St = enc_query.shape[1]
-    D = HD // heads
-    out = tuple(torch.empty(B, heads, Sv + St, D, dtype=query.dtype, device=query.device) for _ in range(3))
-    core.qkv_prep(query, key, value, heads, out=out, out_row0=0, norm=core.NORM_RMS_HEAD, gamma_q=norm_q_weight,
-                  gamma_k=norm_k_weight, eps=eps, rope=1, cos=cos, sin=sin, rope_lo=0, rope_n=Sv)
-    core.qkv_prep(enc_query, enc_key, enc_value, heads, out=out, out_row0=Sv,
-                  norm=core.NORM_RMS_HEAD if norm_added_q_weight is not None else core.NORM_NONE,
+    Sv, St = query.shape[1], enc_query.shape[1]
+    video = dict(out_row0=0, norm=core.NORM_RMS_HEAD, gamma_q=norm_q_weight, gamma_k=norm_k_weight, eps=eps, rope=1,
+                 cos=cos, sin=sin, rope_lo=0, rope_n=Sv)
+    prompt = dict(out_row0=Sv, norm=core.NORM_RMS_HEAD if norm_added_q_weight is not None else core.NORM_NONE,
                   gamma_q=norm_added_q_weight, gamma_k=norm_added_k_weight, eps=eps)
-    return out
+    return core.qkv_prep_streams([((query, key, value), video), ((enc_query, enc_key, enc_value), prompt)], heads,
+                                 Sv + St)
 
 
 def wan_qkv(query, key, value, heads, norm_q_weight, norm_k_weight, eps, freqs_real, freqs_imag):
