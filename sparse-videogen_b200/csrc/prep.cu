@@ -13,6 +13,8 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "../../include/svgb200.h"
 #include "host_common.h"
 
@@ -91,21 +93,27 @@ __device__ __forceinline__ void ln_apply(float (&f)[8], const float (&g)[8], con
 #pragma unroll
   for (int i = 0; i < 8; ++i) f[i] = (f[i] - mean) * inv * g[i] + b[i];
 }
+// RoPE rotations; kT selects the transpose (the backward; not the inverse rotation: cos / sin need not repeat within
+// a pair).
 // interleaved pairs (2i, 2i+1): out[e] = x[e]*cos[e] + (e even ? -x[e^1] : x[e^1]) * sin[e]
+//   transpose: dx[2i] = dy[2i]*c[2i] + dy[2i+1]*s[2i+1],  dx[2i+1] = dy[2i+1]*c[2i+1] - dy[2i]*s[2i]
+template <bool kT>
 __device__ __forceinline__ void rope_apply(float (&f)[8], const float (&c)[8], const float (&s)[8]) {
   float o[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) o[i] = f[i] * c[i] + ((i & 1) ? f[i ^ 1] : -f[i ^ 1]) * s[i];
+  for (int i = 0; i < 8; ++i) o[i] = f[i] * c[i] + (((i & 1) != 0) != kT ? f[i ^ 1] : -f[i ^ 1]) * s[kT ? i ^ 1 : i];
 #pragma unroll
   for (int i = 0; i < 8; ++i) f[i] = o[i];
 }
-template <bool BF16>
+// complex pairs (a, b): a' = a*c - b*s, b' = b*c + a*s (transpose: a' = a*c + b*s, b' = b*c - a*s), in fp64 with
+// one rounding
+template <bool BF16, bool kT>
 __device__ __forceinline__ void rope_apply_complex(float (&f)[8], const float (&c)[4], const float (&s)[4]) {
   float o[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const double x = f[i], y = f[i ^ 1], cc = c[i >> 1], sn = s[i >> 1];
-    o[i] = round16d<BF16>(x * cc + ((i & 1) ? y : -y) * sn);
+    o[i] = round16d<BF16>(x * cc + (((i & 1) != 0) != kT ? y : -y) * sn);
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) f[i] = o[i];
@@ -120,6 +128,19 @@ __device__ __forceinline__ void load_f8(const float* p, float (&f)[8]) {
 __device__ __forceinline__ void load_f4(const float* p, float (&f)[4]) {
   const float4 a = __ldg(reinterpret_cast<const float4*>(p));
   f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+}
+// this thread's cos / sin of table row `row`: interleaved [n, D] into c8 / s8, complex [n, D/2] into c4 / s4
+template <int D>
+__device__ __forceinline__ void load_rope_tables(const float* cos_t, const float* sin_t, long long row, int seg,
+                                                 bool complex, float (&c8)[8], float (&s8)[8], float (&c4)[4],
+                                                 float (&s4)[4]) {
+  if (complex) {
+    load_f4(cos_t + row * (D / 2) + seg * 4, c4);
+    load_f4(sin_t + row * (D / 2) + seg * 4, s4);
+  } else {
+    load_f8(cos_t + row * D + seg * 8, c8);
+    load_f8(sin_t + row * D + seg * 8, s8);
+  }
 }
 
 constexpr int kThreads = 256;
@@ -159,6 +180,8 @@ row_norm_kernel(uint4* __restrict__ x, const uint4* __restrict__ gamma, const ui
 }
 
 // ---- in-place RoPE on q [B,Hq,S,D], k [B,Hk,S,D]; rows [row0, row0+valid) of every head ------------
+// qk_rope_bwd_kernel is the same head walk, out of place.  This one keeps its own body and so its instruction stream;
+// merged into one kernel with the transpose it took 0.25-0.36% longer at HunyuanVideo 720p (DESIGN.md §5).
 template <bool BF16, int D, bool kComplex>
 __global__ void __launch_bounds__(kThreads)
 qk_rope_kernel(uint4* __restrict__ q, uint4* __restrict__ k, const float* __restrict__ cos_t,
@@ -168,13 +191,7 @@ qk_rope_kernel(uint4* __restrict__ q, uint4* __restrict__ k, const float* __rest
   const int t = blockIdx.x * RPB + threadIdx.x / LPR;
   if (t >= valid) return;
   float c8[8], s8[8], c4[4], s4[4];
-  if constexpr (kComplex) {
-    load_f4(cos_t + static_cast<long long>(t) * (D / 2) + seg * 4, c4);
-    load_f4(sin_t + static_cast<long long>(t) * (D / 2) + seg * 4, s4);
-  } else {
-    load_f8(cos_t + static_cast<long long>(t) * D + seg * 8, c8);
-    load_f8(sin_t + static_cast<long long>(t) * D + seg * 8, s8);
-  }
+  load_rope_tables<D>(cos_t, sin_t, t, seg, kComplex, c8, s8, c4, s4);
   const long long hs = static_cast<long long>(S) * LPR;
 #pragma unroll 1
   for (int which = 0; which < 2; ++which) {
@@ -191,8 +208,8 @@ qk_rope_kernel(uint4* __restrict__ q, uint4* __restrict__ k, const float* __rest
         if (h0 + u < H) {
           float f[8];
           unpack8<BF16>(v[u], f);
-          if constexpr (kComplex) rope_apply_complex<BF16>(f, c4, s4);
-          else rope_apply(f, c8, s8);
+          if constexpr (kComplex) rope_apply_complex<BF16, false>(f, c4, s4);
+          else rope_apply<false>(f, c8, s8);
           p[(h0 + u) * hs] = pack8<BF16>(f);
         }
       }
@@ -200,17 +217,65 @@ qk_rope_kernel(uint4* __restrict__ q, uint4* __restrict__ k, const float* __rest
   }
 }
 
+// ---- RoPE backward, out of place: every row of dq [B,Hq,S,D] / dk [B,Hk,S,D]; rows [row0, row0+valid) transposed,
+// the others copied
+template <bool BF16, int D, bool kComplex>
+__global__ void __launch_bounds__(kThreads)
+qk_rope_bwd_kernel(const uint4* __restrict__ dq, const uint4* __restrict__ dk, uint4* __restrict__ gq,
+                   uint4* __restrict__ gk, const float* __restrict__ cos_t, const float* __restrict__ sin_t, int Hq,
+                   int Hk, int S, int row0, int valid) {
+  constexpr int LPR = D / 8, RPB = kThreads / LPR;
+  const int seg = threadIdx.x % LPR;
+  const int t = blockIdx.x * RPB + threadIdx.x / LPR;
+  if (t >= S) return;
+  const bool rot = t >= row0 && t < row0 + valid;
+  float c8[8], s8[8], c4[4], s4[4];
+  if (rot) load_rope_tables<D>(cos_t, sin_t, t - row0, seg, kComplex, c8, s8, c4, s4);
+  const long long hs = static_cast<long long>(S) * LPR;
+#pragma unroll 1
+  for (int which = 0; which < 2; ++which) {
+    const int H = which ? Hk : Hq;
+    const long long o = (static_cast<long long>(blockIdx.y) * H * S + t) * LPR + seg;
+    const uint4* src = (which ? dk : dq) + o;
+    uint4* dst = (which ? gk : gq) + o;
+#pragma unroll 1
+    for (int h0 = 0; h0 < H; h0 += kUnrollRows) {
+      uint4 v[kUnrollRows];
+#pragma unroll
+      for (int u = 0; u < kUnrollRows; ++u)
+        if (h0 + u < H) v[u] = __ldg(src + (h0 + u) * hs);
+#pragma unroll
+      for (int u = 0; u < kUnrollRows; ++u) {
+        if (h0 + u < H) {
+          if (rot) {
+            float f[8];
+            unpack8<BF16>(v[u], f);
+            if constexpr (kComplex) rope_apply_complex<BF16, true>(f, c4, s4);
+            else rope_apply<true>(f, c8, s8);
+            v[u] = pack8<BF16>(f);
+          }
+          dst[(h0 + u) * hs] = v[u];
+        }
+      }
+    }
+  }
+}
+
 // ---- fused transpose + norm + RoPE ----------------------------------------------------------------
-struct PrepArgs {
-  const uint16_t* in[3];   // q, k, v projection outputs [B, S_in, H*D] (token stride / batch stride below)
-  uint16_t* out[3];        // [B, H, S_out, D]; this call fills rows [out_row0, out_row0 + S_in)
-  const uint16_t* gamma[2];
-  const uint16_t* beta[2];
+// what the fused pass and its backward share: the layout, the norm and the RoPE tables and range
+struct PrepGeom {
   const float* cos_t;
   const float* sin_t;
   long long in_token_stride, in_batch_stride, out_head_stride, out_batch_stride;
   int S_in, H, out_row0, norm, rope, rope_lo, rope_n;
   float eps;
+};
+struct PrepArgs {
+  const uint16_t* in[3];   // q, k, v projection outputs [B, S_in, H*D] (token stride / batch stride in geo)
+  uint16_t* out[3];        // [B, H, S_out, D]; this call fills rows [out_row0, out_row0 + S_in)
+  const uint16_t* gamma[2];
+  const uint16_t* beta[2];
+  PrepGeom geo;
 };
 
 template <bool BF16, int D>
@@ -220,35 +285,26 @@ qkv_prep_kernel(const PrepArgs a) {
   const int seg = threadIdx.x % LPR;
   const int t = blockIdx.x * RPB + threadIdx.x / LPR;
   const int which = blockIdx.z;  // 0 q, 1 k, 2 v
-  const bool live = t < a.S_in;
-  const int tt = live ? t : a.S_in - 1;  // keep the whole warp in the shuffles; dead lanes never store
-  const uint16_t* in = a.in[which] + blockIdx.y * a.in_batch_stride + tt * a.in_token_stride + seg * 8;
-  uint16_t* out = a.out[which] + blockIdx.y * a.out_batch_stride + static_cast<long long>(a.out_row0 + tt) * D + seg * 8;
-  const int norm = which < 2 ? a.norm : 0;
-  const int rp = a.rope;
-  const bool rot = which < 2 && rp != 0 && tt >= a.rope_lo && tt < a.rope_lo + a.rope_n;
+  const bool live = t < a.geo.S_in;
+  const int tt = live ? t : a.geo.S_in - 1;  // keep the whole warp in the shuffles; dead lanes never store
+  const uint16_t* in = a.in[which] + blockIdx.y * a.geo.in_batch_stride + tt * a.geo.in_token_stride + seg * 8;
+  uint16_t* out = a.out[which] + blockIdx.y * a.geo.out_batch_stride + static_cast<long long>(a.geo.out_row0 + tt) * D + seg * 8;
+  const int norm = which < 2 ? a.geo.norm : 0;
+  const int rp = a.geo.rope;
+  const bool rot = which < 2 && rp != 0 && tt >= a.geo.rope_lo && tt < a.geo.rope_lo + a.geo.rope_n;
   float g[8], b[8], c8[8], s8[8], c4[4], s4[4];
   if (norm == 1 || norm == 2) unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(a.gamma[which]) + seg), g);
   if (norm == 2) unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(a.beta[which]) + seg), b);
-  if (rot) {
-    const long long tr = tt - a.rope_lo;
-    if (rp == 2) {
-      load_f4(a.cos_t + tr * (D / 2) + seg * 4, c4);
-      load_f4(a.sin_t + tr * (D / 2) + seg * 4, s4);
-    } else {
-      load_f8(a.cos_t + tr * D + seg * 8, c8);
-      load_f8(a.sin_t + tr * D + seg * 8, s8);
-    }
-  }
+  if (rot) load_rope_tables<D>(a.geo.cos_t, a.geo.sin_t, tt - a.geo.rope_lo, seg, rp == 2, c8, s8, c4, s4);
   float inv_full = 0.f;
   if (norm == 3) {  // RMS over the full hidden row H*D (Wan QK-norm before the head split, wan/attention.py:107-120)
     float ss = 0.f;
 #pragma unroll 1
-    for (int h0 = 0; h0 < a.H; h0 += kUnrollRows) {
+    for (int h0 = 0; h0 < a.geo.H; h0 += kUnrollRows) {
       uint4 v[kUnrollRows];
 #pragma unroll
       for (int u = 0; u < kUnrollRows; ++u)
-        v[u] = h0 + u < a.H ? *reinterpret_cast<const uint4*>(in + (h0 + u) * D) : make_uint4(0, 0, 0, 0);
+        v[u] = h0 + u < a.geo.H ? *reinterpret_cast<const uint4*>(in + (h0 + u) * D) : make_uint4(0, 0, 0, 0);
 #pragma unroll
       for (int u = 0; u < kUnrollRows; ++u) {
         float f[8];
@@ -258,21 +314,21 @@ qkv_prep_kernel(const PrepArgs a) {
       }
     }
     ss = group_sum<LPR>(ss);
-    inv_full = 1.0f / sqrtf(ss / (a.H * D) + a.eps);
+    inv_full = 1.0f / sqrtf(ss / (a.geo.H * D) + a.geo.eps);
   }
 #pragma unroll 1
-  for (int h0 = 0; h0 < a.H; h0 += kUnrollRows) {
+  for (int h0 = 0; h0 < a.geo.H; h0 += kUnrollRows) {
     uint4 v[kUnrollRows];
 #pragma unroll
     for (int u = 0; u < kUnrollRows; ++u)
-      if (h0 + u < a.H) v[u] = *reinterpret_cast<const uint4*>(in + (h0 + u) * D);
+      if (h0 + u < a.geo.H) v[u] = *reinterpret_cast<const uint4*>(in + (h0 + u) * D);
 #pragma unroll
     for (int u = 0; u < kUnrollRows; ++u) {
-      if (h0 + u < a.H) {  // block-uniform
+      if (h0 + u < a.geo.H) {  // block-uniform
         if (norm != 0 || rot) {
           float f[8];
           unpack8<BF16>(v[u], f);
-          if (norm == 1) rms_apply<D>(f, g, a.eps);
+          if (norm == 1) rms_apply<D>(f, g, a.geo.eps);
           else if (norm == 2) ln_apply<D>(f, g, b);
           else if (norm == 3) {
             float gw[8];
@@ -285,77 +341,18 @@ qkv_prep_kernel(const PrepArgs a) {
 #pragma unroll
               for (int i = 0; i < 8; ++i) f[i] = round16f<BF16>(f[i]);
             }
-            if (rp == 2) rope_apply_complex<BF16>(f, c4, s4);
-            else rope_apply(f, c8, s8);
+            if (rp == 2) rope_apply_complex<BF16, false>(f, c4, s4);
+            else rope_apply<false>(f, c8, s8);
           }
           v[u] = pack8<BF16>(f);
         }
-        if (live) *reinterpret_cast<uint4*>(out + (h0 + u) * a.out_head_stride) = v[u];
+        if (live) *reinterpret_cast<uint4*>(out + (h0 + u) * a.geo.out_head_stride) = v[u];
       }
     }
   }
 }
 
-template <bool BF16, bool kLayer>
-static int launch_row_norm(void* x, const void* gamma, const void* beta, float eps, long long m, int n,
-                           cudaStream_t st) {
-  const long long rpb = kThreads / (n / 8);
-  long long blocks = (m + rpb * kUnrollRows - 1) / (rpb * kUnrollRows);
-  if (blocks > 148 * 32) blocks = 148 * 32;
-  if (blocks < 1) blocks = 1;
-  auto X = static_cast<uint4*>(x);
-  auto G = static_cast<const uint4*>(gamma);
-  auto B = static_cast<const uint4*>(beta);
-  const unsigned gb = static_cast<unsigned>(blocks);
-  switch (n) {
-    case 32: row_norm_kernel<BF16, 32, kLayer><<<gb, kThreads, 0, st>>>(X, G, B, eps, m); break;
-    case 64: row_norm_kernel<BF16, 64, kLayer><<<gb, kThreads, 0, st>>>(X, G, B, eps, m); break;
-    case 128: row_norm_kernel<BF16, 128, kLayer><<<gb, kThreads, 0, st>>>(X, G, B, eps, m); break;
-    default: row_norm_kernel<BF16, 256, kLayer><<<gb, kThreads, 0, st>>>(X, G, B, eps, m); break;
-  }
-  SVGB_LAUNCH_OK();
-  return 0;
-}
-
-template <bool BF16, bool kComplex>
-static int launch_rope(void* q, void* k, const float* c, const float* s, int B, int Hq, int Hk, int S, int D, int row0,
-                       int valid, cudaStream_t st) {
-  const int rpb = kThreads / (D / 8);
-  dim3 grid((valid + rpb - 1) / rpb, B);
-  auto Q = static_cast<uint4*>(q);
-  auto K = static_cast<uint4*>(k);
-  switch (D) {
-    case 64: qk_rope_kernel<BF16, 64, kComplex><<<grid, kThreads, 0, st>>>(Q, K, c, s, Hq, Hk, S, row0, valid); break;
-    case 128: qk_rope_kernel<BF16, 128, kComplex><<<grid, kThreads, 0, st>>>(Q, K, c, s, Hq, Hk, S, row0, valid); break;
-    default: qk_rope_kernel<BF16, 256, kComplex><<<grid, kThreads, 0, st>>>(Q, K, c, s, Hq, Hk, S, row0, valid); break;
-  }
-  SVGB_LAUNCH_OK();
-  return 0;
-}
-
 // ================================= backward (DESIGN.md §5) =====================================================
-// The RoPE transposes (not the inverse rotations: cos / sin need not repeat within a pair):
-//   dx[2i] = dy[2i]*c[2i] + dy[2i+1]*s[2i+1],  dx[2i+1] = dy[2i+1]*c[2i+1] - dy[2i]*s[2i]
-__device__ __forceinline__ void rope_apply_t(float (&f)[8], const float (&c)[8], const float (&s)[8]) {
-  float o[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) o[i] = f[i] * c[i] + ((i & 1) ? -f[i ^ 1] : f[i ^ 1]) * s[i ^ 1];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) f[i] = o[i];
-}
-// complex pairs (a, b): da = dy_a*c + dy_b*s, db = dy_b*c - dy_a*s in fp64, one rounding (as the forward)
-template <bool BF16>
-__device__ __forceinline__ void rope_apply_complex_t(float (&f)[8], const float (&c)[4], const float (&s)[4]) {
-  float o[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const double x = f[i], y = f[i ^ 1], cc = c[i >> 1], sn = s[i >> 1];
-    o[i] = round16d<BF16>(x * cc + ((i & 1) ? -y : y) * sn);
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) f[i] = o[i];
-}
-
 // Norm backwards on one head row.  x = the saved 16-bit input (f), d = the gradient at the norm output, replaced by
 // dx; r and x^ are recomputed exactly as rms_apply / ln_apply compute them.  u = gamma*d:
 //   RMS: dx = r*(u - x^*mean(u*x^))          LayerNorm: dx = r*(u - mean(u) - x^*mean(u*x^))
@@ -486,72 +483,15 @@ row_norm_bwd_kernel(const uint4* __restrict__ x, const uint4* __restrict__ dy, c
   if constexpr (kLayer) cta_column_sum<N>(ab, part + static_cast<long long>(blockIdx.x) * 2 * N + N);
 }
 
-// ---- RoPE backward, out of place: every row of dq [B,Hq,S,D] / dk [B,Hk,S,D]; rows [row0, row0+valid) transposed,
-// the others copied ------------------------------------------------------------------------------------------------
-template <bool BF16, int D, bool kComplex>
-__global__ void __launch_bounds__(kThreads)
-qk_rope_bwd_kernel(const uint4* __restrict__ dq, const uint4* __restrict__ dk, uint4* __restrict__ gq,
-                   uint4* __restrict__ gk, const float* __restrict__ cos_t, const float* __restrict__ sin_t, int Hq,
-                   int Hk, int S, int row0, int valid) {
-  constexpr int LPR = D / 8, RPB = kThreads / LPR;
-  const int seg = threadIdx.x % LPR;
-  const int t = blockIdx.x * RPB + threadIdx.x / LPR;
-  if (t >= S) return;
-  const bool rot = t >= row0 && t < row0 + valid;
-  float c8[8], s8[8], c4[4], s4[4];
-  if (rot) {
-    const long long tr = t - row0;
-    if constexpr (kComplex) {
-      load_f4(cos_t + tr * (D / 2) + seg * 4, c4);
-      load_f4(sin_t + tr * (D / 2) + seg * 4, s4);
-    } else {
-      load_f8(cos_t + tr * D + seg * 8, c8);
-      load_f8(sin_t + tr * D + seg * 8, s8);
-    }
-  }
-  const long long hs = static_cast<long long>(S) * LPR;
-#pragma unroll 1
-  for (int which = 0; which < 2; ++which) {
-    const int H = which ? Hk : Hq;
-    const long long o = (static_cast<long long>(blockIdx.y) * H * S + t) * LPR + seg;
-    const uint4* src = (which ? dk : dq) + o;
-    uint4* dst = (which ? gk : gq) + o;
-#pragma unroll 1
-    for (int h0 = 0; h0 < H; h0 += kUnrollRows) {
-      uint4 v[kUnrollRows];
-#pragma unroll
-      for (int u = 0; u < kUnrollRows; ++u)
-        if (h0 + u < H) v[u] = __ldg(src + (h0 + u) * hs);
-#pragma unroll
-      for (int u = 0; u < kUnrollRows; ++u) {
-        if (h0 + u < H) {
-          if (rot) {
-            float f[8];
-            unpack8<BF16>(v[u], f);
-            if constexpr (kComplex) rope_apply_complex_t<BF16>(f, c4, s4);
-            else rope_apply_t(f, c8, s8);
-            v[u] = pack8<BF16>(f);
-          }
-          dst[(h0 + u) * hs] = v[u];
-        }
-      }
-    }
-  }
-}
-
 // ---- fused backward of qkv_prep_kernel -----------------------------------------------------------------------------
 struct PrepBwdArgs {
   const uint16_t* dy[3];   // dQ, dK, dV [B, H, S_out, D]: rows [out_row0, out_row0 + S_in) are read, no others
-  const uint16_t* x[2];    // the forward's q_in, k_in (token stride / batch stride below)
+  const uint16_t* x[2];    // the forward's q_in, k_in (token stride / batch stride in geo)
   uint16_t* dx[3];         // dq_in, dk_in, dv_in: contiguous [B, S_in, H*D]
   const uint16_t* gamma[2];
-  const float* cos_t;
-  const float* sin_t;
   float* part[2];          // q, k: per-CTA [dgamma | dbeta] partials (NORM_RMS_HIDDEN: per-split dgamma [H*D])
   float2* stats[2];        // NORM_RMS_HIDDEN: per token (r, mean(u*x^) over the hidden row)
-  long long in_token_stride, in_batch_stride, out_head_stride, out_batch_stride;
-  int S_in, H, out_row0, norm, rope, rope_lo, rope_n;
-  float eps;
+  PrepGeom geo;
 };
 
 // the gradient at the norm output of one head row: the RoPE transpose, rounded to the 16-bit dtype when a norm
@@ -561,27 +501,13 @@ __device__ __forceinline__ void prep_dn(float (&f)[8], bool rot, int rope, bool 
                                         const float (&s8)[8], const float (&c4)[4], const float (&s4)[4]) {
   if (!rot) return;
   if (rope == 2) {
-    rope_apply_complex_t<BF16>(f, c4, s4);
+    rope_apply_complex<BF16, true>(f, c4, s4);
   } else {
-    rope_apply_t(f, c8, s8);
+    rope_apply<true>(f, c8, s8);
     if (round) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) f[i] = round16f<BF16>(f[i]);
     }
-  }
-}
-
-template <int D>
-__device__ __forceinline__ void prep_tables(const PrepBwdArgs& a, int tt, int seg, bool rot, float (&c8)[8],
-                                            float (&s8)[8], float (&c4)[4], float (&s4)[4]) {
-  if (!rot) return;
-  const long long tr = tt - a.rope_lo;
-  if (a.rope == 2) {
-    load_f4(a.cos_t + tr * (D / 2) + seg * 4, c4);
-    load_f4(a.sin_t + tr * (D / 2) + seg * 4, s4);
-  } else {
-    load_f8(a.cos_t + tr * D + seg * 8, c8);
-    load_f8(a.sin_t + tr * D + seg * 8, s8);
   }
 }
 
@@ -593,41 +519,41 @@ qkv_prep_bwd_kernel(const PrepBwdArgs a) {
   constexpr int LPR = D / 8, RPB = kThreads / LPR;
   const int seg = threadIdx.x % LPR, sub = threadIdx.x / LPR;
   const int which = blockIdx.z;  // 0 q, 1 k, 2 v
-  const int norm = which < 2 ? a.norm : 0;
-  const long long HD = static_cast<long long>(a.H) * D;
+  const int norm = which < 2 ? a.geo.norm : 0;
+  const long long HD = static_cast<long long>(a.geo.H) * D;
   float g[8], ag[8] = {}, ab[8] = {}, c8[8], s8[8], c4[4], s4[4];
   if (norm == 1 || norm == 2) unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(a.gamma[which]) + seg), g);
 #pragma unroll 1
-  for (int t0 = blockIdx.x * RPB; t0 < a.S_in; t0 += gridDim.x * RPB) {  // block-uniform
+  for (int t0 = blockIdx.x * RPB; t0 < a.geo.S_in; t0 += gridDim.x * RPB) {  // block-uniform
     const int t = t0 + sub;
-    const bool live = t < a.S_in;
-    const int tt = live ? t : a.S_in - 1;  // keep the whole warp in the shuffles; dead lanes add and store nothing
+    const bool live = t < a.geo.S_in;
+    const int tt = live ? t : a.geo.S_in - 1;  // keep the whole warp in the shuffles; dead lanes add and store nothing
     const uint16_t* dy =
-        a.dy[which] + blockIdx.y * a.out_batch_stride + static_cast<long long>(a.out_row0 + tt) * D + seg * 8;
-    const uint16_t* x = which < 2 ? a.x[which] + blockIdx.y * a.in_batch_stride + tt * a.in_token_stride + seg * 8
+        a.dy[which] + blockIdx.y * a.geo.out_batch_stride + static_cast<long long>(a.geo.out_row0 + tt) * D + seg * 8;
+    const uint16_t* x = which < 2 ? a.x[which] + blockIdx.y * a.geo.in_batch_stride + tt * a.geo.in_token_stride + seg * 8
                                   : nullptr;
-    uint16_t* dx = a.dx[which] + (static_cast<long long>(blockIdx.y) * a.S_in + tt) * HD + seg * 8;
-    const bool rot = which < 2 && a.rope != 0 && tt >= a.rope_lo && tt < a.rope_lo + a.rope_n;
-    prep_tables<D>(a, tt, seg, rot, c8, s8, c4, s4);
+    uint16_t* dx = a.dx[which] + (static_cast<long long>(blockIdx.y) * a.geo.S_in + tt) * HD + seg * 8;
+    const bool rot = which < 2 && a.geo.rope != 0 && tt >= a.geo.rope_lo && tt < a.geo.rope_lo + a.geo.rope_n;
+    if (rot) load_rope_tables<D>(a.geo.cos_t, a.geo.sin_t, tt - a.geo.rope_lo, seg, a.geo.rope == 2, c8, s8, c4, s4);
     if (norm == 3) {  // first pass over the hidden row: sum x^2 and (gamma*dn)*x over all H heads
       float ss = 0.f, ux = 0.f;
 #pragma unroll 1
-      for (int h0 = 0; h0 < a.H; h0 += kUnrollRows) {
+      for (int h0 = 0; h0 < a.geo.H; h0 += kUnrollRows) {
         uint4 dv[kUnrollRows], xv[kUnrollRows];
 #pragma unroll
         for (int u = 0; u < kUnrollRows; ++u) {
-          const bool in = h0 + u < a.H;
-          dv[u] = in ? *reinterpret_cast<const uint4*>(dy + (h0 + u) * a.out_head_stride) : make_uint4(0, 0, 0, 0);
+          const bool in = h0 + u < a.geo.H;
+          dv[u] = in ? *reinterpret_cast<const uint4*>(dy + (h0 + u) * a.geo.out_head_stride) : make_uint4(0, 0, 0, 0);
           xv[u] = in ? *reinterpret_cast<const uint4*>(x + (h0 + u) * D) : make_uint4(0, 0, 0, 0);
         }
 #pragma unroll
         for (int u = 0; u < kUnrollRows; ++u) {
-          if (h0 + u < a.H) {
+          if (h0 + u < a.geo.H) {
             float f[8], d[8], gw[8];
             unpack8<BF16>(xv[u], f);
             unpack8<BF16>(dv[u], d);
             unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(a.gamma[which] + (h0 + u) * D) + seg), gw);
-            prep_dn<BF16, D>(d, rot, a.rope, true, c8, s8, c4, s4);
+            prep_dn<BF16, D>(d, rot, a.geo.rope, true, c8, s8, c4, s4);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               ss += f[i] * f[i];
@@ -638,28 +564,28 @@ qkv_prep_bwd_kernel(const PrepBwdArgs a) {
       }
       ss = group_sum<LPR>(ss);
       ux = group_sum<LPR>(ux);
-      const float inv = 1.0f / sqrtf(ss / HD + a.eps);
+      const float inv = 1.0f / sqrtf(ss / HD + a.geo.eps);
       if (live && seg == 0)
-        a.stats[which][static_cast<long long>(blockIdx.y) * a.S_in + t] = make_float2(inv, inv * ux / HD);
+        a.stats[which][static_cast<long long>(blockIdx.y) * a.geo.S_in + t] = make_float2(inv, inv * ux / HD);
       continue;
     }
 #pragma unroll 1
-    for (int h0 = 0; h0 < a.H; h0 += kUnrollRows) {
+    for (int h0 = 0; h0 < a.geo.H; h0 += kUnrollRows) {
       uint4 dv[kUnrollRows], xv[kUnrollRows];
 #pragma unroll
       for (int u = 0; u < kUnrollRows; ++u) {
-        if (h0 + u < a.H) {
-          dv[u] = *reinterpret_cast<const uint4*>(dy + (h0 + u) * a.out_head_stride);
+        if (h0 + u < a.geo.H) {
+          dv[u] = *reinterpret_cast<const uint4*>(dy + (h0 + u) * a.geo.out_head_stride);
           if (norm != 0) xv[u] = *reinterpret_cast<const uint4*>(x + (h0 + u) * D);
         }
       }
 #pragma unroll
       for (int u = 0; u < kUnrollRows; ++u) {
-        if (h0 + u < a.H) {  // block-uniform
+        if (h0 + u < a.geo.H) {  // block-uniform
           if (norm != 0 || rot) {
             float d[8];
             unpack8<BF16>(dv[u], d);
-            prep_dn<BF16, D>(d, rot, a.rope, norm != 0, c8, s8, c4, s4);
+            prep_dn<BF16, D>(d, rot, a.geo.rope, norm != 0, c8, s8, c4, s4);
             if (norm != 0) {
               float f[8];
               unpack8<BF16>(xv[u], f);
@@ -667,7 +593,7 @@ qkv_prep_bwd_kernel(const PrepBwdArgs a) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) d[i] = 0.f;
               }
-              if (norm == 1) rms_bwd<D>(f, d, g, a.eps, ag);
+              if (norm == 1) rms_bwd<D>(f, d, g, a.geo.eps, ag);
               else ln_bwd<D>(f, d, g, ag, ab);
             }
             dv[u] = pack8<BF16>(d);
@@ -693,10 +619,10 @@ hidden_rms_bwd_kernel(const PrepBwdArgs a, int B) {
   constexpr int LPR = D / 8;
   const int which = blockIdx.z;
   const int c = blockIdx.x * kHiddenThreads + threadIdx.x;
-  if (c >= a.H * LPR) return;
+  if (c >= a.geo.H * LPR) return;
   const int h = c / LPR, seg = c % LPR;
-  const long long HD = static_cast<long long>(a.H) * D;
-  const long long T = static_cast<long long>(B) * a.S_in;
+  const long long HD = static_cast<long long>(a.geo.H) * D;
+  const long long T = static_cast<long long>(B) * a.geo.S_in;
   const long long per = (T + gridDim.y - 1) / gridDim.y;
   const long long lo = blockIdx.y * per, hi = lo + per < T ? lo + per : T;
   float g[8], ag[8] = {};
@@ -708,23 +634,23 @@ hidden_rms_bwd_kernel(const PrepBwdArgs a, int B) {
     for (int u = 0; u < kUnrollRows; ++u) {
       const long long i = i0 + u;
       if (i < hi) {
-        const long long b = i / a.S_in, t = i % a.S_in;
-        dv[u] = *reinterpret_cast<const uint4*>(a.dy[which] + b * a.out_batch_stride + h * a.out_head_stride +
-                                                (a.out_row0 + t) * D + seg * 8);
-        xv[u] = *reinterpret_cast<const uint4*>(a.x[which] + b * a.in_batch_stride + t * a.in_token_stride + c * 8);
+        const long long b = i / a.geo.S_in, t = i % a.geo.S_in;
+        dv[u] = *reinterpret_cast<const uint4*>(a.dy[which] + b * a.geo.out_batch_stride + h * a.geo.out_head_stride +
+                                                (a.geo.out_row0 + t) * D + seg * 8);
+        xv[u] = *reinterpret_cast<const uint4*>(a.x[which] + b * a.geo.in_batch_stride + t * a.geo.in_token_stride + c * 8);
       }
     }
 #pragma unroll
     for (int u = 0; u < kUnrollRows; ++u) {
       const long long i = i0 + u;
       if (i < hi) {
-        const int t = static_cast<int>(i % a.S_in);
-        const bool rot = a.rope != 0 && t >= a.rope_lo && t < a.rope_lo + a.rope_n;
+        const int t = static_cast<int>(i % a.geo.S_in);
+        const bool rot = a.geo.rope != 0 && t >= a.geo.rope_lo && t < a.geo.rope_lo + a.geo.rope_n;
         float c8[8], s8[8], c4[4], s4[4], f[8], d[8];
-        prep_tables<D>(a, t, seg, rot, c8, s8, c4, s4);
+        if (rot) load_rope_tables<D>(a.geo.cos_t, a.geo.sin_t, t - a.geo.rope_lo, seg, a.geo.rope == 2, c8, s8, c4, s4);
         unpack8<BF16>(xv[u], f);
         unpack8<BF16>(dv[u], d);
-        prep_dn<BF16, D>(d, rot, a.rope, true, c8, s8, c4, s4);
+        prep_dn<BF16, D>(d, rot, a.geo.rope, true, c8, s8, c4, s4);
         const float2 st = a.stats[which][i];
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
@@ -741,12 +667,15 @@ hidden_rms_bwd_kernel(const PrepBwdArgs a, int B) {
   for (int k = 0; k < 8; ++k) p[k] = ag[k];
 }
 
-// Grid sizes of the backward launches; the workspace sizes are derived from them, so both sides agree.
+
+// ================================= host side ===================================================================
+// Grid sizes; the backward's workspace sizes are derived from them, so both sides agree.
 constexpr int kBwdCtas = 148 * 4;  // persistent grids: a few waves, which bounds the partial rows
-static int row_norm_bwd_blocks(long long m, int n) {
+// a walk over the rows of [m, n], kUnrollRows rows per thread per pass, on at most cap CTAs
+static int row_blocks(long long m, int n, int cap) {
   const long long rpb = kThreads / (n / 8);
-  long long blocks = (m + rpb * kUnrollRows - 1) / (rpb * kUnrollRows);
-  return static_cast<int>(blocks < 1 ? 1 : blocks > kBwdCtas ? kBwdCtas : blocks);
+  const long long blocks = (m + rpb * kUnrollRows - 1) / (rpb * kUnrollRows);
+  return static_cast<int>(blocks < 1 ? 1 : blocks > cap ? cap : blocks);
 }
 static int prep_bwd_blocks(int B, int S_in, int D) {
   const int rpb = kThreads / (D / 8);
@@ -757,6 +686,26 @@ static int hidden_cols(int H, int D) { return (H * (D / 8) + kHiddenThreads - 1)
 static int hidden_splits(int B, int S_in, int H, int D) {
   const long long want = kBwdCtas / hidden_cols(H, D), T = static_cast<long long>(B) * S_in;
   return static_cast<int>(want < 1 ? 1 : want > T ? T : want);
+}
+
+// The row widths a kernel family is instantiated for.  dispatch() calls f(bf16, n) with both as compile-time
+// constants (std::bool_constant, std::integral_constant) and returns its result; check() first.
+template <int... Ns>
+struct Dims {
+  static int check(int n) {
+    SVGB_REQUIRE(((n == Ns) || ...), "Unsupported head_dim: %d", n);
+    return 0;
+  }
+};
+using NormDims = Dims<32, 64, 128, 256>;  // the row norms: n
+using HeadDims = Dims<64, 128, 256>;      // RoPE and the fused prep: D
+
+template <int... Ns, class F>
+static int dispatch(Dims<Ns...>, int dtype, int n, F&& f) {
+  int rc = 0;
+  const auto run = [&](auto N) { rc = dtype == SVGB_BF16 ? f(std::true_type{}, N) : f(std::false_type{}, N); };
+  ((n == Ns ? run(std::integral_constant<int, Ns>{}) : void()), ...);
+  return rc;
 }
 
 static int launch_column_sum(const float* const* in, float* const* out, int n, long long stride, int rows, int cols,
@@ -774,187 +723,48 @@ static int launch_column_sum(const float* const* in, float* const* out, int n, l
   return 0;
 }
 
-template <bool BF16, bool kLayer>
-static int launch_row_norm_bwd(const void* x, const void* dy, const void* gamma, void* dx, float* dgamma,
-                               float* dbeta, float eps, long long m, int n, float* part, cudaStream_t st) {
-  const int blocks = row_norm_bwd_blocks(m, n);
-  auto X = static_cast<const uint4*>(x);
-  auto DY = static_cast<const uint4*>(dy);
-  auto G = static_cast<const uint4*>(gamma);
-  auto DX = static_cast<uint4*>(dx);
-  switch (n) {
-    case 32: row_norm_bwd_kernel<BF16, 32, kLayer><<<blocks, kThreads, 0, st>>>(X, DY, G, DX, eps, m, part); break;
-    case 64: row_norm_bwd_kernel<BF16, 64, kLayer><<<blocks, kThreads, 0, st>>>(X, DY, G, DX, eps, m, part); break;
-    case 128: row_norm_bwd_kernel<BF16, 128, kLayer><<<blocks, kThreads, 0, st>>>(X, DY, G, DX, eps, m, part); break;
-    default: row_norm_bwd_kernel<BF16, 256, kLayer><<<blocks, kThreads, 0, st>>>(X, DY, G, DX, eps, m, part); break;
-  }
-  SVGB_LAUNCH_OK();
-  const float* in[2] = {part, part + n};
-  float* out[2] = {dgamma, dbeta};
-  return launch_column_sum(in, out, kLayer ? 2 : 1, 2LL * n, blocks, n, st);
-}
-
-template <bool BF16, bool kComplex>
-static int launch_rope_bwd(const void* dq, const void* dk, void* gq, void* gk, const float* c, const float* s, int B,
-                           int Hq, int Hk, int S, int D, int row0, int valid, cudaStream_t st) {
-  const int rpb = kThreads / (D / 8);
-  dim3 grid((S + rpb - 1) / rpb, B);
-  auto Q = static_cast<const uint4*>(dq);
-  auto K = static_cast<const uint4*>(dk);
-  auto GQ = static_cast<uint4*>(gq);
-  auto GK = static_cast<uint4*>(gk);
-  switch (D) {
-    case 64: qk_rope_bwd_kernel<BF16, 64, kComplex><<<grid, kThreads, 0, st>>>(Q, K, GQ, GK, c, s, Hq, Hk, S, row0, valid); break;
-    case 128: qk_rope_bwd_kernel<BF16, 128, kComplex><<<grid, kThreads, 0, st>>>(Q, K, GQ, GK, c, s, Hq, Hk, S, row0, valid); break;
-    default: qk_rope_bwd_kernel<BF16, 256, kComplex><<<grid, kThreads, 0, st>>>(Q, K, GQ, GK, c, s, Hq, Hk, S, row0, valid); break;
-  }
-  SVGB_LAUNCH_OK();
-  return 0;
-}
-
 template <bool BF16, int D>
 static int launch_prep_bwd(const PrepBwdArgs& a, int B, cudaStream_t st) {
-  const int gx = prep_bwd_blocks(B, a.S_in, D);
+  const int gx = prep_bwd_blocks(B, a.geo.S_in, D);
   qkv_prep_bwd_kernel<BF16, D><<<dim3(gx, B, 3), kThreads, 0, st>>>(a);
   SVGB_LAUNCH_OK();
-  if (a.norm == SVGB_NORM_RMS_HIDDEN) {
-    const int splits = hidden_splits(B, a.S_in, a.H, D);
-    hidden_rms_bwd_kernel<BF16, D><<<dim3(hidden_cols(a.H, D), splits, 2), kHiddenThreads, 0, st>>>(a, B);
+  if (a.geo.norm == SVGB_NORM_RMS_HIDDEN) {
+    const int splits = hidden_splits(B, a.geo.S_in, a.geo.H, D);
+    hidden_rms_bwd_kernel<BF16, D><<<dim3(hidden_cols(a.geo.H, D), splits, 2), kHiddenThreads, 0, st>>>(a, B);
     SVGB_LAUNCH_OK();
   }
   return 0;
 }
 
-}  // namespace svgb
-
-using namespace svgb;
-
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" {
-
-int svgb_rms_norm(void* x, const void* gamma, long long m, int n, float eps, int dtype, void* stream) {
-  SVGB_REQUIRE(x && gamma && m >= 0, "null pointer");
-  SVGB_REQUIRE(n == 32 || n == 64 || n == 128 || n == 256, "Unsupported head_dim: %d", n);
+// svgb_rms_norm / svgb_layer_norm (layer: beta, and eps is LayerNorm's fixed 1e-5)
+static int row_norm(void* x, const void* gamma, const void* beta, long long m, int n, float eps, int dtype,
+                    bool layer, void* stream) {
+  SVGB_REQUIRE(x && gamma && (beta || !layer) && m >= 0, "null pointer");
+  if (NormDims::check(n)) return -1;
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
-  SVGB_REQUIRE(aligned16(x) && aligned16(gamma), "pointers must be 16-byte aligned");
+  SVGB_REQUIRE(aligned16(x) && aligned16(gamma) && (!layer || aligned16(beta)), "pointers must be 16-byte aligned");
   if (m == 0) return 0;
+  const unsigned blocks = row_blocks(m, n, 148 * 32);
+  auto X = static_cast<uint4*>(x);
+  auto G = static_cast<const uint4*>(gamma);
+  auto Bt = static_cast<const uint4*>(beta);
   auto st = static_cast<cudaStream_t>(stream);
-  return dtype == SVGB_BF16 ? launch_row_norm<true, false>(x, gamma, nullptr, eps, m, n, st)
-                            : launch_row_norm<false, false>(x, gamma, nullptr, eps, m, n, st);
+  return dispatch(NormDims{}, dtype, n, [&](auto bf, auto N) {
+    const auto kernel = layer ? row_norm_kernel<bf, N, true> : row_norm_kernel<bf, N, false>;
+    kernel<<<blocks, kThreads, 0, st>>>(X, G, Bt, eps, m);
+    SVGB_LAUNCH_OK();
+    return 0;
+  });
 }
 
-int svgb_layer_norm(void* x, const void* gamma, const void* beta, long long m, int n, int dtype, void* stream) {
-  SVGB_REQUIRE(x && gamma && beta && m >= 0, "null pointer");
-  SVGB_REQUIRE(n == 32 || n == 64 || n == 128 || n == 256, "Unsupported head_dim: %d", n);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
-  SVGB_REQUIRE(aligned16(x) && aligned16(gamma) && aligned16(beta), "pointers must be 16-byte aligned");
-  if (m == 0) return 0;
-  auto st = static_cast<cudaStream_t>(stream);
-  return dtype == SVGB_BF16 ? launch_row_norm<true, true>(x, gamma, beta, 0.f, m, n, st)
-                            : launch_row_norm<false, true>(x, gamma, beta, 0.f, m, n, st);
-}
-
-int svgb_qk_rope(void* q, void* k, const float* cos_t, const float* sin_t, int B, int Hq, int Hk, int S, int D,
-                 int len_text, int mode, int dtype, void* stream) {
-  SVGB_REQUIRE(q && k && cos_t && sin_t, "null pointer");
-  SVGB_REQUIRE(B > 0 && Hq > 0 && Hk > 0 && S > 0, "bad sizes");
-  SVGB_REQUIRE(D == 64 || D == 128 || D == 256, "Unsupported head_dim: %d", D);
-  SVGB_REQUIRE(len_text >= 0 && len_text < S, "len_text_prompt must leave at least one rotated row");
-  SVGB_REQUIRE(mode >= SVGB_ROPE_TXT_FIRST && mode <= SVGB_ROPE_COMPLEX_TXT_FIRST, "mode %d unknown", mode);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
-  SVGB_REQUIRE(aligned16(q) && aligned16(k) && aligned16(cos_t) && aligned16(sin_t), "pointers must be 16-byte aligned");
-  const int valid = S - len_text;
-  const int row0 = mode == SVGB_ROPE_TXT_LAST ? 0 : len_text;
-  auto st = static_cast<cudaStream_t>(stream);
-  if (mode == SVGB_ROPE_COMPLEX_TXT_FIRST)
-    return dtype == SVGB_BF16 ? launch_rope<true, true>(q, k, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st)
-                              : launch_rope<false, true>(q, k, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st);
-  return dtype == SVGB_BF16 ? launch_rope<true, false>(q, k, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st)
-                            : launch_rope<false, false>(q, k, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st);
-}
-
-int svgb_qkv_prep(const void* q_in, const void* k_in, const void* v_in, long long in_token_stride,
-                  long long in_batch_stride, void* q_out, void* k_out, void* v_out, long long out_head_stride,
-                  long long out_batch_stride, int B, int S_in, int H, int D, int out_row0, int norm,
-                  const void* gamma_q, const void* gamma_k, const void* beta_q, const void* beta_k, float eps,
-                  int rope, const float* cos_t, const float* sin_t, int rope_lo, int rope_n, int dtype,
-                  void* stream) {
-  SVGB_REQUIRE(q_in && k_in && v_in && q_out && k_out && v_out, "null pointer");
-  SVGB_REQUIRE(B > 0 && S_in > 0 && H > 0 && out_row0 >= 0, "bad sizes");
-  SVGB_REQUIRE(D == 64 || D == 128 || D == 256, "Unsupported head_dim: %d", D);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
-  SVGB_REQUIRE(norm >= SVGB_NORM_NONE && norm <= SVGB_NORM_RMS_HIDDEN, "norm %d unknown", norm);
-  SVGB_REQUIRE(norm == SVGB_NORM_NONE || (gamma_q && gamma_k), "norm needs gamma_q and gamma_k");
-  SVGB_REQUIRE(norm != SVGB_NORM_LAYER || (beta_q && beta_k), "layer norm needs beta_q and beta_k");
-  SVGB_REQUIRE(rope >= 0 && rope <= 2, "rope %d unknown (0 none, 1 cos/sin [n,D], 2 complex [n,D/2])", rope);
-  SVGB_REQUIRE(rope == 0 || (cos_t && sin_t && rope_lo >= 0 && rope_n >= 0 && rope_lo + rope_n <= S_in),
-               "rope needs tables and a token range inside [0, S_in)");
-  SVGB_REQUIRE(in_token_stride % 8 == 0 && in_batch_stride % 8 == 0 && out_head_stride % 8 == 0 &&
-                   out_batch_stride % 8 == 0,
-               "strides must be multiples of 8 elements (16 bytes)");
-  SVGB_REQUIRE(aligned16(q_in) && aligned16(k_in) && aligned16(v_in) && aligned16(q_out) && aligned16(k_out) &&
-                   aligned16(v_out),
-               "pointers must be 16-byte aligned");
-  PrepArgs a;
-  a.in[0] = static_cast<const uint16_t*>(q_in);
-  a.in[1] = static_cast<const uint16_t*>(k_in);
-  a.in[2] = static_cast<const uint16_t*>(v_in);
-  a.out[0] = static_cast<uint16_t*>(q_out);
-  a.out[1] = static_cast<uint16_t*>(k_out);
-  a.out[2] = static_cast<uint16_t*>(v_out);
-  a.gamma[0] = static_cast<const uint16_t*>(gamma_q);
-  a.gamma[1] = static_cast<const uint16_t*>(gamma_k);
-  a.beta[0] = static_cast<const uint16_t*>(beta_q);
-  a.beta[1] = static_cast<const uint16_t*>(beta_k);
-  a.cos_t = cos_t;
-  a.sin_t = sin_t;
-  a.in_token_stride = in_token_stride;
-  a.in_batch_stride = in_batch_stride;
-  a.out_head_stride = out_head_stride;
-  a.out_batch_stride = out_batch_stride;
-  a.S_in = S_in;
-  a.H = H;
-  a.out_row0 = out_row0;
-  a.norm = norm;
-  a.rope = rope;
-  a.rope_lo = rope_lo;
-  a.rope_n = rope_n;
-  a.eps = eps;
-  const int rpb = kThreads / (D / 8);
-  dim3 grid((S_in + rpb - 1) / rpb, B, 3);
-  auto st = static_cast<cudaStream_t>(stream);
-  const bool bf = dtype == SVGB_BF16;
-  switch (D) {
-    case 64:
-      if (bf) qkv_prep_kernel<true, 64><<<grid, kThreads, 0, st>>>(a);
-      else qkv_prep_kernel<false, 64><<<grid, kThreads, 0, st>>>(a);
-      break;
-    case 128:
-      if (bf) qkv_prep_kernel<true, 128><<<grid, kThreads, 0, st>>>(a);
-      else qkv_prep_kernel<false, 128><<<grid, kThreads, 0, st>>>(a);
-      break;
-    default:
-      if (bf) qkv_prep_kernel<true, 256><<<grid, kThreads, 0, st>>>(a);
-      else qkv_prep_kernel<false, 256><<<grid, kThreads, 0, st>>>(a);
-      break;
-  }
-  SVGB_LAUNCH_OK();
-  return 0;
-}
-
-int svgb_row_norm_bwd_bytes(long long m, int n, size_t* bytes) {
-  SVGB_REQUIRE(bytes && m >= 0, "bad arguments");
-  SVGB_REQUIRE(n == 32 || n == 64 || n == 128 || n == 256, "Unsupported head_dim: %d", n);
-  *bytes = align_up(sizeof(float) * 2 * n * static_cast<size_t>(row_norm_bwd_blocks(m, n)), 256);
-  return 0;
-}
-
+// svgb_rms_norm_bwd / svgb_layer_norm_bwd
 static int row_norm_bwd(const void* x, const void* dy, const void* gamma, void* dx, float* dgamma, float* dbeta,
                         long long m, int n, float eps, int dtype, bool layer, void* ws, size_t ws_bytes,
                         void* stream) {
   SVGB_REQUIRE(x && dy && gamma && dx && dgamma && (dbeta || !layer) && m >= 0, "null pointer");
-  SVGB_REQUIRE(n == 32 || n == 64 || n == 128 || n == 256, "Unsupported head_dim: %d", n);
+  if (NormDims::check(n)) return -1;
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
   SVGB_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(gamma) && aligned16(dx), "pointers must be 16-byte aligned");
   size_t need = 0;
@@ -966,12 +776,139 @@ static int row_norm_bwd(const void* x, const void* dy, const void* gamma, void* 
     if (layer) SVGB_CUDA(cudaMemsetAsync(dbeta, 0, sizeof(float) * n, st));
     return 0;
   }
+  const int blocks = row_blocks(m, n, kBwdCtas);
+  auto X = static_cast<const uint4*>(x);
+  auto DY = static_cast<const uint4*>(dy);
+  auto G = static_cast<const uint4*>(gamma);
+  auto DX = static_cast<uint4*>(dx);
   auto part = static_cast<float*>(ws);
-  if (layer)
-    return dtype == SVGB_BF16 ? launch_row_norm_bwd<true, true>(x, dy, gamma, dx, dgamma, dbeta, 0.f, m, n, part, st)
-                              : launch_row_norm_bwd<false, true>(x, dy, gamma, dx, dgamma, dbeta, 0.f, m, n, part, st);
-  return dtype == SVGB_BF16 ? launch_row_norm_bwd<true, false>(x, dy, gamma, dx, dgamma, nullptr, eps, m, n, part, st)
-                            : launch_row_norm_bwd<false, false>(x, dy, gamma, dx, dgamma, nullptr, eps, m, n, part, st);
+  const int rc = dispatch(NormDims{}, dtype, n, [&](auto bf, auto N) {
+    const auto kernel = layer ? row_norm_bwd_kernel<bf, N, true> : row_norm_bwd_kernel<bf, N, false>;
+    kernel<<<blocks, kThreads, 0, st>>>(X, DY, G, DX, eps, m, part);
+    SVGB_LAUNCH_OK();
+    return 0;
+  });
+  if (rc) return rc;
+  const float* in[2] = {part, part + n};
+  float* out[2] = {dgamma, dbeta};
+  return launch_column_sum(in, out, layer ? 2 : 1, 2LL * n, blocks, n, st);
+}
+
+// svgb_qk_rope (in place: q_out = q, k_out = k) / svgb_qk_rope_bwd (transpose: the RoPE transpose, out of place)
+static int qk_rope(const void* q, const void* k, void* q_out, void* k_out, const float* cos_t, const float* sin_t,
+                   int B, int Hq, int Hk, int S, int D, int len_text, int mode, int dtype, bool transpose,
+                   void* stream) {
+  SVGB_REQUIRE(q && k && q_out && k_out && cos_t && sin_t, "null pointer");
+  SVGB_REQUIRE(B > 0 && Hq > 0 && Hk > 0 && S > 0, "bad sizes");
+  if (HeadDims::check(D)) return -1;
+  SVGB_REQUIRE(len_text >= 0 && len_text < S, "len_text_prompt must leave at least one rotated row");
+  SVGB_REQUIRE(mode >= SVGB_ROPE_TXT_FIRST && mode <= SVGB_ROPE_COMPLEX_TXT_FIRST, "mode %d unknown", mode);
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
+  SVGB_REQUIRE(aligned16(q) && aligned16(k) && aligned16(q_out) && aligned16(k_out) && aligned16(cos_t) &&
+                   aligned16(sin_t),
+               "pointers must be 16-byte aligned");
+  const int valid = S - len_text;
+  const int row0 = mode == SVGB_ROPE_TXT_LAST ? 0 : len_text;
+  const bool complex = mode == SVGB_ROPE_COMPLEX_TXT_FIRST;
+  const int rpb = kThreads / (D / 8);
+  const dim3 grid(((transpose ? S : valid) + rpb - 1) / rpb, B);
+  auto Q = static_cast<const uint4*>(q);
+  auto K = static_cast<const uint4*>(k);
+  auto QO = static_cast<uint4*>(q_out);
+  auto KO = static_cast<uint4*>(k_out);
+  auto st = static_cast<cudaStream_t>(stream);
+  return dispatch(HeadDims{}, dtype, D, [&](auto bf, auto d) {
+    if (transpose) {
+      const auto kernel = complex ? qk_rope_bwd_kernel<bf, d, true> : qk_rope_bwd_kernel<bf, d, false>;
+      kernel<<<grid, kThreads, 0, st>>>(Q, K, QO, KO, cos_t, sin_t, Hq, Hk, S, row0, valid);
+    } else {
+      const auto kernel = complex ? qk_rope_kernel<bf, d, true> : qk_rope_kernel<bf, d, false>;
+      kernel<<<grid, kThreads, 0, st>>>(QO, KO, cos_t, sin_t, Hq, Hk, S, row0, valid);
+    }
+    SVGB_LAUNCH_OK();
+    return 0;
+  });
+}
+
+// The checks svgb_qkv_prep and svgb_qkv_prep_bwd share, and the geometry they pass to the kernels.
+static int prep_geom(PrepGeom& g, long long in_token_stride, long long in_batch_stride, long long out_head_stride,
+                     long long out_batch_stride, int B, int S_in, int H, int D, int out_row0, int norm, float eps,
+                     int rope, const float* cos_t, const float* sin_t, int rope_lo, int rope_n, int dtype) {
+  SVGB_REQUIRE(B > 0 && S_in > 0 && H > 0 && out_row0 >= 0, "bad sizes");
+  if (HeadDims::check(D)) return -1;
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
+  SVGB_REQUIRE(norm >= SVGB_NORM_NONE && norm <= SVGB_NORM_RMS_HIDDEN, "norm %d unknown", norm);
+  SVGB_REQUIRE(rope >= 0 && rope <= 2, "rope %d unknown (0 none, 1 cos/sin [n,D], 2 complex [n,D/2])", rope);
+  SVGB_REQUIRE(rope == 0 || (cos_t && sin_t && rope_lo >= 0 && rope_n >= 0 && rope_lo + rope_n <= S_in),
+               "rope needs tables and a token range inside [0, S_in)");
+  SVGB_REQUIRE(in_token_stride % 8 == 0 && in_batch_stride % 8 == 0 && out_head_stride % 8 == 0 &&
+                   out_batch_stride % 8 == 0,
+               "strides must be multiples of 8 elements (16 bytes)");
+  g = PrepGeom{cos_t,    sin_t, in_token_stride, in_batch_stride, out_head_stride, out_batch_stride, S_in, H,
+               out_row0, norm,  rope,            rope_lo,         rope_n,          eps};
+  return 0;
+}
+
+}  // namespace svgb
+
+using namespace svgb;
+
+extern "C" {
+
+int svgb_rms_norm(void* x, const void* gamma, long long m, int n, float eps, int dtype, void* stream) {
+  return row_norm(x, gamma, nullptr, m, n, eps, dtype, false, stream);
+}
+
+int svgb_layer_norm(void* x, const void* gamma, const void* beta, long long m, int n, int dtype, void* stream) {
+  return row_norm(x, gamma, beta, m, n, 0.f, dtype, true, stream);
+}
+
+int svgb_qk_rope(void* q, void* k, const float* cos_t, const float* sin_t, int B, int Hq, int Hk, int S, int D,
+                 int len_text, int mode, int dtype, void* stream) {
+  return qk_rope(q, k, q, k, cos_t, sin_t, B, Hq, Hk, S, D, len_text, mode, dtype, false, stream);
+}
+
+int svgb_qkv_prep(const void* q_in, const void* k_in, const void* v_in, long long in_token_stride,
+                  long long in_batch_stride, void* q_out, void* k_out, void* v_out, long long out_head_stride,
+                  long long out_batch_stride, int B, int S_in, int H, int D, int out_row0, int norm,
+                  const void* gamma_q, const void* gamma_k, const void* beta_q, const void* beta_k, float eps,
+                  int rope, const float* cos_t, const float* sin_t, int rope_lo, int rope_n, int dtype,
+                  void* stream) {
+  SVGB_REQUIRE(q_in && k_in && v_in && q_out && k_out && v_out, "null pointer");
+  PrepArgs a;
+  if (prep_geom(a.geo, in_token_stride, in_batch_stride, out_head_stride, out_batch_stride, B, S_in, H, D, out_row0,
+                norm, eps, rope, cos_t, sin_t, rope_lo, rope_n, dtype))
+    return -1;
+  SVGB_REQUIRE(norm == SVGB_NORM_NONE || (gamma_q && gamma_k), "norm needs gamma_q and gamma_k");
+  SVGB_REQUIRE(norm != SVGB_NORM_LAYER || (beta_q && beta_k), "layer norm needs beta_q and beta_k");
+  SVGB_REQUIRE(aligned16(q_in) && aligned16(k_in) && aligned16(v_in) && aligned16(q_out) && aligned16(k_out) &&
+                   aligned16(v_out),
+               "pointers must be 16-byte aligned");
+  a.in[0] = static_cast<const uint16_t*>(q_in);
+  a.in[1] = static_cast<const uint16_t*>(k_in);
+  a.in[2] = static_cast<const uint16_t*>(v_in);
+  a.out[0] = static_cast<uint16_t*>(q_out);
+  a.out[1] = static_cast<uint16_t*>(k_out);
+  a.out[2] = static_cast<uint16_t*>(v_out);
+  a.gamma[0] = static_cast<const uint16_t*>(gamma_q);
+  a.gamma[1] = static_cast<const uint16_t*>(gamma_k);
+  a.beta[0] = static_cast<const uint16_t*>(beta_q);
+  a.beta[1] = static_cast<const uint16_t*>(beta_k);
+  const int rpb = kThreads / (D / 8);
+  const dim3 grid((S_in + rpb - 1) / rpb, B, 3);
+  auto st = static_cast<cudaStream_t>(stream);
+  return dispatch(HeadDims{}, dtype, D, [&](auto bf, auto d) {
+    qkv_prep_kernel<bf, d><<<grid, kThreads, 0, st>>>(a);
+    SVGB_LAUNCH_OK();
+    return 0;
+  });
+}
+
+int svgb_row_norm_bwd_bytes(long long m, int n, size_t* bytes) {
+  SVGB_REQUIRE(bytes && m >= 0, "bad arguments");
+  if (NormDims::check(n)) return -1;
+  *bytes = align_up(sizeof(float) * 2 * n * static_cast<size_t>(row_blocks(m, n, kBwdCtas)), 256);
+  return 0;
 }
 
 int svgb_rms_norm_bwd(const void* x, const void* dy, const void* gamma, void* dx, float* dgamma, long long m, int n,
@@ -987,30 +924,12 @@ int svgb_layer_norm_bwd(const void* x, const void* dy, const void* gamma, void* 
 int svgb_qk_rope_bwd(const void* dq, const void* dk, void* dq_out, void* dk_out, const float* cos_t,
                      const float* sin_t, int B, int Hq, int Hk, int S, int D, int len_text, int mode, int dtype,
                      void* stream) {
-  SVGB_REQUIRE(dq && dk && dq_out && dk_out && cos_t && sin_t, "null pointer");
-  SVGB_REQUIRE(B > 0 && Hq > 0 && Hk > 0 && S > 0, "bad sizes");
-  SVGB_REQUIRE(D == 64 || D == 128 || D == 256, "Unsupported head_dim: %d", D);
-  SVGB_REQUIRE(len_text >= 0 && len_text < S, "len_text_prompt must leave at least one rotated row");
-  SVGB_REQUIRE(mode >= SVGB_ROPE_TXT_FIRST && mode <= SVGB_ROPE_COMPLEX_TXT_FIRST, "mode %d unknown", mode);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
-  SVGB_REQUIRE(aligned16(dq) && aligned16(dk) && aligned16(dq_out) && aligned16(dk_out) && aligned16(cos_t) &&
-                   aligned16(sin_t),
-               "pointers must be 16-byte aligned");
-  const int valid = S - len_text;
-  const int row0 = mode == SVGB_ROPE_TXT_LAST ? 0 : len_text;
-  auto st = static_cast<cudaStream_t>(stream);
-  if (mode == SVGB_ROPE_COMPLEX_TXT_FIRST)
-    return dtype == SVGB_BF16
-               ? launch_rope_bwd<true, true>(dq, dk, dq_out, dk_out, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st)
-               : launch_rope_bwd<false, true>(dq, dk, dq_out, dk_out, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st);
-  return dtype == SVGB_BF16
-             ? launch_rope_bwd<true, false>(dq, dk, dq_out, dk_out, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st)
-             : launch_rope_bwd<false, false>(dq, dk, dq_out, dk_out, cos_t, sin_t, B, Hq, Hk, S, D, row0, valid, st);
+  return qk_rope(dq, dk, dq_out, dk_out, cos_t, sin_t, B, Hq, Hk, S, D, len_text, mode, dtype, true, stream);
 }
 
 int svgb_qkv_prep_bwd_bytes(int B, int S_in, int H, int D, int norm, size_t* bytes) {
   SVGB_REQUIRE(bytes && B > 0 && S_in > 0 && H > 0, "bad arguments");
-  SVGB_REQUIRE(D == 64 || D == 128 || D == 256, "Unsupported head_dim: %d", D);
+  if (HeadDims::check(D)) return -1;
   SVGB_REQUIRE(norm >= SVGB_NORM_NONE && norm <= SVGB_NORM_RMS_HIDDEN, "norm %d unknown", norm);
   size_t n = 0;
   if (norm == SVGB_NORM_RMS_HEAD || norm == SVGB_NORM_LAYER)  // q, k: [blocks * B][dgamma | dbeta]
@@ -1030,26 +949,19 @@ int svgb_qkv_prep_bwd(const void* dq, const void* dk, const void* dv, long long 
                       float* dgamma_k, float* dbeta_q, float* dbeta_k, int dtype, void* ws, size_t ws_bytes,
                       void* stream) {
   SVGB_REQUIRE(dq && dk && dv && dq_in && dk_in && dv_in, "null pointer");
-  SVGB_REQUIRE(B > 0 && S_in > 0 && H > 0 && out_row0 >= 0, "bad sizes");
-  SVGB_REQUIRE(D == 64 || D == 128 || D == 256, "Unsupported head_dim: %d", D);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "dtype %d unsupported", dtype);
-  SVGB_REQUIRE(norm >= SVGB_NORM_NONE && norm <= SVGB_NORM_RMS_HIDDEN, "norm %d unknown", norm);
+  PrepBwdArgs a{};
+  if (prep_geom(a.geo, in_token_stride, in_batch_stride, out_head_stride, out_batch_stride, B, S_in, H, D, out_row0,
+                norm, eps, rope, cos_t, sin_t, rope_lo, rope_n, dtype))
+    return -1;
   SVGB_REQUIRE(norm == SVGB_NORM_NONE || (q_in && k_in && gamma_q && gamma_k && dgamma_q && dgamma_k),
                "norm needs q_in, k_in, gamma_q, gamma_k, dgamma_q and dgamma_k");
   SVGB_REQUIRE(norm != SVGB_NORM_LAYER || (dbeta_q && dbeta_k), "layer norm needs dbeta_q and dbeta_k");
-  SVGB_REQUIRE(rope >= 0 && rope <= 2, "rope %d unknown (0 none, 1 cos/sin [n,D], 2 complex [n,D/2])", rope);
-  SVGB_REQUIRE(rope == 0 || (cos_t && sin_t && rope_lo >= 0 && rope_n >= 0 && rope_lo + rope_n <= S_in),
-               "rope needs tables and a token range inside [0, S_in)");
-  SVGB_REQUIRE(in_token_stride % 8 == 0 && in_batch_stride % 8 == 0 && out_head_stride % 8 == 0 &&
-                   out_batch_stride % 8 == 0,
-               "strides must be multiples of 8 elements (16 bytes)");
   SVGB_REQUIRE(aligned16(dq) && aligned16(dk) && aligned16(dv) && aligned16(dq_in) && aligned16(dk_in) &&
                    aligned16(dv_in) && (norm == SVGB_NORM_NONE || (aligned16(q_in) && aligned16(k_in))),
                "pointers must be 16-byte aligned");
   size_t need = 0;
   if (svgb_qkv_prep_bwd_bytes(B, S_in, H, D, norm, &need)) return -1;
   SVGB_REQUIRE(need == 0 || (ws && ws_bytes >= need), "backward workspace too small: %zu < %zu", ws_bytes, need);
-  PrepBwdArgs a{};
   a.dy[0] = static_cast<const uint16_t*>(dq);
   a.dy[1] = static_cast<const uint16_t*>(dk);
   a.dy[2] = static_cast<const uint16_t*>(dv);
@@ -1060,20 +972,6 @@ int svgb_qkv_prep_bwd(const void* dq, const void* dk, const void* dv, long long 
   a.dx[2] = static_cast<uint16_t*>(dv_in);
   a.gamma[0] = static_cast<const uint16_t*>(gamma_q);
   a.gamma[1] = static_cast<const uint16_t*>(gamma_k);
-  a.cos_t = cos_t;
-  a.sin_t = sin_t;
-  a.in_token_stride = in_token_stride;
-  a.in_batch_stride = in_batch_stride;
-  a.out_head_stride = out_head_stride;
-  a.out_batch_stride = out_batch_stride;
-  a.S_in = S_in;
-  a.H = H;
-  a.out_row0 = out_row0;
-  a.norm = norm;
-  a.rope = rope;
-  a.rope_lo = rope_lo;
-  a.rope_n = rope_n;
-  a.eps = eps;
   // workspace: the q then the k partials, each need / 2 (NORM_RMS_HIDDEN: partials, then stats)
   auto base = static_cast<char*>(ws);
   long long rows = 0, stride = 0;
@@ -1095,13 +993,7 @@ int svgb_qkv_prep_bwd(const void* dq, const void* dk, const void* dv, long long 
     a.stats[1] = reinterpret_cast<float2*>(base + 2 * pb + align_up(sizeof(float) * 2 * static_cast<size_t>(B) * S_in, 256));
   }
   auto st = static_cast<cudaStream_t>(stream);
-  const bool bf = dtype == SVGB_BF16;
-  int rc;
-  switch (D) {
-    case 64: rc = bf ? launch_prep_bwd<true, 64>(a, B, st) : launch_prep_bwd<false, 64>(a, B, st); break;
-    case 128: rc = bf ? launch_prep_bwd<true, 128>(a, B, st) : launch_prep_bwd<false, 128>(a, B, st); break;
-    default: rc = bf ? launch_prep_bwd<true, 256>(a, B, st) : launch_prep_bwd<false, 256>(a, B, st); break;
-  }
+  const int rc = dispatch(HeadDims{}, dtype, D, [&](auto bf, auto d) { return launch_prep_bwd<bf, d>(a, B, st); });
   if (rc || norm == SVGB_NORM_NONE) return rc;
   const float* in[4] = {a.part[0], a.part[0] + D, a.part[1], a.part[1] + D};
   float* out[4] = {dgamma_q, norm == SVGB_NORM_LAYER ? dbeta_q : nullptr, dgamma_k,

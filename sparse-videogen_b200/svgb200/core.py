@@ -139,28 +139,26 @@ def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.T
     return AttnPlan(desc, ws, None if gather else (m, r, c, (m._version, r._version, c._version)))
 
 
-def plan_band(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device) -> AttnPlan:
+def _plan_band(bytes_fn, plan_fn, name, mask_mode, m0, m1, m2, BH, S, device) -> AttnPlan:
     nbytes = C.c_size_t()
-    check(lib().svgb_attn_plan_band_bytes(S, C.byref(nbytes)), "plan_band_bytes")
+    check(bytes_fn(S, C.byref(nbytes)), f"{name}_bytes")
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan (long-lived)
     desc = Plan()
-    check(lib().svgb_attn_plan_band(mask_mode, m0, m1, m2, BH, S, ws.data_ptr(), ws.numel(),
-                                    C.byref(desc), torch.cuda.current_stream(device).cuda_stream),
-          "svgb_attn_plan_band")
+    check(plan_fn(mask_mode, m0, m1, m2, BH, S, ws.data_ptr(), ws.numel(), C.byref(desc),
+                  torch.cuda.current_stream(device).cuda_stream), f"svgb_attn_{name}")
     _bump()
     return AttnPlan(desc, ws)
+
+
+def plan_band(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device) -> AttnPlan:
+    return _plan_band(lib().svgb_attn_plan_band_bytes, lib().svgb_attn_plan_band, "plan_band", mask_mode, m0, m1, m2,
+                      BH, S, device)
 
 
 def plan_band_t(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, device) -> AttnPlan:
     """Key-major form of plan_band's mask (include/svgb200.h svgb_attn_plan_band_t), for attn_bwd."""
-    nbytes = C.c_size_t()
-    check(lib().svgb_attn_plan_band_t_bytes(S, C.byref(nbytes)), "plan_band_t_bytes")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
-    desc = Plan()
-    check(lib().svgb_attn_plan_band_t(mask_mode, m0, m1, m2, BH, S, ws.data_ptr(), ws.numel(), C.byref(desc),
-                                      torch.cuda.current_stream(device).cuda_stream), "svgb_attn_plan_band_t")
-    _bump()
-    return AttnPlan(desc, ws)
+    return _plan_band(lib().svgb_attn_plan_band_t_bytes, lib().svgb_attn_plan_band_t, "plan_band_t", mask_mode, m0,
+                      m1, m2, BH, S, device)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -178,6 +176,16 @@ def _attn(q, k, v, scales, o, dtype, plan, BH, S, D, rs, hs, o_rows, q_rows, kv_
     return (o, lse) if return_lse else o
 
 
+def _geometry(q, layout):
+    if layout == "bhsd":
+        B, H, S, D = q.shape
+        return B * H, S, D, D, S * D
+    if layout == "shd":
+        S, H, D = q.shape
+        return H, S, D, H * D, D
+    raise SvgbError(f"unknown layout {layout}")
+
+
 def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[torch.Tensor] = None,
              q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
              return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
@@ -189,27 +197,10 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
         raise SvgbError("q, k, v must be contiguous")
     if not (q.dtype == k.dtype == v.dtype) or not (q.shape == k.shape == v.shape):
         raise SvgbError("q, k, v must share dtype and shape")
-    if layout == "bhsd":
-        B, H, S, D = q.shape
-        BH, rs, hs = B * H, D, S * D
-    elif layout == "shd":
-        S, H, D = q.shape
-        BH, rs, hs = H, H * D, D
-    else:
-        raise SvgbError(f"unknown layout {layout}")
+    BH, S, D, rs, hs = _geometry(q, layout)
     o = torch.empty_like(q) if out is None else out
     return _attn(q, k, v, (None, None, None), o, _dt(q), plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows,
                  return_lse, sm_scale)
-
-
-def _geometry(q, layout):
-    if layout == "bhsd":
-        B, H, S, D = q.shape
-        return B * H, S, D, D, S * D
-    if layout == "shd":
-        S, H, D = q.shape
-        return H, S, D, H * D, D
-    raise SvgbError(f"unknown layout {layout}")
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
@@ -763,6 +754,28 @@ def qk_rope_(q: torch.Tensor, k: torch.Tensor, cos: torch.Tensor, sin: torch.Ten
     return q, k
 
 
+def _check_tables_and_weights(D, HD, dtype, norm, rope, cos, sin, rope_n, weights):
+    """The checks qkv_prep and qkv_prep_bwd share.  RoPE tables: float32, contiguous, [rope_n, D] (complex mode:
+    [rope_n, D/2]), rope_n defaulting to the tables' rows.  weights: (name, tensor or None) pairs of norm weights, each
+    contiguous [D] (NORM_RMS_HIDDEN: [H*D]) of dtype.  Returns rope_n (0 without RoPE)."""
+    if rope:
+        if cos is None or sin is None or cos.dtype != torch.float32 or sin.dtype != torch.float32:
+            raise SvgbError("rope needs float32 cos / sin tables")
+        _contig(cos, sin)
+        if rope_n is None:
+            rope_n = cos.shape[0]
+        width = D // 2 if rope == 2 else D
+        if tuple(cos.shape) != (rope_n, width) or tuple(sin.shape) != (rope_n, width):
+            raise SvgbError(f"cos / sin must be [{rope_n}, {width}]")
+    else:
+        rope_n = 0
+    want = HD if norm == NORM_RMS_HIDDEN else D
+    for name, g in weights:
+        if g is not None and (g.dtype != dtype or g.numel() != want or not g.is_contiguous()):
+            raise SvgbError(f"{name} must be contiguous [{want}] of the input dtype")
+    return rope_n
+
+
 def qkv_prep_bwd(dq, dk, dv, heads: int, S_in: int, *, q_in=None, k_in=None, out_row0: int = 0,
                  norm: int = NORM_NONE, gamma_q=None, gamma_k=None, eps: float = 1e-6, rope: int = 0, cos=None,
                  sin=None, rope_lo: int = 0, rope_n: Optional[int] = None):
@@ -785,21 +798,8 @@ def qkv_prep_bwd(dq, dk, dv, heads: int, S_in: int, *, q_in=None, k_in=None, out
             if tuple(t.shape) != (B, S_in, H * D) or t.dtype != dq.dtype or t.stride(2) != 1 or t.stride() != q_in.stride():
                 raise SvgbError("q_in, k_in must be [B, S_in, H*D] of the gradients' dtype with one set of strides")
         ts, bs = q_in.stride(1), q_in.stride(0)
-        want = H * D if norm == NORM_RMS_HIDDEN else D
-        for g in (gamma_q, gamma_k):
-            if g.dtype != dq.dtype or g.numel() != want or not g.is_contiguous():
-                raise SvgbError(f"gamma_q / gamma_k must be contiguous [{want}] of the input dtype")
-    if rope:
-        if cos is None or sin is None or cos.dtype != torch.float32 or sin.dtype != torch.float32:
-            raise SvgbError("rope needs float32 cos / sin tables")
-        _contig(cos, sin)
-        if rope_n is None:
-            rope_n = cos.shape[0]
-        width = D // 2 if rope == 2 else D
-        if tuple(cos.shape) != (rope_n, width) or tuple(sin.shape) != (rope_n, width):
-            raise SvgbError(f"cos / sin must be [{rope_n}, {width}]")
-    else:
-        rope_n = 0
+    weights = (("gamma_q / gamma_k", gamma_q), ("gamma_q / gamma_k", gamma_k)) if norm != NORM_NONE else ()
+    rope_n = _check_tables_and_weights(D, H * D, dq.dtype, norm, rope, cos, sin, rope_n, weights)
     nbytes = C.c_size_t()
     check(lib().svgb_qkv_prep_bwd_bytes(B, S_in, H, D, int(norm), C.byref(nbytes)), "svgb_qkv_prep_bwd_bytes")
     ws = workspace("qkv_prep_bwd", nbytes.value, dq.device)
@@ -818,6 +818,17 @@ def qkv_prep_bwd(dq, dk, dv, heads: int, S_in: int, *, q_in=None, k_in=None, out
     return (*dx, *cast)
 
 
+def _prep_streams(heads, S_out, calls, ts):
+    """One new (q, k, v) [B, heads, S_out, D] filled by one _qkv_prep per call: ts holds each call's q_in, k_in, v_in,
+    gamma_q, gamma_k, beta_q, beta_k, and calls its other keyword arguments."""
+    B, _, HD = ts[0].shape
+    out = tuple(torch.empty(B, heads, S_out, HD // heads, dtype=ts[0].dtype, device=ts[0].device) for _ in range(3))
+    for i, kw in enumerate(calls):
+        q_in, k_in, v_in, gq, gk, bq, bk = ts[7 * i:7 * i + 7]
+        _qkv_prep(q_in, k_in, v_in, heads, out=out, gamma_q=gq, gamma_k=gk, beta_q=bq, beta_k=bk, **kw)
+    return out
+
+
 class _QkvPrep(torch.autograd.Function):
     """One or more qkv_prep calls into one shared output (a single block: one call; the double block: its video and
     prompt streams) under autograd.  Inputs per call: q_in, k_in, v_in, gamma_q, gamma_k, beta_q, beta_k; `calls` holds
@@ -826,13 +837,10 @@ class _QkvPrep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, heads, S_out, calls, *ts):
-        B, _, HD = ts[0].shape
-        out = tuple(torch.empty(B, heads, S_out, HD // heads, dtype=ts[0].dtype, device=ts[0].device)
-                    for _ in range(3))
+        out = _prep_streams(heads, S_out, calls, ts)
         saved = []
         for i, call in enumerate(calls):
-            q_in, k_in, v_in, gq, gk, bq, bk = ts[7 * i:7 * i + 7]
-            _qkv_prep(q_in, k_in, v_in, heads, out=out, gamma_q=gq, gamma_k=gk, beta_q=bq, beta_k=bk, **call)
+            q_in, k_in, _, gq, gk = ts[7 * i:7 * i + 5]
             keep = call["norm"] != NORM_NONE  # the norm backward reads x; a transpose or a rotation does not
             saved += [q_in if keep else None, k_in if keep else None, gq, gk]
         ctx.save_for_backward(*saved)
@@ -866,13 +874,7 @@ def qkv_prep_streams(streams, heads: int, S_out: int):
             _tables_no_grad(kw.get("cos"), kw.get("sin"))
             kw.setdefault("norm", NORM_NONE)
         return _QkvPrep.apply(heads, S_out, calls, *ts)
-    q0 = ts[0]
-    B, _, HD = q0.shape
-    out = tuple(torch.empty(B, heads, S_out, HD // heads, dtype=q0.dtype, device=q0.device) for _ in range(3))
-    for i, kw in enumerate(calls):
-        q_in, k_in, v_in, gq, gk, bq, bk = ts[7 * i:7 * i + 7]
-        _qkv_prep(q_in, k_in, v_in, heads, out=out, gamma_q=gq, gamma_k=gk, beta_q=bq, beta_k=bk, **kw)
-    return out
+    return _prep_streams(heads, S_out, calls, ts)
 
 
 def qkv_prep(q_in, k_in, v_in, heads: int, *, out=None, out_row0: int = 0, out_rows: Optional[int] = None,
@@ -913,22 +915,8 @@ def _qkv_prep(q_in, k_in, v_in, heads: int, *, out=None, out_row0: int = 0, out_
             raise SvgbError("outputs must be contiguous [B, H, S_out, D] of the input dtype")
     if out_row0 + S_in > S_out:
         raise SvgbError("out_row0 + S_in exceeds the output rows")
-    if rope:
-        if cos is None or sin is None or cos.dtype != torch.float32 or sin.dtype != torch.float32:
-            raise SvgbError("rope needs float32 cos / sin tables")
-        _contig(cos, sin)
-        if rope_n is None:
-            rope_n = cos.shape[0]
-        width = D // 2 if rope == 2 else D
-        if tuple(cos.shape) != (rope_n, width) or tuple(sin.shape) != (rope_n, width):
-            raise SvgbError(f"cos / sin must be [{rope_n}, {width}]")
-    else:
-        rope_n = 0
-    for g, n in ((gamma_q, "gamma_q"), (gamma_k, "gamma_k"), (beta_q, "beta_q"), (beta_k, "beta_k")):
-        if g is not None:
-            want = HD if norm == NORM_RMS_HIDDEN else D
-            if g.dtype != q_in.dtype or g.numel() != want or not g.is_contiguous():
-                raise SvgbError(f"{n} must be contiguous [{want}] of the input dtype")
+    weights = (("gamma_q", gamma_q), ("gamma_k", gamma_k), ("beta_q", beta_q), ("beta_k", beta_k))
+    rope_n = _check_tables_and_weights(D, HD, q_in.dtype, norm, rope, cos, sin, rope_n, weights)
     check(lib().svgb_qkv_prep(q_in.data_ptr(), k_in.data_ptr(), v_in.data_ptr(), q_in.stride(1), q_in.stride(0),
                               out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(), S_out * D, heads * S_out * D,
                               B, S_in, heads, D, int(out_row0), int(norm), _p(gamma_q), _p(gamma_k), _p(beta_q),
