@@ -68,6 +68,9 @@ typedef struct svgb_plan {
 } svgb_plan;
 /* A plan built with BH == 1 may serve every head of a launch (one map for all heads, e.g. BSR masks):
  * set items_stride = 0 in the host struct. */
+/* S is the query length.  A variable-block plan has no element mask (mask_mode = SVGB_MASK_NONE), and its m0 holds the
+ * key/value length Skv when svgb_attn_plan_varblock_kv built it; m0 = 0 (every other planner) means Skv = S.  The
+ * attention entries reject a plan whose lengths differ from the call's. */
 
 /* SVG2 / BSR / dense: q-block i of head h attends k-block j iff map[h,i,j] != 0.
  * Stands behind dynamic_block_sparse_fwd_flashinfer's wrapper.plan (svg/kmeans_utils.py:1355-1385).
@@ -77,6 +80,15 @@ int svgb_attn_plan_varblock_bytes(int BH, int S, int QC, int KC, size_t* bytes);
 int svgb_attn_plan_varblock(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH,
                             int S, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
                             void* stream);
+
+/* Rectangular form, for queries attending a key/value sequence of another length (cross-attention, a chunk of frames
+ * against context frames): row sizes sum to Sq, column sizes to Skv; the items cover Sq query rows and the chunk lists
+ * Skv keys.  plan->kind = SVGB_PLAN_VARBLOCK, plan->S = Sq, plan->m0 = Skv; runs with svgb_attn_fwd_kv / svgb_attn_bwd_kv.
+ * Its key-major companion for the backward is the same planner on the transpose: (map^T, col_sz, row_sz, Skv, Sq). */
+int svgb_attn_plan_varblock_kv_bytes(int BH, int Sq, int Skv, int QC, int KC, size_t* bytes);
+int svgb_attn_plan_varblock_kv(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int Sq,
+                               int Skv, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
+                               void* stream);
 
 /* Same map, lowered for the row-gather kernel path: the selected key ranges are kept as runs and the
  * kernel gathers exactly-full 128-key chunks across run boundaries with cp.async (no padded tail chunk per
@@ -129,6 +141,18 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream);
+/* svgb_attn_fwd with queries of length Sq against keys / values of length Skv:
+ *   q     : [BH, Sq, D] at q_row_stride / q_head_stride;  k, v : [BH, Skv, D] at kv_row_stride / kv_head_stride;
+ *   o     : [BH, Sq, D] at its own strides;  lse : optional float [BH, Sq].
+ *   plan  : SVGB_PLAN_VARBLOCK built for (Sq, Skv) -- svgb_attn_plan_varblock_kv, or svgb_attn_plan_varblock when
+ *           Sq == Skv.  16-bit inputs only (SVGB_BF16 / SVGB_F16), D in {64,128}; alignment as svgb_attn_fwd.
+ * Same kernel as svgb_attn_fwd: a key chunk past Skv is cut by its valid count and TMA fills rows past Skv with zeros.
+ * Band, gather and profiling plans, row-index vectors and e4m3 inputs need Sq == Skv and svgb_attn_fwd.  With
+ * Sq == Skv and equal strides the result is svgb_attn_fwd's, bit for bit. */
+int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BH, int Sq,
+                     int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
+                     long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
+                     const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
 
 /* Backward of svgb_attn_fwd: dq, dk, dv from q, k, v, the forward's o and natural-log lse, and the output gradient dO.
@@ -146,6 +170,20 @@ int svgb_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
                   void* dq, void* dk, void* dv, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                   const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream);
+
+/* Backward of svgb_attn_fwd_kv: q, o, dO, dq [BH, Sq, D] at the q strides; k, v, dk, dv [BH, Skv, D] at the k/v
+ * strides; lse float [BH, Sq].  plan: the forward's SVGB_PLAN_VARBLOCK plan for (Sq, Skv); plan_t: its key-major
+ * companion svgb_attn_plan_varblock_kv(map^T, col_sz, row_sz, Skv, Sq) (svgb_attn_plan_varblock(map^T, ...) when
+ * Sq == Skv).  ws: device scratch of svgb_attn_bwd_kv_bytes (the delta over Sq rows).  The dQ launch walks plan with
+ * K / V over Skv rows; the dK / dV launch walks plan_t with K / V as its rows and Q / dO (Sq rows) as its chunks.
+ * Guarantees as svgb_attn_bwd: every gradient row written, no atomics, deterministic; with Sq == Skv and equal
+ * strides the gradients are svgb_attn_bwd's, bit for bit.  Variable-block plans and 16-bit inputs only. */
+int svgb_attn_bwd_kv_bytes(int BH, int Sq, int Skv, size_t* bytes);
+int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                     void* dq, void* dk, void* dv, int dtype, int BH, int Sq, int Skv, int D, long long q_row_stride,
+                     long long q_head_stride, long long kv_row_stride, long long kv_head_stride, float sm_scale,
+                     const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws,
+                     void* ws, size_t ws_bytes, void* stream);
 
 /* density of a variable-block map (density_calculation, svg/kmeans_utils.py:13-31) -> float [BH] */
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

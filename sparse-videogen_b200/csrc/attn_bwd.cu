@@ -38,6 +38,89 @@ static AttnBwdArgs bwd_args(const svgb_plan* p, const void* ws) {
   return a;
 }
 
+// Every backward entry: q, o, dO, dq over Sq rows with the q strides, k, v, dk, dv over Skv rows with the k/v strides.
+// The dQ launch walks the forward plan (X / Y = Q / dO, U / W = K / V), the dK / dV launch the key-major plan (X / Y =
+// K / V, U / W = Q / dO); lse and delta are per query row in both.
+static int attn_bwd_run(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                        void* dq, void* dk, void* dv, int dtype, int BH, int Sq, int Skv, int D, long long q_rs,
+                        long long q_hs, long long kv_rs, long long kv_hs, float sm_scale, const svgb_plan* plan,
+                        const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws, void* ws,
+                        size_t ws_bytes, void* stream) {
+  SVGB_REQUIRE(q && k && v && o && dout && lse && dq && dk && dv && plan && plan_ws && plan_t && plan_t_ws && ws,
+               "null pointer");
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
+               "attention backward takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no backward)", dtype);
+  SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND,
+               "attention backward needs a variable-block or band plan (kind %d; gather plans have no backward)",
+               plan->kind);
+  SVGB_REQUIRE(plan_t->kind == (plan->kind == SVGB_PLAN_BAND ? SVGB_PLAN_BAND_T : SVGB_PLAN_VARBLOCK),
+               "plan_t (kind %d) is not the key-major companion of a kind-%d plan", plan_t->kind, plan->kind);
+  SVGB_REQUIRE(plan->mask_mode >= MASK_NONE && plan->mask_mode <= MASK_COG,
+               "attention backward supports the executed band masks NONE / HY / WAN / COG (mask mode %d)",
+               plan->mask_mode);
+  // a variable-block plan's m0 is its Skv (svgb200.h), checked with the lengths below
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || (plan_t->mask_mode == plan->mask_mode && plan_t->m0 == plan->m0 &&
+                                                plan_t->m1 == plan->m1 && plan_t->m2 == plan->m2),
+               "plan_t was built for another mask than plan");
+  // the key-major plan has the keys as rows: its S is Skv and its Skv is Sq
+  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH),
+               "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
+               plan_kv_len(plan), BH, Sq, Skv);
+  SVGB_REQUIRE(plan_t->S == Skv && plan_kv_len(plan_t) == Sq && (plan_t->items_stride == 0 || plan_t->BH == BH),
+               "plan_t was built for BH=%d S=%d Skv=%d; the key-major plan of this call has BH=%d S=%d Skv=%d",
+               plan_t->BH, plan_t->S, plan_kv_len(plan_t), BH, Skv, Sq);
+  size_t need = 0;
+  if (svgb_attn_bwd_bytes(BH, Sq, &need)) return -1;
+  SVGB_REQUIRE(ws_bytes >= need, "backward workspace too small: %zu < %zu", ws_bytes, need);
+  for (const void* t : {dq, dk, dv})
+    SVGB_REQUIRE((reinterpret_cast<uintptr_t>(t) & 15) == 0, "gradients must be 16-byte aligned");
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0 &&
+                   q_rs % 8 == 0 && q_hs % 8 == 0 && kv_rs % 8 == 0 && kv_hs % 8 == 0,
+               "o / dO must be 16-byte aligned with strides multiple of 8 elements");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* delta = static_cast<float*>(ws);
+
+  const long long rows = static_cast<long long>(BH) * Sq;
+  const unsigned blocks = static_cast<unsigned>((rows + 7) / 8);
+  if (dtype == SVGB_BF16)
+    attn_bwd_delta_kernel<true><<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o),
+                                                        static_cast<const uint16_t*>(dout), q_rs, q_hs, BH, Sq, D,
+                                                        delta);
+  else
+    attn_bwd_delta_kernel<false><<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o),
+                                                         static_cast<const uint16_t*>(dout), q_rs, q_hs, BH, Sq, D,
+                                                         delta);
+  SVGB_LAUNCH_OK();
+
+  CUtensorMap qm, km, vm, dom;
+  if (encode_tmap_hsd(&qm, q, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
+  if (encode_tmap_hsd(&km, k, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
+  if (encode_tmap_hsd(&vm, v, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
+  if (encode_tmap_hsd(&dom, dout, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
+  AttnBwdArgs aq = bwd_args(plan, plan_ws), ak = bwd_args(plan_t, plan_t_ws);
+  for (AttnBwdArgs* a : {&aq, &ak}) {
+    a->lse = lse;
+    a->delta = delta;
+    a->scale_log2 = sm_scale * 1.4426950408889634f;
+    a->sm_scale = sm_scale;
+    a->S = Sq;
+  }
+  aq.row_stride = q_rs;  // dQ is stored with q's strides, dK and dV with k's
+  aq.head_stride = q_hs;
+  ak.row_stride = kv_rs;
+  ak.head_stride = kv_hs;
+  aq.g0 = dq;
+  ak.g0 = dk;
+  ak.g1 = dv;
+  const dim3 gq(plan->max_items, BH), gk(plan_t->max_items, BH);
+  if (D == 128)
+    return dtype == SVGB_BF16 ? launch_bwd_pair<128, DT_BF16>(qm, km, vm, dom, aq, gq, ak, gk, st)
+                              : launch_bwd_pair<128, DT_F16>(qm, km, vm, dom, aq, gq, ak, gk, st);
+  return dtype == SVGB_BF16 ? launch_bwd_pair<64, DT_BF16>(qm, km, vm, dom, aq, gq, ak, gk, st)
+                            : launch_bwd_pair<64, DT_F16>(qm, km, vm, dom, aq, gq, ak, gk, st);
+}
+
 }  // namespace svgb
 
 using namespace svgb;
@@ -54,72 +137,26 @@ int svgb_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
                   void* dq, void* dk, void* dv, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                   const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
-  SVGB_REQUIRE(q && k && v && o && dout && lse && dq && dk && dv && plan && plan_ws && plan_t && plan_t_ws && ws,
-               "null pointer");
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
-               "attention backward takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no backward)", dtype);
-  SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND,
-               "attention backward needs a variable-block or band plan (kind %d; gather plans have no backward)",
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, S, S, D, row_stride, head_stride, row_stride,
+                      head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
+}
+
+int svgb_attn_bwd_kv_bytes(int BH, int Sq, int Skv, size_t* bytes) {
+  SVGB_REQUIRE(Skv > 0, "bad arguments");
+  return svgb_attn_bwd_bytes(BH, Sq, bytes);  // the per-query-row delta
+}
+
+int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                     void* dq, void* dk, void* dv, int dtype, int BH, int Sq, int Skv, int D, long long q_row_stride,
+                     long long q_head_stride, long long kv_row_stride, long long kv_head_stride, float sm_scale,
+                     const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws,
+                     void* ws, size_t ws_bytes, void* stream) {
+  SVGB_REQUIRE(plan, "null pointer");
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK,
+               "svgb_attn_bwd_kv takes variable-block plans only (kind %d; band plans need Sq == Skv, svgb_attn_bwd)",
                plan->kind);
-  SVGB_REQUIRE(plan_t->kind == (plan->kind == SVGB_PLAN_BAND ? SVGB_PLAN_BAND_T : SVGB_PLAN_VARBLOCK),
-               "plan_t (kind %d) is not the key-major companion of a kind-%d plan", plan_t->kind, plan->kind);
-  SVGB_REQUIRE(plan->mask_mode >= MASK_NONE && plan->mask_mode <= MASK_COG,
-               "attention backward supports the executed band masks NONE / HY / WAN / COG (mask mode %d)",
-               plan->mask_mode);
-  SVGB_REQUIRE(plan_t->mask_mode == plan->mask_mode && plan_t->m0 == plan->m0 && plan_t->m1 == plan->m1 &&
-                   plan_t->m2 == plan->m2,
-               "plan_t was built for another mask than plan");
-  for (const svgb_plan* p : {plan, plan_t})
-    SVGB_REQUIRE(p->S == S && (p->items_stride == 0 || p->BH == BH),
-                 "plan was built for BH=%d S=%d, called with BH=%d S=%d", p->BH, p->S, BH, S);
-  size_t need = 0;
-  if (svgb_attn_bwd_bytes(BH, S, &need)) return -1;
-  SVGB_REQUIRE(ws_bytes >= need, "backward workspace too small: %zu < %zu", ws_bytes, need);
-  for (const void* t : {dq, dk, dv})
-    SVGB_REQUIRE((reinterpret_cast<uintptr_t>(t) & 15) == 0, "gradients must be 16-byte aligned");
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0 &&
-                   row_stride % 8 == 0 && head_stride % 8 == 0,
-               "o / dO must be 16-byte aligned with strides multiple of 8 elements");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  float* delta = static_cast<float*>(ws);
-
-  const long long rows = static_cast<long long>(BH) * S;
-  const unsigned blocks = static_cast<unsigned>((rows + 7) / 8);
-  if (dtype == SVGB_BF16)
-    attn_bwd_delta_kernel<true><<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o),
-                                                        static_cast<const uint16_t*>(dout), row_stride, head_stride,
-                                                        BH, S, D, delta);
-  else
-    attn_bwd_delta_kernel<false><<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o),
-                                                         static_cast<const uint16_t*>(dout), row_stride, head_stride,
-                                                         BH, S, D, delta);
-  SVGB_LAUNCH_OK();
-
-  CUtensorMap qm, km, vm, dom;
-  if (encode_tmap_hsd(&qm, q, dtype, BH, S, D, row_stride, head_stride)) return -1;
-  if (encode_tmap_hsd(&km, k, dtype, BH, S, D, row_stride, head_stride)) return -1;
-  if (encode_tmap_hsd(&vm, v, dtype, BH, S, D, row_stride, head_stride)) return -1;
-  if (encode_tmap_hsd(&dom, dout, dtype, BH, S, D, row_stride, head_stride)) return -1;
-  AttnBwdArgs aq = bwd_args(plan, plan_ws), ak = bwd_args(plan_t, plan_t_ws);
-  for (AttnBwdArgs* a : {&aq, &ak}) {
-    a->lse = lse;
-    a->delta = delta;
-    a->row_stride = row_stride;
-    a->head_stride = head_stride;
-    a->scale_log2 = sm_scale * 1.4426950408889634f;
-    a->sm_scale = sm_scale;
-    a->S = S;
-  }
-  aq.g0 = dq;
-  ak.g0 = dk;
-  ak.g1 = dv;
-  const dim3 gq(plan->max_items, BH), gk(plan_t->max_items, BH);
-  if (D == 128)
-    return dtype == SVGB_BF16 ? launch_bwd_pair<128, DT_BF16>(qm, km, vm, dom, aq, gq, ak, gk, st)
-                              : launch_bwd_pair<128, DT_F16>(qm, km, vm, dom, aq, gq, ak, gk, st);
-  return dtype == SVGB_BF16 ? launch_bwd_pair<64, DT_BF16>(qm, km, vm, dom, aq, gq, ak, gk, st)
-                            : launch_bwd_pair<64, DT_F16>(qm, km, vm, dom, aq, gq, ak, gk, st);
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, Sq, Skv, D, q_row_stride, q_head_stride,
+                      kv_row_stride, kv_head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
 }
 
 }  // extern "C"

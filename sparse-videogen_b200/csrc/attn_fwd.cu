@@ -421,43 +421,39 @@ int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const v
                             : launch_attn<64, DT_F16>(qm, km, vm, a, gather, grid, st);
 }
 
-static int varblock_chunk_cap(int S, int KC) { return S / kChunkCols + (KC + 1) / 2 + 2; }
-static int varblock_max_items(int S, int QC) { return S / kItemRows + QC + 1; }
+// a chunk list covers the key side (Skv columns), the items the query side (Sq rows)
+static int varblock_chunk_cap(int Skv, int KC) { return Skv / kChunkCols + (KC + 1) / 2 + 2; }
+static int varblock_max_items(int Sq, int QC) { return Sq / kItemRows + QC + 1; }
 
-}  // namespace svgb
-
-using namespace svgb;
-
-extern "C" {
-
-int svgb_attn_plan_varblock_bytes(int BH, int S, int QC, int KC, size_t* bytes) {
-  SVGB_REQUIRE(BH > 0 && S > 0 && QC > 0 && KC > 0 && bytes, "bad arguments");
+static int plan_varblock_bytes(int BH, int Sq, int Skv, int QC, int KC, size_t* bytes) {
+  SVGB_REQUIRE(BH > 0 && Sq > 0 && Skv > 0 && QC > 0 && KC > 0 && bytes, "bad arguments");
   const size_t counts = align_up(sizeof(int) * BH, 256);
-  const size_t items = align_up(2 * sizeof(int4) * BH * varblock_max_items(S, QC), 256);
-  const size_t chunks = align_up(sizeof(int2) * static_cast<size_t>(BH) * QC * varblock_chunk_cap(S, KC), 256);
+  const size_t items = align_up(2 * sizeof(int4) * BH * varblock_max_items(Sq, QC), 256);
+  const size_t chunks = align_up(sizeof(int2) * static_cast<size_t>(BH) * QC * varblock_chunk_cap(Skv, KC), 256);
   const size_t lens = align_up(sizeof(int) * static_cast<size_t>(BH) * QC, 256);  // per q-block list length
   *bytes = counts + items + chunks + lens;
   return 0;
 }
 
-static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH,
-                              int S, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
-                              void* stream, bool gather) {
+// rect: the plan of svgb_attn_plan_varblock_kv, which records Skv in m0 (0 leaves Skv = S, svgb200.h)
+static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int Sq,
+                              int Skv, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
+                              bool gather, bool rect) {
   size_t need = 0;
-  if (svgb_attn_plan_varblock_bytes(BH, S, QC, KC, &need)) return -1;
+  if (plan_varblock_bytes(BH, Sq, Skv, QC, KC, &need)) return -1;
   SVGB_REQUIRE(map && row_sz && col_sz && plan_ws && plan, "null pointer");
   SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(static_cast<size_t>(BH) * QC * varblock_chunk_cap(S, KC) < (1ull << 31),
+  SVGB_REQUIRE(static_cast<size_t>(BH) * QC * varblock_chunk_cap(Skv, KC) < (1ull << 31),
                "plan too large for 32-bit chunk offsets");
-  const int max_items = varblock_max_items(S, QC);
-  const int cap = varblock_chunk_cap(S, KC);
+  const int max_items = varblock_max_items(Sq, QC);
+  const int cap = varblock_chunk_cap(Skv, KC);
   plan->kind = gather ? SVGB_PLAN_GATHER : SVGB_PLAN_VARBLOCK;
   plan->BH = BH;
-  plan->S = S;
+  plan->S = Sq;
   plan->max_items = max_items;
   plan->items_stride = max_items;
   plan->mask_mode = MASK_NONE;
-  plan->m0 = 0;
+  plan->m0 = rect ? Skv : 0;
   plan->m1 = 0;
   plan->m2 = 0;
   plan->counts_off = 0;
@@ -482,16 +478,90 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   return 0;
 }
 
+// Every forward entry: q / o over Sq rows, k / v over Skv rows, each pair with its own strides.
+static int attn_fwd_run(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
+                        const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
+                        const int32_t* o_rows, int dtype, int BH, int Sq, int Skv, int D, long long q_rs,
+                        long long q_hs, long long kv_rs, long long kv_hs, long long o_rs, long long o_hs,
+                        float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
+  SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
+  SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
+               "fp8 attention needs the three per-head scale vectors");
+  SVGB_REQUIRE(dtype == SVGB_E4M3 || (!q_scale && !k_scale && !v_scale),
+               "per-head scale vectors are for e4m3 inputs only (dtype %d)", dtype);
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND_T,
+               "a key-major band plan (svgb_attn_plan_band_t) is for svgb_attn_bwd; the forward takes svgb_attn_plan_band");
+  const bool gather = plan->kind == SVGB_PLAN_GATHER;
+  SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
+               "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");
+  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH),
+               "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
+               plan_kv_len(plan), BH, Sq, Skv);
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && o_rs % 8 == 0 && o_hs % 8 == 0,
+               "output must be 16-byte aligned with strides multiple of 8 elements");
+  const char* ws = static_cast<const char*>(plan_ws);
+  AttnArgs a;
+  a.items = reinterpret_cast<const int4*>(ws + plan->items_off);
+  a.item_count = reinterpret_cast<const int*>(ws + plan->counts_off);
+  a.chunks = reinterpret_cast<const int2*>(ws + plan->chunks_off);
+  a.items_stride = plan->items_stride;
+  a.o = o;
+  a.o_row_stride = o_rs;
+  a.o_head_stride = o_hs;
+  a.o_rows = o_rows;
+  a.lse = lse;
+  a.scale_log2 = sm_scale * 1.4426950408889634f;
+  a.S = Sq;
+  if (plan->kind == SVGB_PLAN_BAND) {  // a variable-block plan's m0 is its Skv, not a mask parameter
+    a.mask_mode = plan->mask_mode;
+    a.m0 = plan->m0;
+    a.m1 = plan->m1;
+    a.m2 = plan->m2;
+  }
+  a.q_scale = q_scale;
+  a.k_scale = k_scale;
+  a.v_scale = v_scale;
+  a.q_rows = q_rows;
+  a.kv_rows = kv_rows;
+  a.q_ptr = q;
+  a.k_ptr = k;
+  a.v_ptr = v;
+  a.in_row_stride = q_rs;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
+  a.in_head_stride = q_hs;
+  return attn_fwd_impl(q, Sq, q_rs, q_hs, k, v, Skv, kv_rs, kv_hs, dtype, BH, D, a, gather, plan->max_items,
+                       static_cast<cudaStream_t>(stream));
+}
+
+}  // namespace svgb
+
+using namespace svgb;
+
+extern "C" {
+
+int svgb_attn_plan_varblock_bytes(int BH, int S, int QC, int KC, size_t* bytes) {
+  return plan_varblock_bytes(BH, S, S, QC, KC, bytes);
+}
+
 int svgb_attn_plan_varblock(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH,
                             int S, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
                             void* stream) {
-  return plan_varblock_impl(map, row_sz, col_sz, BH, S, QC, KC, plan_ws, ws_bytes, plan, stream, false);
+  return plan_varblock_impl(map, row_sz, col_sz, BH, S, S, QC, KC, plan_ws, ws_bytes, plan, stream, false, false);
+}
+
+int svgb_attn_plan_varblock_kv_bytes(int BH, int Sq, int Skv, int QC, int KC, size_t* bytes) {
+  return plan_varblock_bytes(BH, Sq, Skv, QC, KC, bytes);
+}
+
+int svgb_attn_plan_varblock_kv(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int Sq,
+                               int Skv, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
+                               void* stream) {
+  return plan_varblock_impl(map, row_sz, col_sz, BH, Sq, Skv, QC, KC, plan_ws, ws_bytes, plan, stream, false, true);
 }
 
 int svgb_attn_plan_varblock_gather(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH,
                                    int S, int QC, int KC, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
                                    void* stream) {
-  return plan_varblock_impl(map, row_sz, col_sz, BH, S, QC, KC, plan_ws, ws_bytes, plan, stream, true);
+  return plan_varblock_impl(map, row_sz, col_sz, BH, S, S, QC, KC, plan_ws, ws_bytes, plan, stream, true, false);
 }
 
 int svgb_attn_plan_band_bytes(int S, size_t* bytes) {
@@ -553,49 +623,29 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream) {
-  SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
-  SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
-               "fp8 attention needs the three per-head scale vectors");
-  SVGB_REQUIRE(dtype == SVGB_E4M3 || (!q_scale && !k_scale && !v_scale),
-               "per-head scale vectors are for e4m3 inputs only (dtype %d)", dtype);
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND_T,
-               "a key-major band plan (svgb_attn_plan_band_t) is for svgb_attn_bwd; the forward takes svgb_attn_plan_band");
-  const bool gather = plan->kind == SVGB_PLAN_GATHER;
-  SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
-               "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");
-  SVGB_REQUIRE(plan->S == S && (plan->items_stride == 0 || plan->BH == BH),
-               "plan was built for BH=%d S=%d, called with BH=%d S=%d", plan->BH, plan->S, BH, S);
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && o_row_stride % 8 == 0 && o_head_stride % 8 == 0,
-               "output must be 16-byte aligned with strides multiple of 8 elements");
-  const char* ws = static_cast<const char*>(plan_ws);
-  AttnArgs a;
-  a.items = reinterpret_cast<const int4*>(ws + plan->items_off);
-  a.item_count = reinterpret_cast<const int*>(ws + plan->counts_off);
-  a.chunks = reinterpret_cast<const int2*>(ws + plan->chunks_off);
-  a.items_stride = plan->items_stride;
-  a.o = o;
-  a.o_row_stride = o_row_stride;
-  a.o_head_stride = o_head_stride;
-  a.o_rows = o_rows;
-  a.lse = lse;
-  a.scale_log2 = sm_scale * 1.4426950408889634f;
-  a.S = S;
-  a.mask_mode = plan->mask_mode;
-  a.m0 = plan->m0;
-  a.m1 = plan->m1;
-  a.m2 = plan->m2;
-  a.q_scale = q_scale;
-  a.k_scale = k_scale;
-  a.v_scale = v_scale;
-  a.q_rows = q_rows;
-  a.kv_rows = kv_rows;
-  a.q_ptr = q;
-  a.k_ptr = k;
-  a.v_ptr = v;
-  a.in_row_stride = row_stride;
-  a.in_head_stride = head_stride;
-  return attn_fwd_impl(q, S, row_stride, head_stride, k, v, S, row_stride, head_stride, dtype, BH, D, a, gather,
-                       plan->max_items, static_cast<cudaStream_t>(stream));
+  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, BH, S, S, D,
+                      row_stride, head_stride, row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan,
+                      plan_ws, stream);
+}
+
+int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BH, int Sq,
+                     int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
+                     long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
+                     const svgb_plan* plan, const void* plan_ws, void* stream) {
+  SVGB_REQUIRE(plan, "null pointer");
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
+               "svgb_attn_fwd_kv takes bf16 or fp16 inputs (dtype %d; e4m3 attention needs Sq == Skv, svgb_attn_fwd)",
+               dtype);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK,
+               "svgb_attn_fwd_kv takes variable-block plans only (kind %d; band, gather and profiling plans need "
+               "Sq == Skv, svgb_attn_fwd)", plan->kind);
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
+                   kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
+               "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
+  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, BH, Sq, Skv, D,
+                      q_row_stride, q_head_stride, kv_row_stride, kv_head_stride, o_row_stride, o_head_stride,
+                      sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "../../include/svgb200.h"
+
 namespace svgb {
 
 // thread-local last-error message (api.cu)
@@ -47,6 +49,10 @@ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 // box = 64 x 128 x 1, 128-byte swizzle.  Returns 0 on success.
 int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S, int D,
                     long long row_stride_elems, long long head_stride_elems, int box_rows = 128);
+
+// key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0 (svgb200.h);
+// every other plan has Skv = S
+inline int plan_kv_len(const svgb_plan* p) { return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S; }
 
 struct AttnArgs;
 // attention launch with independent query / key-value geometry (attn_fwd.cu); used by svgb_attn_fwd

@@ -38,6 +38,8 @@ _PROTOS = {
     "svgb_device_check": [C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)],
     "svgb_attn_plan_varblock_bytes": [_i, _i, _i, _i, _psz],
     "svgb_attn_plan_varblock": [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_varblock_kv_bytes": [_i, _i, _i, _i, _i, _psz],
+    "svgb_attn_plan_varblock_kv": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_plan_varblock_gather": [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_plan_band_bytes": [_i, _psz],
     "svgb_attn_plan_band": [_i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
@@ -45,10 +47,15 @@ _PROTOS = {
     "svgb_attn_plan_band_t": [_i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                       _pplan, _vp, _vp],
+    "svgb_attn_fwd_kv": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan, _vp,
+                         _vp],
     "svgb_quantize_e4m3": [_vp, _i, _vp, _vp, _i, _i, _i, _vp],
     "svgb_attn_bwd_bytes": [_i, _i, _psz],
     "svgb_attn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _f, _pplan, _vp, _pplan,
                       _vp, _vp, _sz, _vp],
+    "svgb_attn_bwd_kv_bytes": [_i, _i, _i, _psz],
+    "svgb_attn_bwd_kv": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
+                         _pplan, _vp, _pplan, _vp, _vp, _sz, _vp],
     "svgb_density": [_vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "svgb_argsort_labels_bytes": [_i, _i, _i, _psz],
     "svgb_argsort_labels": [_vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp],

@@ -85,6 +85,12 @@ class AttnPlan:
     def S(self):
         return self.desc.S
 
+    @property
+    def S_kv(self):
+        """Key/value length: a rectangular variable-block plan records it in m0 (include/svgb200.h, svgb_plan)."""
+        d = self.desc
+        return d.m0 if d.kind == PLAN_VARBLOCK and d.m0 > 0 else d.S
+
     def key_major(self) -> "AttnPlan":
         """The plan the backward's dK / dV kernel walks (one work list per key range), built on first use: the band
         mask's transposed plan, or the variable-block planner on the transposed map with row and column sizes swapped.
@@ -103,7 +109,7 @@ class AttnPlan:
                     raise SvgbError("attention backward: the block map or block sizes of this plan were modified in "
                                     "place after the plan was built; rebuild the plan")
                 m, r, c = ts
-                kt = plan_varblock(m.transpose(1, 2), c, r, d.S)
+                kt = plan_varblock(m.transpose(1, 2), c, r, self.S_kv, S_kv=d.S)
                 if d.items_stride == 0:  # one map shared by every head (svgb200.h, svgb_plan): so is its transpose
                     kt.desc.items_stride = 0
                 self._key_major = kt
@@ -115,10 +121,14 @@ class AttnPlan:
 
 
 def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.Tensor, S: int,
-                  gather: bool = False) -> AttnPlan:
+                  gather: bool = False, *, S_kv: Optional[int] = None) -> AttnPlan:
     """block_map [BH,QC,KC] bool/uint8, row_sz [BH,QC], col_sz [BH,KC] (any int dtype) on GPU.
     gather=True lowers the map for the row-gather kernel path (exactly-full chunks, optional fused
     permutation through attn_fwd(..., q_rows=, kv_rows=)).
+    S_kv: key/value length when it differs from the query length S (row sizes sum to S, column sizes to S_kv): the
+    rectangular plan of svgb_attn_plan_varblock_kv, which attn_fwd / attn_bwd / attention run on k, v of S_kv rows.
+    S_kv == S (or None) is the square planner's call.  As for the square planner, the sizes are device tensors and are
+    not checked against S / S_kv: sizes that overrun them make the kernels read and store rows past the tensors.
 
     Every plan owns its device work list (torch's caching allocator makes the per-call allocation free of
     cudaMalloc / syncs), so plans of one shape can be held and executed in any order or on different streams."""
@@ -129,9 +139,19 @@ def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.T
     r = row_sz.reshape(BH, QC).to(torch.int32).contiguous()
     c = col_sz.reshape(BH, KC).to(torch.int32).contiguous()
     nbytes = C.c_size_t()
+    desc = Plan()
+    if S_kv is not None and S_kv != S:
+        if gather:
+            raise SvgbError(f"gather plans need S_kv == S (got S={S}, S_kv={S_kv}): the rectangular plan is TMA only")
+        check(lib().svgb_attn_plan_varblock_kv_bytes(BH, S, S_kv, QC, KC, C.byref(nbytes)), "plan_varblock_kv_bytes")
+        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=m.device)
+        check(lib().svgb_attn_plan_varblock_kv(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, S, S_kv, QC, KC,
+                                               ws.data_ptr(), ws.numel(), C.byref(desc), _stream(m)),
+              "svgb_attn_plan_varblock_kv")
+        _bump()
+        return AttnPlan(desc, ws, (m, r, c, (m._version, r._version, c._version)))
     check(lib().svgb_attn_plan_varblock_bytes(BH, S, QC, KC, C.byref(nbytes)), "plan_varblock_bytes")
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=m.device)
-    desc = Plan()
     fn = lib().svgb_attn_plan_varblock_gather if gather else lib().svgb_attn_plan_varblock
     check(fn(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, S, QC, KC, ws.data_ptr(), ws.numel(), C.byref(desc),
              _stream(m)), "svgb_attn_plan_varblock")
@@ -186,21 +206,70 @@ def _geometry(q, layout):
     raise SvgbError(f"unknown layout {layout}")
 
 
+def _kv_geometry(q, k, layout):
+    """(BH, Sq, Skv, D, q strides, k/v strides) when k's sequence length differs from q's; k must match q in every
+    other dimension."""
+    BH, Sq, D, qrs, qhs = _geometry(q, layout)
+    if q.dim() != k.dim():
+        raise SvgbError(f"q {tuple(q.shape)} and k {tuple(k.shape)} differ in rank")
+    BHk, Skv, Dk, kvrs, kvhs = _geometry(k, layout)
+    seq = 2 if layout == "bhsd" else 0
+    if [n for i, n in enumerate(q.shape) if i != seq] != [n for i, n in enumerate(k.shape) if i != seq]:
+        raise SvgbError(f"q {tuple(q.shape)} and k, v {tuple(k.shape)} may differ in the sequence length only")
+    return BH, Sq, Skv, D, (qrs, qhs), (kvrs, kvhs)
+
+
+def _attn_kv(q, k, v, o, plan, layout, return_lse, sm_scale):
+    """One svgb_attn_fwd_kv launch: q and o over Sq rows, k and v over Skv rows, each pair with its own strides.
+    Variable-block plans, 16-bit inputs.  attn_fwd takes it when the lengths differ; with equal lengths it gives
+    attn_fwd's bits (the svgb_attn_fwd launch)."""
+    BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
+    lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device) if return_lse else None
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    check(lib().svgb_attn_fwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), _dt(q), BH, Sq,
+                                 Skv, D, *qs, *kvs, *qs, scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
+          "svgb_attn_fwd_kv")
+    _bump()
+    return (o, lse) if return_lse else o
+
+
 def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[torch.Tensor] = None,
              q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
              return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
     """layout 'bhsd': q,k,v [B,H,S,D] contiguous;  'shd': [S,H,D] contiguous (ops API).
     o_rows scatters the output rows; q_rows / kv_rows gather the input rows and need a gather plan
-    (plan_varblock(..., gather=True)); all three are int [BH,S] (include/svgb200.h, svgb_attn_fwd)."""
+    (plan_varblock(..., gather=True)); all three are int [BH,S] (include/svgb200.h, svgb_attn_fwd).
+    k, v may have another sequence length S_kv than q (same batch, heads, D and dtype): the plan is then a rectangular
+    variable-block plan (plan_varblock(..., S_kv=)), o has q's shape, and row vectors are not taken."""
     _need_cuda(q, k, v)
     if not (q.is_contiguous() and k.is_contiguous() and v.is_contiguous()):
         raise SvgbError("q, k, v must be contiguous")
-    if not (q.dtype == k.dtype == v.dtype) or not (q.shape == k.shape == v.shape):
-        raise SvgbError("q, k, v must share dtype and shape")
-    BH, S, D, rs, hs = _geometry(q, layout)
+    if not (q.dtype == k.dtype == v.dtype) or k.shape != v.shape:
+        raise SvgbError("q, k, v must share dtype, and k, v their shape")
     o = torch.empty_like(q) if out is None else out
+    if q.shape != k.shape:
+        if o_rows is not None or q_rows is not None or kv_rows is not None:
+            raise SvgbError("row vectors (o_rows / q_rows / kv_rows) need k, v of q's sequence length")
+        return _attn_kv(q, k, v, o, plan, layout, return_lse, sm_scale)
+    BH, S, D, rs, hs = _geometry(q, layout)
     return _attn(q, k, v, (None, None, None), o, _dt(q), plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows,
                  return_lse, sm_scale)
+
+
+def _attn_bwd_kv(q, k, v, o, do, lse, plan, plan_t, dq, dk, dv, layout, sm_scale):
+    """One svgb_attn_bwd_kv call (the delta and two kernel launches): q, o, do, dq over Sq rows, k, v, dk, dv over Skv
+    rows.  attn_bwd takes it when the lengths differ; with equal lengths it gives attn_bwd's bits."""
+    BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_bwd_kv_bytes(BH, Sq, Skv, C.byref(nbytes)), "svgb_attn_bwd_kv_bytes")
+    ws = workspace(("attn_bwd", BH, Sq), nbytes.value, q.device)
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    check(lib().svgb_attn_bwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                 lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, Sq, Skv, D,
+                                 *qs, *kvs, scale, C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc),
+                                 plan_t.ws.data_ptr(), ws.data_ptr(), ws.numel(), _stream(q)), "svgb_attn_bwd_kv")
+    _bump(3)
+    return dq, dk, dv
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
@@ -208,15 +277,24 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
     """Gradients (dq, dk, dv) of o = attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale) for the output gradient
     do; lse is the forward's return_lse output.  Variable-block and band plans (mask NONE / HY / WAN / COG); the plan's
     key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits.
-    out: optional (dq, dk, dv) tensors of q's dtype and shape, contiguous, written and returned instead of new ones."""
+    k, v may have another sequence length than q under a rectangular variable-block plan; dk, dv then have k's shape.
+    out: optional (dq, dk, dv) tensors of q's, k's and v's dtype and shape, contiguous, written and returned instead
+    of new ones."""
     _need_cuda(q, k, v, o, do, lse)
     ts = (q, k, v, o, do) + (tuple(out) if out is not None else ())
     if out is not None and len(out) != 3:
         raise SvgbError("out must be a (dq, dk, dv) tuple")
     if not all(t.is_contiguous() for t in ts):
         raise SvgbError("q, k, v, o, do (and out) must be contiguous")
-    if not all(t.dtype == q.dtype and t.shape == q.shape for t in ts):
-        raise SvgbError("q, k, v, o, do (and out) must share dtype and shape")
+    like = (q, k, k, q, q) + ((q, k, k) if out is not None else ())
+    if not all(t.dtype == q.dtype and t.shape == r.shape for t, r in zip(ts, like)):
+        raise SvgbError("q, k, v, o, do (and out) must share dtype; o, do, dq have q's shape, v, dk, dv k's")
+    if q.shape != k.shape:
+        plan_t = plan.key_major()
+        dq, dk, dv = (torch.empty_like(t) for t in (q, k, v)) if out is None else out
+        _need_cuda(dq, dk, dv)
+        return _attn_bwd_kv(q, k, v, o, do, lse.to(torch.float32).contiguous(), plan, plan_t, dq, dk, dv, layout,
+                            sm_scale)
     BH, S, D, rs, hs = _geometry(q, layout)
     plan_t = plan.key_major()
     lse = lse.to(torch.float32).contiguous()

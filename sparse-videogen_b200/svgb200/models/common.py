@@ -76,16 +76,42 @@ def sparse_flex_attention_fp8(query, key, value, block_mask: BandMask):
     return fp8_attention(query, key, value, block_mask.plan)
 
 
-def dense_attention(query, key, value, seg_lens=None):
+def check_segments(what, segs, kv_segs, S, S_kv):
+    """Segment lists that pair query segment i with key segment i must be as many and sum to the two lengths: the plan's
+    block sizes are not checked on the device, and key blocks past S_kv would have dK / dV rows stored past the end of
+    k's gradient.  Only the call with equal lengths and equal lists skips this check, as it did before S_kv existed."""
+    if S_kv == S and kv_segs == segs:
+        return
+    if len(kv_segs) != len(segs) or sum(segs) != S or sum(kv_segs) != S_kv:
+        raise core.SvgbError(f"{what}: query segments {segs} must sum to {S} and key segments {kv_segs} to {S_kv}, "
+                             "one key segment per query segment")
+
+
+def dense_attention(query, key, value, seg_lens=None, kv_seg_lens=None):
     """Dense fall-back (b11).  seg_lens: optional list of segment lengths that only attend inside
-    themselves (HunyuanVideo's padded-prompt varlen split, hyvideo/attention.py:308-316,807-875)."""
+    themselves (HunyuanVideo's padded-prompt varlen split, hyvideo/attention.py:308-316,807-875).
+    key / value may be longer or shorter than query (cross-attention, [cfg,H,S_kv,D]); kv_seg_lens then gives their
+    segments, query segment i attending key segment i (None: the whole key sequence, or seg_lens when the lengths
+    match).  Differentiable when an input requires grad (core.attention)."""
     cfg, H, S, D = query.shape
+    S_kv = key.shape[2]
     dev = query.device
     segs = [S] if seg_lens is None else [int(x) for x in seg_lens]
+    if kv_seg_lens is None and seg_lens is None:
+        kv_segs = [S_kv]
+    elif kv_seg_lens is None and S_kv == S:
+        kv_segs = segs
+    elif kv_seg_lens is None:
+        raise core.SvgbError(f"dense_attention: {len(segs)} query segments and a key sequence of another length "
+                             f"({S} vs {S_kv}) need kv_seg_lens")
+    else:
+        kv_segs = [int(x) for x in kv_seg_lens]
+    check_segments("dense_attention", segs, kv_segs, S, S_kv)
     n = len(segs)
     bm = torch.eye(n, dtype=torch.bool, device=dev).expand(cfg * H, n, n).contiguous()
     sz = torch.tensor(segs, dtype=torch.int32, device=dev).expand(cfg * H, n).contiguous()
-    plan = core.plan_varblock(bm, sz, sz, S)
+    kv_sz = sz if kv_segs == segs else torch.tensor(kv_segs, dtype=torch.int32, device=dev).expand(cfg * H, n).contiguous()
+    plan = core.plan_varblock(bm, sz, kv_sz, S, S_kv=S_kv)
     if core.needs_grad(query, key, value):
         return core.attention(query, key, value, plan)
     return core.attn_fwd(query, key, value, plan)

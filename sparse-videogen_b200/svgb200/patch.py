@@ -61,28 +61,52 @@ def flex_attention_fp8(query, key, value, block_mask=None, **kw):
     return _flex_attention("flex_attention_fp8", sparse_flex_attention_fp8, query, key, value, block_mask, kw)
 
 
+def _varlen_segments(cu_seqlens_q, cu_seqlens_kv):
+    """(query segments, key segments) of a varlen call: segment i of the queries attends segment i of the keys.  When
+    the two give the same lengths both are the non-empty query segments (the same object); otherwise only the pairs
+    where both sides are empty are dropped (queries whose key segment is empty have no keys and get 0)."""
+    seg_q = (cu_seqlens_q[1:] - cu_seqlens_q[:-1]).tolist()
+    seg_kv = seg_q if cu_seqlens_kv is cu_seqlens_q else (cu_seqlens_kv[1:] - cu_seqlens_kv[:-1]).tolist()
+    if seg_kv == seg_q:
+        seg = [n for n in seg_q if n > 0]
+        return seg, seg
+    if len(seg_kv) != len(seg_q):
+        from .core import SvgbError
+
+        raise SvgbError(f"cu_seqlens_q and cu_seqlens_kv must hold the same number of segments "
+                        f"({len(seg_q)} vs {len(seg_kv)})")
+    pairs = [(a, b) for a, b in zip(seg_q, seg_kv) if a > 0 or b > 0]
+    return [a for a, _ in pairs], [b for _, b in pairs]
+
+
 def flashinfer_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv):
-    """hyvideo/attention.py:807-875: dense attention inside each cu_seqlens segment, q,k,v [B,H,S,D]."""
+    """hyvideo/attention.py:807-875: dense attention inside each cu_seqlens segment, q,k,v [B,H,S,D].  Query segment i
+    attends key segment i (cu_seqlens_kv; k, v may be longer or shorter than q)."""
     from .models.common import dense_attention
 
-    seg = [n for n in (cu_seqlens_q[1:] - cu_seqlens_q[:-1]).tolist() if n > 0]
-    return dense_attention(q, k, v, seg)
+    seg, seg_kv = _varlen_segments(cu_seqlens_q, cu_seqlens_kv)
+    return dense_attention(q, k, v, seg, None if seg_kv is seg and k.shape[2] == q.shape[2] else seg_kv)
 
 
 def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, **kw):
     """flash_attn.flash_attn_interface.flash_attn_varlen_func as hyvideo/attention.py:452-470 calls it: q,k,v
-    [L, B*H, D] (sequence first), segments given by cu_seqlens."""
+    [L, B*H, D] (sequence first), segments given by cu_seqlens: query segment i attends key segment i (k, v may have
+    another length than q)."""
     from . import core
+    from .models.common import check_segments
 
     S, BH, D = q.shape
-    seg = [n for n in (cu_seqlens_q[1:] - cu_seqlens_q[:-1]).tolist() if n > 0]
+    S_kv = k.shape[0]
+    seg, seg_kv = _varlen_segments(cu_seqlens_q, cu_seqlens_kv)
+    check_segments("flash_attn_varlen_func", seg, seg_kv, S, S_kv)
     dev = q.device
     n = len(seg)
     import torch
 
     bm = torch.eye(n, dtype=torch.bool, device=dev).expand(BH, n, n).contiguous()
     sz = torch.tensor(seg, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
-    plan = core.plan_varblock(bm, sz, sz, S)
+    sz_kv = sz if seg_kv is seg else torch.tensor(seg_kv, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
+    plan = core.plan_varblock(bm, sz, sz_kv, S, S_kv=S_kv)
     if core.needs_grad(q, k, v):
         return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
     return core.attn_fwd(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
