@@ -1018,6 +1018,21 @@ def _mod_vec(v, N):
     return v, v.shape[0]
 
 
+def _out_dt(out_dtype) -> int:
+    if out_dtype not in _TORCH_DT:
+        raise SvgbError(f"unsupported out_dtype {out_dtype}: bfloat16, float16 or float32")
+    return _TORCH_DT[out_dtype]
+
+
+def _norm_weights(N, weight, bias=None):
+    """The glue's norm weight and bias: [N] each, and one dtype (the kernel reads both with one w_dtype)."""
+    for name, t in (("weight", weight), ("bias", bias)):
+        if t is not None and t.numel() != N:
+            raise SvgbError(f"{name} must hold the hidden size {N} elements, got {t.numel()}")
+    if weight is not None and bias is not None and bias.dtype != weight.dtype:
+        raise SvgbError(f"bias dtype {bias.dtype} differs from weight dtype {weight.dtype}")
+
+
 def _rows_per_batch(rows, nb):
     if nb == 1:
         return 0
@@ -1028,10 +1043,11 @@ def _rows_per_batch(rows, nb):
 
 def layernorm_modulate(x, weight=None, bias=None, eps=1e-6, scale=None, shift=None, out_dtype=None):
     _no_backward("layernorm_modulate", x, weight, bias, scale, shift)
-    _need_cuda(x, weight, bias, scale, shift)
-    _contig(x, weight, bias)
     N = x.shape[-1]
     rows = x.numel() // N
+    out_dtype = out_dtype or torch.float32
+    y_dt = _out_dt(out_dtype)
+    _norm_weights(N, weight, bias)
     rpb = 0
     if scale is not None:
         scale, nb = _mod_vec(scale, N)
@@ -1039,10 +1055,12 @@ def layernorm_modulate(x, weight=None, bias=None, eps=1e-6, scale=None, shift=No
         if nb != nb2:
             raise SvgbError("scale and shift must have the same batch")
         rpb = _rows_per_batch(rows, nb)
-    y = torch.empty(x.shape, dtype=out_dtype or torch.float32, device=x.device)
+    _need_cuda(x, weight, bias, scale, shift)
+    _contig(x, weight, bias)
+    y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
     check(lib().svgb_layernorm_modulate(x.data_ptr(), _dt3(x), _p(weight), _p(bias),
                                         _dt3(weight) if weight is not None else 0, float(eps), _p(scale), _p(shift),
-                                        rpb, y.data_ptr(), _TORCH_DT[y.dtype], rows, N, _stream(x)),
+                                        rpb, y.data_ptr(), y_dt, rows, N, _stream(x)),
           "svgb_layernorm_modulate")
     _bump()
     return y
@@ -1050,43 +1068,52 @@ def layernorm_modulate(x, weight=None, bias=None, eps=1e-6, scale=None, shift=No
 
 def rmsnorm_hidden(x, weight, eps, out_dtype=None):
     _no_backward("rmsnorm_hidden", x, weight)
+    N = x.shape[-1]
+    out_dtype = out_dtype or x.dtype
+    y_dt = _out_dt(out_dtype)
+    _norm_weights(N, weight)
     _need_cuda(x, weight)
     _contig(x, weight)
-    N = x.shape[-1]
-    y = torch.empty(x.shape, dtype=out_dtype or x.dtype, device=x.device)
+    y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
     check(lib().svgb_rmsnorm_hidden(x.data_ptr(), _dt3(x), weight.data_ptr(), _dt3(weight), float(eps), y.data_ptr(),
-                                    _TORCH_DT[y.dtype], x.numel() // N, N, _stream(x)), "svgb_rmsnorm_hidden")
+                                    y_dt, x.numel() // N, N, _stream(x)), "svgb_rmsnorm_hidden")
     _bump()
     return y
 
 
 def modulate_shift(x, scale, shift, out_dtype=torch.float32):
     _no_backward("modulate_shift", x, scale, shift)
-    _need_cuda(x, scale, shift)
-    _contig(x)
     N = x.shape[-1]
     rows = x.numel() // N
+    y_dt = _out_dt(out_dtype)
     scale, nb = _mod_vec(scale, N)
-    shift, _ = _mod_vec(shift, N)
+    shift, nb2 = _mod_vec(shift, N)
+    if nb != nb2:
+        raise SvgbError("scale and shift must have the same batch")
+    rpb = _rows_per_batch(rows, nb)
+    _need_cuda(x, scale, shift)
+    _contig(x)
     y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
-    check(lib().svgb_modulate_shift(x.data_ptr(), _dt3(x), scale.data_ptr(), shift.data_ptr(), _rows_per_batch(rows, nb),
-                                    y.data_ptr(), _TORCH_DT[y.dtype], rows, N, _stream(x)), "svgb_modulate_shift")
+    check(lib().svgb_modulate_shift(x.data_ptr(), _dt3(x), scale.data_ptr(), shift.data_ptr(), rpb, y.data_ptr(), y_dt,
+                                    rows, N, _stream(x)), "svgb_modulate_shift")
     _bump()
     return y
 
 
 def gate_residual(residual, x, gate, out_dtype=torch.float32):
     _no_backward("gate_residual", residual, x, gate)
-    _need_cuda(residual, x, gate)
-    _contig(residual, x)
     if residual.shape != x.shape:
         raise SvgbError("residual and x must have the same shape")
     N = x.shape[-1]
     rows = x.numel() // N
+    y_dt = _out_dt(out_dtype)
     gate, nb = _mod_vec(gate, N)
+    rpb = _rows_per_batch(rows, nb)
+    _need_cuda(residual, x, gate)
+    _contig(residual, x)
     y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
     check(lib().svgb_gate_residual(residual.data_ptr(), _dt3(residual), x.data_ptr(), _dt3(x), gate.data_ptr(),
-                                   _rows_per_batch(rows, nb), y.data_ptr(), _TORCH_DT[y.dtype], rows, N, _stream(x)),
+                                   rpb, y.data_ptr(), y_dt, rows, N, _stream(x)),
           "svgb_gate_residual")
     _bump()
     return y
