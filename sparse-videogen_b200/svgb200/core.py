@@ -138,23 +138,18 @@ def plan_varblock(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.T
     m = m.view(torch.uint8) if m.dtype == torch.bool else m.to(torch.uint8)
     r = row_sz.reshape(BH, QC).to(torch.int32).contiguous()
     c = col_sz.reshape(BH, KC).to(torch.int32).contiguous()
+    rect = S_kv is not None and S_kv != S
+    if rect and gather:
+        raise SvgbError(f"gather plans need S_kv == S (got S={S}, S_kv={S_kv}): the rectangular plan is TMA only")
+    # the rectangular planner pair takes S_kv after S; the square and gather planners share one workspace query
+    name, lens = ("svgb_attn_plan_varblock_kv", (S, S_kv)) if rect else ("svgb_attn_plan_varblock", (S,))
     nbytes = C.c_size_t()
-    desc = Plan()
-    if S_kv is not None and S_kv != S:
-        if gather:
-            raise SvgbError(f"gather plans need S_kv == S (got S={S}, S_kv={S_kv}): the rectangular plan is TMA only")
-        check(lib().svgb_attn_plan_varblock_kv_bytes(BH, S, S_kv, QC, KC, C.byref(nbytes)), "plan_varblock_kv_bytes")
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=m.device)
-        check(lib().svgb_attn_plan_varblock_kv(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, S, S_kv, QC, KC,
-                                               ws.data_ptr(), ws.numel(), C.byref(desc), _stream(m)),
-              "svgb_attn_plan_varblock_kv")
-        _bump()
-        return AttnPlan(desc, ws, (m, r, c, (m._version, r._version, c._version)))
-    check(lib().svgb_attn_plan_varblock_bytes(BH, S, QC, KC, C.byref(nbytes)), "plan_varblock_bytes")
+    check(getattr(lib(), name + "_bytes")(BH, *lens, QC, KC, C.byref(nbytes)), name + "_bytes")
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=m.device)
-    fn = lib().svgb_attn_plan_varblock_gather if gather else lib().svgb_attn_plan_varblock
-    check(fn(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, S, QC, KC, ws.data_ptr(), ws.numel(), C.byref(desc),
-             _stream(m)), "svgb_attn_plan_varblock")
+    desc = Plan()
+    name += "_gather" if gather else ""
+    check(getattr(lib(), name)(m.data_ptr(), r.data_ptr(), c.data_ptr(), BH, *lens, QC, KC, ws.data_ptr(), ws.numel(),
+                               C.byref(desc), _stream(m)), name)
     _bump()
     return AttnPlan(desc, ws, None if gather else (m, r, c, (m._version, r._version, c._version)))
 
@@ -184,18 +179,6 @@ def plan_band_t(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, devi
 # ----------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------
-def _attn(q, k, v, scales, o, dtype, plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows, return_lse, sm_scale):
-    """One svgb_attn_fwd launch; q, k, v and o share the row / head strides rs, hs (elements)."""
-    rows = [None if r is None else r.reshape(BH, S).to(torch.int32).contiguous() for r in (q_rows, kv_rows, o_rows)]
-    lse = torch.empty(BH, S, dtype=torch.float32, device=q.device) if return_lse else None
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    check(lib().svgb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), *map(_p, scales), o.data_ptr(), _p(lse),
-                              *map(_p, rows), dtype, BH, S, D, rs, hs, rs, hs, scale, C.byref(plan.desc),
-                              plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd")
-    _bump()
-    return (o, lse) if return_lse else o
-
-
 def _geometry(q, layout):
     if layout == "bhsd":
         B, H, S, D = q.shape
@@ -207,8 +190,8 @@ def _geometry(q, layout):
 
 
 def _kv_geometry(q, k, layout):
-    """(BH, Sq, Skv, D, q strides, k/v strides) when k's sequence length differs from q's; k must match q in every
-    other dimension."""
+    """(BH, Sq, Skv, D, q strides, k/v strides); k's sequence length may differ from q's, every other dimension must
+    match."""
     BH, Sq, D, qrs, qhs = _geometry(q, layout)
     if q.dim() != k.dim():
         raise SvgbError(f"q {tuple(q.shape)} and k {tuple(k.shape)} differ in rank")
@@ -219,16 +202,22 @@ def _kv_geometry(q, k, layout):
     return BH, Sq, Skv, D, (qrs, qhs), (kvrs, kvhs)
 
 
-def _attn_kv(q, k, v, o, plan, layout, return_lse, sm_scale):
-    """One svgb_attn_fwd_kv launch: q and o over Sq rows, k and v over Skv rows, each pair with its own strides.
-    Variable-block plans, 16-bit inputs.  attn_fwd takes it when the lengths differ; with equal lengths it gives
-    attn_fwd's bits (the svgb_attn_fwd launch)."""
+def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
+    """One attention launch.  Equal sequence lengths take svgb_attn_fwd: 16-bit or e4m3 (dtype) with its per-head
+    scales, and the row vectors rows = (q_rows, kv_rows, o_rows).  Otherwise svgb_attn_fwd_kv: q and o over Sq rows,
+    k and v over Skv rows, each pair with its own strides; 16-bit, no scales, no row vectors."""
     BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
     lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    check(lib().svgb_attn_fwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), _dt(q), BH, Sq,
-                                 Skv, D, *qs, *kvs, *qs, scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
-          "svgb_attn_fwd_kv")
+    if Sq == Skv:
+        rows = [None if r is None else r.reshape(BH, Sq).to(torch.int32).contiguous() for r in rows]
+        check(lib().svgb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), *map(_p, scales), o.data_ptr(), _p(lse),
+                                  *map(_p, rows), dtype, BH, Sq, D, *qs, *qs, scale, C.byref(plan.desc),
+                                  plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd")
+    else:
+        check(lib().svgb_attn_fwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), dtype, BH, Sq,
+                                     Skv, D, *qs, *kvs, *qs, scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
+              "svgb_attn_fwd_kv")
     _bump()
     return (o, lse) if return_lse else o
 
@@ -247,29 +236,9 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     if not (q.dtype == k.dtype == v.dtype) or k.shape != v.shape:
         raise SvgbError("q, k, v must share dtype, and k, v their shape")
     o = torch.empty_like(q) if out is None else out
-    if q.shape != k.shape:
-        if o_rows is not None or q_rows is not None or kv_rows is not None:
-            raise SvgbError("row vectors (o_rows / q_rows / kv_rows) need k, v of q's sequence length")
-        return _attn_kv(q, k, v, o, plan, layout, return_lse, sm_scale)
-    BH, S, D, rs, hs = _geometry(q, layout)
-    return _attn(q, k, v, (None, None, None), o, _dt(q), plan, BH, S, D, rs, hs, o_rows, q_rows, kv_rows,
-                 return_lse, sm_scale)
-
-
-def _attn_bwd_kv(q, k, v, o, do, lse, plan, plan_t, dq, dk, dv, layout, sm_scale):
-    """One svgb_attn_bwd_kv call (the delta and two kernel launches): q, o, do, dq over Sq rows, k, v, dk, dv over Skv
-    rows.  attn_bwd takes it when the lengths differ; with equal lengths it gives attn_bwd's bits."""
-    BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
-    nbytes = C.c_size_t()
-    check(lib().svgb_attn_bwd_kv_bytes(BH, Sq, Skv, C.byref(nbytes)), "svgb_attn_bwd_kv_bytes")
-    ws = workspace(("attn_bwd", BH, Sq), nbytes.value, q.device)
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    check(lib().svgb_attn_bwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
-                                 lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, Sq, Skv, D,
-                                 *qs, *kvs, scale, C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc),
-                                 plan_t.ws.data_ptr(), ws.data_ptr(), ws.numel(), _stream(q)), "svgb_attn_bwd_kv")
-    _bump(3)
-    return dq, dk, dv
+    if q.shape != k.shape and (o_rows is not None or q_rows is not None or kv_rows is not None):
+        raise SvgbError("row vectors (o_rows / q_rows / kv_rows) need k, v of q's sequence length")
+    return _attn(q, k, v, o, plan, layout, _dt(q), (None, None, None), (q_rows, kv_rows, o_rows), return_lse, sm_scale)
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
@@ -289,25 +258,21 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
     like = (q, k, k, q, q) + ((q, k, k) if out is not None else ())
     if not all(t.dtype == q.dtype and t.shape == r.shape for t, r in zip(ts, like)):
         raise SvgbError("q, k, v, o, do (and out) must share dtype; o, do, dq have q's shape, v, dk, dv k's")
-    if q.shape != k.shape:
-        plan_t = plan.key_major()
-        dq, dk, dv = (torch.empty_like(t) for t in (q, k, v)) if out is None else out
-        _need_cuda(dq, dk, dv)
-        return _attn_bwd_kv(q, k, v, o, do, lse.to(torch.float32).contiguous(), plan, plan_t, dq, dk, dv, layout,
-                            sm_scale)
-    BH, S, D, rs, hs = _geometry(q, layout)
+    BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
     plan_t = plan.key_major()
     lse = lse.to(torch.float32).contiguous()
+    # equal lengths take svgb_attn_bwd, whose q and k share one length and one pair of strides
+    name, lens, strides = ("svgb_attn_bwd", (Sq,), qs) if Sq == Skv else ("svgb_attn_bwd_kv", (Sq, Skv), qs + kvs)
     nbytes = C.c_size_t()
-    check(lib().svgb_attn_bwd_bytes(BH, S, C.byref(nbytes)), "svgb_attn_bwd_bytes")
-    ws = workspace(("attn_bwd", BH, S), nbytes.value, q.device)
-    dq, dk, dv = (torch.empty_like(q) for _ in range(3)) if out is None else out
+    check(getattr(lib(), name + "_bytes")(BH, *lens, C.byref(nbytes)), name + "_bytes")
+    ws = workspace(("attn_bwd", BH, Sq), nbytes.value, q.device)
+    dq, dk, dv = (torch.empty_like(t) for t in (q, k, v)) if out is None else out
     _need_cuda(dq, dk, dv)
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    check(lib().svgb_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
-                              dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, S, D, rs, hs, scale,
-                              C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc), plan_t.ws.data_ptr(),
-                              ws.data_ptr(), ws.numel(), _stream(q)), "svgb_attn_bwd")
+    check(getattr(lib(), name)(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
+                               dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, *lens, D, *strides, scale,
+                               C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc), plan_t.ws.data_ptr(),
+                               ws.data_ptr(), ws.numel(), _stream(q)), name)
     _bump(3)
     return dq, dk, dv
 
@@ -328,16 +293,20 @@ class _Attention(torch.autograd.Function):
 
 
 def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None):
-    """attn_fwd as a differentiable op: the forward keeps its LSE and the backward runs attn_bwd.  Plans without a
-    backward (gather plans, the profiling masks) are rejected here, before the forward runs."""
+    """attn_fwd, differentiable when an input requires grad (needs_grad): the forward then keeps its LSE and the
+    backward runs attn_bwd, and plans without a backward (gather plans, the profiling masks) are rejected before the
+    forward runs.  Otherwise it is exactly attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale): one launch, no
+    LSE, and the plan is not read here."""
+    if not needs_grad(q, k, v):
+        return attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale)
     if plan.desc.kind == PLAN_GATHER or (plan.desc.kind == PLAN_BAND and plan.desc.mask_mode > MASK_COG):
         plan.key_major()  # raises, naming what has no backward
     return _Attention.apply(q, k, v, plan, layout, sm_scale)
 
 
 def needs_grad(*ts) -> bool:
-    """True when autograd would record an op on these tensors: the attention entry points then take attention(), the
-    layout ops _HeadPlacement / _Permute, the pre-attention chain _RowNorm / _QkRope / _QkvPrep."""
+    """True when autograd would record an op on these tensors: attention() then records _Attention, and the layout
+    ops _HeadPlacement / _Permute and the pre-attention chain _RowNorm / _QkRope / _QkvPrep their own functions."""
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
 
 
@@ -417,8 +386,7 @@ def attn_fwd_fp8(q8, k8, v8, q_scale, k_scale, v_scale, plan: AttnPlan, *, o_row
     # by the allocator for the next one and alias two operands)
     q8c, k8c, v8c = q8.contiguous(), k8.contiguous(), v8.contiguous()
     scales = tuple(t.to(torch.float32).contiguous() for t in (q_scale, k_scale, v_scale))
-    return _attn(q8c, k8c, v8c, scales, o, _E4M3, plan, B * H, S, D, D, S * D, o_rows, q_rows, kv_rows, return_lse,
-                 sm_scale)
+    return _attn(q8c, k8c, v8c, o, plan, "bhsd", _E4M3, scales, (q_rows, kv_rows, o_rows), return_lse, sm_scale)
 
 
 def density(block_map, row_sz, col_sz):
@@ -660,8 +628,8 @@ def _contig(*ts):
 
 
 def _no_backward(what, *ts):
-    """Ops without a backward raise under grad rather than return a result detached from the graph (the message of
-    models.common.check_no_grad)."""
+    """Ops and attention paths without a backward raise under grad rather than return a result detached from the
+    graph."""
     if needs_grad(*ts):
         raise SvgbError(f"{what} has no backward: call it on tensors that do not require grad "
                         "(or under torch.no_grad())")

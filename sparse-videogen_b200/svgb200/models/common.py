@@ -37,16 +37,7 @@ class BandMask:
 def sparse_flex_attention(query, key, value, block_mask: BandMask):
     """hyvideo/attention.py:401-403: flex_attention(q, k, v, block_mask=...)  [cfg,H,S,D].  Differentiable when an input
     requires grad (core.attention)."""
-    if core.needs_grad(query, key, value):
-        return core.attention(query, key, value, block_mask.plan)
-    return core.attn_fwd(query, key, value, block_mask.plan)
-
-
-def check_no_grad(what, *ts):
-    """Attention paths without a backward raise rather than return a result detached from the graph."""
-    if core.needs_grad(*ts):
-        raise core.SvgbError(f"{what} has no backward: call it on tensors that do not require grad "
-                             "(or under torch.no_grad())")
+    return core.attention(query, key, value, block_mask.plan)
 
 
 def check_fp8_head_dim(D):
@@ -63,7 +54,7 @@ def fp8_attention(query, key, value, plan: core.AttnPlan, **rows):
     """Attention under `plan` in FP8: Q, K, V [B,H,S,128] quantised to e4m3 per head and run on the e4m3 kernel
     (rows: q_rows / kv_rows / o_rows of core.attn_fwd_fp8).  The kernel writes bf16; the result comes back in
     query.dtype.  FP8 attention has no backward: an input that requires grad raises."""
-    check_no_grad("fp8 attention", query, key, value)
+    core._no_backward("fp8 attention", query, key, value)
     check_fp8_head_dim(query.shape[-1])
     (q8, sq), (k8, sk), (v8, sv) = quantize_qkv(query, key, value)
     return core.attn_fwd_fp8(q8, k8, v8, sq, sk, sv, plan, **rows).to(query.dtype)
@@ -71,7 +62,7 @@ def fp8_attention(query, key, value, plan: core.AttnPlan, **rows):
 
 def sparse_flex_attention_fp8(query, key, value, block_mask: BandMask):
     """sparse_flex_attention in FP8 (fp8_attention under the band plan)."""
-    check_no_grad("fp8 attention", query, key, value)
+    core._no_backward("fp8 attention", query, key, value)
     check_fp8_head_dim(query.shape[-1])  # before block_mask is read: a head_dim-64 model fails on its cause
     return fp8_attention(query, key, value, block_mask.plan)
 
@@ -87,15 +78,34 @@ def check_segments(what, segs, kv_segs, S, S_kv):
                              "one key segment per query segment")
 
 
+def segment_attention(what, query, key, value, segs, kv_segs, layout="bhsd"):
+    """core.attention in which query segment i attends key segment i only: the segment lists pass check_segments
+    (`what` names the caller in its error), then one rectangular plan of the diagonal block map over them.  layout
+    'bhsd' or 'shd', as core.attention takes it."""
+    seq = 2 if layout == "bhsd" else 0
+    S, S_kv = query.shape[seq], key.shape[seq]
+    check_segments(what, segs, kv_segs, S, S_kv)
+    BH = query.shape[0] * query.shape[1] if layout == "bhsd" else query.shape[1]
+    n, dev = len(segs), query.device
+    bm = torch.eye(n, dtype=torch.bool, device=dev).expand(BH, n, n).contiguous()
+    sz = torch.tensor(segs, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
+    kv_sz = sz if kv_segs == segs else torch.tensor(kv_segs, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
+    plan = core.plan_varblock(bm, sz, kv_sz, S, S_kv=S_kv)
+    return core.attention(query, key, value, plan, layout=layout)
+
+
+def segment_lengths(cu_seqlens):
+    """The non-empty segment lengths of one cu_seqlens row, as a host list."""
+    return [s for s in (cu_seqlens[1:] - cu_seqlens[:-1]).tolist() if s > 0]
+
+
 def dense_attention(query, key, value, seg_lens=None, kv_seg_lens=None):
     """Dense fall-back (b11).  seg_lens: optional list of segment lengths that only attend inside
     themselves (HunyuanVideo's padded-prompt varlen split, hyvideo/attention.py:308-316,807-875).
     key / value may be longer or shorter than query (cross-attention, [cfg,H,S_kv,D]); kv_seg_lens then gives their
     segments, query segment i attending key segment i (None: the whole key sequence, or seg_lens when the lengths
     match).  Differentiable when an input requires grad (core.attention)."""
-    cfg, H, S, D = query.shape
-    S_kv = key.shape[2]
-    dev = query.device
+    S, S_kv = query.shape[2], key.shape[2]
     segs = [S] if seg_lens is None else [int(x) for x in seg_lens]
     if kv_seg_lens is None and seg_lens is None:
         kv_segs = [S_kv]
@@ -106,15 +116,7 @@ def dense_attention(query, key, value, seg_lens=None, kv_seg_lens=None):
                              f"({S} vs {S_kv}) need kv_seg_lens")
     else:
         kv_segs = [int(x) for x in kv_seg_lens]
-    check_segments("dense_attention", segs, kv_segs, S, S_kv)
-    n = len(segs)
-    bm = torch.eye(n, dtype=torch.bool, device=dev).expand(cfg * H, n, n).contiguous()
-    sz = torch.tensor(segs, dtype=torch.int32, device=dev).expand(cfg * H, n).contiguous()
-    kv_sz = sz if kv_segs == segs else torch.tensor(kv_segs, dtype=torch.int32, device=dev).expand(cfg * H, n).contiguous()
-    plan = core.plan_varblock(bm, sz, kv_sz, S, S_kv=S_kv)
-    if core.needs_grad(query, key, value):
-        return core.attention(query, key, value, plan)
-    return core.attn_fwd(query, key, value, plan)
+    return segment_attention("dense_attention", query, key, value, segs, kv_segs)
 
 
 class KMeansState:
@@ -199,7 +201,7 @@ class SVG1Core:
     # -- the sparse branch ---------------------------------------------------------------------------
     def sparse_core(self, query, key, value, sampled_rows=None, attn_events=None):
         if self.fp8:
-            check_no_grad("the SVG1 core with fp8 attention", query, key, value)
+            core._no_backward("the SVG1 core with fp8 attention", query, key, value)
         # stage labels = the reference's TIME_BENCH table (hyvideo/attention.py:375,401,405,439)
         with time_logging_decorator("Level 3 - sample mse"):
             sampled_mses = self.sample_mse(query, key, value, sampled_rows)
@@ -229,7 +231,7 @@ class SVG1Core:
         NVLink transfer of head i overlaps the attention of head i+1 (svgb200.parallel.HeadParallel).
         Returns the full [1, H_local * world, S, D] output (heads interleaved: global h = i*world + rank)."""
         # the output is assembled by all-gathers into a plain buffer, outside the autograd graph
-        check_no_grad("the head-parallel SVG1 core (sparse_core_head_parallel)", query, key, value)
+        core._no_backward("the head-parallel SVG1 core (sparse_core_head_parallel)", query, key, value)
         cfg, Hl, S, D = query.shape
         assert cfg == 1
         if trace is not None:
@@ -266,7 +268,7 @@ class SVG1Core:
         group's output is additionally all-gathered into `gathered` [1, H_local*world, S, D] on the device (the
         downstream projection needs every head) on hp's communication stream, overlapping the next group."""
         # heads travel through staging copies, outside the autograd graph
-        check_no_grad("the host-pipelined SVG1 core (sparse_core_from_host)", hq, hk, hv)
+        core._no_backward("the host-pipelined SVG1 core (sparse_core_from_host)", hq, hk, hv)
         cfg, H, S, D = hq.shape
         assert cfg == 1
         dev = self.block_mask.plan.ws.device
@@ -339,11 +341,7 @@ class SVG1Core:
         return ho
 
     def dense_core(self, query, key, value, cu_max_seqlens=None):
-        seg = None
-        if cu_max_seqlens is not None:
-            cu = cu_max_seqlens[0]
-            seg = (cu[1:] - cu[:-1]).tolist()
-            seg = [s for s in seg if s > 0]
+        seg = None if cu_max_seqlens is None else segment_lengths(cu_max_seqlens[0])
         with time_logging_decorator("Level 3 - Dense Flash Attention"):
             return dense_attention(query, key, value, seg)
 
@@ -426,7 +424,7 @@ class SAPCore:
         cfg, H, S, D = query.shape
         assert cfg == 1, "Batch size must be 1 for kmeans block sparse attention"
         # the permutations and the fused inverse-permutation store have no backward
-        check_no_grad("the SVG2 sparse core (clustered permutation, o_rows)", query, key, value)
+        core._no_backward("the SVG2 sparse core (clustered permutation, o_rows)", query, key, value)
         if self.fp8:
             check_fp8_head_dim(D)
         layer_idx = self.layer_idx if layer_idx is None else layer_idx
@@ -493,9 +491,6 @@ class SAPCore:
             if self.zero_step_kmeans_init:
                 V = self.num_frame * self.frame_size
                 self.kmeans_clustering(query[:, :, :V].contiguous(), key[:, :, :V].contiguous(), layer_idx)
-            seg = None
-            if cu_max_seqlens is not None:
-                cu = cu_max_seqlens[0]
-                seg = [s for s in (cu[1:] - cu[:-1]).tolist() if s > 0]
+            seg = None if cu_max_seqlens is None else segment_lengths(cu_max_seqlens[0])
             return dense_attention(query, key, value, seg)
         return self.sparse_core(query, key, value, layer_idx, timestep)

@@ -92,24 +92,11 @@ def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, m
     """flash_attn.flash_attn_interface.flash_attn_varlen_func as hyvideo/attention.py:452-470 calls it: q,k,v
     [L, B*H, D] (sequence first), segments given by cu_seqlens: query segment i attends key segment i (k, v may have
     another length than q)."""
-    from . import core
-    from .models.common import check_segments
+    from .models.common import segment_attention
 
-    S, BH, D = q.shape
-    S_kv = k.shape[0]
     seg, seg_kv = _varlen_segments(cu_seqlens_q, cu_seqlens_kv)
-    check_segments("flash_attn_varlen_func", seg, seg_kv, S, S_kv)
-    dev = q.device
-    n = len(seg)
-    import torch
-
-    bm = torch.eye(n, dtype=torch.bool, device=dev).expand(BH, n, n).contiguous()
-    sz = torch.tensor(seg, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
-    sz_kv = sz if seg_kv is seg else torch.tensor(seg_kv, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
-    plan = core.plan_varblock(bm, sz, sz_kv, S, S_kv=S_kv)
-    if core.needs_grad(q, k, v):
-        return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
-    return core.attn_fwd(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
+    return segment_attention("flash_attn_varlen_func", q.contiguous(), k.contiguous(), v.contiguous(), seg, seg_kv,
+                             layout="shd")
 
 
 def _model_of(module):

@@ -222,6 +222,65 @@ def test_autograd_wiring(cuda):
     assert torch.equal(y, ref)
 
 
+@pytest.mark.parametrize("entry", ["sparse_flex_attention", "dense_attention", "dynamic_block_sparse_fwd_flashinfer",
+                                   "flash_attn_varlen_func", "sparse_attn_forward", "wan_sparse_attn_forward",
+                                   "flashinfer_sparse_attn_forward"])
+def test_entries_without_grad_make_one_forward_launch(cuda, entry):
+    """The 16-bit attention entries run core.attention; on inputs that do not require grad that is core.attn_fwd:
+    the entry's own planner launch (none for a prebuilt BandMask plan) and one attention launch, with attn_fwd's bits
+    under the same plan."""
+    from svgb200 import core, kmeans_utils, ops, patch
+    from svgb200.models import common
+    from svgb200.models import hyvideo as hy
+
+    H, D, dtype = 2, 128, torch.bfloat16
+    gen = torch.Generator().manual_seed(17)
+    S, layout, planned = 600, "bhsd", 1
+    if entry == "sparse_flex_attention":
+        ctx, F, P = 64, 3, 128
+        S, planned = ctx + F * P, 0
+        bmask = hy.prepare_flexattention(1, H, D, dtype, cuda, ctx, 20, F, P, diag_width=1.3, multiplier=1.3)
+        call = lambda a, b, c: common.sparse_flex_attention(a, b, c, bmask)  # noqa: E731
+        plan = lambda: bmask.plan  # noqa: E731
+    elif entry in ("dense_attention", "flash_attn_varlen_func"):
+        segs = [S - 77, 77]
+        cu = torch.tensor([0, S - 77, S], dtype=torch.int32, device=cuda)
+        if entry == "dense_attention":
+            call = lambda a, b, c: common.dense_attention(a, b, c, segs)  # noqa: E731
+        else:
+            layout = "shd"
+            call = lambda a, b, c: patch.flash_attn_varlen_func(a, b, c, cu, cu, S - 77, S - 77)  # noqa: E731
+
+        def plan():
+            bm, row, _, _ = varblock_case("varlen", H, S, gen)
+            return core.plan_varblock(bm.to(cuda), row.to(cuda), row.to(cuda), S)
+    elif entry == "dynamic_block_sparse_fwd_flashinfer":
+        maps = [t[None] for t in varblock_case("vb0.5", H, S, gen)[:3]]  # [B, H, ...] on the host, as the reference
+        call = lambda a, b, c: kmeans_utils.dynamic_block_sparse_fwd_flashinfer(a, b, c, *maps)  # noqa: E731
+        plan = lambda: kmeans_utils._flashinfer_plan(q, *maps)  # noqa: E731
+    elif entry == "sparse_attn_forward":  # text first, [S, H, D]; each mask object plans once (ops.bsr_to_plan cache)
+        F, P, T = 6, 160, 16
+        S, layout = F * P + T, "shd"
+        meta = ops.FAMetadata(T, F, P, ops._gen_temporal_mask(F, P, 1.8, device=cuda), None)
+        call = lambda a, b, c: ops.sparse_attn_forward(a, b, c, meta, "temporal")  # noqa: E731
+        plan = lambda: ops.bsr_to_plan(*meta.temporal_mask_metadata, F * P, T, cuda)  # noqa: E731
+    else:
+        F, P = 5, 240
+        S = F * P
+        md = ops.gen_temporal_mask(F, P, 1.3, device=cuda)
+        if entry == "wan_sparse_attn_forward":  # [S, H, D]
+            layout = "shd"
+            call = lambda a, b, c: ops.wan_sparse_attn_forward(a, b, c, ops.WanFAMetadata(F, P, md))  # noqa: E731
+        else:
+            call = lambda a, b, c: ops.flashinfer_sparse_attn_forward(a, b, c, md)  # noqa: E731
+        plan = lambda: ops.bsr_to_plan(*md, S, 0, cuda)  # noqa: E731
+    q, k, v = (to_layout(t, layout).to(cuda) for t in inputs(H, S, D, dtype, gen)[:3])
+    n0 = core.launch_count
+    y = call(q, k, v)
+    assert core.launch_count - n0 == planned + 1
+    assert torch.equal(y, core.attn_fwd(q, k, v, plan(), layout=layout))
+
+
 def test_no_backward_paths_raise(cuda):
     """FP8 attention and gather plans have no backward: under grad they raise SvgbError instead of returning a result
     detached from the graph."""

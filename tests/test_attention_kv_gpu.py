@@ -74,6 +74,30 @@ def plan_kv(bm, row, col, Sq, Skv, dev):
     return core.AttnPlan(d, ws, (m, r, c, (m._version, r._version, c._version)))
 
 
+def kv_entries(q, k, v, do, plan, layout):
+    """(o, lse, dq, dk, dv) of svgb_attn_fwd_kv and svgb_attn_bwd_kv called directly with the arguments core passes
+    them when Sq != Skv (core.attn_fwd / attn_bwd take the square entries when Sq == Skv)"""
+    from svgb200 import core
+    from svgb200._lib import check, lib
+
+    BH, Sq, Skv, D, qs, kvs = core._kv_geometry(q, k, layout)
+    scale, dt, stream = float(D) ** -0.5, core._dt(q), torch.cuda.current_stream().cuda_stream
+    o, dq, dk, dv = (torch.empty_like(t) for t in (q, q, k, v))
+    lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device)
+    check(lib().svgb_attn_fwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), dt, BH, Sq,
+                                 Skv, D, *qs, *kvs, *qs, scale, C.byref(plan.desc), plan.ws.data_ptr(), stream),
+          "fwd_kv")
+    plan_t = plan.key_major()
+    n = C.c_size_t()
+    check(lib().svgb_attn_bwd_kv_bytes(BH, Sq, Skv, C.byref(n)), "bwd_kv_bytes")
+    ws = torch.empty(n.value, dtype=torch.uint8, device=q.device)
+    check(lib().svgb_attn_bwd_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
+                                 dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), dt, BH, Sq, Skv, D, *qs, *kvs, scale,
+                                 C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc), plan_t.ws.data_ptr(),
+                                 ws.data_ptr(), ws.numel(), stream), "bwd_kv")
+    return o, lse, dq, dk, dv
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # key census
 # ------------------------------------------------------------------------------------------------------------------
@@ -133,7 +157,7 @@ def test_key_census(cuda, Skv, Sq, D, dtype):
 @pytest.mark.parametrize("layout", ["bhsd", "shd"])
 @pytest.mark.parametrize("kind", ["varblock", "dense"])
 @pytest.mark.parametrize("rect_plan", [False, True])
-def test_equal_lengths_match_square_entries(cuda, kind, layout, rect_plan):
+def test_kv_abi_entries_match_square_entries_at_equal_lengths(cuda, kind, layout, rect_plan):
     """svgb_attn_fwd_kv / svgb_attn_bwd_kv at Sq == Skv give svgb_attn_fwd / svgb_attn_bwd's o, lse, dq, dk, dv bit for
     bit, under the square planner's plan and under svgb_attn_plan_varblock_kv's plan of the same map."""
     from svgb200 import core
@@ -151,9 +175,7 @@ def test_equal_lengths_match_square_entries(cuda, kind, layout, rect_plan):
     q, k, v, do = (torch.randn(*shape, generator=gen).to(dtype).to(cuda) for _ in range(4))
     o, lse = core.attn_fwd(q, k, v, sq, layout=layout, return_lse=True)
     g = core.attn_bwd(q, k, v, o, do, lse, sq, layout=layout)
-    o2, lse2 = core._attn_kv(q, k, v, torch.empty_like(q), plan, layout, True, None)
-    g2 = core._attn_bwd_kv(q, k, v, o2, do, lse2, plan, plan.key_major(), *(torch.empty_like(t) for t in (q, k, v)),
-                           layout, None)
+    o2, lse2, *g2 = kv_entries(q, k, v, do, plan, layout)
     assert torch.equal(o, o2) and torch.equal(lse, lse2)
     for a, b in zip(g, g2):
         assert torch.equal(a, b)
