@@ -153,6 +153,21 @@ int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float
                      int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                      long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                      const svgb_plan* plan, const void* plan_ws, void* stream);
+/* Grouped-query attention (GQA; multi-query when BHkv = 1): svgb_attn_fwd_kv with fewer key/value heads than query
+ * heads, FlashInfer's head mapping.
+ *   q, o  : [BHq, Sq, D] at the q / o strides;  k, v : [BHkv, Skv, D] at the k/v strides;  lse : optional [BHq, Sq].
+ *   BHq = G * BHkv: flattened query head h attends with key/value head h / G (for a batch of B, query head hq of batch
+ *           element b is h = b * Hq + hq and reads head b * Hkv + hq / G).
+ *   plan  : SVGB_PLAN_VARBLOCK built over the BHkv key/value heads (map [BHkv, QC, KC]; plan->BH = BHkv), shared by the
+ *           G query heads of a group, rectangular (Sq != Skv) or not; or SVGB_PLAN_BAND (one work list for every head,
+ *           Sq == Skv).
+ * 16-bit inputs, D in {64,128}, alignment as svgb_attn_fwd; no gather plans, row vectors or e4m3 inputs.  The kernel
+ * is svgb_attn_fwd's, so each output row is bit for bit the one of svgb_attn_fwd / _kv on K / V repeated G times per
+ * head under the map repeated per query head. */
+int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BHq, int BHkv,
+                      int Sq, int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
+                      long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
+                      const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
 
 /* Backward of svgb_attn_fwd: dq, dk, dv from q, k, v, the forward's o and natural-log lse, and the output gradient dO.
@@ -184,6 +199,21 @@ int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o,
                      long long q_head_stride, long long kv_row_stride, long long kv_head_stride, float sm_scale,
                      const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws,
                      void* ws, size_t ws_bytes, void* stream);
+
+/* Backward of svgb_attn_fwd_gqa: q, o, dO, dq [BHq, Sq, D] at the q strides; k, v, dk, dv [BHkv, Skv, D] at the k/v
+ * strides; lse float [BHq, Sq].  plan and plan_t are svgb_attn_bwd_kv's (band: svgb_attn_bwd's) built over the BHkv
+ * key/value heads.  ws: device scratch of svgb_attn_bwd_gqa_bytes (the delta over BHq * Sq rows).  The dQ launch runs
+ * one CTA row per query head on its group's plan; the dK / dV launch one CTA row per key/value head, whose key items
+ * walk their chunk list once per query head of the group (g = 0 .. G-1 in order), so dk and dv are the sums over the
+ * group's G query heads, kept in registers and stored once.  Guarantees as svgb_attn_bwd (every row written, no
+ * atomics, deterministic); dq is bit for bit svgb_attn_bwd / _kv's on K / V repeated per head.  Variable-block and band
+ * plans with the backward's masks, 16-bit inputs. */
+int svgb_attn_bwd_gqa_bytes(int BHq, int BHkv, int Sq, int Skv, size_t* bytes);
+int svgb_attn_bwd_gqa(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                      void* dq, void* dk, void* dv, int dtype, int BHq, int BHkv, int Sq, int Skv, int D,
+                      long long q_row_stride, long long q_head_stride, long long kv_row_stride,
+                      long long kv_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
+                      const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream);
 
 /* density of a variable-block map (density_calculation, svg/kmeans_utils.py:13-31) -> float [BH] */
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

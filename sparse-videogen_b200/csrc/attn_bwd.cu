@@ -38,11 +38,12 @@ static AttnBwdArgs bwd_args(const svgb_plan* p, const void* ws) {
   return a;
 }
 
-// Every backward entry: q, o, dO, dq over Sq rows with the q strides, k, v, dk, dv over Skv rows with the k/v strides.
-// The dQ launch walks the forward plan (X / Y = Q / dO, U / W = K / V), the dK / dV launch the key-major plan (X / Y =
-// K / V, U / W = Q / dO); lse and delta are per query row in both.
+// Every backward entry: q, o, dO, dq over Sq rows, BH heads and the q strides, k, v, dk, dv over Skv rows, BH / kv_group
+// heads and the k/v strides.  The dQ launch walks the forward plan (X / Y = Q / dO, U / W = K / V), one CTA row per
+// query head; the dK / dV launch the key-major plan (X / Y = K / V, U / W = Q / dO), one CTA row per key/value head;
+// lse and delta are per query row in both.
 static int attn_bwd_run(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
-                        void* dq, void* dk, void* dv, int dtype, int BH, int Sq, int Skv, int D, long long q_rs,
+                        void* dq, void* dk, void* dv, int dtype, int BH, int kv_group, int Sq, int Skv, int D, long long q_rs,
                         long long q_hs, long long kv_rs, long long kv_hs, float sm_scale, const svgb_plan* plan,
                         const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws, void* ws,
                         size_t ws_bytes, void* stream) {
@@ -64,12 +65,14 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
                                                 plan_t->m1 == plan->m1 && plan_t->m2 == plan->m2),
                "plan_t was built for another mask than plan");
   // the key-major plan has the keys as rows: its S is Skv and its Skv is Sq
-  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH),
+  // both plans are per key/value head
+  const int BHkv = BH / kv_group;
+  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BHkv),
                "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
-               plan_kv_len(plan), BH, Sq, Skv);
-  SVGB_REQUIRE(plan_t->S == Skv && plan_kv_len(plan_t) == Sq && (plan_t->items_stride == 0 || plan_t->BH == BH),
+               plan_kv_len(plan), BHkv, Sq, Skv);
+  SVGB_REQUIRE(plan_t->S == Skv && plan_kv_len(plan_t) == Sq && (plan_t->items_stride == 0 || plan_t->BH == BHkv),
                "plan_t was built for BH=%d S=%d Skv=%d; the key-major plan of this call has BH=%d S=%d Skv=%d",
-               plan_t->BH, plan_t->S, plan_kv_len(plan_t), BH, Skv, Sq);
+               plan_t->BH, plan_t->S, plan_kv_len(plan_t), BHkv, Skv, Sq);
   size_t need = 0;
   if (svgb_attn_bwd_bytes(BH, Sq, &need)) return -1;
   SVGB_REQUIRE(ws_bytes >= need, "backward workspace too small: %zu < %zu", ws_bytes, need);
@@ -95,8 +98,8 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
 
   CUtensorMap qm, km, vm, dom;
   if (encode_tmap_hsd(&qm, q, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
-  if (encode_tmap_hsd(&km, k, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
-  if (encode_tmap_hsd(&vm, v, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
+  if (encode_tmap_hsd(&km, k, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
+  if (encode_tmap_hsd(&vm, v, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
   if (encode_tmap_hsd(&dom, dout, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
   AttnBwdArgs aq = bwd_args(plan, plan_ws), ak = bwd_args(plan_t, plan_t_ws);
   for (AttnBwdArgs* a : {&aq, &ak}) {
@@ -105,6 +108,7 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
     a->scale_log2 = sm_scale * 1.4426950408889634f;
     a->sm_scale = sm_scale;
     a->S = Sq;
+    a->kv_group = kv_group;
   }
   aq.row_stride = q_rs;  // dQ is stored with q's strides, dK and dV with k's
   aq.head_stride = q_hs;
@@ -113,7 +117,7 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
   aq.g0 = dq;
   ak.g0 = dk;
   ak.g1 = dv;
-  const dim3 gq(plan->max_items, BH), gk(plan_t->max_items, BH);
+  const dim3 gq(plan->max_items, BH), gk(plan_t->max_items, BHkv);
   if (D == 128)
     return dtype == SVGB_BF16 ? launch_bwd_pair<128, DT_BF16>(qm, km, vm, dom, aq, gq, ak, gk, st)
                               : launch_bwd_pair<128, DT_F16>(qm, km, vm, dom, aq, gq, ak, gk, st);
@@ -137,7 +141,7 @@ int svgb_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
                   void* dq, void* dk, void* dv, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                   const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
-  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, S, S, D, row_stride, head_stride, row_stride,
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, 1, S, S, D, row_stride, head_stride, row_stride,
                       head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
 }
 
@@ -155,8 +159,28 @@ int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o,
   SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK,
                "svgb_attn_bwd_kv takes variable-block plans only (kind %d; band plans need Sq == Skv, svgb_attn_bwd)",
                plan->kind);
-  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, Sq, Skv, D, q_row_stride, q_head_stride,
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, 1, Sq, Skv, D, q_row_stride, q_head_stride,
                       kv_row_stride, kv_head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
+}
+
+int svgb_attn_bwd_gqa_bytes(int BHq, int BHkv, int Sq, int Skv, size_t* bytes) {
+  SVGB_REQUIRE(BHkv > 0 && Skv > 0, "bad arguments");
+  return svgb_attn_bwd_bytes(BHq, Sq, bytes);  // the per-query-row delta
+}
+
+int svgb_attn_bwd_gqa(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                      void* dq, void* dk, void* dv, int dtype, int BHq, int BHkv, int Sq, int Skv, int D,
+                      long long q_row_stride, long long q_head_stride, long long kv_row_stride,
+                      long long kv_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
+                      const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
+  if (attn_gqa_check(dtype, BHq, BHkv, Sq, Skv, plan, "svgb_attn_bwd_gqa")) return -1;
+  SVGB_REQUIRE(plan_t, "null pointer");
+  SVGB_REQUIRE(plan_t->items_stride == 0 || plan_t->BH == BHkv,
+               "svgb_attn_bwd_gqa: a per-head plan_t is built over the BHkv=%d key/value heads (plan_t BH=%d)", BHkv,
+               plan_t->BH);
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BHq, BHq / BHkv, Sq, Skv, D, q_row_stride,
+                      q_head_stride, kv_row_stride, kv_head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws,
+                      ws_bytes, stream);
 }
 
 }  // extern "C"

@@ -33,6 +33,10 @@ struct AttnBwdArgs {
   const int* item_count = nullptr;  // [BH] when items_stride != 0, else [1]
   const int2* chunks = nullptr;     // chunk lists
   int items_stride = 0;
+  // query heads per key/value head (grouped-query attention).  Query-major: CTA head bh is a query head, its plan and
+  // K / V are at bh / kv_group.  Key-major: bh is a key/value head with its own plan, and each stream walks its chunk
+  // list once for every query head bh * kv_group + g of the group.
+  int kv_group = 1;
   const float* lse = nullptr;    // [BH, S] natural-log LSE of the forward (query rows)
   const float* delta = nullptr;  // [BH, S] rowsum(dO * O)
   void* g0 = nullptr;            // query-major: dQ; key-major: dK
@@ -99,10 +103,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
   using Cfg = AttnCfg<D, DT>;
   constexpr bool BF16 = DT == DT_BF16;
   constexpr int kTile = Cfg::kTileBytes;
-  const int bh = blockIdx.y;
-  const int n_items = args.item_count[args.items_stride ? bh : 0];
+  const int bh = blockIdx.y;  // head of the stationary tiles X, Y and of the gradients this CTA stores
+  const int G = args.kv_group;
+  const int ph = kKeyMajor ? bh : bh / G;  // head of the plan (a key/value head)
+  const int n_items = args.item_count[args.items_stride ? ph : 0];
   if (static_cast<int>(blockIdx.x) >= n_items) return;
-  const int4* desc = args.items + 2 * (static_cast<size_t>(bh) * args.items_stride + blockIdx.x);
+  const int4* desc = args.items + 2 * (static_cast<size_t>(ph) * args.items_stride + blockIdx.x);
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_u32 = smem_u32(smem_raw);
@@ -125,12 +131,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
   }
   __syncthreads();
 
-  // thread 0: the two tiles of `row` (rows row .. row + 127 of the head) into dst0 / dst1, on one barrier
-  auto load_pair = [&](uint32_t b, uint32_t dst0, const CUtensorMap* m0, uint32_t dst1, const CUtensorMap* m1, int row) {
+  // thread 0: the two tiles of `row` (rows row .. row + 127 of head `head`) into dst0 / dst1, on one barrier
+  auto load_pair = [&](uint32_t b, uint32_t dst0, const CUtensorMap* m0, uint32_t dst1, const CUtensorMap* m1, int row,
+                       int head) {
     mbar_expect_tx(b, 2 * kTile);
     for (int h = 0; h < Cfg::kHalves; ++h) {
-      tma_load_3d(dst0 + h * Cfg::kPanelBytes, m0, b, h * Cfg::kPanelElems, row, bh);
-      tma_load_3d(dst1 + h * Cfg::kPanelBytes, m1, b, h * Cfg::kPanelElems, row, bh);
+      tma_load_3d(dst0 + h * Cfg::kPanelBytes, m0, b, h * Cfg::kPanelElems, row, head);
+      tma_load_3d(dst1 + h * Cfg::kPanelBytes, m1, b, h * Cfg::kPanelElems, row, head);
     }
   };
   auto stage_u = [&](int n) { return sU0 + 2 * (n & 1) * kTile; };
@@ -138,7 +145,6 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
 
   const float c = args.scale_log2;
   const int mode = args.mask_mode, m0 = args.m0, m1 = args.m1, m2 = args.m2;
-  const size_t qbase = static_cast<size_t>(bh) * args.S;  // lse / delta of this head
   // this thread's accumulator rows: rloc and rloc + 8 of the stream's 128; columns 8j + 2 * (lane % 4) (+1)
   const int rloc = 64 * wg + 16 * wq + (lane >> 2);
   const uint32_t sXw = sX + 64 * wg * 128, sYw = sY + 64 * wg * 128;
@@ -150,16 +156,21 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
     const int4 d = __ldg(&desc[st]);
     const int r0 = d.x, nr = d.y, nch = d.w;
     const int2* __restrict__ chunks = args.chunks + d.z;
+    // step t of the stream takes chunk t % nch of the streamed tiles' head uhead(t): the query-major kernel walks the
+    // list once (K / V of head bh / G), the key-major kernel once per query head of the group, g = t / nch in order
+    const int steps = kKeyMajor ? G * nch : nch;
+    auto uhead = [&](int t) { return kKeyMajor ? bh * G + t / nch : ph; };
     if (tid == 0 && nch > 0) {
-      load_pair(bar_xy, sX, &xmap, sY, &ymap, r0);
-      for (int j = 0; j < 2 && j < nch; ++j) {
-        const uint32_t su = stage_u(n + j);
-        load_pair(bar_u(n + j), su, &umap, su + kTile, &wmap, __ldg(&chunks[j].x));
+      load_pair(bar_xy, sX, &xmap, sY, &ymap, r0, bh);
+      for (int t = 0; t < 2 && t < steps; ++t) {
+        const uint32_t su = stage_u(n + t);
+        load_pair(bar_u(n + t), su, &umap, su + kTile, &wmap, __ldg(&chunks[t % nch].x), uhead(t));
       }
     }
     // query-major: the rows are queries, their lse / delta are fixed for the stream (rows past nr: P = 0)
     float lse_r[2] = {0.f, 0.f}, dl_r[2] = {0.f, 0.f};
     if constexpr (!kKeyMajor) {
+      const size_t qbase = static_cast<size_t>(bh) * args.S;
 #pragma unroll
       for (int v1 = 0; v1 < 2; ++v1) {
         const int row = rloc + 8 * v1;
@@ -174,8 +185,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
     for (int i = 0; i < (kKeyMajor ? D / 2 : 1); ++i) acc2[i] = 0.f;
 
     if (nch > 0) mbar_wait(bar_xy, nx & 1, 21);
-    for (int j = 0; j < nch; ++j) {
-      const int nn = n + j;
+    // key-major: lse / delta of the step's query head (the columns are its queries)
+    const float* lse_h = args.lse + static_cast<size_t>(bh) * G * args.S;
+    const float* dl_h = args.delta + static_cast<size_t>(bh) * G * args.S;
+    for (int t = 0, j = 0; t < steps; ++t) {
+      const int nn = n + t;
       const int2 ch = __ldg(&chunks[j]);
       const int c0 = ch.x, valid = chunk_valid(ch.y);
       const bool elem = (ch.y & kChunkElem) != 0;
@@ -198,8 +212,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
             float lse_c = INFINITY, dl_c = 0.f;
             if constexpr (kKeyMajor) {  // the columns are queries
               if (in) {
-                lse_c = bwd_lse2(__ldg(&args.lse[qbase + c0 + col]));
-                dl_c = __ldg(&args.delta[qbase + c0 + col]);
+                lse_c = bwd_lse2(__ldg(&lse_h[c0 + col]));
+                dl_c = __ldg(&dl_h[c0 + col]);
               }
             }
 #pragma unroll
@@ -227,12 +241,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
         attn_wait<0>(acc1);
         wg_fence_regs(acc2);
       }
-      __syncthreads();  // both warpgroups' wgmma on this stage have retired: refill it with chunk j + 2
-      if (tid == 0 && j + 2 < nch) {
-        load_pair(bar_u(nn + 2), sU, &umap, sW, &wmap, __ldg(&chunks[j + 2].x));
+      __syncthreads();  // both warpgroups' wgmma on this stage have retired: refill it with step t + 2
+      if (tid == 0 && t + 2 < steps) {
+        load_pair(bar_u(nn + 2), sU, &umap, sW, &wmap, __ldg(&chunks[(t + 2) % nch].x), uhead(t + 2));
+      }
+      if (++j == nch) {  // key-major: on to the next query head of the group
+        j = 0;
+        lse_h += args.S;
+        dl_h += args.S;
       }
     }
-    n += nch;
+    n += steps;
     nx += nch > 0;
 
     // ---- epilogue: A1 * sm_scale (dQ or dK), A2 (dV); rows past nr belong to other streams

@@ -254,6 +254,9 @@ struct AttnArgs {
   const int* item_count = nullptr;  // [BH] when items_stride != 0, else [1]
   const int2* chunks = nullptr;     // chunk or run lists
   int items_stride = 0;             // 0: one plan shared by all heads (band masks); else items per head
+  // query heads per key/value head (grouped-query attention): query head bh reads K / V head bh / kv_group, and so
+  // does the plan (built over the key/value heads); Q, O and LSE stay at bh
+  int kv_group = 1;
   void* o = nullptr;
   long long o_row_stride = 0;   // elements
   long long o_head_stride = 0;  // elements

@@ -405,9 +405,10 @@ int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const v
   SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16 || dtype == SVGB_E4M3, "dtype %d unsupported", dtype);
   CUtensorMap qm, km, vm;
+  const int BHkv = BH / a.kv_group;  // BH counts the query heads
   if (encode_tmap_hsd(&qm, q, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
-  if (encode_tmap_hsd(&km, k, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
-  if (encode_tmap_hsd(&vm, v, dtype, BH, Skv, D, kv_rs, kv_hs)) return -1;
+  if (encode_tmap_hsd(&km, k, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
+  if (encode_tmap_hsd(&vm, v, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
   dim3 grid(grid_x, BH);
   if (dtype == SVGB_E4M3) {
     SVGB_REQUIRE(D == 128, "the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle", D);
@@ -478,10 +479,11 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   return 0;
 }
 
-// Every forward entry: q / o over Sq rows, k / v over Skv rows, each pair with its own strides.
+// Every forward entry: q / o over Sq rows and BH heads, k / v over Skv rows and BH / kv_group heads, each pair with
+// its own strides.
 static int attn_fwd_run(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
                         const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
-                        const int32_t* o_rows, int dtype, int BH, int Sq, int Skv, int D, long long q_rs,
+                        const int32_t* o_rows, int dtype, int BH, int kv_group, int Sq, int Skv, int D, long long q_rs,
                         long long q_hs, long long kv_rs, long long kv_hs, long long o_rs, long long o_hs,
                         float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
   SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
@@ -494,9 +496,9 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   const bool gather = plan->kind == SVGB_PLAN_GATHER;
   SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
                "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");
-  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH),
+  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH / kv_group),
                "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
-               plan_kv_len(plan), BH, Sq, Skv);
+               plan_kv_len(plan), BH / kv_group, Sq, Skv);
   SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && o_rs % 8 == 0 && o_hs % 8 == 0,
                "output must be 16-byte aligned with strides multiple of 8 elements");
   const char* ws = static_cast<const char*>(plan_ws);
@@ -505,6 +507,7 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.item_count = reinterpret_cast<const int*>(ws + plan->counts_off);
   a.chunks = reinterpret_cast<const int2*>(ws + plan->chunks_off);
   a.items_stride = plan->items_stride;
+  a.kv_group = kv_group;
   a.o = o;
   a.o_row_stride = o_rs;
   a.o_head_stride = o_hs;
@@ -623,7 +626,7 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream) {
-  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, BH, S, S, D,
+  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, BH, 1, S, S, D,
                       row_stride, head_stride, row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan,
                       plan_ws, stream);
 }
@@ -643,9 +646,23 @@ int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float
                    (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
                    kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
                "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
-  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, BH, Sq, Skv, D,
+  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, BH, 1, Sq, Skv, D,
                       q_row_stride, q_head_stride, kv_row_stride, kv_head_stride, o_row_stride, o_head_stride,
                       sm_scale, plan, plan_ws, stream);
+}
+
+int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BHq, int BHkv,
+                      int Sq, int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
+                      long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
+                      const svgb_plan* plan, const void* plan_ws, void* stream) {
+  if (attn_gqa_check(dtype, BHq, BHkv, Sq, Skv, plan, "svgb_attn_fwd_gqa")) return -1;
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
+                   kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
+               "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
+  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, BHq, BHq / BHkv,
+                      Sq, Skv, D, q_row_stride, q_head_stride, kv_row_stride, kv_head_stride, o_row_stride,
+                      o_head_stride, sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

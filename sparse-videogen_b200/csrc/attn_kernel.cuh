@@ -138,10 +138,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   constexpr bool FP8 = DT == DT_E4M3;
   constexpr bool kPBF16 = DT == DT_BF16;  // format of P and V in the P V product (fp8: fp16)
   using Elem = typename std::conditional<FP8, uint8_t, uint16_t>::type;  // storage element of Q / K / V
-  const int bh = blockIdx.y;
-  const int n_items = args.item_count[args.items_stride ? bh : 0];
+  const int bh = blockIdx.y;  // query head: Q, O, LSE
+  // key/value head: K, V and the plan's work list.  Gather plans take no groups (their kv_rows are per query head; the
+  // host refuses them with kv_group > 1), so the row-gather kernel keeps bh and its code of kv_group = 1.
+  const int kvh = kGather ? bh : bh / args.kv_group;
+  const int n_items = args.item_count[args.items_stride ? kvh : 0];
   if (static_cast<int>(blockIdx.x) >= n_items) return;
-  const int4* desc = args.items + 2 * (static_cast<size_t>(bh) * args.items_stride + blockIdx.x);
+  const int4* desc = args.items + 2 * (static_cast<size_t>(kvh) * args.items_stride + blockIdx.x);
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_u32 = smem_u32(smem_raw);
@@ -208,8 +211,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   if (wg == 0) {
     // ======================= producer: every load, and the FP8 widening of V
     setmaxnreg_dec<kProducerRegs>();
-    const Elem* kp = static_cast<const Elem*>(args.k_ptr) + bh * args.in_head_stride;
-    const Elem* vp = static_cast<const Elem*>(args.v_ptr) + bh * args.in_head_stride;
+    const Elem* kp = static_cast<const Elem*>(args.k_ptr) + kvh * args.in_head_stride;
+    const Elem* vp = static_cast<const Elem*>(args.v_ptr) + kvh * args.in_head_stride;
     const int* kv_rows = (kGather && args.kv_rows) ? args.kv_rows + static_cast<size_t>(bh) * args.S : nullptr;
 
     // gather: piece p (16 B) of row r -> panel p/8, byte r*128 + ((p%8) ^ (r%8))*16; a row is kRowBytes bytes
@@ -319,10 +322,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
           const int kv0 = __ldg(&sm.list[j].x);
           mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
           mbar_expect_tx(kf, Cfg::kTileBytes);
-          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, kf, h * Cfg::kPanelElems, kv0, bh);
+          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, kf, h * Cfg::kPanelElems, kv0, kvh);
           mbar_wait(smem_u32(&ctl->v_empty[s]), par, 7);
           mbar_expect_tx(vf, Cfg::kTileBytes);
-          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sV + h * Cfg::kPanelBytes, &vmap, vf, h * Cfg::kPanelElems, kv0, bh);
+          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sV + h * Cfg::kPanelBytes, &vmap, vf, h * Cfg::kPanelElems, kv0, kvh);
         }
         // FP8: widen the previous chunk's V, requested one chunk earlier, rather than wait here for V(j) to land
         if constexpr (FP8) {

@@ -54,6 +54,24 @@ int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S
 // every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) { return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S; }
 
+// the checks svgb_attn_fwd_gqa and svgb_attn_bwd_gqa share, before any device work: BHq query heads in groups over
+// BHkv key/value heads, 16-bit inputs, and a variable-block plan over the key/value heads or a band plan (one work
+// list for every head, Sq == Skv)
+inline int attn_gqa_check(int dtype, int BHq, int BHkv, int Sq, int Skv, const svgb_plan* plan, const char* who) {
+  SVGB_REQUIRE(plan, "null pointer");
+  SVGB_REQUIRE(BHq > 0 && BHkv > 0 && BHq % BHkv == 0,
+               "%s: the query heads BHq=%d must be a multiple of the key/value heads BHkv=%d", who, BHq, BHkv);
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
+               "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no GQA path)", who, dtype);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND,
+               "%s takes variable-block or band plans (kind %d; gather and key-major plans have no GQA path)", who,
+               plan->kind);
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
+  SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
+               "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
+  return 0;
+}
+
 struct AttnArgs;
 // attention launch with independent query / key-value geometry (attn_fwd.cu); used by svgb_attn_fwd
 // and by sample_mse's split-KV passes.  Checks D and dtype; gather selects the row-gather kernel (run lists).

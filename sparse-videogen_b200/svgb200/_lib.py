@@ -49,6 +49,8 @@ _PROTOS = {
                       _pplan, _vp, _vp],
     "svgb_attn_fwd_kv": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan, _vp,
                          _vp],
+    "svgb_attn_fwd_gqa": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan,
+                          _vp, _vp],
     "svgb_quantize_e4m3": [_vp, _i, _vp, _vp, _i, _i, _i, _vp],
     "svgb_attn_bwd_bytes": [_i, _i, _psz],
     "svgb_attn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _f, _pplan, _vp, _pplan,
@@ -56,6 +58,9 @@ _PROTOS = {
     "svgb_attn_bwd_kv_bytes": [_i, _i, _i, _psz],
     "svgb_attn_bwd_kv": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                          _pplan, _vp, _pplan, _vp, _vp, _sz, _vp],
+    "svgb_attn_bwd_gqa_bytes": [_i, _i, _i, _i, _psz],
+    "svgb_attn_bwd_gqa": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
+                          _pplan, _vp, _pplan, _vp, _vp, _sz, _vp],
     "svgb_density": [_vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "svgb_argsort_labels_bytes": [_i, _i, _i, _psz],
     "svgb_argsort_labels": [_vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp],

@@ -190,26 +190,43 @@ def _geometry(q, layout):
 
 
 def _kv_geometry(q, k, layout):
-    """(BH, Sq, Skv, D, q strides, k/v strides); k's sequence length may differ from q's, every other dimension must
-    match."""
+    """(BH, Sq, Skv, D, q strides, k/v strides), BH counting q's heads.  k's sequence length may differ from q's, and
+    its head count (dim 1 in both layouts) may be q's divided by a whole G = _kv_group(q, k) (grouped-query attention:
+    query head h attends with key/value head h // G); every other dimension must match."""
     BH, Sq, D, qrs, qhs = _geometry(q, layout)
     if q.dim() != k.dim():
         raise SvgbError(f"q {tuple(q.shape)} and k {tuple(k.shape)} differ in rank")
     BHk, Skv, Dk, kvrs, kvhs = _geometry(k, layout)
     seq = 2 if layout == "bhsd" else 0
-    if [n for i, n in enumerate(q.shape) if i != seq] != [n for i, n in enumerate(k.shape) if i != seq]:
-        raise SvgbError(f"q {tuple(q.shape)} and k, v {tuple(k.shape)} may differ in the sequence length only")
+    if ([n for i, n in enumerate(q.shape) if i not in (seq, 1)] != [n for i, n in enumerate(k.shape) if i not in (seq, 1)]
+            or k.shape[1] == 0 or q.shape[1] % k.shape[1]):
+        raise SvgbError(f"q {tuple(q.shape)} and k, v {tuple(k.shape)} may differ in the sequence length only, and "
+                        "in a key/value head count that divides q's (grouped-query attention)")
     return BH, Sq, Skv, D, (qrs, qhs), (kvrs, kvhs)
 
 
+def _kv_group(q, k):
+    """Query heads per key/value head, once _kv_geometry has accepted q and k."""
+    return q.shape[1] // k.shape[1]
+
+
 def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
-    """One attention launch.  Equal sequence lengths take svgb_attn_fwd: 16-bit or e4m3 (dtype) with its per-head
-    scales, and the row vectors rows = (q_rows, kv_rows, o_rows).  Otherwise svgb_attn_fwd_kv: q and o over Sq rows,
-    k and v over Skv rows, each pair with its own strides; 16-bit, no scales, no row vectors."""
+    """One attention launch.  Fewer key/value heads than query heads (G > 1) take svgb_attn_fwd_gqa: 16-bit, no
+    scales, no row vectors, no gather plan.  Otherwise equal sequence lengths take svgb_attn_fwd: 16-bit or e4m3
+    (dtype) with its per-head scales, and the row vectors rows = (q_rows, kv_rows, o_rows); other lengths
+    svgb_attn_fwd_kv: q and o over Sq rows, k and v over Skv rows, each pair with its own strides; 16-bit, no scales,
+    no row vectors."""
     BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
+    G = _kv_group(q, k)
+    if G > 1:
+        _gqa_check(dtype, plan, rows)
     lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    if Sq == Skv:
+    if G > 1:
+        check(lib().svgb_attn_fwd_gqa(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), dtype, BH,
+                                      BH // G, Sq, Skv, D, *qs, *kvs, *qs, scale, C.byref(plan.desc),
+                                      plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd_gqa")
+    elif Sq == Skv:
         rows = [None if r is None else r.reshape(BH, Sq).to(torch.int32).contiguous() for r in rows]
         check(lib().svgb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), *map(_p, scales), o.data_ptr(), _p(lse),
                                   *map(_p, rows), dtype, BH, Sq, D, *qs, *qs, scale, C.byref(plan.desc),
@@ -222,6 +239,19 @@ def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
     return (o, lse) if return_lse else o
 
 
+def _gqa_check(dtype, plan, rows=()):
+    """What grouped-query attention does not take, refused before any device work."""
+    if dtype == _E4M3:
+        raise SvgbError("grouped-query attention (fewer k, v heads than q heads) has no FP8 path: the per-head scales "
+                        "are indexed by query head")
+    if any(r is not None for r in rows):
+        raise SvgbError("grouped-query attention (fewer k, v heads than q heads) takes no row vectors "
+                        "(o_rows / q_rows / kv_rows)")
+    if plan.desc.kind == PLAN_GATHER:
+        raise SvgbError("grouped-query attention (fewer k, v heads than q heads) takes no gather plan: its kv_rows are "
+                        "indexed by query head")
+
+
 def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[torch.Tensor] = None,
              q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
              return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
@@ -229,14 +259,18 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     o_rows scatters the output rows; q_rows / kv_rows gather the input rows and need a gather plan
     (plan_varblock(..., gather=True)); all three are int [BH,S] (include/svgb200.h, svgb_attn_fwd).
     k, v may have another sequence length S_kv than q (same batch, heads, D and dtype): the plan is then a rectangular
-    variable-block plan (plan_varblock(..., S_kv=)), o has q's shape, and row vectors are not taken."""
+    variable-block plan (plan_varblock(..., S_kv=)), o has q's shape, and row vectors are not taken.
+    k, v may have fewer heads than q, Hq = G * Hkv (grouped-query attention, FlashInfer's mapping: query head h attends
+    with key/value head h // G): a variable-block plan is then built over the B * Hkv key/value heads and shared by
+    each group, band plans are shared by every head already; no row vectors, FP8 or gather plans."""
     _need_cuda(q, k, v)
     if not (q.is_contiguous() and k.is_contiguous() and v.is_contiguous()):
         raise SvgbError("q, k, v must be contiguous")
     if not (q.dtype == k.dtype == v.dtype) or k.shape != v.shape:
         raise SvgbError("q, k, v must share dtype, and k, v their shape")
     o = torch.empty_like(q) if out is None else out
-    if q.shape != k.shape and (o_rows is not None or q_rows is not None or kv_rows is not None):
+    if q.shape[1] == k.shape[1] and q.shape != k.shape and (o_rows is not None or q_rows is not None
+                                                           or kv_rows is not None):
         raise SvgbError("row vectors (o_rows / q_rows / kv_rows) need k, v of q's sequence length")
     return _attn(q, k, v, o, plan, layout, _dt(q), (None, None, None), (q_rows, kv_rows, o_rows), return_lse, sm_scale)
 
@@ -246,7 +280,8 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
     """Gradients (dq, dk, dv) of o = attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale) for the output gradient
     do; lse is the forward's return_lse output.  Variable-block and band plans (mask NONE / HY / WAN / COG); the plan's
     key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits.
-    k, v may have another sequence length than q under a rectangular variable-block plan; dk, dv then have k's shape.
+    k, v may have another sequence length than q under a rectangular variable-block plan, and fewer heads (grouped-query
+    attention, as attn_fwd); dk, dv then have k's shape, a group's dk and dv summing over its query heads.
     out: optional (dq, dk, dv) tensors of q's, k's and v's dtype and shape, contiguous, written and returned instead
     of new ones."""
     _need_cuda(q, k, v, o, do, lse)
@@ -259,18 +294,26 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
     if not all(t.dtype == q.dtype and t.shape == r.shape for t, r in zip(ts, like)):
         raise SvgbError("q, k, v, o, do (and out) must share dtype; o, do, dq have q's shape, v, dk, dv k's")
     BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
+    G = _kv_group(q, k)
+    if G > 1:
+        _gqa_check(_dt(q), plan)
     plan_t = plan.key_major()
     lse = lse.to(torch.float32).contiguous()
-    # equal lengths take svgb_attn_bwd, whose q and k share one length and one pair of strides
-    name, lens, strides = ("svgb_attn_bwd", (Sq,), qs) if Sq == Skv else ("svgb_attn_bwd_kv", (Sq, Skv), qs + kvs)
+    # equal lengths and heads take svgb_attn_bwd, whose q and k share one length and one pair of strides
+    if G > 1:
+        name, lens, strides = "svgb_attn_bwd_gqa", (BH, BH // G, Sq, Skv), qs + kvs
+    elif Sq == Skv:
+        name, lens, strides = "svgb_attn_bwd", (BH, Sq), qs
+    else:
+        name, lens, strides = "svgb_attn_bwd_kv", (BH, Sq, Skv), qs + kvs
     nbytes = C.c_size_t()
-    check(getattr(lib(), name + "_bytes")(BH, *lens, C.byref(nbytes)), name + "_bytes")
+    check(getattr(lib(), name + "_bytes")(*lens, C.byref(nbytes)), name + "_bytes")
     ws = workspace(("attn_bwd", BH, Sq), nbytes.value, q.device)
     dq, dk, dv = (torch.empty_like(t) for t in (q, k, v)) if out is None else out
     _need_cuda(dq, dk, dv)
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
     check(getattr(lib(), name)(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
-                               dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), BH, *lens, D, *strides, scale,
+                               dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), *lens, D, *strides, scale,
                                C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc), plan_t.ws.data_ptr(),
                                ws.data_ptr(), ws.numel(), _stream(q)), name)
     _bump(3)
@@ -378,6 +421,8 @@ def attn_fwd_fp8(q8, k8, v8, q_scale, k_scale, v_scale, plan: AttnPlan, *, o_row
     With a gather plan (plan_varblock(..., gather=True)), q_rows / kv_rows read the rows through index vectors, as in
     attn_fwd."""
     _need_cuda(q8, k8, v8, q_scale, k_scale, v_scale)
+    if q8.dim() == k8.dim() and q8.dim() > 1 and q8.shape[1] != k8.shape[1]:
+        _gqa_check(_E4M3, plan)
     if not (q8.dtype == k8.dtype == v8.dtype == torch.uint8) or not (q8.shape == k8.shape == v8.shape):
         raise SvgbError("q8, k8, v8 must be uint8 tensors of one shape")
     B, H, S, D = q8.shape

@@ -81,11 +81,12 @@ def check_segments(what, segs, kv_segs, S, S_kv):
 def segment_attention(what, query, key, value, segs, kv_segs, layout="bhsd"):
     """core.attention in which query segment i attends key segment i only: the segment lists pass check_segments
     (`what` names the caller in its error), then one rectangular plan of the diagonal block map over them.  layout
-    'bhsd' or 'shd', as core.attention takes it."""
+    'bhsd' or 'shd', as core.attention takes it.  The map is built over key's heads, so key / value may have fewer
+    heads than query (grouped-query attention)."""
     seq = 2 if layout == "bhsd" else 0
     S, S_kv = query.shape[seq], key.shape[seq]
     check_segments(what, segs, kv_segs, S, S_kv)
-    BH = query.shape[0] * query.shape[1] if layout == "bhsd" else query.shape[1]
+    BH = key.shape[0] * key.shape[1] if layout == "bhsd" else key.shape[1]
     n, dev = len(segs), query.device
     bm = torch.eye(n, dtype=torch.bool, device=dev).expand(BH, n, n).contiguous()
     sz = torch.tensor(segs, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
