@@ -70,31 +70,40 @@ def _hash(*vals):
     return h
 
 
-def row_params(seed, rows, row0=0, device="cpu"):
-    """(m, j) of rows [row0, row0 + rows): int64 tensors."""
-    r = torch.arange(row0, row0 + rows, dtype=torch.int64, device=device)
-    h = _hash(r, seed + 7)
-    return (h >> 4) % (2 * MMAX + 1) - MMAX, torch.tensor(JS, device=device)[(h >> 12) % len(JS)]
+def _rows(rows, row0, device, idx):
+    """The int64 row indices [row0, row0 + rows), or idx (any int64 tensor of row indices) when given."""
+    if idx is not None:
+        return idx.to(device=device, dtype=torch.int64)
+    return torch.arange(row0, row0 + rows, dtype=torch.int64, device=device)
 
 
-def row_x(seed, rows, N, *, centred, row0=0, device="cpu"):
-    """x [rows, N] float32 of integers (rows row0...) and rstd [rows] float64, exact: see the module docstring."""
+def row_params(seed, rows, row0=0, device="cpu", *, js=JS, idx=None):
+    """(m, j) of rows [row0, row0 + rows) (or of the rows idx): int64 tensors, j drawn from js."""
+    h = _hash(_rows(rows, row0, device, idx), seed + 7)
+    return (h >> 4) % (2 * MMAX + 1) - MMAX, torch.tensor(js, device=device)[(h >> 12) % len(js)]
+
+
+def block_hash(seed, r, nb):
+    """The hash h [n, nb], the BLOCKS index [n, nb] and the permutation [n, nb, 8] of each 8-block of rows r."""
+    dev = r.device
+    h = _hash(r[:, None], torch.arange(nb, dtype=torch.int64, device=dev)[None, :], seed)
+    return h, (h >> 3) % BLOCKS.shape[0], PERMS.to(dev)[_hash(h, 3) % PERMS.shape[0]]
+
+
+def row_x(seed, rows, N, *, centred, row0=0, device="cpu", js=JS, idx=None):
+    """x [rows, N] float32 of integers (rows row0..., or the rows idx) and rstd [rows] float64, exact: see the module
+    docstring.  js: the exponents j a row may draw (LayerNorm's backward census keeps to var >= 256)."""
     assert N % 8 == 0
-    nb = N // 8
-    r = torch.arange(row0, row0 + rows, dtype=torch.int64, device=device)[:, None]
-    b = torch.arange(nb, dtype=torch.int64, device=device)[None, :]
-    h = _hash(r, b, seed)
-    blk = BLOCKS.to(device)[(h >> 3) % BLOCKS.shape[0]]                    # [rows, nb, 8]
-    perm = PERMS.to(device)[_hash(h, 3) % PERMS.shape[0]]
-    d = torch.gather(blk, 2, perm)
-    m, j = row_params(seed, rows, row0, device)
+    r = _rows(rows, row0, device, idx)
+    _, bi, perm = block_hash(seed, r, N // 8)
+    d = torch.gather(BLOCKS.to(device)[bi], 2, perm)                       # [rows, nb, 8]
+    m, j = row_params(seed, rows, row0, device, js=js, idx=idx)
     if not centred:
         m = torch.zeros_like(m)
     # powers of two from exact tables: torch.pow on CUDA may be an ulp off
-    k = j - min(JS)
-    scale = torch.tensor([2.0 ** v for v in JS], device=device)[k]
-    rstd = torch.tensor([2.0 ** -(2 + v) for v in JS], dtype=torch.float64, device=device)[k]
-    return d.reshape(rows, N) * scale[:, None] + m.float()[:, None], rstd
+    scale = torch.tensor([2.0 ** v for v in range(max(js) + 1)], device=device)[j]
+    rstd = torch.tensor([2.0 ** -(2 + v) for v in range(max(js) + 1)], dtype=torch.float64, device=device)[j]
+    return d.reshape(r.shape[0], N) * scale[:, None] + m.float()[:, None], rstd
 
 
 def multiples(shape, step, lo, hi, gen, odd=False):
@@ -205,8 +214,9 @@ def exact_in(t, dtype):
 def norm_margin_ok(v, scale, dtype):
     """Element-wise: v is representable in the 16-bit dtype, and it lies further than ERR_REL * scale (scale = |x^ g|
     + |b|, the size of the terms the approximate path rounds) from the midpoints to its neighbours, so rsqrtf a few
-    ulps off, an unabsorbed eps and the fp32 roundings of x^ g + b cannot move its rounding.  Returns (ok, the smallest
-    ratio of the margin to the error bound)."""
+    ulps off, an unabsorbed eps and the fp32 roundings of x^ g + b cannot move its rounding.  Any per-element scale
+    works: the backward census (oracle/rowwise_bwd.py) passes r (|u| + |x^ m0|).  Returns (ok, the smallest ratio of the
+    margin to the error bound)."""
     v = v.double()
     if not exact_in(v, dtype):
         return False, 0.0

@@ -357,6 +357,7 @@ qkv_prep_kernel(const PrepArgs a) {
 // dx; r and x^ are recomputed exactly as rms_apply / ln_apply compute them.  u = gamma*d:
 //   RMS: dx = r*(u - x^*mean(u*x^))          LayerNorm: dx = r*(u - mean(u) - x^*mean(u*x^))
 // ag += d*x^ (dgamma), ab += d (dbeta): per-thread fp32 partials of this thread's 8 columns.
+// Everything below is pinned bit for bit by tests/test_rowwise_bwd_census_gpu.py (oracle/rowwise_bwd.py).
 template <int D>
 __device__ __forceinline__ void rms_bwd(const float (&f)[8], float (&d)[8], const float (&g)[8], float eps,
                                         float (&ag)[8]) {
