@@ -168,6 +168,23 @@ int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, floa
                       int Sq, int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                       long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                       const svgb_plan* plan, const void* plan_ws, void* stream);
+/* Attention on strided [B, H, S, D] views: svgb_attn_fwd_gqa with a batch dimension and strides per tensor, so that
+ * a transposed [B, S, H, D] projection, one third of a packed [B, S, 3, H, D] QKV, every other head or a batch slice is
+ * read and written in place.
+ *   q, o  : [B, Hq, Sq, D];  k, v : [B, Hkv, Skv, D];  lse : optional float [B * Hq, Sq], contiguous.
+ *   x_strides : {batch, head, row} element strides of tensor x (the last dimension is contiguous), each a nonzero
+ *           multiple of 8; bases 16-byte aligned.  Element (b, h, s, d) of x is at x + b*st[0] + h*st[1] + s*st[2] + d.
+ *   Hq = G * Hkv: query head hq of batch element b attends with key/value head hq / G of b.
+ *   plan  : SVGB_PLAN_VARBLOCK built over the B * Hkv key/value heads (flat head b * Hkv + hkv; rectangular or not), or
+ *           SVGB_PLAN_BAND (Sq == Skv).
+ * 16-bit inputs, D in {64,128}; no gather plans, row vectors or e4m3 inputs.  The TMA maps are 4-D (d, row, head,
+ * batch) and o is stored at its own strides (only the view's elements are written); each output row is bit for bit
+ * the one svgb_attn_fwd_gqa (svgb_attn_fwd / _kv when Hq == Hkv) gives on contiguous copies.  svgb_attn_fwd, _kv and
+ * _gqa run the same host path with B = 1 and batch stride = heads * head stride. */
+int svgb_attn_fwd_strided(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int B, int Hq,
+                          int Hkv, int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
+                          const long long* v_strides, const long long* o_strides, float sm_scale,
+                          const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
 
 /* Backward of svgb_attn_fwd: dq, dk, dv from q, k, v, the forward's o and natural-log lse, and the output gradient dO.
@@ -214,6 +231,22 @@ int svgb_attn_bwd_gqa(const void* q, const void* k, const void* v, const void* o
                       long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                       long long kv_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                       const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream);
+
+/* Backward of svgb_attn_fwd_strided: q, o, dO, dq [B, Hq, Sq, D]; k, v, dk, dv [B, Hkv, Skv, D]; each of the eight
+ * tensors with its own {batch, head, row} strides under the rules of svgb_attn_fwd_strided, so dO may be a transposed
+ * view and the gradients may be written into views (every element of each view is written, nothing outside it).
+ * lse float [B * Hq, Sq] contiguous.  plan and plan_t as svgb_attn_bwd_gqa's, built over the B * Hkv key/value heads.
+ * ws: device scratch of svgb_attn_bwd_strided_bytes (the delta over B * Hq * Sq rows, read from o and dO at their own
+ * strides).  Guarantees as svgb_attn_bwd_gqa, and the gradients are bit for bit its gradients on contiguous copies.
+ * svgb_attn_bwd, _kv and _gqa run the same host path with B = 1. */
+int svgb_attn_bwd_strided_bytes(int B, int Hq, int Hkv, int Sq, int Skv, size_t* bytes);
+int svgb_attn_bwd_strided(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                          const float* lse, void* dq, void* dk, void* dv, int dtype, int B, int Hq, int Hkv, int Sq,
+                          int Skv, int D, const long long* q_strides, const long long* k_strides,
+                          const long long* v_strides, const long long* o_strides, const long long* do_strides,
+                          const long long* dq_strides, const long long* dk_strides, const long long* dv_strides,
+                          float sm_scale, const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t,
+                          const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream);
 
 /* density of a variable-block map (density_calculation, svg/kmeans_utils.py:13-31) -> float [BH] */
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

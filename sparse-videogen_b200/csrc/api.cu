@@ -32,28 +32,43 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
-int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S, int D,
-                    long long row_stride_elems, long long head_stride_elems, int box_rows) {
+// rank-D TMA descriptor of 16-bit or e4m3 rows: dims[0] = D elements per row, byte strides of dims 1.., box of one
+// 128-byte panel x box_rows rows x 1 ...
+static int encode_rows(CUtensorMap* map, const void* base, int dtype, int rank, const cuuint64_t* dims,
+                       const long long* strides_elems, int box_rows) {
   PFN_encodeTiled enc = get_encode();
   SVGB_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
   SVGB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor base must be 16-byte aligned");
-  cuuint64_t dims[3] = {static_cast<cuuint64_t>(D), static_cast<cuuint64_t>(S),
-                        static_cast<cuuint64_t>(BH)};
   const int eb = dtype == SVGB_E4M3 ? 1 : 2;  // bytes per element
-  SVGB_REQUIRE((row_stride_elems * eb) % 16 == 0 && (head_stride_elems * eb) % 16 == 0,
-               "strides must be multiples of 16 bytes");
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(row_stride_elems) * eb,
-                           static_cast<cuuint64_t>(head_stride_elems) * eb};
-  cuuint32_t box[3] = {static_cast<cuuint32_t>(128 / eb), static_cast<cuuint32_t>(box_rows), 1};  // 128-byte rows
-  cuuint32_t estr[3] = {1, 1, 1};
+  cuuint64_t strides[3];
+  for (int i = 0; i + 1 < rank; ++i) {
+    SVGB_REQUIRE((strides_elems[i] * eb) % 16 == 0, "strides must be multiples of 16 bytes");
+    strides[i] = static_cast<cuuint64_t>(strides_elems[i]) * eb;
+  }
+  cuuint32_t box[4] = {static_cast<cuuint32_t>(128 / eb), static_cast<cuuint32_t>(box_rows), 1, 1};  // 128-byte rows
+  cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(map, dtype == SVGB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                         : dtype == SVGB_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                             : CU_TENSOR_MAP_DATA_TYPE_UINT8,
-                   3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SVGB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
   return 0;
+}
+
+int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S, int D,
+                    long long row_stride_elems, long long head_stride_elems, int box_rows) {
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(D), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(BH)};
+  const long long st[2] = {row_stride_elems, head_stride_elems};
+  return encode_rows(map, base, dtype, 3, dims, st, box_rows);
+}
+
+int encode_tmap_bhsd(CUtensorMap* map, const void* base, int dtype, int B, int H, int S, int D, Strides st) {
+  const cuuint64_t dims[4] = {static_cast<cuuint64_t>(D), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(H),
+                              static_cast<cuuint64_t>(B)};
+  const long long s[3] = {st.r, st.h, st.b};
+  return encode_rows(map, base, dtype, 4, dims, s, 128);
 }
 
 }  // namespace svgb

@@ -38,15 +38,15 @@ static AttnBwdArgs bwd_args(const svgb_plan* p, const void* ws) {
   return a;
 }
 
-// Every backward entry: q, o, dO, dq over Sq rows, BH heads and the q strides, k, v, dk, dv over Skv rows, BH / kv_group
-// heads and the k/v strides.  The dQ launch walks the forward plan (X / Y = Q / dO, U / W = K / V), one CTA row per
-// query head; the dK / dV launch the key-major plan (X / Y = K / V, U / W = Q / dO), one CTA row per key/value head;
-// lse and delta are per query row in both.
+// Every backward entry: q, o, dO, dq over Sq rows and BH heads in B batch elements, k, v, dk, dv over Skv rows and
+// BH / kv_group heads, each tensor with its own strides.  The dQ launch walks the forward plan (X / Y = Q / dO, U / W =
+// K / V), one CTA row per query head; the dK / dV launch the key-major plan (X / Y = K / V, U / W = Q / dO), one CTA
+// row per key/value head; lse and delta are per query row in both.
 static int attn_bwd_run(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
-                        void* dq, void* dk, void* dv, int dtype, int BH, int kv_group, int Sq, int Skv, int D, long long q_rs,
-                        long long q_hs, long long kv_rs, long long kv_hs, float sm_scale, const svgb_plan* plan,
-                        const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws, void* ws,
-                        size_t ws_bytes, void* stream) {
+                        void* dq, void* dk, void* dv, int dtype, int B, int BH, int kv_group, int Sq, int Skv, int D,
+                        Strides qs, Strides ks, Strides vs, Strides os, Strides dos, Strides dqs, Strides dks,
+                        Strides dvs, float sm_scale, const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t,
+                        const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
   SVGB_REQUIRE(q && k && v && o && dout && lse && dq && dk && dv && plan && plan_ws && plan_t && plan_t_ws && ws,
                "null pointer");
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
@@ -78,29 +78,27 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
   SVGB_REQUIRE(ws_bytes >= need, "backward workspace too small: %zu < %zu", ws_bytes, need);
   for (const void* t : {dq, dk, dv})
     SVGB_REQUIRE((reinterpret_cast<uintptr_t>(t) & 15) == 0, "gradients must be 16-byte aligned");
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0 &&
-                   q_rs % 8 == 0 && q_hs % 8 == 0 && kv_rs % 8 == 0 && kv_hs % 8 == 0,
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0,
                "o / dO must be 16-byte aligned with strides multiple of 8 elements");
+  for (const Strides& s : {qs, ks, vs, os, dos, dqs, dks, dvs})
+    SVGB_REQUIRE(s.r % 8 == 0 && s.h % 8 == 0 && s.b % 8 == 0,
+                 "every stride must be a multiple of 8 elements (got %lld, %lld, %lld)", s.b, s.h, s.r);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* delta = static_cast<float*>(ws);
+  const int Hq = BH / B, Hkv = BHkv / B;
 
   const long long rows = static_cast<long long>(BH) * Sq;
   const unsigned blocks = static_cast<unsigned>((rows + 7) / 8);
-  if (dtype == SVGB_BF16)
-    attn_bwd_delta_kernel<true><<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o),
-                                                        static_cast<const uint16_t*>(dout), q_rs, q_hs, BH, Sq, D,
-                                                        delta);
-  else
-    attn_bwd_delta_kernel<false><<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o),
-                                                         static_cast<const uint16_t*>(dout), q_rs, q_hs, BH, Sq, D,
-                                                         delta);
+  auto delta_kernel = dtype == SVGB_BF16 ? attn_bwd_delta_kernel<true> : attn_bwd_delta_kernel<false>;
+  delta_kernel<<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(o), static_cast<const uint16_t*>(dout), os.b, os.h,
+                                       os.r, dos.b, dos.h, dos.r, BH, Hq, Sq, D, delta);
   SVGB_LAUNCH_OK();
 
   CUtensorMap qm, km, vm, dom;
-  if (encode_tmap_hsd(&qm, q, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
-  if (encode_tmap_hsd(&km, k, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
-  if (encode_tmap_hsd(&vm, v, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
-  if (encode_tmap_hsd(&dom, dout, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
+  if (encode_tmap_bhsd(&qm, q, dtype, B, Hq, Sq, D, qs)) return -1;
+  if (encode_tmap_bhsd(&km, k, dtype, B, Hkv, Skv, D, ks)) return -1;
+  if (encode_tmap_bhsd(&vm, v, dtype, B, Hkv, Skv, D, vs)) return -1;
+  if (encode_tmap_bhsd(&dom, dout, dtype, B, Hq, Sq, D, dos)) return -1;
   AttnBwdArgs aq = bwd_args(plan, plan_ws), ak = bwd_args(plan_t, plan_t_ws);
   for (AttnBwdArgs* a : {&aq, &ak}) {
     a->lse = lse;
@@ -110,13 +108,14 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
     a->S = Sq;
     a->kv_group = kv_group;
   }
-  aq.row_stride = q_rs;  // dQ is stored with q's strides, dK and dV with k's
-  aq.head_stride = q_hs;
-  ak.row_stride = kv_rs;
-  ak.head_stride = kv_hs;
+  aq.Hx = Hq;
+  ak.Hx = Hkv;
   aq.g0 = dq;
+  aq.g0_bs = dqs.b, aq.g0_hs = dqs.h, aq.g0_rs = dqs.r;
   ak.g0 = dk;
+  ak.g0_bs = dks.b, ak.g0_hs = dks.h, ak.g0_rs = dks.r;
   ak.g1 = dv;
+  ak.g1_bs = dvs.b, ak.g1_hs = dvs.h, ak.g1_rs = dvs.r;
   const dim3 gq(plan->max_items, BH), gk(plan_t->max_items, BHkv);
   if (D == 128)
     return dtype == SVGB_BF16 ? launch_bwd_pair<128, DT_BF16>(qm, km, vm, dom, aq, gq, ak, gk, st)
@@ -141,8 +140,9 @@ int svgb_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
                   void* dq, void* dk, void* dv, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                   const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
-  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, 1, S, S, D, row_stride, head_stride, row_stride,
-                      head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
+  const Strides x = flat_strides(row_stride, head_stride, BH);
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, 1, BH, 1, S, S, D, x, x, x, x, x, x, x, x, sm_scale,
+                      plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
 }
 
 int svgb_attn_bwd_kv_bytes(int BH, int Sq, int Skv, size_t* bytes) {
@@ -159,8 +159,9 @@ int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o,
   SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK,
                "svgb_attn_bwd_kv takes variable-block plans only (kind %d; band plans need Sq == Skv, svgb_attn_bwd)",
                plan->kind);
-  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BH, 1, Sq, Skv, D, q_row_stride, q_head_stride,
-                      kv_row_stride, kv_head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
+  const Strides x = flat_strides(q_row_stride, q_head_stride, BH), y = flat_strides(kv_row_stride, kv_head_stride, BH);
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, 1, BH, 1, Sq, Skv, D, x, y, y, x, x, x, y, y, sm_scale,
+                      plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
 }
 
 int svgb_attn_bwd_gqa_bytes(int BHq, int BHkv, int Sq, int Skv, size_t* bytes) {
@@ -178,9 +179,36 @@ int svgb_attn_bwd_gqa(const void* q, const void* k, const void* v, const void* o
   SVGB_REQUIRE(plan_t->items_stride == 0 || plan_t->BH == BHkv,
                "svgb_attn_bwd_gqa: a per-head plan_t is built over the BHkv=%d key/value heads (plan_t BH=%d)", BHkv,
                plan_t->BH);
-  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, BHq, BHq / BHkv, Sq, Skv, D, q_row_stride,
-                      q_head_stride, kv_row_stride, kv_head_stride, sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws,
-                      ws_bytes, stream);
+  const Strides x = flat_strides(q_row_stride, q_head_stride, BHq), y = flat_strides(kv_row_stride, kv_head_stride, BHkv);
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, 1, BHq, BHq / BHkv, Sq, Skv, D, x, y, y, x, x, x, y, y,
+                      sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);
+}
+
+int svgb_attn_bwd_strided_bytes(int B, int Hq, int Hkv, int Sq, int Skv, size_t* bytes) {
+  SVGB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Skv > 0, "bad arguments");
+  return svgb_attn_bwd_bytes(B * Hq, Sq, bytes);  // the per-query-row delta
+}
+
+int svgb_attn_bwd_strided(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                          const float* lse, void* dq, void* dk, void* dv, int dtype, int B, int Hq, int Hkv, int Sq,
+                          int Skv, int D, const long long* q_strides, const long long* k_strides,
+                          const long long* v_strides, const long long* o_strides, const long long* do_strides,
+                          const long long* dq_strides, const long long* dk_strides, const long long* dv_strides,
+                          float sm_scale, const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t,
+                          const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
+  Strides st[8];
+  if (attn_strided_check(B, Hq, Hkv, {q, k, v, o, dout, dq, dk, dv},
+                         {q_strides, k_strides, v_strides, o_strides, do_strides, dq_strides, dk_strides, dv_strides},
+                         st, "svgb_attn_bwd_strided"))
+    return -1;
+  if (attn_gqa_check(dtype, B * Hq, B * Hkv, Sq, Skv, plan, "svgb_attn_bwd_strided")) return -1;
+  SVGB_REQUIRE(plan_t, "null pointer");
+  SVGB_REQUIRE(plan_t->items_stride == 0 || plan_t->BH == B * Hkv,
+               "svgb_attn_bwd_strided: a per-head plan_t is built over the B*Hkv=%d key/value heads (plan_t BH=%d)",
+               B * Hkv, plan_t->BH);
+  return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, B, B * Hq, Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2],
+                      st[3], st[4], st[5], st[6], st[7], sm_scale, plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes,
+                      stream);
 }
 
 }  // extern "C"

@@ -37,11 +37,16 @@ struct AttnBwdArgs {
   // K / V are at bh / kv_group.  Key-major: bh is a key/value head with its own plan, and each stream walks its chunk
   // list once for every query head bh * kv_group + g of the group.
   int kv_group = 1;
+  // heads of the stationary tiles per batch element (query-major: Hq, key-major: Hkv): CTA head bh is head bh % Hx of
+  // batch element bh / Hx in the tensor maps (d, row, head, batch) and the gradient stores; the plan, LSE and delta
+  // index the flat head
+  int Hx = 1;
   const float* lse = nullptr;    // [BH, S] natural-log LSE of the forward (query rows)
   const float* delta = nullptr;  // [BH, S] rowsum(dO * O)
   void* g0 = nullptr;            // query-major: dQ; key-major: dK
   void* g1 = nullptr;            // key-major: dV
-  long long row_stride = 0, head_stride = 0;  // elements, shared by the inputs and the gradients
+  long long g0_bs = 0, g0_hs = 0, g0_rs = 0;  // element strides (batch, head, row) of g0
+  long long g1_bs = 0, g1_hs = 0, g1_rs = 0;  // and of g1
   float scale_log2 = 0, sm_scale = 0;
   int S = 0;
   int mask_mode = 0, m0 = 0, m1 = 0, m2 = 0;
@@ -106,6 +111,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
   const int bh = blockIdx.y;  // head of the stationary tiles X, Y and of the gradients this CTA stores
   const int G = args.kv_group;
   const int ph = kKeyMajor ? bh : bh / G;  // head of the plan (a key/value head)
+  // batch element and head within it of the stationary tiles; the streamed tiles are in the same batch element
+  const int batch = bh / args.Hx, xh = bh - batch * args.Hx;
   const int n_items = args.item_count[args.items_stride ? ph : 0];
   if (static_cast<int>(blockIdx.x) >= n_items) return;
   const int4* desc = args.items + 2 * (static_cast<size_t>(ph) * args.items_stride + blockIdx.x);
@@ -131,13 +138,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
   }
   __syncthreads();
 
-  // thread 0: the two tiles of `row` (rows row .. row + 127 of head `head`) into dst0 / dst1, on one barrier
+  // thread 0: the two tiles of `row` (rows row .. row + 127 of head `head` of this CTA's batch element) into dst0 /
+  // dst1, on one barrier
   auto load_pair = [&](uint32_t b, uint32_t dst0, const CUtensorMap* m0, uint32_t dst1, const CUtensorMap* m1, int row,
                        int head) {
     mbar_expect_tx(b, 2 * kTile);
     for (int h = 0; h < Cfg::kHalves; ++h) {
-      tma_load_3d(dst0 + h * Cfg::kPanelBytes, m0, b, h * Cfg::kPanelElems, row, head);
-      tma_load_3d(dst1 + h * Cfg::kPanelBytes, m1, b, h * Cfg::kPanelElems, row, head);
+      tma_load_4d(dst0 + h * Cfg::kPanelBytes, m0, b, h * Cfg::kPanelElems, row, head, batch);
+      tma_load_4d(dst1 + h * Cfg::kPanelBytes, m1, b, h * Cfg::kPanelElems, row, head, batch);
     }
   };
   auto stage_u = [&](int n) { return sU0 + 2 * (n & 1) * kTile; };
@@ -159,9 +167,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
     // step t of the stream takes chunk t % nch of the streamed tiles' head uhead(t): the query-major kernel walks the
     // list once (K / V of head bh / G), the key-major kernel once per query head of the group, g = t / nch in order
     const int steps = kKeyMajor ? G * nch : nch;
-    auto uhead = [&](int t) { return kKeyMajor ? bh * G + t / nch : ph; };
+    auto uhead = [&](int t) { return kKeyMajor ? xh * G + t / nch : xh / G; };
     if (tid == 0 && nch > 0) {
-      load_pair(bar_xy, sX, &xmap, sY, &ymap, r0, bh);
+      load_pair(bar_xy, sX, &xmap, sY, &ymap, r0, xh);
       for (int t = 0; t < 2 && t < steps; ++t) {
         const uint32_t su = stage_u(n + t);
         load_pair(bar_u(n + t), su, &umap, su + kTile, &wmap, __ldg(&chunks[t % nch].x), uhead(t));
@@ -259,14 +267,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
     for (int v1 = 0; v1 < 2; ++v1) {
       const int row = rloc + 8 * v1;
       if (row >= nr) continue;
-      const long long off = bh * args.head_stride + static_cast<long long>(r0 + row) * args.row_stride + 2 * (lane & 3);
-      uint16_t* g0 = reinterpret_cast<uint16_t*>(args.g0) + off;
+      const long long r = r0 + row, c0 = 2 * (lane & 3);
+      uint16_t* g0 = reinterpret_cast<uint16_t*>(args.g0) + batch * args.g0_bs + xh * args.g0_hs + r * args.g0_rs + c0;
 #pragma unroll
       for (int jj = 0; jj < D / 8; ++jj)
         *reinterpret_cast<uint32_t*>(g0 + 8 * jj) =
             pack2<BF16>(acc1[4 * jj + 2 * v1] * args.sm_scale, acc1[4 * jj + 2 * v1 + 1] * args.sm_scale);
       if constexpr (kKeyMajor) {
-        uint16_t* g1 = reinterpret_cast<uint16_t*>(args.g1) + off;
+        uint16_t* g1 = reinterpret_cast<uint16_t*>(args.g1) + batch * args.g1_bs + xh * args.g1_hs + r * args.g1_rs + c0;
 #pragma unroll
         for (int jj = 0; jj < D / 8; ++jj)
           *reinterpret_cast<uint32_t*>(g1 + 8 * jj) = pack2<BF16>(acc2[4 * jj + 2 * v1], acc2[4 * jj + 2 * v1 + 1]);
@@ -275,27 +283,30 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
   }
 }
 
-// delta[h, s] = sum_d dO[h, s, d] * O[h, s, d] in fp32: one warp per row
+// delta[bh, s] = sum_d dO[bh, s, d] * O[bh, s, d] in fp32: one warp per row; head bh is head bh % H of batch element
+// bh / H in o and dO, each at its own element strides (batch, head, row)
 template <bool kBF16>
 __global__ void __launch_bounds__(256)
-attn_bwd_delta_kernel(const uint16_t* __restrict__ o, const uint16_t* __restrict__ dout, long long row_stride,
-                      long long head_stride, int BH, int S, int D, float* __restrict__ delta) {
+attn_bwd_delta_kernel(const uint16_t* __restrict__ o, const uint16_t* __restrict__ dout, long long o_bs, long long o_hs,
+                      long long o_rs, long long do_bs, long long do_hs, long long do_rs, int BH, int H, int S, int D,
+                      float* __restrict__ delta) {
   const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (r >= static_cast<long long>(BH) * S) return;
   const int lane = threadIdx.x & 31;
-  const long long h = r / S, s = r - h * S;
-  const long long off = h * head_stride + s * row_stride;
+  const long long bh = r / S, s = r - bh * S, b = bh / H, h = bh - b * H;
+  const uint16_t* orow = o + b * o_bs + h * o_hs + s * o_rs;
+  const uint16_t* drow = dout + b * do_bs + h * do_hs + s * do_rs;
   float acc = 0.f;
   for (int d = 2 * lane; d < D; d += 64) {
-    const uint32_t a = *reinterpret_cast<const uint32_t*>(o + off + d);
-    const uint32_t b = *reinterpret_cast<const uint32_t*>(dout + off + d);
+    const uint32_t x = *reinterpret_cast<const uint32_t*>(orow + d);
+    const uint32_t y = *reinterpret_cast<const uint32_t*>(drow + d);
     float2 fa, fb;
     if constexpr (kBF16) {
-      fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&a));
-      fb = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&b));
+      fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&x));
+      fb = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&y));
     } else {
-      fa = __half22float2(*reinterpret_cast<const __half2*>(&a));
-      fb = __half22float2(*reinterpret_cast<const __half2*>(&b));
+      fa = __half22float2(*reinterpret_cast<const __half2*>(&x));
+      fb = __half22float2(*reinterpret_cast<const __half2*>(&y));
     }
     acc = fmaf(fa.x, fb.x, fmaf(fa.y, fb.y, acc));
   }

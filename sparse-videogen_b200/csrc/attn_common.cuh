@@ -257,9 +257,13 @@ struct AttnArgs {
   // query heads per key/value head (grouped-query attention): query head bh reads K / V head bh / kv_group, and so
   // does the plan (built over the key/value heads); Q, O and LSE stay at bh
   int kv_group = 1;
+  // query heads per batch element: CTA head bh is query head bh % Hq of batch element bh / Hq, which the tensor maps
+  // (d, row, head, batch) and the o store address; the plan, LSE and the row vectors index the flat bh
+  int Hq = 1;
   void* o = nullptr;
-  long long o_row_stride = 0;   // elements
-  long long o_head_stride = 0;  // elements
+  long long o_row_stride = 0;    // elements
+  long long o_head_stride = 0;   // elements
+  long long o_batch_stride = 0;  // elements
   const int* o_rows = nullptr;  // optional [BH, S]: output row for query row q (fused inverse permutation)
   float* lse = nullptr;         // optional [BH, S] (natural log), indexed like o rows
   float scale_log2 = 0;         // softmax scale * log2(e)

@@ -399,27 +399,28 @@ static int launch_selftest(const CUtensorMap& qm, const CUtensorMap& km, const C
   return 0;
 }
 
-int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const void* k, const void* v, int Skv,
-                  long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, bool gather,
-                  int grid_x, cudaStream_t st) {
+int attn_fwd_impl(const void* q, Strides qs, int Sq, const void* k, Strides ks, const void* v, Strides vs, int Skv,
+                  int dtype, int B, int BH, int D, const AttnArgs& a, bool gather, int grid_x, cudaStream_t st) {
   SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16 || dtype == SVGB_E4M3, "dtype %d unsupported", dtype);
   CUtensorMap qm, km, vm;
-  const int BHkv = BH / a.kv_group;  // BH counts the query heads
-  if (encode_tmap_hsd(&qm, q, dtype, BH, Sq, D, q_rs, q_hs)) return -1;
-  if (encode_tmap_hsd(&km, k, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
-  if (encode_tmap_hsd(&vm, v, dtype, BHkv, Skv, D, kv_rs, kv_hs)) return -1;
+  const int Hq = BH / B, Hkv = Hq / a.kv_group;  // BH counts the query heads
+  if (encode_tmap_bhsd(&qm, q, dtype, B, Hq, Sq, D, qs)) return -1;
+  if (encode_tmap_bhsd(&km, k, dtype, B, Hkv, Skv, D, ks)) return -1;
+  if (encode_tmap_bhsd(&vm, v, dtype, B, Hkv, Skv, D, vs)) return -1;
+  AttnArgs args = a;
+  args.Hq = Hq;
   dim3 grid(grid_x, BH);
   if (dtype == SVGB_E4M3) {
     SVGB_REQUIRE(D == 128, "the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle", D);
-    return launch_attn<128, DT_E4M3>(qm, km, vm, a, gather, grid, st);
+    return launch_attn<128, DT_E4M3>(qm, km, vm, args, gather, grid, st);
   }
   if (D == 128) {
-    return dtype == SVGB_BF16 ? launch_attn<128, DT_BF16>(qm, km, vm, a, gather, grid, st)
-                              : launch_attn<128, DT_F16>(qm, km, vm, a, gather, grid, st);
+    return dtype == SVGB_BF16 ? launch_attn<128, DT_BF16>(qm, km, vm, args, gather, grid, st)
+                              : launch_attn<128, DT_F16>(qm, km, vm, args, gather, grid, st);
   }
-  return dtype == SVGB_BF16 ? launch_attn<64, DT_BF16>(qm, km, vm, a, gather, grid, st)
-                            : launch_attn<64, DT_F16>(qm, km, vm, a, gather, grid, st);
+  return dtype == SVGB_BF16 ? launch_attn<64, DT_BF16>(qm, km, vm, args, gather, grid, st)
+                            : launch_attn<64, DT_F16>(qm, km, vm, args, gather, grid, st);
 }
 
 // a chunk list covers the key side (Skv columns), the items the query side (Sq rows)
@@ -479,13 +480,13 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   return 0;
 }
 
-// Every forward entry: q / o over Sq rows and BH heads, k / v over Skv rows and BH / kv_group heads, each pair with
-// its own strides.
+// Every forward entry: q / o over Sq rows and BH heads in B batch elements, k / v over Skv rows and BH / kv_group
+// heads, each tensor with its own strides.
 static int attn_fwd_run(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
                         const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
-                        const int32_t* o_rows, int dtype, int BH, int kv_group, int Sq, int Skv, int D, long long q_rs,
-                        long long q_hs, long long kv_rs, long long kv_hs, long long o_rs, long long o_hs,
-                        float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
+                        const int32_t* o_rows, int dtype, int B, int BH, int kv_group, int Sq, int Skv, int D,
+                        Strides qs, Strides ks, Strides vs, Strides os, float sm_scale, const svgb_plan* plan,
+                        const void* plan_ws, void* stream) {
   SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
   SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
                "fp8 attention needs the three per-head scale vectors");
@@ -499,7 +500,7 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH / kv_group),
                "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
                plan_kv_len(plan), BH / kv_group, Sq, Skv);
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && o_rs % 8 == 0 && o_hs % 8 == 0,
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && os.r % 8 == 0 && os.h % 8 == 0 && os.b % 8 == 0,
                "output must be 16-byte aligned with strides multiple of 8 elements");
   const char* ws = static_cast<const char*>(plan_ws);
   AttnArgs a;
@@ -509,8 +510,9 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.items_stride = plan->items_stride;
   a.kv_group = kv_group;
   a.o = o;
-  a.o_row_stride = o_rs;
-  a.o_head_stride = o_hs;
+  a.o_row_stride = os.r;
+  a.o_head_stride = os.h;
+  a.o_batch_stride = os.b;
   a.o_rows = o_rows;
   a.lse = lse;
   a.scale_log2 = sm_scale * 1.4426950408889634f;
@@ -529,9 +531,9 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.q_ptr = q;
   a.k_ptr = k;
   a.v_ptr = v;
-  a.in_row_stride = q_rs;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
-  a.in_head_stride = q_hs;
-  return attn_fwd_impl(q, Sq, q_rs, q_hs, k, v, Skv, kv_rs, kv_hs, dtype, BH, D, a, gather, plan->max_items,
+  a.in_row_stride = qs.r;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
+  a.in_head_stride = qs.h;
+  return attn_fwd_impl(q, qs, Sq, k, ks, v, vs, Skv, dtype, B, BH, D, a, gather, plan->max_items,
                        static_cast<cudaStream_t>(stream));
 }
 
@@ -626,9 +628,9 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream) {
-  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, BH, 1, S, S, D,
-                      row_stride, head_stride, row_stride, head_stride, o_row_stride, o_head_stride, sm_scale, plan,
-                      plan_ws, stream);
+  const Strides in = flat_strides(row_stride, head_stride, BH);
+  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, 1, BH, 1, S, S, D,
+                      in, in, in, flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BH, int Sq,
@@ -646,9 +648,10 @@ int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float
                    (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
                    kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
                "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
-  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, BH, 1, Sq, Skv, D,
-                      q_row_stride, q_head_stride, kv_row_stride, kv_head_stride, o_row_stride, o_head_stride,
-                      sm_scale, plan, plan_ws, stream);
+  const Strides kv = flat_strides(kv_row_stride, kv_head_stride, BH);
+  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 1, BH, 1, Sq, Skv,
+                      D, flat_strides(q_row_stride, q_head_stride, BH), kv, kv,
+                      flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BHq, int BHkv,
@@ -660,9 +663,23 @@ int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, floa
                    (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
                    kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
                "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
-  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, BHq, BHq / BHkv,
-                      Sq, Skv, D, q_row_stride, q_head_stride, kv_row_stride, kv_head_stride, o_row_stride,
-                      o_head_stride, sm_scale, plan, plan_ws, stream);
+  const Strides kv = flat_strides(kv_row_stride, kv_head_stride, BHkv);
+  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 1, BHq, BHq / BHkv,
+                      Sq, Skv, D, flat_strides(q_row_stride, q_head_stride, BHq), kv, kv,
+                      flat_strides(o_row_stride, o_head_stride, BHq), sm_scale, plan, plan_ws, stream);
+}
+
+int svgb_attn_fwd_strided(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int B, int Hq,
+                          int Hkv, int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
+                          const long long* v_strides, const long long* o_strides, float sm_scale,
+                          const svgb_plan* plan, const void* plan_ws, void* stream) {
+  Strides st[4];
+  if (attn_strided_check(B, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st,
+                         "svgb_attn_fwd_strided"))
+    return -1;
+  if (attn_gqa_check(dtype, B * Hq, B * Hkv, Sq, Skv, plan, "svgb_attn_fwd_strided")) return -1;
+  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, B, B * Hq,
+                      Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, stream);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

@@ -284,6 +284,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     // writes that wgmma reads through the async proxy; the writer cannot fence after an asynchronous copy, so each
     // consumer thread fences (fence.proxy.async) after its full-barrier wait, before its warpgroup's wgmma.
     const bool leader = wt == 0;
+    // the tensor maps' (head, batch) coordinates: query head hq and key/value head hkv of batch element `batch`
+    const int batch = bh / args.Hq, hq = bh - batch * args.Hq, hkv = hq / args.kv_group;
     int g = 0, nq = 0;  // chunks and Q tiles of the earlier streams
     for (int st = 0; st < nstreams; ++st) {
       const Stream sm = stream(st);
@@ -302,7 +304,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         const uint32_t qb = smem_u32(&ctl->q_full);
         mbar_wait(smem_u32(&ctl->q_empty), (nq & 1) ^ 1, 5);
         mbar_expect_tx(qb, Cfg::kTileBytes);
-        for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sQ + h * Cfg::kPanelBytes, &qmap, qb, h * Cfg::kPanelElems, sm.q0, bh);
+        for (int x = 0; x < Cfg::kHalves; ++x) tma_load_4d(sQ + x * Cfg::kPanelBytes, &qmap, qb, x * Cfg::kPanelElems, sm.q0, hq, batch);
       }
       for (int j = 0; j < sm.nch; ++j) {
         const int n = g + j, s = n % kKvStages, par = ((n / kKvStages) & 1) ^ 1;
@@ -322,10 +324,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
           const int kv0 = __ldg(&sm.list[j].x);
           mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
           mbar_expect_tx(kf, Cfg::kTileBytes);
-          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sK + h * Cfg::kPanelBytes, &kmap, kf, h * Cfg::kPanelElems, kv0, kvh);
+          for (int x = 0; x < Cfg::kHalves; ++x) tma_load_4d(sK + x * Cfg::kPanelBytes, &kmap, kf, x * Cfg::kPanelElems, kv0, hkv, batch);
           mbar_wait(smem_u32(&ctl->v_empty[s]), par, 7);
           mbar_expect_tx(vf, Cfg::kTileBytes);
-          for (int h = 0; h < Cfg::kHalves; ++h) tma_load_3d(sV + h * Cfg::kPanelBytes, &vmap, vf, h * Cfg::kPanelElems, kv0, kvh);
+          for (int x = 0; x < Cfg::kHalves; ++x) tma_load_4d(sV + x * Cfg::kPanelBytes, &vmap, vf, x * Cfg::kPanelElems, kv0, hkv, batch);
         }
         // FP8: widen the previous chunk's V, requested one chunk earlier, rather than wait here for V(j) to land
         if constexpr (FP8) {
@@ -506,6 +508,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     }
 
     // ---------------- epilogue: O / l -> global (optionally scattered rows), LSE
+    // batch element and head of the o store (the row gather: its one batch element), derived per stream rather than
+    // kept live through the chunk loop, since the consumers are register-bound
+    long long o_base = bh * args.o_head_stride;
+    if constexpr (!kGather) {
+      const int bhe = ctaid_y_here(), batch = bhe / args.Hq;
+      o_base = batch * args.o_batch_stride + (bhe - batch * args.Hq) * args.o_head_stride;
+    }
 #pragma unroll
     for (int v1 = 0; v1 < 2; ++v1) {
       float l = l_run[v1];
@@ -519,13 +528,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       if (args.o_rows) out_row = __ldg(&args.o_rows[static_cast<size_t>(bh) * args.S + q]);
       const int col0 = 2 * (lane & 3);
       if (args.out_f32) {
-        float* optr = reinterpret_cast<float*>(args.o) + bh * args.o_head_stride + out_row * args.o_row_stride;
+        float* optr = reinterpret_cast<float*>(args.o) + o_base + out_row * args.o_row_stride;
 #pragma unroll
         for (int jj = 0; jj < D / 8; ++jj)
           *reinterpret_cast<float2*>(optr + 8 * jj + col0) =
               make_float2(o[4 * jj + 2 * v1] * inv_l, o[4 * jj + 2 * v1 + 1] * inv_l);
       } else {
-        uint16_t* optr = reinterpret_cast<uint16_t*>(args.o) + bh * args.o_head_stride + out_row * args.o_row_stride;
+        uint16_t* optr = reinterpret_cast<uint16_t*>(args.o) + o_base + out_row * args.o_row_stride;
 #pragma unroll
         for (int jj = 0; jj < D / 8; ++jj)
           *reinterpret_cast<uint32_t*>(optr + 8 * jj + col0) =

@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <initializer_list>
+
 #include "../../include/svgb200.h"
 
 namespace svgb {
@@ -50,34 +52,67 @@ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 int encode_tmap_hsd(CUtensorMap* map, const void* base, int dtype, int BH, int S, int D,
                     long long row_stride_elems, long long head_stride_elems, int box_rows = 128);
 
+// element strides of one [B, H, S, D] attention operand; the last dimension is contiguous
+struct Strides {
+  long long b, h, r;
+};
+// the (row, head) stride pair of a flat [BH, S, D] operand: one batch element of BH heads
+inline Strides flat_strides(long long rs, long long hs, int BH) { return {BH * hs, hs, rs}; }
+
+// 4-D TMA descriptor over a [B, H, S, D] operand addressed as (d, s, h, b) with the byte strides of st.
+// box = one 128-byte panel x 128 rows x 1 x 1, 128-byte swizzle.  Returns 0 on success.
+int encode_tmap_bhsd(CUtensorMap* map, const void* base, int dtype, int B, int H, int S, int D, Strides st);
+
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0 (svgb200.h);
 // every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) { return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S; }
 
-// the checks svgb_attn_fwd_gqa and svgb_attn_bwd_gqa share, before any device work: BHq query heads in groups over
-// BHkv key/value heads, 16-bit inputs, and a variable-block plan over the key/value heads or a band plan (one work
-// list for every head, Sq == Skv)
+// the checks the grouped-query and strided entries (svgb_attn_{fwd,bwd}_{gqa,strided}) share, before any device
+// work: BHq query heads in groups over BHkv key/value heads, 16-bit inputs, and a variable-block plan over the
+// key/value heads or a band plan (one work list for every head, Sq == Skv)
 inline int attn_gqa_check(int dtype, int BHq, int BHkv, int Sq, int Skv, const svgb_plan* plan, const char* who) {
   SVGB_REQUIRE(plan, "null pointer");
   SVGB_REQUIRE(BHq > 0 && BHkv > 0 && BHq % BHkv == 0,
                "%s: the query heads BHq=%d must be a multiple of the key/value heads BHkv=%d", who, BHq, BHkv);
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
-               "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no GQA path)", who, dtype);
+               "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no GQA or strided path)", who, dtype);
   SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND,
-               "%s takes variable-block or band plans (kind %d; gather and key-major plans have no GQA path)", who,
-               plan->kind);
+               "%s takes variable-block or band plans (kind %d; gather and key-major plans have no GQA or strided "
+               "path)", who, plan->kind);
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
   SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
                "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
   return 0;
 }
 
+// the operands of a strided entry (svgb_attn_fwd_strided, svgb_attn_bwd_strided), before any device work: B batch
+// elements of Hq query heads over Hkv key/value heads, 16-byte aligned bases, and (batch, head, row) strides that are
+// nonzero multiples of 8 elements, copied to st[i]
+inline int attn_strided_check(int B, int Hq, int Hkv, std::initializer_list<const void*> ptrs,
+                              std::initializer_list<const long long*> strides, Strides* st, const char* who) {
+  SVGB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0, "%s: bad head counts B=%d Hq=%d Hkv=%d", who, B, Hq, Hkv);
+  for (const void* p : ptrs) {
+    SVGB_REQUIRE(p, "null pointer");
+    SVGB_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, "%s: every tensor must be 16-byte aligned", who);
+  }
+  for (const long long* s : strides) {
+    SVGB_REQUIRE(s, "null pointer");
+    for (int i = 0; i < 3; ++i)
+      SVGB_REQUIRE(s[i] != 0 && s[i] % 8 == 0,
+                   "%s: every (batch, head, row) stride must be a nonzero multiple of 8 elements (got %lld, %lld, %lld)",
+                   who, s[0], s[1], s[2]);
+    *st++ = {s[0], s[1], s[2]};
+  }
+  return 0;
+}
+
 struct AttnArgs;
 // attention launch with independent query / key-value geometry (attn_fwd.cu); used by svgb_attn_fwd
-// and by sample_mse's split-KV passes.  Checks D and dtype; gather selects the row-gather kernel (run lists).
-int attn_fwd_impl(const void* q, int Sq, long long q_rs, long long q_hs, const void* k, const void* v, int Skv,
-                  long long kv_rs, long long kv_hs, int dtype, int BH, int D, const AttnArgs& a, bool gather,
-                  int grid_x, cudaStream_t st);
+// and by sample_mse's split-KV passes.  q over B batch elements of BH / B heads and Sq rows, k and v over
+// BH / a.kv_group heads and Skv rows, each with its own strides.  Checks D and dtype; gather selects the row-gather
+// kernel (run lists, B = 1).
+int attn_fwd_impl(const void* q, Strides qs, int Sq, const void* k, Strides ks, const void* v, Strides vs, int Skv,
+                  int dtype, int B, int BH, int D, const AttnArgs& a, bool gather, int grid_x, cudaStream_t st);
 
 // stable counting-sort argsort (layout_ops.cu); `offs` (optional) receives the exclusive prefix of
 // counts per head; `skip_flag` (optional, device) turns the three kernels into no-ops when non-zero.

@@ -216,8 +216,9 @@ int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* 
     a.m2 = layout == 2 ? (thres | (ctx << 12)) : thres;
     a.q_index = reinterpret_cast<const int*>(w + L.qidx);
     a.out_f32 = 1;
-    if (attn_fwd_impl(w + L.qg, rows_per_head, D, static_cast<long long>(rows_per_head) * D, k, v, S, D,
-                      static_cast<long long>(S) * D, dtype, BH, D, a, false, L.nsplit, st))
+    const Strides kv = flat_strides(D, static_cast<long long>(S) * D, BH);
+    if (attn_fwd_impl(w + L.qg, flat_strides(D, static_cast<long long>(rows_per_head) * D, BH), rows_per_head, k, kv,
+                      v, kv, S, dtype, 1, BH, D, a, false, L.nsplit, st))
       return -1;
   }
   smse_combine_kernel<<<dim3(BH, kCombineParts), 256, 0, st>>>(

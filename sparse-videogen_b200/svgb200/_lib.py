@@ -30,6 +30,7 @@ class Plan(C.Structure):
 
 _vp, _i, _f, _ll, _sz = C.c_void_p, C.c_int, C.c_float, C.c_longlong, C.c_size_t
 _psz = C.POINTER(C.c_size_t)
+_pll = C.POINTER(C.c_longlong)  # a {batch, head, row} stride triple
 _pplan = C.POINTER(Plan)
 
 # name -> argtypes (restype is int unless noted).  Kept in declaration order of svgb200.h.
@@ -51,6 +52,8 @@ _PROTOS = {
                          _vp],
     "svgb_attn_fwd_gqa": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan,
                           _vp, _vp],
+    "svgb_attn_fwd_strided": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll, _pll, _f, _pplan,
+                              _vp, _vp],
     "svgb_quantize_e4m3": [_vp, _i, _vp, _vp, _i, _i, _i, _vp],
     "svgb_attn_bwd_bytes": [_i, _i, _psz],
     "svgb_attn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _f, _pplan, _vp, _pplan,
@@ -61,6 +64,9 @@ _PROTOS = {
     "svgb_attn_bwd_gqa_bytes": [_i, _i, _i, _i, _psz],
     "svgb_attn_bwd_gqa": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                           _pplan, _vp, _pplan, _vp, _vp, _sz, _vp],
+    "svgb_attn_bwd_strided_bytes": [_i, _i, _i, _i, _i, _psz],
+    "svgb_attn_bwd_strided": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, *[_pll] * 8, _f,
+                              _pplan, _vp, _pplan, _vp, _vp, _sz, _vp],
     "svgb_density": [_vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "svgb_argsort_labels_bytes": [_i, _i, _i, _psz],
     "svgb_argsort_labels": [_vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp],

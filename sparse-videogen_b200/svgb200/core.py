@@ -210,19 +210,53 @@ def _kv_group(q, k):
     return q.shape[1] // k.shape[1]
 
 
+def _strides(t, layout):
+    """(batch, head, row) element strides of an attention operand, as the strided entries take them; 'shd' is one batch
+    element.  A dimension of extent 1 is never stepped, so a stride there that the ABI would refuse is replaced by 8."""
+    if layout == "bhsd":
+        n, st = t.shape[:3], t.stride()[:3]
+    else:
+        n, st = (1, t.shape[1], t.shape[0]), (t.shape[1] * t.stride(1), t.stride(1), t.stride(0))
+    return tuple(8 if e == 1 and not (x and x % 8 == 0) else x for e, x in zip(n, st))
+
+
+def _addressable(t, layout):
+    """True when the strided entries (svgb_attn_fwd_strided / svgb_attn_bwd_strided) read or write t in place: the
+    last stride is 1, the base 16-byte aligned and the (batch, head, row) strides nonzero multiples of 8 elements."""
+    return t.stride(-1) == 1 and t.data_ptr() % 16 == 0 and all(x and x % 8 == 0 for x in _strides(t, layout))
+
+
+def _addressed(t, layout):
+    """t itself when the strided entries can read it, otherwise a contiguous copy (a zero stride such as the expanded
+    gradient of o.sum(), a misaligned view, a last stride other than 1).  A clone rather than .contiguous(), which
+    would return a misaligned contiguous tensor itself."""
+    return t if _addressable(t, layout) else t.clone(memory_format=torch.contiguous_format)
+
+
+def _st(t, layout):
+    return (C.c_longlong * 3)(*_strides(t, layout))
+
+
 def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
-    """One attention launch.  Fewer key/value heads than query heads (G > 1) take svgb_attn_fwd_gqa: 16-bit, no
-    scales, no row vectors, no gather plan.  Otherwise equal sequence lengths take svgb_attn_fwd: 16-bit or e4m3
-    (dtype) with its per-head scales, and the row vectors rows = (q_rows, kv_rows, o_rows); other lengths
-    svgb_attn_fwd_kv: q and o over Sq rows, k and v over Skv rows, each pair with its own strides; 16-bit, no scales,
-    no row vectors."""
+    """One attention launch.  Operands that are not all contiguous take svgb_attn_fwd_strided, each at its own strides
+    (_addressable): 16-bit, no scales, no row vectors, no gather plan.  Otherwise fewer key/value heads than query
+    heads (G > 1) take svgb_attn_fwd_gqa: 16-bit, no scales, no row vectors, no gather plan.  Otherwise equal sequence
+    lengths take svgb_attn_fwd: 16-bit or e4m3 (dtype) with its per-head scales, and the row vectors rows = (q_rows,
+    kv_rows, o_rows); other lengths svgb_attn_fwd_kv: q and o over Sq rows, k and v over Skv rows, each pair with its
+    own strides; 16-bit, no scales, no row vectors."""
     BH, Sq, Skv, D, qs, kvs = _kv_geometry(q, k, layout)
     G = _kv_group(q, k)
     if G > 1:
         _gqa_check(dtype, plan, rows)
     lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    if G > 1:
+    if not all(t.is_contiguous() for t in (q, k, v, o)):
+        B = q.shape[0] if layout == "bhsd" else 1
+        check(lib().svgb_attn_fwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), dtype, B,
+                                          q.shape[1], k.shape[1], Sq, Skv, D, *(_st(t, layout) for t in (q, k, v, o)),
+                                          scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
+              "svgb_attn_fwd_strided")
+    elif G > 1:
         check(lib().svgb_attn_fwd_gqa(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), dtype, BH,
                                       BH // G, Sq, Skv, D, *qs, *kvs, *qs, scale, C.byref(plan.desc),
                                       plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd_gqa")
@@ -255,24 +289,41 @@ def _gqa_check(dtype, plan, rows=()):
 def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[torch.Tensor] = None,
              q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
              return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
-    """layout 'bhsd': q,k,v [B,H,S,D] contiguous;  'shd': [S,H,D] contiguous (ops API).
+    """layout 'bhsd': q,k,v [B,H,S,D];  'shd': [S,H,D] (ops API).  q, k, v may be views ([B, S, H, D] passed as
+    x.transpose(1, 2), one of a packed projection's unbind(2), every other head, a batch slice): they are read in place
+    when their last stride is 1, their base 16-byte aligned and their other strides nonzero multiples of 8 elements,
+    and copied with .contiguous() otherwise.  o is torch.empty_like(q), so it keeps a view's memory order; out= may be
+    a view too, and only its elements are written.
     o_rows scatters the output rows; q_rows / kv_rows gather the input rows and need a gather plan
-    (plan_varblock(..., gather=True)); all three are int [BH,S] (include/svgb200.h, svgb_attn_fwd).
+    (plan_varblock(..., gather=True)); all three are int [BH,S] (include/svgb200.h, svgb_attn_fwd).  Row vectors and
+    gather plans take contiguous q, k, v and out only.
     k, v may have another sequence length S_kv than q (same batch, heads, D and dtype): the plan is then a rectangular
     variable-block plan (plan_varblock(..., S_kv=)), o has q's shape, and row vectors are not taken.
     k, v may have fewer heads than q, Hq = G * Hkv (grouped-query attention, FlashInfer's mapping: query head h attends
     with key/value head h // G): a variable-block plan is then built over the B * Hkv key/value heads and shared by
     each group, band plans are shared by every head already; no row vectors, FP8 or gather plans."""
     _need_cuda(q, k, v)
-    if not (q.is_contiguous() and k.is_contiguous() and v.is_contiguous()):
-        raise SvgbError("q, k, v must be contiguous")
+    rows = (q_rows, kv_rows, o_rows)
+    if any(r is not None for r in rows) or plan.desc.kind == PLAN_GATHER:
+        # the row vectors and the row-gather kernel index one flat [BH, S, D] stride pair
+        if not (q.is_contiguous() and k.is_contiguous() and v.is_contiguous()):
+            raise SvgbError("q, k, v must be contiguous")
+        if out is not None and not out.is_contiguous():
+            raise SvgbError("out must be contiguous with row vectors or a gather plan")
+    else:
+        q, k, v = (_addressed(t, layout) for t in (q, k, v))
     if not (q.dtype == k.dtype == v.dtype) or k.shape != v.shape:
         raise SvgbError("q, k, v must share dtype, and k, v their shape")
-    o = torch.empty_like(q) if out is None else out
-    if q.shape[1] == k.shape[1] and q.shape != k.shape and (o_rows is not None or q_rows is not None
-                                                           or kv_rows is not None):
+    if out is not None and (out.shape != q.shape or out.dtype != q.dtype):
+        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype")
+    o = torch.empty_like(q) if out is None or not _addressable(out, layout) else out
+    if q.shape[1] == k.shape[1] and q.shape != k.shape and any(r is not None for r in rows):
         raise SvgbError("row vectors (o_rows / q_rows / kv_rows) need k, v of q's sequence length")
-    return _attn(q, k, v, o, plan, layout, _dt(q), (None, None, None), (q_rows, kv_rows, o_rows), return_lse, sm_scale)
+    res = _attn(q, k, v, o, plan, layout, _dt(q), (None, None, None), rows, return_lse, sm_scale)
+    if out is None or o is out:
+        return res
+    out.copy_(o)  # an out= the kernels cannot address
+    return (out, res[1]) if return_lse else out
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
@@ -282,14 +333,16 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
     key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits.
     k, v may have another sequence length than q under a rectangular variable-block plan, and fewer heads (grouped-query
     attention, as attn_fwd); dk, dv then have k's shape, a group's dk and dv summing over its query heads.
-    out: optional (dq, dk, dv) tensors of q's, k's and v's dtype and shape, contiguous, written and returned instead
-    of new ones."""
+    Every tensor may be a view, as in attn_fwd: q, k, v, o, do are read in place where the strided entry can address
+    them and copied with .contiguous() otherwise (do with a zero stride, for instance).
+    out: optional (dq, dk, dv) tensors of q's, k's and v's dtype and shape, written and returned instead of new ones;
+    each may be a view, whose every element is written and nothing outside it.  Without out, dq, dk, dv are
+    torch.empty_like(q / k / v) and keep the inputs' memory order."""
     _need_cuda(q, k, v, o, do, lse)
-    ts = (q, k, v, o, do) + (tuple(out) if out is not None else ())
     if out is not None and len(out) != 3:
         raise SvgbError("out must be a (dq, dk, dv) tuple")
-    if not all(t.is_contiguous() for t in ts):
-        raise SvgbError("q, k, v, o, do (and out) must be contiguous")
+    q, k, v, o, do = (_addressed(t, layout) for t in (q, k, v, o, do))
+    ts = (q, k, v, o, do) + (tuple(out) if out is not None else ())
     like = (q, k, k, q, q) + ((q, k, k) if out is not None else ())
     if not all(t.dtype == q.dtype and t.shape == r.shape for t, r in zip(ts, like)):
         raise SvgbError("q, k, v, o, do (and out) must share dtype; o, do, dq have q's shape, v, dk, dv k's")
@@ -299,6 +352,24 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
         _gqa_check(_dt(q), plan)
     plan_t = plan.key_major()
     lse = lse.to(torch.float32).contiguous()
+    grads = (torch.empty_like(t) for t in (q, k, v)) if out is None else out
+    dq, dk, dv = (g if _addressable(g, layout) else torch.empty_like(r) for g, r in zip(grads, (q, k, v)))
+    _need_cuda(dq, dk, dv)
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    if not all(t.is_contiguous() for t in (q, k, v, o, do, dq, dk, dv)):
+        B = q.shape[0] if layout == "bhsd" else 1
+        lens = (B, q.shape[1], k.shape[1], Sq, Skv)
+        nbytes = C.c_size_t()
+        check(lib().svgb_attn_bwd_strided_bytes(*lens, C.byref(nbytes)), "svgb_attn_bwd_strided_bytes")
+        ws = workspace(("attn_bwd", BH, Sq), nbytes.value, q.device)
+        check(lib().svgb_attn_bwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                          lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), *lens, D,
+                                          *(_st(t, layout) for t in (q, k, v, o, do, dq, dk, dv)), scale,
+                                          C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc),
+                                          plan_t.ws.data_ptr(), ws.data_ptr(), ws.numel(), _stream(q)),
+              "svgb_attn_bwd_strided")
+        _bump(3)
+        return _written(out, (dq, dk, dv))
     # equal lengths and heads take svgb_attn_bwd, whose q and k share one length and one pair of strides
     if G > 1:
         name, lens, strides = "svgb_attn_bwd_gqa", (BH, BH // G, Sq, Skv), qs + kvs
@@ -309,15 +380,22 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_sc
     nbytes = C.c_size_t()
     check(getattr(lib(), name + "_bytes")(*lens, C.byref(nbytes)), name + "_bytes")
     ws = workspace(("attn_bwd", BH, Sq), nbytes.value, q.device)
-    dq, dk, dv = (torch.empty_like(t) for t in (q, k, v)) if out is None else out
-    _need_cuda(dq, dk, dv)
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
     check(getattr(lib(), name)(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(),
                                dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), _dt(q), *lens, D, *strides, scale,
                                C.byref(plan.desc), plan.ws.data_ptr(), C.byref(plan_t.desc), plan_t.ws.data_ptr(),
                                ws.data_ptr(), ws.numel(), _stream(q)), name)
     _bump(3)
-    return dq, dk, dv
+    return _written(out, (dq, dk, dv))
+
+
+def _written(out, gs):
+    """The gradients, copied into those of the out= tensors the kernels could not address."""
+    if out is None:
+        return gs
+    for o, g in zip(out, gs):
+        if o is not g:
+            o.copy_(g)
+    return tuple(out)
 
 
 class _Attention(torch.autograd.Function):
@@ -331,7 +409,7 @@ class _Attention(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do):
         q, k, v, o, lse = ctx.saved_tensors
-        dq, dk, dv = attn_bwd(q, k, v, o, do.contiguous(), lse, ctx.plan, layout=ctx.layout, sm_scale=ctx.sm_scale)
+        dq, dk, dv = attn_bwd(q, k, v, o, do, lse, ctx.plan, layout=ctx.layout, sm_scale=ctx.sm_scale)
         return dq, dk, dv, None, None, None
 
 

@@ -100,7 +100,7 @@ def dynamic_block_sparse_fwd_flashinfer(q, k, v, block_mask_map, block_row_sz, b
     """svg/kmeans_utils.py:1319-1392.  q,k,v [B,H,S,D]; map bool [B,H,QC,KC]; sizes [B,H,QC]/[B,H,KC]
     (on CPU when is_cpu, like the reference's default; moved to the GPU here)."""
     plan = _flashinfer_plan(q, block_mask_map, block_row_sz, block_col_sz)
-    return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan)
+    return core.attention(q, k, v, plan)
 
 
 def dynamic_block_sparse_fwd_triton(q, k, v, dynamic_map, qc_size, kc_size):

@@ -100,4 +100,4 @@ def sparse_attn_forward(q, k, v, metadata: FAMetadata, sparse_pattern: str = "te
     indptr, indices, block_size = md
     T = metadata.len_text_promt
     plan = bsr_to_plan(indptr, indices, block_size, q.shape[0] - T, T, q.device)
-    return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
+    return core.attention(q, k, v, plan, layout="shd")

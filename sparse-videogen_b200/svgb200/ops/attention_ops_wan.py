@@ -53,7 +53,7 @@ def wan_sparse_attn_forward(q, k, v, metadata: WanFAMetadata):
     assert k.shape[0] % block_size[1] == 0, f"Key length {k.shape[0]} % block_size {block_size[1]} != 0"
     assert k.shape[0] == v.shape[0], f"Key length {k.shape[0]} != Value length {v.shape[0]}"
     plan = bsr_to_plan(indptr, indices, block_size, q.shape[0], 0, q.device)
-    return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan, layout="shd")
+    return core.attention(q, k, v, plan, layout="shd")
 
 
 def flashinfer_sparse_attn_forward(q, k, v, temporal_mask_metadata):
@@ -62,4 +62,4 @@ def flashinfer_sparse_attn_forward(q, k, v, temporal_mask_metadata):
     cfg, H, S, D = q.shape
     assert S % block_size[0] == 0 and S % block_size[1] == 0
     plan = bsr_to_plan(indptr, indices, block_size, S, 0, q.device)
-    return core.attention(q.contiguous(), k.contiguous(), v.contiguous(), plan)
+    return core.attention(q, k, v, plan)

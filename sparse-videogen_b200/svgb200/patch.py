@@ -95,7 +95,7 @@ def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, m
     from .models.common import segment_attention
 
     seg, seg_kv = _varlen_segments(cu_seqlens_q, cu_seqlens_kv)
-    return segment_attention("flash_attn_varlen_func", q.contiguous(), k.contiguous(), v.contiguous(), seg, seg_kv,
+    return segment_attention("flash_attn_varlen_func", q, k, v, seg, seg_kv,
                              layout="shd")
 
 
