@@ -43,6 +43,11 @@ extern "C" {
 #define SVGB_MASK_PROF_WAN_T 7  /* ... temporal                                                           */
 #define SVGB_MASK_PROF_COG_S 8  /* cog/utils.py:61-88 spatial, text first (text rows / columns attend)    */
 #define SVGB_MASK_PROF_COG_T 9  /* ... temporal, video x video only (text rows / columns see nothing)     */
+/* Local band with attention sinks: m0 = sink, m1 = left, m2 = right, all >= 0 (so every row keeps its diagonal key).
+ *   allowed(q, kv) = (kv < sink) | ((q - kv <= left) & (kv - q <= right))
+ * Causal attention is (0, S, 0); FlashAttention's window_size = (l, r) is (0, l, r) with -1 taken as S; a streaming
+ * sink-plus-window is (sink, l, 0).  SVGB_MASK_WAN(P, W) is SVGB_MASK_LOCAL(P, W, W).  Forward and backward. */
+#define SVGB_MASK_LOCAL 10
 
 /* ---- library ---------------------------------------------------------------------------- */
 int svgb_version(void);
@@ -99,7 +104,10 @@ int svgb_attn_plan_varblock_gather(const uint8_t* map, const int32_t* row_sz, co
                                    void* stream);
 
 /* SVG1: one element-exact band mask shared by every head.  Stands behind prepare_flexattention /
- * create_block_mask (svg/models/hyvideo/attention.py:527-551). */
+ * create_block_mask (svg/models/hyvideo/attention.py:527-551), and, with SVGB_MASK_LOCAL, behind causal and
+ * sliding-window attention (a negative sink, left or right is an error).  Items are issued heaviest first: under
+ * SVGB_MASK_LOCAL with left > right the query-major plan lists its items from the last rows back, and with right > left
+ * the key-major plan does. */
 int svgb_attn_plan_band_bytes(int S, size_t* bytes);
 int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
                         size_t ws_bytes, svgb_plan* plan, void* stream);
@@ -192,7 +200,7 @@ int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH,
  *           row_stride / head_stride pair (elements; 16-byte aligned bases, strides multiples of 8 elements).
  *   lse   : float [BH,S] written by svgb_attn_fwd under the same plan and sm_scale.
  *   plan  : the forward (query-major) plan, SVGB_PLAN_VARBLOCK or SVGB_PLAN_BAND with mask SVGB_MASK_NONE / HY / WAN /
- *           COG.  plan_t: its key-major companion -- svgb_attn_plan_band_t with the same mask for a band plan,
+ *           COG / LOCAL (not the profiling masks 4-9).  plan_t: its key-major companion -- svgb_attn_plan_band_t with the same mask for a band plan,
  *           svgb_attn_plan_varblock(map^T, col_sz, row_sz) for a variable-block plan.
  *   ws    : device scratch of svgb_attn_bwd_bytes (per-row delta = rowsum(dO * O)).
  * Every row of dq, dk, dv is written (rows without an allowed key: dq = 0; keys no row reaches: dk = dv = 0); the

@@ -61,6 +61,10 @@ enum MaskMode : int {
   //             (cog/utils.py:76-86) -- a sampled text row has no allowed key at all
   MASK_PROF_COG_S = 8,
   MASK_PROF_COG_T = 9,
+  // Local band with attention sinks (causal, sliding window, StreamingLLM):
+  //   m0 = sink, m1 = left, m2 = right (all >= 0)   : kv < sink | (q - kv <= left & kv - q <= right)
+  // MASK_WAN(P, W) is MASK_LOCAL(P, W, W).
+  MASK_LOCAL = 10,
 };
 
 __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, int m1, int m2) {
@@ -74,8 +78,10 @@ __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, in
       const bool vid = (d < m2) | (kv >= m0) | (q >= m0);
       return (real & vid) | fake;
     }
-    case MASK_WAN:
+    case MASK_WAN:  // MASK_LOCAL(m0, m2, m2), kept as |q - kv| (DESIGN §1: fewer instructions in the ELEM chunks)
       return (kv < m0) | (d <= m2);
+    case MASK_LOCAL:
+      return (kv < m0) | ((q - kv <= m1) & (kv - q <= m2));
     case MASK_COG:
       return (kv < m0) | (q < m1) | (d < m2);
     case MASK_PROF_COG_S: {
@@ -242,6 +248,7 @@ struct ElemMask {
     if (mode == MASK_HY) bits_direct<MASK_HY>(kvb, keep);
     else if (mode == MASK_WAN) bits_direct<MASK_WAN>(kvb, keep);
     else if (mode == MASK_COG) bits_direct<MASK_COG>(kvb, keep);
+    else if (mode == MASK_LOCAL) bits_direct<MASK_LOCAL>(kvb, keep);
     else if (mode == MASK_PROF_COG_S) bits_direct<MASK_PROF_COG_S>(kvb, keep);
     else if (mode == MASK_PROF_HY_S || mode == MASK_PROF_WAN_S) bits_banded<false>(kvb, keep);
     else if (banded(mode)) bits_banded<true>(kvb, keep);

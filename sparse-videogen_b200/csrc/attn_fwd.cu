@@ -197,6 +197,7 @@ struct BandSegs {
   int bound[6];      // bound[s] .. bound[s+1]
   int item_base[6];  // first item index of segment s (launch order)
   int item_cnt[6];
+  int reversed[6];   // the segment's items run from its last rows back (heaviest first under a one-sided band)
 };
 
 // transposed = 1 builds the KEY-MAJOR plan of the backward pass: rows are keys, chunks are query ranges, and the vote
@@ -208,7 +209,8 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
   int seg = 0;
   for (int s = 0; s < segs.n; ++s)
     if (item >= segs.item_base[s] && item < segs.item_base[s] + segs.item_cnt[s]) seg = s;
-  const int q_row0 = segs.bound[seg] + (item - segs.item_base[seg]) * kItemRows;
+  const int k = item - segs.item_base[seg];
+  const int q_row0 = segs.bound[seg] + (segs.reversed[seg] ? segs.item_cnt[seg] - 1 - k : k) * kItemRows;
   const int nrows = min(kItemRows, segs.bound[seg + 1] - q_row0);
   const int q = q_row0 + threadIdx.x;
   const bool row_live = static_cast<int>(threadIdx.x) < nrows;
@@ -239,9 +241,11 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
 }
 
 // row-region boundaries of each mask family, and the launch order of the segments.  Key-major (transposed): the
-// HunyuanVideo regions are the same; the Wan sink keys (kv < P) and the CogVideoX first columns (kv < m0) are seen by
-// every query and form the heavy first segment.
-static BandSegs band_segments(int mode, int m0, int m1, int S, bool transposed = false) {
+// HunyuanVideo regions are the same; the Wan and local sink keys (kv < m0) and the CogVideoX first columns (kv < m0)
+// are seen by every query and form the heavy first segment.  A one-sided local band (left != right) makes list length
+// grow along the rows: query-major with left > right the last rows see the most keys, key-major with right > left the
+// last keys are reached by the most queries, and that segment's items are then issued from its end (LPT).
+static BandSegs band_segments(int mode, int m0, int m1, int m2, int S, bool transposed = false) {
   int cuts[4], nc = 0;
   auto add = [&](int c) {
     if (c > 0 && c < S && (nc == 0 || cuts[nc - 1] < c)) cuts[nc++] = c;
@@ -251,8 +255,8 @@ static BandSegs band_segments(int mode, int m0, int m1, int S, bool transposed =
     add(m1);  // end of real prompt
   } else if (mode == MASK_COG) {
     add(transposed ? m0 : m1);  // end of the first columns (key-major) / of the text prefix
-  } else if (mode == MASK_WAN && transposed) {
-    add(m0);  // end of the first-frame sink keys
+  } else if ((mode == MASK_WAN || mode == MASK_LOCAL) && transposed) {
+    add(m0);  // end of the sink keys
   }
   BandSegs sg{};
   sg.n = nc + 1;
@@ -272,6 +276,7 @@ static BandSegs band_segments(int mode, int m0, int m1, int S, bool transposed =
       base += sg.item_cnt[s];
     }
   }
+  if (mode == MASK_LOCAL && (transposed ? m2 > m1 : m1 > m2)) sg.reversed[sg.n - 1] = 1;  // the band, after any sinks
   return sg;
 }
 static int band_total_items(const BandSegs& sg) {
@@ -583,8 +588,10 @@ static int plan_band_impl(int mask_mode, int m0, int m1, int m2, int BH, int S, 
   if (svgb_attn_plan_band_bytes(S, &need)) return -1;
   SVGB_REQUIRE(plan_ws && plan, "null pointer");
   SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_PROF_COG_T, "unknown mask mode %d", mask_mode);
-  const BandSegs sg = band_segments(mask_mode, m0, m1, S, transposed);
+  SVGB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_LOCAL, "unknown mask mode %d", mask_mode);
+  SVGB_REQUIRE(mask_mode != MASK_LOCAL || (m0 >= 0 && m1 >= 0 && m2 >= 0),
+               "local mask: sink (m0 = %d), left (m1 = %d) and right (m2 = %d) must be >= 0", m0, m1, m2);
+  const BandSegs sg = band_segments(mask_mode, m0, m1, m2, S, transposed);
   const int n_items = band_total_items(sg);
   const int n_items_cap = (S + kItemRows - 1) / kItemRows + 4;
   const int n_chunks = (S + kChunkCols - 1) / kChunkCols;

@@ -14,6 +14,8 @@ from ._lib import Plan, SvgbError, check, lib
 MASK_NONE, MASK_HY, MASK_WAN, MASK_COG = 0, 1, 2, 3
 # SVG1 profiling masks (include/svgb200.h SVGB_MASK_PROF_*): the element masks of sample_mse, also accepted by plan_band
 MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_S, MASK_PROF_COG_T = 4, 5, 6, 7, 8, 9
+# local band with attention sinks (SVGB_MASK_LOCAL): m0 = sink, m1 = left, m2 = right; plan_local builds it
+MASK_LOCAL = 10
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
 PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T = 1, 2, 3, 4
 _E4M3 = 2  # SVGB_E4M3 (the 16-bit dtype ids come from _dt)
@@ -98,9 +100,9 @@ class AttnPlan:
         if self._key_major is None:
             d = self.desc
             if d.kind == PLAN_BAND:
-                if d.mask_mode > MASK_COG:
+                if _is_profiling(d.mask_mode):
                     raise SvgbError(f"attention backward: the profiling mask mode {d.mask_mode} has no backward "
-                                    "(executed masks NONE / HY / WAN / COG only)")
+                                    "(executed masks NONE / HY / WAN / COG / LOCAL only)")
                 self._key_major = plan_band_t(d.mask_mode, d.m0, d.m1, d.m2, d.BH, d.S, self.ws.device)
             elif d.kind == PLAN_VARBLOCK and self.source is not None:
                 *ts, versions = self.source
@@ -174,6 +176,25 @@ def plan_band_t(mask_mode: int, m0: int, m1: int, m2: int, BH: int, S: int, devi
     """Key-major form of plan_band's mask (include/svgb200.h svgb_attn_plan_band_t), for attn_bwd."""
     return _plan_band(lib().svgb_attn_plan_band_t_bytes, lib().svgb_attn_plan_band_t, "plan_band_t", mask_mode, m0,
                       m1, m2, BH, S, device)
+
+
+def plan_local(BH: int, S: int, device, *, causal: bool = False, window_size=(-1, -1), sink: int = 0) -> AttnPlan:
+    """Causal or sliding-window attention with attention sinks, in FlashAttention's conventions: query q sees key kv
+    when kv < sink, or when kv lies at most window_size[0] positions behind q and at most window_size[1] ahead of it
+    (-1: unbounded); causal=True sets the right window to 0 and conflicts with a positive window_size[1].  A band plan
+    of MASK_LOCAL(sink, left, right), so every entry that runs band plans runs it, forward and backward."""
+    left, right = (int(w) for w in window_size)
+    if causal:
+        if right > 0:
+            raise SvgbError(f"plan_local: causal=True looks no key ahead, but window_size[1] = {right}")
+        right = 0
+    left, right = (S if w == -1 else w for w in (left, right))
+    return plan_band(MASK_LOCAL, int(sink), left, right, BH, S, device)
+
+
+def _is_profiling(mask_mode: int) -> bool:
+    """The SVG1 profiling masks (modes 4-9): band plans the forward runs and the backward does not."""
+    return MASK_PROF_HY_S <= mask_mode <= MASK_PROF_COG_T
 
 
 # ----------------------------------------------------------------------------------------------
@@ -329,7 +350,7 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
              out: Optional[tuple] = None):
     """Gradients (dq, dk, dv) of o = attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale) for the output gradient
-    do; lse is the forward's return_lse output.  Variable-block and band plans (mask NONE / HY / WAN / COG); the plan's
+    do; lse is the forward's return_lse output.  Variable-block and band plans (mask NONE / HY / WAN / COG / LOCAL); the plan's
     key-major companion is built on the first call (AttnPlan.key_major).  Deterministic: two calls give the same bits.
     k, v may have another sequence length than q under a rectangular variable-block plan, and fewer heads (grouped-query
     attention, as attn_fwd); dk, dv then have k's shape, a group's dk and dv summing over its query heads.
@@ -420,7 +441,7 @@ def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Option
     LSE, and the plan is not read here."""
     if not needs_grad(q, k, v):
         return attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale)
-    if plan.desc.kind == PLAN_GATHER or (plan.desc.kind == PLAN_BAND and plan.desc.mask_mode > MASK_COG):
+    if plan.desc.kind == PLAN_GATHER or (plan.desc.kind == PLAN_BAND and _is_profiling(plan.desc.mask_mode)):
         plan.key_major()  # raises, naming what has no backward
     return _Attention.apply(q, k, v, plan, layout, sm_scale)
 
