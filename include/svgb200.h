@@ -62,6 +62,8 @@ int svgb_device_check(int* sm_major, int* sm_minor, int* num_sms);
 #define SVGB_PLAN_BAND 2     /* element-exact band mask (svgb_attn_plan_band) */
 #define SVGB_PLAN_GATHER 3   /* variable-block map, row gather (svgb_attn_plan_varblock_gather) */
 #define SVGB_PLAN_BAND_T 4   /* key-major band plan of the backward pass (svgb_attn_plan_band_t) */
+#define SVGB_PLAN_SEG 5      /* local mask inside packed variable-length segments (svgb_attn_plan_local_varlen) */
+#define SVGB_PLAN_SEG_T 6    /* its key-major companion for the backward (svgb_attn_plan_local_varlen_t) */
 typedef struct svgb_plan {
   int32_t kind;          /* SVGB_PLAN_* */
   int32_t BH, S;
@@ -75,7 +77,11 @@ typedef struct svgb_plan {
  * set items_stride = 0 in the host struct. */
 /* S is the query length.  A variable-block plan has no element mask (mask_mode = SVGB_MASK_NONE), and its m0 holds the
  * key/value length Skv when svgb_attn_plan_varblock_kv built it; m0 = 0 (every other planner) means Skv = S.  The
- * attention entries reject a plan whose lengths differ from the call's. */
+ * attention entries reject a plan whose lengths differ from the call's.  A segment plan (SVGB_PLAN_SEG / _SEG_T) serves
+ * every head (items_stride = 0), so its BH holds its key/value length instead (key-major: the query length); its
+ * segment count and its copy of the bounds are in its workspace, int32 {nseg, cu_q[0..nseg], cu_k[0..nseg]} at byte
+ * SVGB_PLAN_SEG_BOUNDS_OFF. */
+#define SVGB_PLAN_SEG_BOUNDS_OFF 16
 
 /* SVG2 / BSR / dense: q-block i of head h attends k-block j iff map[h,i,j] != 0.
  * Stands behind dynamic_block_sparse_fwd_flashinfer's wrapper.plan (svg/kmeans_utils.py:1355-1385).
@@ -119,6 +125,39 @@ int svgb_attn_plan_band_t_bytes(int S, size_t* bytes);
 int svgb_attn_plan_band_t(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
                           size_t ws_bytes, svgb_plan* plan, void* stream);
 
+/* Local mask inside packed variable-length segments (FlashAttention's flash_attn_varlen_func with causal= /
+ * window_size=), one plan shared by every head.  cu_q, cu_k: device int32 [nseg + 1], query segment i = rows
+ * [cu_q[i], cu_q[i+1]) of length Lq_i, key segment i = keys [cu_k[i], cu_k[i+1]) of length Lk_i.  With qi, kj the
+ * positions inside segment i and off_i = Lk_i - Lq_i (bottom-right alignment):
+ *   allowed(q, kv) = same segment & (kj < sink | ((qi + off_i) - kj <= left & kj - (qi + off_i) <= right))
+ * sink, left, right >= 0 (a negative one is an error); causal is right = 0.  With nseg = 1 and Sq == Skv this is
+ * SVGB_MASK_LOCAL(sink, left, right) and the results are svgb_attn_plan_band's, bit for bit.  A row without an allowed
+ * key gets o = 0, lse = -inf, dq = 0; a key no row reaches dk = dv = 0.  Empty segments are legal.
+ * The planner copies the bounds into the workspace (the plan owns them) and reads nothing on the host: the item count
+ * stays on the device, plan->max_items is a host bound.  The first bound is taken as 0 and the last as Sq (Skv), the
+ * others are clamped to [0, Sq] ([0, Skv]) and made monotone (running maximum), so bounds out of range or out of order
+ * give an unspecified result that stays inside the tensors.  No stream straddles a query segment and no chunk a key
+ * segment (chunks start at cu_k[i] + 128 j); each chunk is FULL, ELEM or omitted, classified from the band's interval
+ * form.  Items are issued in row order (segments in turn).
+ * plan->kind = SVGB_PLAN_SEG, mask_mode = SVGB_MASK_LOCAL, m0..m2 = sink, left, right, S = Sq, BH = Skv.  Runs
+ * with svgb_attn_fwd (Sq == Skv), _kv, _gqa and _strided, 16-bit inputs only (no e4m3, gather plans or row vectors).
+ * Workspace (one size for the plan and its key-major companion; integer division, n = nseg):
+ *   I = max over R in {Sq, Skv} of min(R, (R + 510 n) / 256)            items (at most one partial item per segment,
+ *                                                                       key-major two)
+ *   C = min(I * ceil(max(Sq, Skv) / 128), (Sq Skv + 510 (Sq + Skv) + 64770 n) / 32768)    chunk slots
+ *   bytes = 16 + align16(4 (2 n + 3)) + align16(8 (n + 1)) + 32 I + 8 C
+ * which depends on nseg, Sq and Skv only; at n = 1 and Sq == Skv == S it never exceeds svgb_attn_plan_band_bytes(S).
+ * Sq, Skv > 0. */
+int svgb_attn_plan_local_varlen_bytes(int nseg, int Sq, int Skv, size_t* bytes);
+int svgb_attn_plan_local_varlen(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink, int left,
+                                int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
+/* Key-major companion for svgb_attn_bwd*: items are key ranges of one key segment (the sink keys of a segment form
+ * items of their own), chunks the query ranges of that segment that reach them.  Same arguments and workspace size;
+ * plan->kind = SVGB_PLAN_SEG_T, S = Skv, BH = Sq.  The backward checks that plan and plan_t have swapped lengths, the
+ * same parameters and the same workspace layout (which is a function of nseg, Sq and Skv). */
+int svgb_attn_plan_local_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                  int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
+
 /* ---- attention -------------------------------------------------------------------------- */
 /* o = softmax(q k^T * sm_scale  [masked by plan]) v, per head.  Stands behind
  * dynamic_block_sparse_fwd_flashinfer (svg/kmeans_utils.py:1319-1392), flex_attention under the
@@ -153,7 +192,8 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
  *   q     : [BH, Sq, D] at q_row_stride / q_head_stride;  k, v : [BH, Skv, D] at kv_row_stride / kv_head_stride;
  *   o     : [BH, Sq, D] at its own strides;  lse : optional float [BH, Sq].
  *   plan  : SVGB_PLAN_VARBLOCK built for (Sq, Skv) -- svgb_attn_plan_varblock_kv, or svgb_attn_plan_varblock when
- *           Sq == Skv.  16-bit inputs only (SVGB_BF16 / SVGB_F16), D in {64,128}; alignment as svgb_attn_fwd.
+ *           Sq == Skv -- or SVGB_PLAN_SEG (svgb_attn_plan_local_varlen).  16-bit inputs only (SVGB_BF16 / SVGB_F16),
+ *           D in {64,128}; alignment as svgb_attn_fwd.
  * Same kernel as svgb_attn_fwd: a key chunk past Skv is cut by its valid count and TMA fills rows past Skv with zeros.
  * Band, gather and profiling plans, row-index vectors and e4m3 inputs need Sq == Skv and svgb_attn_fwd.  With
  * Sq == Skv and equal strides the result is svgb_attn_fwd's, bit for bit. */
@@ -168,7 +208,7 @@ int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float
  *           element b is h = b * Hq + hq and reads head b * Hkv + hq / G).
  *   plan  : SVGB_PLAN_VARBLOCK built over the BHkv key/value heads (map [BHkv, QC, KC]; plan->BH = BHkv), shared by the
  *           G query heads of a group, rectangular (Sq != Skv) or not; or SVGB_PLAN_BAND (one work list for every head,
- *           Sq == Skv).
+ *           Sq == Skv); or SVGB_PLAN_SEG (one work list for every head).
  * 16-bit inputs, D in {64,128}, alignment as svgb_attn_fwd; no gather plans, row vectors or e4m3 inputs.  The kernel
  * is svgb_attn_fwd's, so each output row is bit for bit the one of svgb_attn_fwd / _kv on K / V repeated G times per
  * head under the map repeated per query head. */
@@ -183,8 +223,8 @@ int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, floa
  *   x_strides : {batch, head, row} element strides of tensor x (the last dimension is contiguous), each a nonzero
  *           multiple of 8; bases 16-byte aligned.  Element (b, h, s, d) of x is at x + b*st[0] + h*st[1] + s*st[2] + d.
  *   Hq = G * Hkv: query head hq of batch element b attends with key/value head hq / G of b.
- *   plan  : SVGB_PLAN_VARBLOCK built over the B * Hkv key/value heads (flat head b * Hkv + hkv; rectangular or not), or
- *           SVGB_PLAN_BAND (Sq == Skv).
+ *   plan  : SVGB_PLAN_VARBLOCK built over the B * Hkv key/value heads (flat head b * Hkv + hkv; rectangular or not),
+ *           SVGB_PLAN_BAND (Sq == Skv) or SVGB_PLAN_SEG (every batch element segmented alike).
  * 16-bit inputs, D in {64,128}; no gather plans, row vectors or e4m3 inputs.  The TMA maps are 4-D (d, row, head,
  * batch) and o is stored at its own strides (only the view's elements are written); each output row is bit for bit
  * the one svgb_attn_fwd_gqa (svgb_attn_fwd / _kv when Hq == Hkv) gives on contiguous copies.  svgb_attn_fwd, _kv and
@@ -200,8 +240,10 @@ int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH,
  *           row_stride / head_stride pair (elements; 16-byte aligned bases, strides multiples of 8 elements).
  *   lse   : float [BH,S] written by svgb_attn_fwd under the same plan and sm_scale.
  *   plan  : the forward (query-major) plan, SVGB_PLAN_VARBLOCK or SVGB_PLAN_BAND with mask SVGB_MASK_NONE / HY / WAN /
- *           COG / LOCAL (not the profiling masks 4-9).  plan_t: its key-major companion -- svgb_attn_plan_band_t with the same mask for a band plan,
- *           svgb_attn_plan_varblock(map^T, col_sz, row_sz) for a variable-block plan.
+ *           COG / LOCAL (not the profiling masks 4-9), or SVGB_PLAN_SEG.  plan_t: its key-major companion --
+ *           svgb_attn_plan_band_t with the same mask for a band plan, svgb_attn_plan_varblock(map^T, col_sz, row_sz)
+ *           for a variable-block plan, svgb_attn_plan_local_varlen_t with the same bounds and parameters for a segment
+ *           plan.
  *   ws    : device scratch of svgb_attn_bwd_bytes (per-row delta = rowsum(dO * O)).
  * Every row of dq, dk, dv is written (rows without an allowed key: dq = 0; keys no row reaches: dk = dv = 0); the
  * result is deterministic (no atomics).  Gather plans, row gathers and e4m3 inputs have no backward. */
@@ -214,7 +256,8 @@ int svgb_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
 /* Backward of svgb_attn_fwd_kv: q, o, dO, dq [BH, Sq, D] at the q strides; k, v, dk, dv [BH, Skv, D] at the k/v
  * strides; lse float [BH, Sq].  plan: the forward's SVGB_PLAN_VARBLOCK plan for (Sq, Skv); plan_t: its key-major
  * companion svgb_attn_plan_varblock_kv(map^T, col_sz, row_sz, Skv, Sq) (svgb_attn_plan_varblock(map^T, ...) when
- * Sq == Skv).  ws: device scratch of svgb_attn_bwd_kv_bytes (the delta over Sq rows).  The dQ launch walks plan with
+ * Sq == Skv), or a segment plan and its svgb_attn_plan_local_varlen_t.  ws: device scratch of svgb_attn_bwd_kv_bytes
+ * (the delta over Sq rows).  The dQ launch walks plan with
  * K / V over Skv rows; the dK / dV launch walks plan_t with K / V as its rows and Q / dO (Sq rows) as its chunks.
  * Guarantees as svgb_attn_bwd: every gradient row written, no atomics, deterministic; with Sq == Skv and equal
  * strides the gradients are svgb_attn_bwd's, bit for bit.  Variable-block plans and 16-bit inputs only. */

@@ -35,6 +35,8 @@ static AttnBwdArgs bwd_args(const svgb_plan* p, const void* ws) {
   a.m0 = p->m0;
   a.m1 = p->m1;
   a.m2 = p->m2;
+  if (p->kind == SVGB_PLAN_SEG || p->kind == SVGB_PLAN_SEG_T)
+    a.segs = reinterpret_cast<const int*>(w + SVGB_PLAN_SEG_BOUNDS_OFF);
   return a;
 }
 
@@ -52,18 +54,26 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
                "attention backward takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no backward)", dtype);
   SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND,
-               "attention backward needs a variable-block or band plan (kind %d; gather plans have no backward)",
-               plan->kind);
-  SVGB_REQUIRE(plan_t->kind == (plan->kind == SVGB_PLAN_BAND ? SVGB_PLAN_BAND_T : SVGB_PLAN_VARBLOCK),
-               "plan_t (kind %d) is not the key-major companion of a kind-%d plan", plan_t->kind, plan->kind);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_SEG,
+               "attention backward needs a variable-block, band or segment plan (kind %d; gather plans have no "
+               "backward, key-major plans go in plan_t)", plan->kind);
+  const int kind_t = plan->kind == SVGB_PLAN_BAND  ? SVGB_PLAN_BAND_T
+                     : plan->kind == SVGB_PLAN_SEG ? SVGB_PLAN_SEG_T
+                                                   : SVGB_PLAN_VARBLOCK;
+  SVGB_REQUIRE(plan_t->kind == kind_t, "plan_t (kind %d) is not the key-major companion of a kind-%d plan",
+               plan_t->kind, plan->kind);
   SVGB_REQUIRE((plan->mask_mode >= MASK_NONE && plan->mask_mode <= MASK_COG) || plan->mask_mode == MASK_LOCAL,
                "attention backward supports the executed band masks NONE / HY / WAN / COG / LOCAL (mask mode %d)",
                plan->mask_mode);
   // a variable-block plan's m0 is its Skv (svgb200.h), checked with the lengths below
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || (plan_t->mask_mode == plan->mask_mode && plan_t->m0 == plan->m0 &&
-                                                plan_t->m1 == plan->m1 && plan_t->m2 == plan->m2),
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK ||
+                   (plan_t->mask_mode == plan->mask_mode && plan_t->m0 == plan->m0 && plan_t->m1 == plan->m1 &&
+                    plan_t->m2 == plan->m2),
                "plan_t was built for another mask than plan");
+  // a segment plan's layout is a function of (nseg, Sq, Skv), so equal layouts mean equal segment counts
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG || (plan_t->items_off == plan->items_off &&
+                                               plan_t->chunks_off == plan->chunks_off && plan_t->bytes == plan->bytes),
+               "plan_t was built for another segmentation than plan (nseg, Sq or Skv)");
   // the key-major plan has the keys as rows: its S is Skv and its Skv is Sq
   // both plans are per key/value head
   const int BHkv = BH / kv_group;
@@ -156,9 +166,9 @@ int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o,
                      const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws,
                      void* ws, size_t ws_bytes, void* stream) {
   SVGB_REQUIRE(plan, "null pointer");
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK,
-               "svgb_attn_bwd_kv takes variable-block plans only (kind %d; band plans need Sq == Skv, svgb_attn_bwd)",
-               plan->kind);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_SEG,
+               "svgb_attn_bwd_kv takes segment plans and variable-block plans only (kind %d; band plans need "
+               "Sq == Skv, svgb_attn_bwd)", plan->kind);
   const Strides x = flat_strides(q_row_stride, q_head_stride, BH), y = flat_strides(kv_row_stride, kv_head_stride, BH);
   return attn_bwd_run(q, k, v, o, dout, lse, dq, dk, dv, dtype, 1, BH, 1, Sq, Skv, D, x, y, y, x, x, x, y, y, sm_scale,
                       plan, plan_ws, plan_t, plan_t_ws, ws, ws_bytes, stream);

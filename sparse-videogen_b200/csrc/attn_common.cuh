@@ -119,6 +119,57 @@ __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, in
   }
 }
 
+// Packed variable-length segments (SVGB_PLAN_SEG / SVGB_PLAN_SEG_T).  The plan keeps its own copy of the bounds at byte
+// SVGB_PLAN_SEG_BOUNDS_OFF of its workspace, seg = {nseg, cq_0 .. cq_nseg, ck_0 .. ck_nseg}: query segment i is rows
+// [cq_i, cq_i+1), key segment i keys [ck_i, ck_i+1).
+// Every stream lies in one segment, so the local mask of segment i is MASK_LOCAL(sink, left, right) with two per-stream
+// constants: query positions shifted by delta_i = cq_i+1 - ck_i+1 (query qi of the segment sits at key position
+// ck_i + qi + Lk_i - Lq_i, FlashAttention's bottom-right alignment) and the sink bound ck_i + sink in place of m0.
+// The same segment is implicit: a stream's chunks are keys (key-major: queries) of its own segment only.
+struct SegOrigin {
+  int shift;     // subtract from a query position
+  int sink_end;  // m0 of the stream: keys below it are sinks
+};
+// origin of the stream whose first row is `row`: a query row (key_major = false) or a key row (true).  Its segment is
+// the last one that starts at or before it, so empty segments are skipped.
+__host__ __device__ inline SegOrigin seg_origin(const int* seg, int row, bool key_major, int sink) {
+  const int nseg = seg[0];
+  const int* segs = seg + 1;
+  const int* b = segs + (key_major ? nseg + 1 : 0);
+  int lo = 0, hi = nseg - 1;  // largest i < nseg with b[i] <= row
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (b[mid] <= row) lo = mid;
+    else hi = mid - 1;
+  }
+  const int* ck = segs + nseg + 1;
+  SegOrigin o;
+  o.shift = segs[lo + 1] - ck[lo + 1];
+  o.sink_end = ck[lo] + sink;
+  return o;
+}
+
+// Kind of a chunk of a segment plan, from the mask's interval form: 0 = omitted (no allowed pair), 1 = FULL (every pair
+// allowed), 2 = ELEM.  Query-major: rows r0..r1 are queries at positions p = q - shift, columns c0..c1 keys.  Key-major:
+// rows are keys, columns queries.  Pairs (p, kv) are allowed when kv < sink_end or p - left <= kv <= p + right; every
+// key of the chunk and of the item lies in the segment (kv >= sink_end - sink).  64-bit: left / right may be large.
+__host__ __device__ inline int seg_chunk_kind(bool key_major, int r0, int r1, int c0, int c1, SegOrigin o, int left,
+                                              int right) {
+  const long long L = left, R = right;
+  if (!key_major) {
+    const long long p0 = static_cast<long long>(r0) - o.shift, p1 = static_cast<long long>(r1) - o.shift;
+    const bool any = c0 < o.sink_end || (c0 <= p1 + R && c1 >= p0 - L);
+    const long long k = c0 > o.sink_end ? c0 : o.sink_end;  // first key past the sinks
+    const bool all = k > c1 || (k >= p1 - L && c1 <= p0 + R);
+    return any ? (all ? 1 : 2) : 0;
+  }
+  // key kv is reached by positions kv - right .. kv + left, i.e. queries kv + shift - right .. kv + shift + left
+  const long long k0 = r0 > o.sink_end ? r0 : o.sink_end;  // first key of the item past the sinks
+  const bool any = r0 < o.sink_end || (c0 <= r1 + o.shift + L && c1 >= r0 + o.shift - R);
+  const bool all = k0 > r1 || (c0 >= r1 + o.shift - R && c1 <= k0 + o.shift + L);
+  return any ? (all ? 1 : 2) : 0;
+}
+
 // Element masks inside the attention kernel.  A thread holds the scores of two query rows at positions q[0], q[1]
 // and key columns kvb + 8*jj + v0 (jj < 16, v0 < 2; kvb = chunk start + 2*(lane % 4)), the wgmma accumulator
 // layout.  ElemMask::bits returns them as two 32-bit masks: bit 2*jj + v0 of keep[v1] <=> mask_allowed(mode, q[v1],
@@ -277,6 +328,8 @@ struct AttnArgs {
   int S = 0;                    // query rows per head (indexing of o_rows / lse / q_index)
   int mask_mode = 0, m0 = 0, m1 = 0, m2 = 0;
   const int* q_index = nullptr;  // optional [S]: query position used by the element mask (sampled rows)
+  // segment plans: the plan's copy of the bounds {nseg, cq[0..nseg], ck[0..nseg]} (seg_origin); nullptr otherwise
+  const int* segs = nullptr;
   int out_f32 = 0;               // 1: o is fp32 (used for split-KV partials)
   // FP8 (e4m3) inputs: per-head dequantisation scales [BH]; s_q * s_k multiplies the logits, s_v the
   // output.  NULL for 16-bit inputs.

@@ -1,5 +1,7 @@
 // Attention plans (device-built work lists), the attention launcher, density, and the tile
 // self-test.  See attn_kernel.cuh for the kernel itself.
+#include <algorithm>
+
 #include "../../include/svgb200.h"
 #include "attn_kernel.cuh"
 #include "host_common.h"
@@ -286,6 +288,127 @@ static int band_total_items(const BandSegs& sg) {
 }
 
 // =============================================================================================
+// Plan: local mask inside packed variable-length segments (svgb_attn_plan_local_varlen[_t]).  Count, scan and fill:
+//   seg_bounds_kernel  one CTA: the plan's copy of the bounds (clamped, monotone), per segment its items and chunk
+//                      slots, their exclusive scans and the item count
+//   seg_lists_kernel   one warp per item: its rows, and its chunk list, classified from the band's interval form
+//                      (seg_chunk_kind) and compacted with a ballot, and its two stream descriptors
+// Items launch in row order (segments in turn, first rows first).  Longest-list-first (LPT) was measured against it
+// (tools/varlen_local_perf.py --order) and came within 1 % either way: the grid walks every head's items before the next
+// head's, so many heads make many waves and only the last head's tail could gain.
+// Item rows are cut in 256 from the start of their segment; key-major, the sink keys of a segment are items of their
+// own.  An item's list has one slot per chunk of its segment, so the chunk storage is the sum over segments of
+// items x chunks (svgb_attn_plan_local_varlen_bytes bounds it).
+// =============================================================================================
+constexpr int kSegThreads = 1024;
+
+// in-place scan of a[0..n) by one CTA of kSegThreads threads, inclusive running maximum (kMax) or exclusive sum:
+// contiguous slices per thread, a warp scan of the slice totals, a serial pass over the 32 warp totals
+template <bool kMax>
+__device__ void seg_block_scan(int* a, int n, int* wtot) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int per = (n + kSegThreads - 1) / kSegThreads;
+  const int j0 = min(n, static_cast<int>(threadIdx.x) * per), j1 = min(n, j0 + per);
+  auto op = [](int x, int y) { return kMax ? max(x, y) : x + y; };
+  const int id = kMax ? INT_MIN : 0;
+  int acc = id;
+  for (int j = j0; j < j1; ++j) acc = op(acc, a[j]);
+  int incl = acc;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int x = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl = op(incl, x);
+  }
+  if (lane == 31) wtot[warp] = incl;
+  __syncthreads();
+  int run = id;
+  for (int w = 0; w < warp; ++w) run = op(run, wtot[w]);
+  const int lane_prev = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane > 0) run = op(run, lane_prev);
+  for (int j = j0; j < j1; ++j) {
+    const int x = a[j];
+    a[j] = kMax ? op(run, x) : run;
+    run = op(run, x);
+  }
+  __syncthreads();
+}
+
+// seg: {nseg, cq[0..nseg], ck[0..nseg]}; base: {item base [nseg + 1], chunk base [nseg + 1]} (exclusive scans, last =
+// total)
+__global__ void __launch_bounds__(kSegThreads)
+seg_bounds_kernel(const int* __restrict__ cu_q, const int* __restrict__ cu_k, int nseg, int Sq, int Skv, int sink,
+                  int transposed, int* __restrict__ seg, int* __restrict__ base, int* __restrict__ counts) {
+  __shared__ int wtot[32];
+  if (threadIdx.x == 0) seg[0] = nseg;
+  int* segs = seg + 1;
+  for (int i = threadIdx.x; i <= nseg; i += kSegThreads) {
+    segs[i] = i == 0 ? 0 : i == nseg ? Sq : min(max(cu_q[i], 0), Sq);
+    segs[nseg + 1 + i] = i == 0 ? 0 : i == nseg ? Skv : min(max(cu_k[i], 0), Skv);
+  }
+  __syncthreads();
+  seg_block_scan<true>(segs, nseg + 1, wtot);
+  seg_block_scan<true>(segs + nseg + 1, nseg + 1, wtot);
+  int* ib = base;
+  int* cb = base + nseg + 1;
+  const int* rb = segs + (transposed ? nseg + 1 : 0);  // rows of the items: queries, or keys (key-major)
+  const int* colb = segs + (transposed ? 0 : nseg + 1);
+  for (int i = threadIdx.x; i <= nseg; i += kSegThreads) {
+    int items = 0, per = 0;
+    if (i < nseg) {
+      const int rows = rb[i + 1] - rb[i], cols = colb[i + 1] - colb[i];
+      const int s = transposed ? min(sink, rows) : 0;
+      items = (s + kItemRows - 1) / kItemRows + (rows - s + kItemRows - 1) / kItemRows;
+      per = (cols + kChunkCols - 1) / kChunkCols;
+    }
+    ib[i] = items;
+    cb[i] = items * per;
+  }
+  __syncthreads();
+  seg_block_scan<false>(ib, nseg + 1, wtot);  // entry nseg is 0, so it receives the total
+  seg_block_scan<false>(cb, nseg + 1, wtot);
+  if (threadIdx.x == 0) counts[0] = ib[nseg];
+}
+
+// One warp per item it < counts[0]: its chunk list and its two stream descriptors, items[2 it], items[2 it + 1].
+__global__ void __launch_bounds__(256)
+seg_lists_kernel(const int* __restrict__ seg, const int* __restrict__ base, const int* __restrict__ counts, int nseg,
+                 int sink, int left, int right, int transposed, int2* __restrict__ chunks, int4* __restrict__ items) {
+  const int* segs = seg + 1;
+  const int lane = threadIdx.x & 31;
+  const int it = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (it >= counts[0]) return;
+  const int* ib = base;
+  const int* cb = base + nseg + 1;
+  int si = 0, hi = nseg - 1;  // the last segment whose first item is at or before `it` (empty ones have no items)
+  while (si < hi) {
+    const int mid = (si + hi + 1) >> 1;
+    if (ib[mid] <= it) si = mid;
+    else hi = mid - 1;
+  }
+  const int k = it - ib[si];
+  const int* rb = segs + (transposed ? nseg + 1 : 0);
+  const int* colb = segs + (transposed ? 0 : nseg + 1);
+  const int rs = rb[si], re = rb[si + 1], cs = colb[si], ce = colb[si + 1];
+  const int s = transposed ? min(sink, re - rs) : 0;  // key-major: the sink keys end an item run of their own
+  const int ns = (s + kItemRows - 1) / kItemRows;
+  const int r0 = k < ns ? rs + k * kItemRows : rs + s + (k - ns) * kItemRows;
+  const int nr = min(kItemRows, (k < ns ? rs + s : re) - r0);
+  const int per = (ce - cs + kChunkCols - 1) / kChunkCols;
+  const int list = cb[si] + k * per;
+  const SegOrigin o = seg_origin(seg, r0, transposed != 0, sink);
+  int n = 0;
+  for (int j0 = 0; j0 < per; j0 += 32) {
+    const int j = j0 + lane;
+    const int c0 = cs + j * kChunkCols, valid = min(kChunkCols, ce - c0);
+    const int kind = j < per ? seg_chunk_kind(transposed != 0, r0, r0 + nr - 1, c0, c0 + valid - 1, o, left, right) : 0;
+    const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
+    if (kind != 0) chunks[list + n + __popc(m & ((1u << lane) - 1u))] = make_int2(c0, chunk_meta(valid, kind == 2));
+    n += __popc(m);
+  }
+  if (lane == 0) put_item(items + 2 * it, r0, nr, list, n);
+}
+
+// =============================================================================================
 // density_calculation (svg/kmeans_utils.py:13-31)
 // =============================================================================================
 __global__ void density_kernel(const uint8_t* __restrict__ map, const int* __restrict__ row_sz,
@@ -485,6 +608,79 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
   return 0;
 }
 
+// Workspace of a segment plan (one layout for both directions), 16-byte aligned pieces:
+//   counts (16 B) | bounds {nseg, 2 (nseg + 1)} | bases 2 (nseg + 1) | items 2 int4 [items] | chunks [C]
+// items: every segment adds at most one partial item (key-major two: its sink keys end an item), so
+//   I = min(R, (R + 510 nseg) / 256) for R = Sq (query-major) and Skv (key-major) covers both.
+// chunks: sum over segments of items x ceil(cols / 128) <= sum (rows + 510)(cols + 127) / 32768 with sum rows x cols <=
+//   Sq Skv, and never more than I x ceil(max(Sq, Skv) / 128).
+struct SegLayout {
+  int max_items;
+  long long max_chunks;
+  size_t segs_off, base_off, items_off, chunks_off, bytes;
+};
+static SegLayout seg_layout(int nseg, int Sq, int Skv) {
+  SegLayout L;
+  const long long n = nseg, q = Sq, k = Skv, mx = q > k ? q : k;
+  const long long iq = std::min(q, (q + 510 * n) / 256), ik = std::min(k, (k + 510 * n) / 256);
+  const long long items = std::max(iq, ik);
+  const long long sum_bound = (q * k + 510 * (q + k) + 510 * 127 * n) / 32768;
+  L.max_items = static_cast<int>(std::min<long long>(items, INT_MAX));
+  L.max_chunks = std::min(items * ((mx + kChunkCols - 1) / kChunkCols), sum_bound);
+  L.segs_off = SVGB_PLAN_SEG_BOUNDS_OFF;
+  L.base_off = L.segs_off + align_up(sizeof(int) * (2 * n + 3), 16);
+  L.items_off = L.base_off + align_up(sizeof(int) * 2 * (n + 1), 16);
+  L.chunks_off = L.items_off + 2 * sizeof(int4) * items;
+  L.bytes = L.chunks_off + sizeof(int2) * L.max_chunks;
+  return L;
+}
+
+static int plan_local_varlen_bytes(int nseg, int Sq, int Skv, size_t* bytes) {
+  SVGB_REQUIRE(nseg > 0 && Sq > 0 && Skv > 0 && bytes, "bad arguments (nseg=%d, Sq=%d, Skv=%d)", nseg, Sq, Skv);
+  *bytes = seg_layout(nseg, Sq, Skv).bytes;
+  return 0;
+}
+
+static int plan_local_varlen_impl(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                  int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
+                                  bool transposed) {
+  size_t need = 0;
+  if (plan_local_varlen_bytes(nseg, Sq, Skv, &need)) return -1;
+  SVGB_REQUIRE(cu_q && cu_k && plan_ws && plan, "null pointer");
+  SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
+  SVGB_REQUIRE(sink >= 0 && left >= 0 && right >= 0,
+               "local varlen mask: sink (%d), left (%d) and right (%d) must be >= 0", sink, left, right);
+  const SegLayout L = seg_layout(nseg, Sq, Skv);
+  SVGB_REQUIRE(L.max_chunks < (1ll << 31) && nseg < (1 << 29), "plan too large for 32-bit chunk offsets");
+  const int rows = transposed ? Skv : Sq, cols = transposed ? Sq : Skv;
+  const int max_items = static_cast<int>(std::min<long long>(rows, (rows + 510ll * nseg) / 256));
+  plan->kind = transposed ? SVGB_PLAN_SEG_T : SVGB_PLAN_SEG;
+  plan->BH = cols;  // a segment plan serves every head: BH holds its key/value length (svgb200.h)
+  plan->S = rows;
+  plan->max_items = max_items;
+  plan->items_stride = 0;
+  plan->mask_mode = MASK_LOCAL;
+  plan->m0 = sink;
+  plan->m1 = left;
+  plan->m2 = right;
+  plan->counts_off = 0;
+  plan->items_off = static_cast<int64_t>(L.items_off);
+  plan->chunks_off = static_cast<int64_t>(L.chunks_off);
+  plan->bytes = static_cast<int64_t>(need);
+  char* ws = static_cast<char*>(plan_ws);
+  int* counts = reinterpret_cast<int*>(ws);
+  int* segs = reinterpret_cast<int*>(ws + L.segs_off);
+  int* base = reinterpret_cast<int*>(ws + L.base_off);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  seg_bounds_kernel<<<1, kSegThreads, 0, st>>>(cu_q, cu_k, nseg, Sq, Skv, sink, transposed ? 1 : 0, segs, base, counts);
+  SVGB_LAUNCH_OK();
+  seg_lists_kernel<<<(max_items + 7) / 8, 256, 0, st>>>(segs, base, counts, nseg, sink, left, right, transposed ? 1 : 0,
+                                                        reinterpret_cast<int2*>(ws + L.chunks_off),
+                                                        reinterpret_cast<int4*>(ws + L.items_off));
+  SVGB_LAUNCH_OK();
+  return 0;
+}
+
 // Every forward entry: q / o over Sq rows and BH heads in B batch elements, k / v over Skv rows and BH / kv_group
 // heads, each tensor with its own strides.
 static int attn_fwd_run(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
@@ -499,6 +695,13 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
                "per-head scale vectors are for e4m3 inputs only (dtype %d)", dtype);
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND_T,
                "a key-major band plan (svgb_attn_plan_band_t) is for svgb_attn_bwd; the forward takes svgb_attn_plan_band");
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG_T,
+               "a key-major segment plan (svgb_attn_plan_local_varlen_t) is for the backward; the forward takes "
+               "svgb_attn_plan_local_varlen");
+  const bool seg = plan->kind == SVGB_PLAN_SEG;
+  SVGB_REQUIRE(!seg || dtype != SVGB_E4M3, "segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs, not e4m3");
+  SVGB_REQUIRE(!seg || (!q_rows && !kv_rows && !o_rows),
+               "segment plans (svgb_attn_plan_local_varlen) take no row vectors (q_rows / kv_rows / o_rows)");
   const bool gather = plan->kind == SVGB_PLAN_GATHER;
   SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
                "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");
@@ -522,12 +725,13 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.lse = lse;
   a.scale_log2 = sm_scale * 1.4426950408889634f;
   a.S = Sq;
-  if (plan->kind == SVGB_PLAN_BAND) {  // a variable-block plan's m0 is its Skv, not a mask parameter
+  if (plan->kind == SVGB_PLAN_BAND || seg) {  // a variable-block plan's m0 is its Skv, not a mask parameter
     a.mask_mode = plan->mask_mode;
     a.m0 = plan->m0;
     a.m1 = plan->m1;
     a.m2 = plan->m2;
   }
+  if (seg) a.segs = reinterpret_cast<const int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF);
   a.q_scale = q_scale;
   a.k_scale = k_scale;
   a.v_scale = v_scale;
@@ -630,6 +834,20 @@ int svgb_attn_plan_band_t(int mask_mode, int m0, int m1, int m2, int BH, int S, 
   return plan_band_impl(mask_mode, m0, m1, m2, BH, S, plan_ws, ws_bytes, plan, stream, true);
 }
 
+int svgb_attn_plan_local_varlen_bytes(int nseg, int Sq, int Skv, size_t* bytes) {
+  return plan_local_varlen_bytes(nseg, Sq, Skv, bytes);
+}
+
+int svgb_attn_plan_local_varlen(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink, int left,
+                                int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
+  return plan_local_varlen_impl(cu_q, cu_k, nseg, Sq, Skv, sink, left, right, plan_ws, ws_bytes, plan, stream, false);
+}
+
+int svgb_attn_plan_local_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                  int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
+  return plan_local_varlen_impl(cu_q, cu_k, nseg, Sq, Skv, sink, left, right, plan_ws, ws_bytes, plan, stream, true);
+}
+
 int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
                   const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
@@ -648,9 +866,9 @@ int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
                "svgb_attn_fwd_kv takes bf16 or fp16 inputs (dtype %d; e4m3 attention needs Sq == Skv, svgb_attn_fwd)",
                dtype);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK,
-               "svgb_attn_fwd_kv takes variable-block plans only (kind %d; band, gather and profiling plans need "
-               "Sq == Skv, svgb_attn_fwd)", plan->kind);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_SEG,
+               "svgb_attn_fwd_kv takes segment plans and variable-block plans only (kind %d; band, gather and "
+               "profiling plans need Sq == Skv, svgb_attn_fwd)", plan->kind);
   SVGB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
                    kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,

@@ -382,13 +382,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     const int rloc = 64 * cw + 16 * wq + (lane >> 2);
     ElemMask em;
     if constexpr (!kGather) {  // gather plans carry no element masks
+      // segment plans: the stream's segment shifts the query positions and moves the sink bound (seg_origin)
+      SegOrigin so{0, m0};
+      if (args.segs) so = seg_origin(args.segs, q0, false, m0);
       int qm[2];
 #pragma unroll
       for (int v1 = 0; v1 < 2; ++v1) {
         const int q = q0 + rloc + 8 * v1;
-        qm[v1] = (args.q_index && q < args.S) ? __ldg(&args.q_index[q]) : q;  // position seen by the mask
+        qm[v1] = ((args.q_index && q < args.S) ? __ldg(&args.q_index[q]) : q) - so.shift;  // position seen by the mask
       }
-      em.init(mode, qm, m0, m1, m2);
+      em.init(mode, qm, so.sink_end, m1, m2);
     }
     float o[D / 2];
 #pragma unroll

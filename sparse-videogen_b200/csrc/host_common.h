@@ -63,22 +63,25 @@ inline Strides flat_strides(long long rs, long long hs, int BH) { return {BH * h
 // box = one 128-byte panel x 128 rows x 1 x 1, 128-byte swizzle.  Returns 0 on success.
 int encode_tmap_bhsd(CUtensorMap* map, const void* base, int dtype, int B, int H, int S, int D, Strides st);
 
-// key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0 (svgb200.h);
-// every other plan has Skv = S
-inline int plan_kv_len(const svgb_plan* p) { return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S; }
+// key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
+// BH (svgb200.h); every other plan has Skv = S
+inline int plan_kv_len(const svgb_plan* p) {
+  if (p->kind == SVGB_PLAN_SEG || p->kind == SVGB_PLAN_SEG_T) return p->BH;
+  return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S;
+}
 
 // the checks the grouped-query and strided entries (svgb_attn_{fwd,bwd}_{gqa,strided}) share, before any device
 // work: BHq query heads in groups over BHkv key/value heads, 16-bit inputs, and a variable-block plan over the
-// key/value heads or a band plan (one work list for every head, Sq == Skv)
+// key/value heads, a band plan (one work list for every head, Sq == Skv) or a segment plan (one work list for every head)
 inline int attn_gqa_check(int dtype, int BHq, int BHkv, int Sq, int Skv, const svgb_plan* plan, const char* who) {
   SVGB_REQUIRE(plan, "null pointer");
   SVGB_REQUIRE(BHq > 0 && BHkv > 0 && BHq % BHkv == 0,
                "%s: the query heads BHq=%d must be a multiple of the key/value heads BHkv=%d", who, BHq, BHkv);
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
                "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no GQA or strided path)", who, dtype);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND,
-               "%s takes variable-block or band plans (kind %d; gather and key-major plans have no GQA or strided "
-               "path)", who, plan->kind);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_SEG,
+               "%s takes variable-block, band or segment plans (kind %d; gather and key-major plans have no GQA or "
+               "strided path)", who, plan->kind);
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
   SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
                "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);

@@ -46,6 +46,9 @@ _PROTOS = {
     "svgb_attn_plan_band": [_i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_plan_band_t_bytes": [_i, _psz],
     "svgb_attn_plan_band_t": [_i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_local_varlen_bytes": [_i, _i, _i, _psz],
+    "svgb_attn_plan_local_varlen": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_local_varlen_t": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                       _pplan, _vp, _vp],
     "svgb_attn_fwd_kv": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan, _vp,

@@ -17,7 +17,8 @@ MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_
 # local band with attention sinks (SVGB_MASK_LOCAL): m0 = sink, m1 = left, m2 = right; plan_local builds it
 MASK_LOCAL = 10
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
-PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T = 1, 2, 3, 4
+PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T, PLAN_SEG, PLAN_SEG_T = 1, 2, 3, 4, 5, 6
+SEG_BOUNDS_OFF = 16  # SVGB_PLAN_SEG_BOUNDS_OFF: a segment plan's {nseg, cu_q, cu_k} in its workspace
 _E4M3 = 2  # SVGB_E4M3 (the 16-bit dtype ids come from _dt)
 
 # launches issued through this module since import (bench.py reports it as gpu_launches)
@@ -77,7 +78,7 @@ def device_check():
 class AttnPlan:
     """Device-resident work list + its host descriptor.  `source` keeps what a variable-block plan was built from
     (map, row sizes, column sizes, and their torch version counters at build time) so that key_major() can plan the
-    transpose; `_key_major` caches that plan."""
+    transpose, and a segment plan's segment count; `_key_major` caches that plan."""
     desc: Plan
     ws: torch.Tensor
     source: Optional[tuple] = None
@@ -89,8 +90,11 @@ class AttnPlan:
 
     @property
     def S_kv(self):
-        """Key/value length: a rectangular variable-block plan records it in m0 (include/svgb200.h, svgb_plan)."""
+        """Key/value length: a rectangular variable-block plan records it in m0, a segment plan (which serves every
+        head) in BH (include/svgb200.h, svgb_plan)."""
         d = self.desc
+        if d.kind in (PLAN_SEG, PLAN_SEG_T):
+            return d.BH
         return d.m0 if d.kind == PLAN_VARBLOCK and d.m0 > 0 else d.S
 
     def key_major(self) -> "AttnPlan":
@@ -104,6 +108,13 @@ class AttnPlan:
                     raise SvgbError(f"attention backward: the profiling mask mode {d.mask_mode} has no backward "
                                     "(executed masks NONE / HY / WAN / COG / LOCAL only)")
                 self._key_major = plan_band_t(d.mask_mode, d.m0, d.m1, d.m2, d.BH, d.S, self.ws.device)
+            elif d.kind == PLAN_SEG:
+                # from the plan's own copy of the bounds {nseg, cu_q, cu_k}, which is what the forward ran; source holds
+                # nseg for the host
+                (nseg,) = self.source
+                cu = self.ws.data_ptr() + SEG_BOUNDS_OFF + 4
+                self._key_major = _plan_local_varlen("svgb_attn_plan_local_varlen_t", cu, cu + 4 * (nseg + 1), nseg,
+                                                     d.S, d.BH, d.m0, d.m1, d.m2, self.ws.device)
             elif d.kind == PLAN_VARBLOCK and self.source is not None:
                 *ts, versions = self.source
                 if tuple(t._version for t in ts) != versions:
@@ -190,6 +201,49 @@ def plan_local(BH: int, S: int, device, *, causal: bool = False, window_size=(-1
         right = 0
     left, right = (S if w == -1 else w for w in (left, right))
     return plan_band(MASK_LOCAL, int(sink), left, right, BH, S, device)
+
+
+def _plan_local_varlen(name, cu_q, cu_k, nseg, Sq, Skv, sink, left, right, device) -> AttnPlan:
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_plan_local_varlen_bytes(nseg, Sq, Skv, C.byref(nbytes)), "svgb_attn_plan_local_varlen_bytes")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the bounds
+    desc = Plan()
+    check(getattr(lib(), name)(cu_q, cu_k, nseg, Sq, Skv, sink, left, right, ws.data_ptr(), ws.numel(), C.byref(desc),
+                               torch.cuda.current_stream(device).cuda_stream), name)
+    _bump(2)
+    return AttnPlan(desc, ws, (nseg,))
+
+
+def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.Tensor] = None, *, total_q: int,
+                      total_k: Optional[int] = None, causal: bool = False, window_size=(-1, -1),
+                      sink: int = 0) -> AttnPlan:
+    """Causal or sliding-window attention with attention sinks inside packed variable-length segments, in
+    FlashAttention's conventions (flash_attn_varlen_func): cu_seqlens_q / cu_seqlens_k are device int [nseg + 1]
+    (cu_seqlens_k None: the same segments), query segment i attends key segment i only, and its queries are aligned to
+    the END of the key segment (bottom-right), so query qi of segment i sits at key position qi + Lk_i - Lq_i.  Query
+    qi sees key kj when kj < sink, or when kj lies at most window_size[0] positions behind that position and at most
+    window_size[1] ahead (-1: unbounded); causal=True sets the right window to 0 and conflicts with a positive
+    window_size[1].  total_q / total_k (default total_q) are the packed lengths, q.shape[0] and k.shape[0] of a
+    [total, H, D] call: they are passed rather than read from cu_seqlens so that planning never waits on the device.
+    One plan for every head (any H, batch, GQA group or view); attention() runs it forward and backward, in 'shd' and in
+    'bhsd' (every batch element segmented alike).  Rows without an allowed key get o = 0 and lse = -inf."""
+    _need_cuda(cu_seqlens_q, cu_seqlens_k)
+    cu_q = cu_seqlens_q.to(torch.int32).contiguous()
+    cu_k = cu_q if cu_seqlens_k is None else cu_seqlens_k.to(torch.int32).contiguous()
+    if cu_q.dim() != 1 or cu_k.shape != cu_q.shape or cu_q.numel() < 2:
+        raise SvgbError(f"plan_local_varlen: cu_seqlens_q {tuple(cu_q.shape)} and cu_seqlens_k {tuple(cu_k.shape)} must "
+                        "be 1-D with the same nseg + 1 >= 2 entries")
+    Sq = int(total_q)
+    Skv = Sq if total_k is None else int(total_k)
+    left, right = (int(w) for w in window_size)
+    if causal:
+        if right > 0:
+            raise SvgbError(f"plan_local_varlen: causal=True looks no key ahead, but window_size[1] = {right}")
+        right = 0
+    # -1: no segment is longer than its total, and no query position lies further than that from a key
+    left, right = (max(Sq, Skv) if w == -1 else w for w in (left, right))
+    return _plan_local_varlen("svgb_attn_plan_local_varlen", cu_q.data_ptr(), cu_k.data_ptr(), cu_q.numel() - 1, Sq,
+                              Skv, int(sink), left, right, cu_q.device)
 
 
 def _is_profiling(mask_mode: int) -> bool:

@@ -78,11 +78,11 @@ def check_segments(what, segs, kv_segs, S, S_kv):
                              "one key segment per query segment")
 
 
-def segment_attention(what, query, key, value, segs, kv_segs, layout="bhsd"):
+def segment_attention(what, query, key, value, segs, kv_segs, layout="bhsd", sm_scale=None):
     """core.attention in which query segment i attends key segment i only: the segment lists pass check_segments
     (`what` names the caller in its error), then one rectangular plan of the diagonal block map over them.  layout
     'bhsd' or 'shd', as core.attention takes it.  The map is built over key's heads, so key / value may have fewer
-    heads than query (grouped-query attention)."""
+    heads than query (grouped-query attention).  sm_scale: the softmax scale (None: head_dim ** -0.5)."""
     seq = 2 if layout == "bhsd" else 0
     S, S_kv = query.shape[seq], key.shape[seq]
     check_segments(what, segs, kv_segs, S, S_kv)
@@ -92,7 +92,9 @@ def segment_attention(what, query, key, value, segs, kv_segs, layout="bhsd"):
     sz = torch.tensor(segs, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
     kv_sz = sz if kv_segs == segs else torch.tensor(kv_segs, dtype=torch.int32, device=dev).expand(BH, n).contiguous()
     plan = core.plan_varblock(bm, sz, kv_sz, S, S_kv=S_kv)
-    return core.attention(query, key, value, plan, layout=layout)
+    if sm_scale is None:
+        return core.attention(query, key, value, plan, layout=layout)
+    return core.attention(query, key, value, plan, layout=layout, sm_scale=sm_scale)
 
 
 def segment_lengths(cu_seqlens):

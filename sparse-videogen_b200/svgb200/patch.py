@@ -88,15 +88,36 @@ def flashinfer_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, m
     return dense_attention(q, k, v, seg, None if seg_kv is seg and k.shape[2] == q.shape[2] else seg_kv)
 
 
-def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, **kw):
-    """flash_attn.flash_attn_interface.flash_attn_varlen_func as hyvideo/attention.py:452-470 calls it: q,k,v
-    [L, B*H, D] (sequence first), segments given by cu_seqlens: query segment i attends key segment i (k, v may have
-    another length than q)."""
+def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, dropout_p=0.0,
+                           softmax_scale=None, causal=False, window_size=(-1, -1), softcap=0.0, alibi_slopes=None,
+                           deterministic=False, return_attn_probs=False, block_table=None):
+    """flash_attn.flash_attn_interface.flash_attn_varlen_func (FlashAttention 2's signature) as hyvideo/attention.py:
+    452-470 calls it: q,k,v [L, B*H, D] (sequence first), segments given by cu_seqlens: query segment i attends key
+    segment i (k, v may have another length than q).  causal= and window_size= mask inside each segment as
+    FlashAttention does (queries aligned to the end of their key segment; core.plan_local_varlen), softmax_scale=
+    replaces head_dim ** -0.5, and deterministic= is accepted (these kernels always are).  dropout_p, softcap,
+    alibi_slopes, return_attn_probs and block_table other than their defaults raise SvgbError rather than being
+    ignored.  Without a mask the call is the dense per-segment attention of models.common.segment_attention."""
+    from .core import SvgbError
+
+    for name, value, ok in (("dropout_p", dropout_p, dropout_p == 0.0), ("softcap", softcap, softcap == 0.0),
+                            ("alibi_slopes", alibi_slopes, alibi_slopes is None),
+                            ("return_attn_probs", return_attn_probs, not return_attn_probs),
+                            ("block_table", block_table, block_table is None)):
+        if not ok:
+            shown = value if isinstance(value, (int, float, bool)) else type(value).__name__
+            raise SvgbError(f"flash_attn_varlen_func: {name}={shown} is not supported (no kernel for it)")
+    if causal or tuple(window_size) != (-1, -1):
+        from . import core
+
+        plan = core.plan_local_varlen(cu_seqlens_q, cu_seqlens_kv, total_q=q.shape[0], total_k=k.shape[0],
+                                      causal=causal, window_size=window_size)
+        return core.attention(q, k, v, plan, layout="shd", sm_scale=softmax_scale)
     from .models.common import segment_attention
 
     seg, seg_kv = _varlen_segments(cu_seqlens_q, cu_seqlens_kv)
     return segment_attention("flash_attn_varlen_func", q, k, v, seg, seg_kv,
-                             layout="shd")
+                             layout="shd", sm_scale=softmax_scale)
 
 
 def _model_of(module):
