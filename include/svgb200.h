@@ -64,6 +64,7 @@ int svgb_device_check(int* sm_major, int* sm_minor, int* num_sms);
 #define SVGB_PLAN_BAND_T 4   /* key-major band plan of the backward pass (svgb_attn_plan_band_t) */
 #define SVGB_PLAN_SEG 5      /* local mask inside packed variable-length segments (svgb_attn_plan_local_varlen) */
 #define SVGB_PLAN_SEG_T 6    /* its key-major companion for the backward (svgb_attn_plan_local_varlen_t) */
+#define SVGB_PLAN_KVCACHE 7  /* local mask into a contiguous or paged KV cache, forward only (svgb_attn_plan_kvcache) */
 typedef struct svgb_plan {
   int32_t kind;          /* SVGB_PLAN_* */
   int32_t BH, S;
@@ -157,6 +158,52 @@ int svgb_attn_plan_local_varlen(const int32_t* cu_q, const int32_t* cu_k, int ns
  * same parameters and the same workspace layout (which is a function of nseg, Sq and Skv). */
 int svgb_attn_plan_local_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
                                   int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
+
+/* ---- KV cache (FlashAttention's flash_attn_with_kvcache) ----------------------------------
+ * A batch of B streams attends into a cache of num_blocks blocks of block_rows rows, Hkv heads, D in {64, 128}:
+ *   contiguous : k_cache, v_cache [B_cache, S_cache, Hkv, D] (num_blocks = B_cache, block_rows = S_cache, block_table
+ *                NULL); stream b lives in block cache_batch_idx[b] (NULL: block b).  Capacity S_cache.
+ *   paged      : k_cache, v_cache [num_pages, page_size, Hkv, D] (num_blocks = num_pages, block_rows = page_size, a
+ *                multiple of 128, so no 128-key chunk straddles two pages) and block_table int32 [B, max_pages]: logical
+ *                key t of stream b is row t % page_size of page block_table[b, t / page_size].  Capacity
+ *                max_pages * page_size; cache_batch_idx must be NULL.
+ * cache_seqlens: device int32 [B], the keys each stream holds before the append.  Nothing is read on the host.
+ * Bad input never makes a kernel touch memory outside the tensors, and gives an unspecified result: a length is clamped
+ * to [0, capacity], a block or page index to [0, num_blocks), and the append skips rows whose key or block falls
+ * outside the cache.  A stream's capacity is at most 2^29 keys and num_blocks * block_rows < 2^31.
+ *
+ * Append: k, v [B, Snew, Hkv, D] (Snew > 0) are written at logical keys cache_seqlens[b] .. cache_seqlens[b] + Snew - 1
+ * of each stream; nothing else is written.  One launch for K and V, 16-byte vectors.  Strides {batch or block, head,
+ * row} in elements per tensor, nonzero multiples of 8; bases 16-byte aligned; 16-bit dtypes. */
+int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
+                        const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew, int Hkv,
+                        int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                        const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                        void* stream);
+/* Plan: stream b has L_b = min(cache_seqlens[b] + Snew, capacity) keys at logical positions 0 .. L_b - 1 (Snew: rows
+ * appended before this attention), and Sq queries, query i at logical position L_b - Sq + i (FlashAttention's
+ * bottom-right alignment).  Query p sees key kv when kv < sink, or when p - kv <= left and kv - p <= right (causal:
+ * right = 0); all three >= 0.  A row without an allowed key gets o = 0 and lse = -inf.
+ * The queries are the packed rows [B * Sq, Hq, D] (query i of stream b is row b Sq + i); k and v are the cache viewed as
+ * num_blocks * block_rows rows.  Runs with svgb_attn_fwd_gqa and svgb_attn_fwd_strided (B = 1 at the ABI, Sq = B * Sq
+ * rows, Skv = num_blocks * block_rows rows), 16-bit inputs; no backward, e4m3, row vectors or gather.
+ * One launch, one warp per item: a stream's queries are cut into items of 256 rows from its first row, and each item
+ * visits only the chunks of its sinks and of its window (the pages behind a window are not read, so pages evicted from
+ * behind a window may be recycled as long as the sink pages are kept).  Chunks are 128 logical keys from position 0,
+ * FULL, ELEM or omitted; a kept chunk records the physical row its TMA box loads from and its logical index (mask
+ * positions).  The 128 - valid rows after a stream's last key in its last chunk are loaded and masked, so they must hold
+ * finite values (any cache allocated with zeros, or rows written earlier, qualifies).
+ * plan->kind = SVGB_PLAN_KVCACHE, mask_mode = SVGB_MASK_LOCAL, m0..m2 = sink, left, right, S = B * Sq,
+ * BH = num_blocks * block_rows (one plan for every head); the workspace keeps int32 {B, Sq, L_0 .. L_B-1} at byte
+ * SVGB_PLAN_SEG_BOUNDS_OFF.
+ * Workspace (integer division; cap = the capacity, I = B ceil(Sq / 256) items):
+ *   slots = min(ceil(cap / 128), ceil(sink / 128) + (255 + left + right) / 128 + 2)   chunk slots per item
+ *   bytes = 16 + align16(4 (B + 2)) + 32 I + 8 I slots
+ * which depends on host-known sizes only. */
+int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes);
+int svgb_attn_plan_kvcache(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table,
+                           int B, int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left,
+                           int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
 
 /* ---- attention -------------------------------------------------------------------------- */
 /* o = softmax(q k^T * sm_scale  [masked by plan]) v, per head.  Stands behind

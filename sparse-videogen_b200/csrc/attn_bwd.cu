@@ -51,6 +51,7 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
                         const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
   SVGB_REQUIRE(q && k && v && o && dout && lse && dq && dk && dv && plan && plan_ws && plan_t && plan_t_ws && ws,
                "null pointer");
+  if (no_kvcache_backward(plan, "attention backward")) return -1;
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
                "attention backward takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no backward)", dtype);
   SVGB_REQUIRE(D == 64 || D == 128, "head_dim %d unsupported (64 or 128)", D);
@@ -165,7 +166,7 @@ int svgb_attn_bwd_kv(const void* q, const void* k, const void* v, const void* o,
                      long long q_head_stride, long long kv_row_stride, long long kv_head_stride, float sm_scale,
                      const svgb_plan* plan, const void* plan_ws, const svgb_plan* plan_t, const void* plan_t_ws,
                      void* ws, size_t ws_bytes, void* stream) {
-  SVGB_REQUIRE(plan, "null pointer");
+  if (no_kvcache_backward(plan, "svgb_attn_bwd_kv")) return -1;
   SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_SEG,
                "svgb_attn_bwd_kv takes segment plans and variable-block plans only (kind %d; band plans need "
                "Sq == Skv, svgb_attn_bwd)", plan->kind);
@@ -184,6 +185,7 @@ int svgb_attn_bwd_gqa(const void* q, const void* k, const void* v, const void* o
                       long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                       long long kv_head_stride, float sm_scale, const svgb_plan* plan, const void* plan_ws,
                       const svgb_plan* plan_t, const void* plan_t_ws, void* ws, size_t ws_bytes, void* stream) {
+  if (no_kvcache_backward(plan, "svgb_attn_bwd_gqa")) return -1;
   if (attn_gqa_check(dtype, BHq, BHkv, Sq, Skv, plan, "svgb_attn_bwd_gqa")) return -1;
   SVGB_REQUIRE(plan_t, "null pointer");
   SVGB_REQUIRE(plan_t->items_stride == 0 || plan_t->BH == BHkv,
@@ -211,6 +213,7 @@ int svgb_attn_bwd_strided(const void* q, const void* k, const void* v, const voi
                          {q_strides, k_strides, v_strides, o_strides, do_strides, dq_strides, dk_strides, dv_strides},
                          st, "svgb_attn_bwd_strided"))
     return -1;
+  if (no_kvcache_backward(plan, "svgb_attn_bwd_strided")) return -1;
   if (attn_gqa_check(dtype, B * Hq, B * Hkv, Sq, Skv, plan, "svgb_attn_bwd_strided")) return -1;
   SVGB_REQUIRE(plan_t, "null pointer");
   SVGB_REQUIRE(plan_t->items_stride == 0 || plan_t->BH == B * Hkv,

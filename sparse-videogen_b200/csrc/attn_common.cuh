@@ -15,7 +15,9 @@ namespace svgb {
 // items of up to kItemRows rows (put_item); a variable-block TMA plan also pairs two tails of different q-blocks,
 // each with its own list.  The list is
 //   TMA plans   : list_len chunks {kv_start, meta}; meta bits [0,8) = valid columns - 1 (0..127), bit 8 = ELEM
-//                 (evaluate the element mask predicate on this chunk), bit 9 = reserved.
+//                 (evaluate the element mask predicate on this chunk), bit 9 = reserved; KV-cache plans only: bits
+//                 [10,32) = the chunk's logical index j (keys 128 j .. of its stream), the position the mask sees, while
+//                 kv_start is the physical row its TMA box loads from.
 //   gather plans: list_len runs {src_start, keys before the run} of the selected key ranges and a sentinel
 //                 {0, total}; the kernel gathers exactly-full 128-key chunks across run boundaries.
 constexpr int kItemRows = 256;
@@ -27,6 +29,11 @@ __host__ __device__ inline int chunk_meta(int valid, bool elem) {
   return ((valid - 1) & 0xff) | (elem ? kChunkElem : 0);
 }
 __host__ __device__ inline int chunk_valid(int meta) { return (meta & 0xff) + 1; }
+constexpr int kChunkLogicalShift = 10;
+// first logical key of a KV-cache chunk (128 j); j < 2^22, so the shift never reaches the sign bit
+__host__ __device__ inline int chunk_logical_kv0(int meta) {
+  return static_cast<int>(static_cast<unsigned>(meta) >> kChunkLogicalShift) * kChunkCols;
+}
 
 // the two streams of an item of nrows (1..kItemRows) consecutive query rows from q0, both over one list
 __device__ inline void put_item(int4* item, int q0, int nrows, int list_off, int list_len) {
@@ -146,6 +153,19 @@ __host__ __device__ inline SegOrigin seg_origin(const int* seg, int row, bool ke
   SegOrigin o;
   o.shift = segs[lo + 1] - ck[lo + 1];
   o.sink_end = ck[lo] + sink;
+  return o;
+}
+
+// KV-cache plans (SVGB_PLAN_KVCACHE).  The plan keeps at byte SVGB_PLAN_SEG_BOUNDS_OFF of its workspace
+// kv = {B, Sq, L_0 .. L_B-1}: stream b has its queries at packed rows [b Sq, (b+1) Sq) and L_b keys at logical positions
+// 0 .. L_b - 1 (clamped to its capacity).  Query row q of stream b sits at logical position L_b - Sq + (q - b Sq), so the
+// mask is MASK_LOCAL(sink, left, right) on logical positions with shift (b+1) Sq - L_b and the sink bound `sink`; the
+// key positions come from each chunk's logical index (chunk_logical_kv0), not from its physical row.
+__host__ __device__ inline SegOrigin kv_origin(const int* kv, int row, int sink) {
+  const int Sq = kv[1], b = row / Sq;
+  SegOrigin o;
+  o.shift = (b + 1) * Sq - kv[2 + b];
+  o.sink_end = sink;
   return o;
 }
 
@@ -330,6 +350,8 @@ struct AttnArgs {
   const int* q_index = nullptr;  // optional [S]: query position used by the element mask (sampled rows)
   // segment plans: the plan's copy of the bounds {nseg, cq[0..nseg], ck[0..nseg]} (seg_origin); nullptr otherwise
   const int* segs = nullptr;
+  // KV-cache plans: segs is the plan's {B, Sq, L_b} (kv_origin) and element masks see each chunk's logical position
+  int kv_logical = 0;
   int out_f32 = 0;               // 1: o is fp32 (used for split-KV partials)
   // FP8 (e4m3) inputs: per-head dequantisation scales [BH]; s_q * s_k multiplies the logits, s_v the
   // output.  NULL for 16-bit inputs.

@@ -698,6 +698,10 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG_T,
                "a key-major segment plan (svgb_attn_plan_local_varlen_t) is for the backward; the forward takes "
                "svgb_attn_plan_local_varlen");
+  const bool kvc = plan->kind == SVGB_PLAN_KVCACHE;
+  SVGB_REQUIRE(!kvc || dtype != SVGB_E4M3, "KV-cache plans (svgb_attn_plan_kvcache) take bf16 or fp16 inputs, not e4m3");
+  SVGB_REQUIRE(!kvc || (!q_rows && !kv_rows && !o_rows),
+               "KV-cache plans (svgb_attn_plan_kvcache) take no row vectors or gathers (q_rows / kv_rows / o_rows)");
   const bool seg = plan->kind == SVGB_PLAN_SEG;
   SVGB_REQUIRE(!seg || dtype != SVGB_E4M3, "segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs, not e4m3");
   SVGB_REQUIRE(!seg || (!q_rows && !kv_rows && !o_rows),
@@ -725,13 +729,14 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.lse = lse;
   a.scale_log2 = sm_scale * 1.4426950408889634f;
   a.S = Sq;
-  if (plan->kind == SVGB_PLAN_BAND || seg) {  // a variable-block plan's m0 is its Skv, not a mask parameter
+  if (plan->kind == SVGB_PLAN_BAND || seg || kvc) {  // a variable-block plan's m0 is its Skv, not a mask parameter
     a.mask_mode = plan->mask_mode;
     a.m0 = plan->m0;
     a.m1 = plan->m1;
     a.m2 = plan->m2;
   }
-  if (seg) a.segs = reinterpret_cast<const int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF);
+  if (seg || kvc) a.segs = reinterpret_cast<const int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF);
+  a.kv_logical = kvc ? 1 : 0;
   a.q_scale = q_scale;
   a.k_scale = k_scale;
   a.v_scale = v_scale;

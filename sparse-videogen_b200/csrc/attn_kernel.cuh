@@ -382,9 +382,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     const int rloc = 64 * cw + 16 * wq + (lane >> 2);
     ElemMask em;
     if constexpr (!kGather) {  // gather plans carry no element masks
-      // segment plans: the stream's segment shifts the query positions and moves the sink bound (seg_origin)
+      // segment plans: the stream's segment shifts the query positions and moves the sink bound (seg_origin); KV-cache
+      // plans: the stream's length shifts them to logical positions (kv_origin)
       SegOrigin so{0, m0};
-      if (args.segs) so = seg_origin(args.segs, q0, false, m0);
+      if (args.segs) so = args.kv_logical ? kv_origin(args.segs, q0, m0) : seg_origin(args.segs, q0, false, m0);
       int qm[2];
 #pragma unroll
       for (int v1 = 0; v1 < 2; ++v1) {
@@ -404,20 +405,22 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     // factor O still has to be scaled by before P(j) V(j) is accumulated
     auto softmax = [&](int j) {
       // ---- mask: partial chunks and element-mask chunks
-      int kv0 = 0, valid = kChunkCols;
+      int kv0 = 0, meta = 0, valid = kChunkCols;
       bool elem = false;
       if constexpr (kGather) {
         valid = min(kChunkCols, total - j * kChunkCols);
       } else {
         const int2 ch = __ldg(&chunks[j]);
         kv0 = ch.x;
+        meta = ch.y;
         valid = chunk_valid(ch.y);
         elem = (ch.y & kChunkElem) != 0;
       }
       if (valid < kChunkCols || elem) {
         // keep[v1] bit 2*jj + v0: column 8*jj + 2*(lane%4) + v0 of row v1 is an allowed key
         uint32_t keep[2] = {~0u, ~0u};
-        if (elem) em.bits(kv0 + 2 * (lane & 3), keep);
+        // KV-cache plans: the mask sees the chunk's logical position, the TMA box loaded its physical row kv0
+        if (elem) em.bits((args.kv_logical ? chunk_logical_kv0(meta) : kv0) + 2 * (lane & 3), keep);
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj)
 #pragma unroll

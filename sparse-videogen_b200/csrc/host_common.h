@@ -66,7 +66,7 @@ int encode_tmap_bhsd(CUtensorMap* map, const void* base, int dtype, int B, int H
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
 // BH (svgb200.h); every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) {
-  if (p->kind == SVGB_PLAN_SEG || p->kind == SVGB_PLAN_SEG_T) return p->BH;
+  if (p->kind == SVGB_PLAN_SEG || p->kind == SVGB_PLAN_SEG_T || p->kind == SVGB_PLAN_KVCACHE) return p->BH;
   return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S;
 }
 
@@ -79,12 +79,21 @@ inline int attn_gqa_check(int dtype, int BHq, int BHkv, int Sq, int Skv, const s
                "%s: the query heads BHq=%d must be a multiple of the key/value heads BHkv=%d", who, BHq, BHkv);
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
                "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no GQA or strided path)", who, dtype);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_SEG,
-               "%s takes variable-block, band or segment plans (kind %d; gather and key-major plans have no GQA or "
-               "strided path)", who, plan->kind);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_SEG ||
+                   plan->kind == SVGB_PLAN_KVCACHE,
+               "%s takes variable-block, band, segment or KV-cache plans (kind %d; gather and key-major plans have no "
+               "GQA or strided path)", who, plan->kind);
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
   SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
                "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
+  return 0;
+}
+
+// KV-cache plans (svgb_attn_plan_kvcache) run forward only, as FlashAttention's flash_attn_with_kvcache
+inline int no_kvcache_backward(const svgb_plan* plan, const char* who) {
+  SVGB_REQUIRE(plan, "null pointer");
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_KVCACHE,
+               "%s: a KV-cache plan (svgb_attn_plan_kvcache) has no backward; it runs forward only", who);
   return 0;
 }
 

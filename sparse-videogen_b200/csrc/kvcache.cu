@@ -1,0 +1,246 @@
+// KV cache: the in-place append of new key / value rows (svgb_kvcache_append) and the plan of the attention of a batch
+// of streams into a contiguous or paged cache (svgb_attn_plan_kvcache), run by the attention forward (attn_kernel.cuh).
+// Both read the per-stream lengths on the device only.
+#include <algorithm>
+
+#include "../../include/svgb200.h"
+#include "attn_common.cuh"
+#include "host_common.h"
+
+namespace svgb {
+
+// Logical keys of stream b after the append, clamped to its capacity: lengths past the capacity or negative give an
+// unspecified result that stays inside the cache
+__device__ __forceinline__ int kv_len(int cache_seqlen, int new_len, int cap) {
+  const long long x = static_cast<long long>(max(cache_seqlen, 0)) + new_len;
+  return static_cast<int>(x < cap ? x : cap);
+}
+
+// The cache is num_blocks blocks of block_rows rows: a contiguous cache [B_cache, S_cache, Hkv, D] (stream b in block
+// cache_batch_idx[b], or b) or a paged one [num_pages, page_size, Hkv, D] (logical key t of stream b in row t % page_size
+// of page block_table[b, t / page_size]).  Out-of-range blocks are clamped to the cache.
+__device__ __forceinline__ int kv_block(const int* __restrict__ batch_idx, const int* __restrict__ table, int b, int t,
+                                        int nblocks, int block_rows, int max_pages) {
+  const int blk = table ? __ldg(&table[static_cast<size_t>(b) * max_pages + t / block_rows])
+                        : (batch_idx ? __ldg(&batch_idx[b]) : b);
+  return min(max(blk, 0), nblocks - 1);
+}
+
+// =============================================================================================
+// Append: new rows k, v [B, Snew, Hkv, D] at logical keys cache_seqlens[b] .. + Snew - 1 of each stream, one 16-byte
+// vector of K and one of V per thread.  Rows whose logical key lies outside [0, capacity) or whose block lies outside
+// the cache are not written.
+// =============================================================================================
+__global__ void __launch_bounds__(256)
+kv_append_kernel(uint16_t* __restrict__ kc, uint16_t* __restrict__ vc, const uint16_t* __restrict__ k,
+                 const uint16_t* __restrict__ v, const int* __restrict__ seqlens, const int* __restrict__ batch_idx,
+                 const int* __restrict__ table, int B, int Snew, int Hkv, int nvec, int nblocks, int block_rows,
+                 int max_pages, int cap, Strides kcs, Strides vcs, Strides ks, Strides vs) {
+  const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(idx % nvec);
+    long long r = idx / nvec;
+    const int h = static_cast<int>(r % Hkv);
+    r /= Hkv;
+    const int i = static_cast<int>(r % Snew), b = static_cast<int>(r / Snew);
+    const long long t = static_cast<long long>(__ldg(&seqlens[b])) + i;
+    if (t < 0 || t >= cap) continue;
+    const int tt = static_cast<int>(t);
+    int blk, row;
+    if (table) {
+      blk = __ldg(&table[static_cast<size_t>(b) * max_pages + tt / block_rows]);
+      row = tt % block_rows;
+    } else {
+      blk = batch_idx ? __ldg(&batch_idx[b]) : b;
+      row = tt;
+    }
+    if (blk < 0 || blk >= nblocks) continue;
+    const long long e = 8ll * c;
+    const uint4 kx = *reinterpret_cast<const uint4*>(k + b * ks.b + i * ks.r + h * ks.h + e);
+    const uint4 vx = *reinterpret_cast<const uint4*>(v + b * vs.b + i * vs.r + h * vs.h + e);
+    *reinterpret_cast<uint4*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) = kx;
+    *reinterpret_cast<uint4*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) = vx;
+  }
+}
+
+// =============================================================================================
+// Plan: one warp per item.  Stream b's Sq query rows (packed rows b Sq ..) are cut into items of 256 rows from its first
+// row, and every item has `slots` chunk slots.  The warp visits the chunks that can hold an allowed key -- those of the
+// sinks and those of the item's window, so the pages behind a window are never read -- classifies each from the band's
+// interval form on logical positions (seg_chunk_kind) and writes the kept ones, compacted with a ballot, with the
+// physical row its TMA box loads from and its logical index in the meta's high bits.
+// =============================================================================================
+__global__ void __launch_bounds__(256)
+kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_idx, const int* __restrict__ table, int B,
+                int Sq, int Snew, int nblocks, int block_rows, int max_pages, int cap, int slots, int sink, int left,
+                int right, int* __restrict__ counts, int* __restrict__ kv, int2* __restrict__ chunks,
+                int4* __restrict__ items) {
+  const int lane = threadIdx.x & 31;
+  const int per = (Sq + kItemRows - 1) / kItemRows;  // items per stream
+  const int it = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (it == 0 && lane == 0) {
+    counts[0] = B * per;
+    kv[0] = B;
+    kv[1] = Sq;
+  }
+  if (it >= B * per) return;
+  const int b = it / per, k = it - b * per;
+  const int L = kv_len(__ldg(&seqlens[b]), Snew, cap);
+  if (k == 0 && lane == 0) kv[2 + b] = L;
+  const int r0 = b * Sq + k * kItemRows, nr = min(kItemRows, Sq - k * kItemRows);
+  SegOrigin o;
+  o.shift = (b + 1) * Sq - L;
+  o.sink_end = sink;
+  // chunks that can hold an allowed key: [0, ns) with sinks, [jlo, jhi] inside the window of positions p0 .. p1
+  const int nch = (L + kChunkCols - 1) / kChunkCols;
+  const int ns = (min(sink, L) + kChunkCols - 1) / kChunkCols;
+  const long long p0 = static_cast<long long>(r0) - o.shift, p1 = p0 + nr - 1;
+  const long long lo = std::max(p0 - left, 0ll), hi = std::min(p1 + right, static_cast<long long>(L) - 1);
+  const int jlo = max(ns, static_cast<int>(lo / kChunkCols));
+  const int jhi = hi < lo ? -1 : min(nch - 1, static_cast<int>(hi / kChunkCols));
+  const int nvis = ns + max(0, jhi - jlo + 1);
+  const int list = it * slots;
+  int n = 0;
+  for (int v0 = 0; v0 < nvis; v0 += 32) {
+    const int vi = v0 + lane;
+    const int j = vi < ns ? vi : jlo + (vi - ns);
+    const int c0 = j * kChunkCols, valid = min(kChunkCols, L - c0);
+    const int kind = vi < nvis ? seg_chunk_kind(false, r0, r0 + nr - 1, c0, c0 + valid - 1, o, left, right) : 0;
+    const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
+    const int at = n + __popc(m & ((1u << lane) - 1u));
+    if (kind != 0 && at < slots) {
+      const int blk = kv_block(batch_idx, table, b, c0, nblocks, block_rows, max_pages);
+      const int row = blk * block_rows + (table ? c0 % block_rows : c0);
+      chunks[list + at] = make_int2(row, chunk_meta(valid, kind == 2) | (j << kChunkLogicalShift));
+    }
+    n += __popc(m);
+  }
+  if (lane == 0) put_item(items + 2 * it, r0, nr, list, min(n, slots));
+}
+
+// Workspace of a KV-cache plan, 16-byte aligned pieces:
+//   counts (16 B) | {B, Sq, L_0 .. L_B-1} | items 2 int4 [B I] | chunks [B I slots]
+// with I = ceil(Sq / 256) items per stream and slots = min(ceil(cap / 128), ceil(sink / 128) + (255 + left + right) / 128
+// + 2), the chunks an item can visit: its sinks and the window of its 256 rows
+struct KvLayout {
+  long long items, slots;
+  size_t items_off, chunks_off, bytes;
+};
+static KvLayout kv_layout(int B, int Sq, int cap, int sink, int left, int right) {
+  KvLayout L;
+  L.items = static_cast<long long>(B) * ((Sq + kItemRows - 1) / kItemRows);
+  const long long win = (static_cast<long long>(sink) + kChunkCols - 1) / kChunkCols +
+                        (kItemRows - 1 + static_cast<long long>(left) + right) / kChunkCols + 2;
+  L.slots = std::min<long long>((static_cast<long long>(cap) + kChunkCols - 1) / kChunkCols, win);
+  L.items_off = SVGB_PLAN_SEG_BOUNDS_OFF + align_up(sizeof(int) * (2 + static_cast<size_t>(B)), 16);
+  L.chunks_off = L.items_off + 2 * sizeof(int4) * L.items;
+  L.bytes = L.chunks_off + sizeof(int2) * L.items * L.slots;
+  return L;
+}
+
+static int kv_plan_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {
+  SVGB_REQUIRE(B > 0 && Sq > 0 && cap > 0 && bytes, "bad arguments (B=%d, Sq=%d, capacity=%d)", B, Sq, cap);
+  SVGB_REQUIRE(sink >= 0 && left >= 0 && right >= 0,
+               "KV-cache plan: sink (%d), left (%d) and right (%d) must be >= 0", sink, left, right);
+  *bytes = kv_layout(B, Sq, cap, sink, left, right).bytes;
+  return 0;
+}
+
+// the cache geometry both entries take: num_blocks blocks of block_rows rows, paged when block_table is given; returns
+// the capacity of a stream in *cap
+static int kv_geometry(const int32_t* cache_batch_idx, const int32_t* block_table, int num_blocks, int block_rows,
+                       int max_pages, int* cap, const char* who) {
+  SVGB_REQUIRE(num_blocks > 0 && block_rows > 0, "%s: bad cache geometry (num_blocks=%d, block_rows=%d)", who,
+               num_blocks, block_rows);
+  SVGB_REQUIRE(static_cast<long long>(num_blocks) * block_rows < (1ll << 31), "%s: cache of %d x %d rows too large",
+               who, num_blocks, block_rows);
+  long long c = block_rows;
+  if (block_table) {
+    SVGB_REQUIRE(block_rows % kChunkCols == 0,
+                 "%s: page_size %d must be a multiple of 128 (no 128-key chunk may straddle two pages)", who, block_rows);
+    SVGB_REQUIRE(max_pages > 0, "%s: block_table needs max_pages > 0 (got %d)", who, max_pages);
+    SVGB_REQUIRE(!cache_batch_idx, "%s: cache_batch_idx is for contiguous caches; a paged cache takes block_table only",
+                 who);
+    c = static_cast<long long>(max_pages) * block_rows;
+  }
+  // the logical chunk index lives in 22 bits of the chunk meta
+  SVGB_REQUIRE(c <= (1ll << 29), "%s: a stream's capacity (%lld keys) exceeds 2^29", who, c);
+  *cap = static_cast<int>(c);
+  return 0;
+}
+
+}  // namespace svgb
+
+using namespace svgb;
+
+extern "C" {
+
+int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
+                        const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew, int Hkv,
+                        int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                        const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                        void* stream) {
+  const char* who = "svgb_kvcache_append";
+  SVGB_REQUIRE(cache_seqlens, "null pointer");
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "%s takes bf16 or fp16 caches (dtype %d)", who, dtype);
+  SVGB_REQUIRE(D == 64 || D == 128, "%s: head_dim %d unsupported (64 or 128)", who, D);
+  SVGB_REQUIRE(Snew > 0, "%s: no new rows (Snew=%d)", who, Snew);
+  Strides st[4];
+  if (attn_strided_check(B, Hkv, Hkv, {k_cache, v_cache, k, v}, {kc_strides, vc_strides, k_strides, v_strides}, st, who))
+    return -1;
+  int cap = 0;
+  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
+  const int nvec = D / 8;
+  const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
+  const unsigned blocks = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 1 << 20));
+  kv_append_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<uint16_t*>(k_cache), static_cast<uint16_t*>(v_cache), static_cast<const uint16_t*>(k),
+      static_cast<const uint16_t*>(v), cache_seqlens, cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks,
+      block_rows, max_pages, cap, st[0], st[1], st[2], st[3]);
+  SVGB_LAUNCH_OK();
+  return 0;
+}
+
+int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {
+  return kv_plan_bytes(B, Sq, cap, sink, left, right, bytes);
+}
+
+int svgb_attn_plan_kvcache(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table,
+                           int B, int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left,
+                           int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
+  const char* who = "svgb_attn_plan_kvcache";
+  SVGB_REQUIRE(cache_seqlens && plan_ws && plan, "null pointer");
+  SVGB_REQUIRE(Snew >= 0, "%s: Snew=%d < 0", who, Snew);
+  int cap = 0;
+  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
+  size_t need = 0;
+  if (kv_plan_bytes(B, Sq, cap, sink, left, right, &need)) return -1;
+  SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
+  SVGB_REQUIRE(static_cast<long long>(B) * Sq < (1ll << 30), "%s: B * Sq = %lld query rows too many", who,
+               static_cast<long long>(B) * Sq);
+  const KvLayout L = kv_layout(B, Sq, cap, sink, left, right);
+  SVGB_REQUIRE(L.items * L.slots < (1ll << 31), "plan too large for 32-bit chunk offsets");
+  plan->kind = SVGB_PLAN_KVCACHE;
+  plan->BH = num_blocks * block_rows;  // a KV-cache plan serves every head: BH holds the cache rows (svgb200.h)
+  plan->S = B * Sq;
+  plan->max_items = static_cast<int>(L.items);
+  plan->items_stride = 0;
+  plan->mask_mode = MASK_LOCAL;
+  plan->m0 = sink;
+  plan->m1 = left;
+  plan->m2 = right;
+  plan->counts_off = 0;
+  plan->items_off = static_cast<int64_t>(L.items_off);
+  plan->chunks_off = static_cast<int64_t>(L.chunks_off);
+  plan->bytes = static_cast<int64_t>(need);
+  char* ws = static_cast<char*>(plan_ws);
+  kv_lists_kernel<<<static_cast<unsigned>((L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, cap,
+      static_cast<int>(L.slots), sink, left, right, reinterpret_cast<int*>(ws), reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF),
+      reinterpret_cast<int2*>(ws + L.chunks_off), reinterpret_cast<int4*>(ws + L.items_off));
+  SVGB_LAUNCH_OK();
+  return 0;
+}
+
+}  // extern "C"

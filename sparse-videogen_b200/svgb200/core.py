@@ -17,8 +17,9 @@ MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_
 # local band with attention sinks (SVGB_MASK_LOCAL): m0 = sink, m1 = left, m2 = right; plan_local builds it
 MASK_LOCAL = 10
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
-PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T, PLAN_SEG, PLAN_SEG_T = 1, 2, 3, 4, 5, 6
-SEG_BOUNDS_OFF = 16  # SVGB_PLAN_SEG_BOUNDS_OFF: a segment plan's {nseg, cu_q, cu_k} in its workspace
+PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T, PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE = 1, 2, 3, 4, 5, 6, 7
+# SVGB_PLAN_SEG_BOUNDS_OFF: a segment plan's {nseg, cu_q, cu_k} in its workspace, a KV-cache plan's {B, Sq, L_b}
+SEG_BOUNDS_OFF = 16
 _E4M3 = 2  # SVGB_E4M3 (the 16-bit dtype ids come from _dt)
 
 # launches issued through this module since import (bench.py reports it as gpu_launches)
@@ -91,9 +92,9 @@ class AttnPlan:
     @property
     def S_kv(self):
         """Key/value length: a rectangular variable-block plan records it in m0, a segment plan (which serves every
-        head) in BH (include/svgb200.h, svgb_plan)."""
+        head) in BH, and so does a KV-cache plan (the cache's rows) (include/svgb200.h, svgb_plan)."""
         d = self.desc
-        if d.kind in (PLAN_SEG, PLAN_SEG_T):
+        if d.kind in (PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE):
             return d.BH
         return d.m0 if d.kind == PLAN_VARBLOCK and d.m0 > 0 else d.S
 
@@ -128,6 +129,9 @@ class AttnPlan:
                 self._key_major = kt
             elif d.kind == PLAN_GATHER:
                 raise SvgbError("attention backward: gather plans (row-gather path, q_rows / kv_rows) have no backward")
+            elif d.kind == PLAN_KVCACHE:
+                raise SvgbError("attention backward: a KV-cache plan (plan_kvcache) has no backward; it runs forward "
+                                "only, as flash_attn_with_kvcache does")
             else:
                 raise SvgbError(f"attention backward: plan kind {d.kind} has no key-major form")
         return self._key_major
@@ -246,6 +250,122 @@ def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.T
                               Skv, int(sink), left, right, cu_q.device)
 
 
+def _seqlens(cache_seqlens, B, device) -> torch.Tensor:
+    """cache_seqlens as a device int32 [B]: an int is broadcast on the device, a tensor converted there."""
+    if isinstance(cache_seqlens, torch.Tensor):
+        _need_cuda(cache_seqlens)
+        t = cache_seqlens.to(torch.int32).reshape(-1).contiguous()
+        if t.numel() != B:
+            raise SvgbError(f"cache_seqlens has {t.numel()} entries for {B} streams")
+        return t
+    return torch.full((B,), int(cache_seqlens), dtype=torch.int32, device=device)
+
+
+def _cache_layout(B, block_table, cache_batch_idx):
+    """(block_table, cache_batch_idx, max_pages) in the form the KV-cache entries take: device int32, contiguous."""
+    if block_table is not None and cache_batch_idx is not None:
+        raise SvgbError("cache_batch_idx is for contiguous caches; a paged cache (block_table) takes no cache_batch_idx")
+    bt = bi = None
+    max_pages = 0
+    if block_table is not None:
+        _need_cuda(block_table)
+        if block_table.dim() != 2 or block_table.shape[0] != B:
+            raise SvgbError(f"block_table {tuple(block_table.shape)} must be [B={B}, max_pages]")
+        bt = block_table.to(torch.int32).contiguous()
+        max_pages = bt.shape[1]
+    if cache_batch_idx is not None:
+        _need_cuda(cache_batch_idx)
+        bi = cache_batch_idx.to(torch.int32).reshape(-1).contiguous()
+        if bi.numel() != B:
+            raise SvgbError(f"cache_batch_idx has {bi.numel()} entries for {B} streams")
+    return bt, bi, max_pages
+
+
+def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cache_seqlens, *,
+                   block_table: Optional[torch.Tensor] = None, cache_batch_idx: Optional[torch.Tensor] = None):
+    """Write the new rows k, v [B, Snew, Hkv, D] into the cache in place, at keys cache_seqlens[b] .. + Snew - 1 of each
+    stream b, in one launch.  The cache is contiguous, k_cache / v_cache [B_cache, S_cache, Hkv, D] with stream b in
+    row cache_batch_idx[b] (default b), or paged, [num_pages, page_size, Hkv, D] with block_table int [B, max_pages]
+    (page_size a multiple of 128).  cache_seqlens: int or device int tensor [B], read on the device only.  Rows whose key
+    or block falls outside the cache are not written (include/svgb200.h, svgb_kvcache_append)."""
+    _need_cuda(k_cache, v_cache, k, v)
+    if k_cache.dim() != 4 or k.dim() != 4 or k_cache.shape != v_cache.shape or k.shape != v.shape:
+        raise SvgbError(f"kvcache_append: k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] and "
+                        f"k, v {tuple(k.shape)} [B, Snew, Hkv, D], each pair of one shape")
+    if k.shape[2:] != k_cache.shape[2:]:
+        raise SvgbError(f"kvcache_append: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
+    if not (k_cache.dtype == v_cache.dtype == k.dtype == v.dtype):
+        raise SvgbError("kvcache_append: the caches and the new rows must share one dtype")
+    dt = _dt(k)
+    B, Snew, Hkv, D = k.shape
+    if Snew == 0:
+        return
+    for c in (k_cache, v_cache):
+        if not _addressable(c.transpose(1, 2), "bhsd"):
+            raise SvgbError("kvcache_append: the cache is written in place, so it must be 16-byte aligned with a last "
+                            "stride of 1 and other strides that are nonzero multiples of 8 elements")
+    k, v = (_addressed(t.transpose(1, 2), "bhsd") for t in (k, v))
+    bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
+    lens = _seqlens(cache_seqlens, B, k.device)
+    check(lib().svgb_kvcache_append(k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(), lens.data_ptr(),
+                                    _p(bi), _p(bt), dt, B, Snew, Hkv, D, k_cache.shape[0], k_cache.shape[1], max_pages,
+                                    _st(k_cache.transpose(1, 2), "bhsd"), _st(v_cache.transpose(1, 2), "bhsd"),
+                                    _st(k, "bhsd"), _st(v, "bhsd"), _stream(k)), "svgb_kvcache_append")
+    _bump()
+
+
+def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0, cache_len: Optional[int] = None,
+                 block_table: Optional[torch.Tensor] = None, page_size: Optional[int] = None,
+                 cache_batch_idx: Optional[torch.Tensor] = None, causal: bool = False, window_size=(-1, -1),
+                 sink: int = 0) -> AttnPlan:
+    """Attention of B streams of q_len queries into a KV cache, in FlashAttention's conventions
+    (flash_attn_with_kvcache): stream b holds L_b = cache_seqlens[b] + new_len keys (new_len rows appended before this
+    attention, e.g. by kvcache_append) and its query i sits at logical position L_b - q_len + i.  Query p sees key kv
+    when kv < sink, or when kv lies at most window_size[0] positions behind p and at most window_size[1] ahead (-1:
+    unbounded); causal=True sets the right window to 0 and conflicts with a positive window_size[1].
+    The cache is k_cache.shape[0] = num_blocks blocks: contiguous, cache_len = S_cache rows each (stream b in block
+    cache_batch_idx[b], default b), or paged, page_size rows each (a multiple of 128) with block_table int [B, max_pages].
+    cache_seqlens: int or device int tensor [B]; nothing is read on the host.  attn_fwd runs the plan on q [B, q_len, Hq,
+    D] and the cache, any Hq = G * Hkv; it has no backward (attention() under grad and key_major() raise)."""
+    if block_table is not None:
+        B = block_table.shape[0]
+        if page_size is None:
+            raise SvgbError("plan_kvcache: a paged cache (block_table) needs page_size")
+        rows = int(page_size)
+        cap = block_table.shape[1] * rows
+    else:
+        if cache_len is None:
+            raise SvgbError("plan_kvcache: a contiguous cache needs cache_len (its rows per stream, k_cache.shape[1])")
+        B = cache_seqlens.numel() if isinstance(cache_seqlens, torch.Tensor) else None
+        if B is None:
+            if cache_batch_idx is None:
+                raise SvgbError("plan_kvcache: with an int cache_seqlens pass a tensor or cache_batch_idx for B")
+            B = cache_batch_idx.numel()
+        rows = cap = int(cache_len)
+    device = (cache_seqlens if isinstance(cache_seqlens, torch.Tensor) else
+              block_table if block_table is not None else cache_batch_idx).device
+    bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
+    lens = _seqlens(cache_seqlens, B, device)
+    Sq = int(q_len)
+    left, right = (int(w) for w in window_size)
+    if causal:
+        if right > 0:
+            raise SvgbError(f"plan_kvcache: causal=True looks no key ahead, but window_size[1] = {right}")
+        right = 0
+    # -1: no query position lies further than cap + Sq from a key
+    left, right = (min(cap + Sq, 2**31 - 1) if w == -1 else w for w in (left, right))
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_plan_kvcache_bytes(B, Sq, cap, int(sink), left, right, C.byref(nbytes)),
+          "svgb_attn_plan_kvcache_bytes")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the lengths
+    desc = Plan()
+    check(lib().svgb_attn_plan_kvcache(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks), rows,
+                                       max_pages, int(sink), left, right, ws.data_ptr(), ws.numel(), C.byref(desc),
+                                       torch.cuda.current_stream(device).cuda_stream), "svgb_attn_plan_kvcache")
+    _bump()
+    return AttnPlan(desc, ws, (B, Sq))
+
+
 def _is_profiling(mask_mode: int) -> bool:
     """The SVG1 profiling masks (modes 4-9): band plans the forward runs and the backward does not."""
     return MASK_PROF_HY_S <= mask_mode <= MASK_PROF_COG_T
@@ -325,7 +445,7 @@ def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
         _gqa_check(dtype, plan, rows)
     lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    if not all(t.is_contiguous() for t in (q, k, v, o)):
+    if plan.desc.kind == PLAN_KVCACHE or not all(t.is_contiguous() for t in (q, k, v, o)):
         B = q.shape[0] if layout == "bhsd" else 1
         check(lib().svgb_attn_fwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), dtype, B,
                                           q.shape[1], k.shape[1], Sq, Skv, D, *(_st(t, layout) for t in (q, k, v, o)),
@@ -378,6 +498,10 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     with key/value head h // G): a variable-block plan is then built over the B * Hkv key/value heads and shared by
     each group, band plans are shared by every head already; no row vectors, FP8 or gather plans."""
     _need_cuda(q, k, v)
+    if plan.desc.kind == PLAN_KVCACHE:
+        if any(r is not None for r in (q_rows, kv_rows, o_rows)):
+            raise SvgbError("a KV-cache plan (plan_kvcache) takes no row vectors (o_rows / q_rows / kv_rows)")
+        return _attn_kvcache(q, k, v, plan, return_lse, sm_scale, out)
     rows = (q_rows, kv_rows, o_rows)
     if any(r is not None for r in rows) or plan.desc.kind == PLAN_GATHER:
         # the row vectors and the row-gather kernel index one flat [BH, S, D] stride pair
@@ -399,6 +523,35 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
         return res
     out.copy_(o)  # an out= the kernels cannot address
     return (out, res[1]) if return_lse else out
+
+
+def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out):
+    """attn_fwd under a KV-cache plan: q [B, Sq, Hq, D] as B * Sq packed rows, the cache [blocks, rows, Hkv, D] as
+    blocks * rows rows (both views), o [B, Sq, Hq, D] and lse [B, Hq, Sq] (flash_attn_with_kvcache's shapes)."""
+    B, Sq = plan.source
+    if q.dim() != 4 or q.shape[:2] != (B, Sq) or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
+        raise SvgbError(f"a KV-cache plan for B={B} streams of Sq={Sq} queries takes q [B, Sq, Hq, D] (got "
+                        f"{tuple(q.shape)}) and k_cache, v_cache [blocks, rows, Hkv, D] of one shape (got "
+                        f"{tuple(k_cache.shape)}, {tuple(v_cache.shape)})")
+    if k_cache.shape[0] * k_cache.shape[1] != plan.S_kv:
+        raise SvgbError(f"the KV-cache plan was built for {plan.S_kv} cache rows, the cache {tuple(k_cache.shape)} has "
+                        f"{k_cache.shape[0] * k_cache.shape[1]}")
+    if not (q.dtype == k_cache.dtype == v_cache.dtype):
+        raise SvgbError("q and the caches must share one dtype")
+    if out is not None and (out.shape != q.shape or out.dtype != q.dtype):
+        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype")
+    Hq, D = q.shape[2:]
+    qf = _addressed(q.reshape(B * Sq, Hq, D), "shd")
+    kf, vf = (_addressed(c.flatten(0, 1), "shd") for c in (k_cache, v_cache))
+    of = torch.empty_like(qf)
+    res = _attn(qf, kf, vf, of, plan, "shd", _dt(q), (None, None, None), (None, None, None), return_lse, sm_scale)
+    o = of.view(B, Sq, Hq, D)
+    if out is not None:
+        out.copy_(o)
+        o = out
+    if not return_lse:
+        return o
+    return o, res[1].view(Hq, B, Sq).transpose(0, 1)
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
@@ -495,7 +648,8 @@ def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Option
     LSE, and the plan is not read here."""
     if not needs_grad(q, k, v):
         return attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale)
-    if plan.desc.kind == PLAN_GATHER or (plan.desc.kind == PLAN_BAND and _is_profiling(plan.desc.mask_mode)):
+    if plan.desc.kind in (PLAN_GATHER, PLAN_KVCACHE) or (plan.desc.kind == PLAN_BAND and
+                                                          _is_profiling(plan.desc.mask_mode)):
         plan.key_major()  # raises, naming what has no backward
     return _Attention.apply(q, k, v, plan, layout, sm_scale)
 

@@ -120,6 +120,49 @@ def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, m
                              layout="shd", sm_scale=softmax_scale)
 
 
+def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None, rotary_sin=None, cache_seqlens=None,
+                            cache_batch_idx=None, cache_leftpad=None, block_table=None, softmax_scale=None, causal=False,
+                            window_size=(-1, -1), softcap=0.0, rotary_interleaved=True, alibi_slopes=None,
+                            num_splits=0, return_softmax_lse=False):
+    """flash_attn.flash_attn_with_kvcache (FlashAttention 2's signature and return convention), forward only.
+    q [B, Sq, Hq, D]; k_cache, v_cache [B_cache, S_cache, Hkv, D] (stream b in row cache_batch_idx[b], default b) or
+    paged [num_pages, page_size, Hkv, D] with block_table int32 [B, max_pages] (page_size a multiple of 128).  k, v
+    [B, Snew, Hkv, D], when given, are written into the cache in place at cache_seqlens[b] (core.kvcache_append), and
+    the queries then attend the cache_seqlens[b] + Snew keys of their stream, aligned to its end (core.plan_kvcache),
+    under causal= / window_size=.  cache_seqlens: int or device int tensor [B] (None: the whole S_cache of a contiguous
+    cache); nothing is read on the host.  Returns out [B, Sq, Hq, D], and lse [B, Hq, Sq] with return_softmax_lse.
+    num_splits is a scheduling hint and is ignored; rotary_cos / rotary_sin, cache_leftpad, softcap and alibi_slopes
+    other than their defaults raise SvgbError rather than being ignored (video models apply their own RoPE before
+    caching)."""
+    from . import core
+    from .core import SvgbError
+
+    for name, value, ok in (("rotary_cos", rotary_cos, rotary_cos is None), ("rotary_sin", rotary_sin, rotary_sin is None),
+                            ("cache_leftpad", cache_leftpad, cache_leftpad is None),
+                            ("softcap", softcap, softcap == 0.0), ("alibi_slopes", alibi_slopes, alibi_slopes is None)):
+        if not ok:
+            shown = value if isinstance(value, (int, float, bool)) else type(value).__name__
+            raise SvgbError(f"flash_attn_with_kvcache: {name}={shown} is not supported (no kernel for it)")
+    if core.needs_grad(q, k_cache, v_cache, k, v):
+        raise SvgbError("flash_attn_with_kvcache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
+    if (k is None) != (v is None):
+        raise SvgbError("flash_attn_with_kvcache: k and v are given together or not at all")
+    B, Sq = q.shape[:2]
+    if cache_seqlens is None:
+        if block_table is not None:
+            raise SvgbError("flash_attn_with_kvcache: a paged cache (block_table) needs cache_seqlens")
+        cache_seqlens = k_cache.shape[1]
+    lens = core._seqlens(cache_seqlens, B, q.device)
+    if k is not None:
+        core.kvcache_append(k_cache, v_cache, k, v, lens, block_table=block_table, cache_batch_idx=cache_batch_idx)
+    paged = block_table is not None
+    plan = core.plan_kvcache(lens, q_len=Sq, num_blocks=k_cache.shape[0], new_len=0 if k is None else k.shape[1],
+                             cache_len=None if paged else k_cache.shape[1], block_table=block_table,
+                             page_size=k_cache.shape[1] if paged else None, cache_batch_idx=cache_batch_idx,
+                             causal=causal, window_size=window_size)
+    return core.attn_fwd(q, k_cache, v_cache, plan, return_lse=return_softmax_lse, sm_scale=softmax_scale)
+
+
 def _model_of(module):
     name = getattr(module, "__name__", "")
     for m in ("hyvideo", "wan", "cosmos", "cog"):

@@ -1,0 +1,147 @@
+"""Attention into a KV cache (core.kvcache_append, core.plan_kvcache, core.attn_fwd) on the H100: the Self-Forcing /
+CausVid streaming shape, a chunk of 3 latent frames (4 680 queries) against a 21-frame cache (32 760 keys, 1 560 tokens
+per frame at 480p) with a one-frame sink and a window of 9 frames (14 040 keys) behind each query, bf16, D = 128, for
+Wan 1.3B (12 heads) and Wan 14B (40 heads).  Ways, each one call sequence as a caller would issue it:
+
+  contiguous      plan + forward on a contiguous [1, 32 760, H, D] cache
+  paged           plan + forward on the same keys in 256-row pages under a shuffled block table
+  append+paged    kvcache_append of the chunk's 4 680 new rows into the pages, then plan + forward
+  index+contig    the caller-side alternative: the new rows written with one slice copy, then plan + forward
+  roll+contig     eviction by shifting: the window part of the cache moved down by one chunk (a slice copy of a clone,
+                  as rolling caches do), the new rows written at the end, then plan + forward
+  sdpa            torch scaled_dot_product_attention on the sliced cache under the same boolean mask (built once)
+  decode          Sq = 1: one query against the same cache, plan + forward (one CTA per head: no split-KV)
+
+Each figure is the median of R rounds with the rounds' min and max; every round times N back-to-back calls of each way
+with CUDA events, the ways alternated within every round.  The card name and power limit are read in the same run.
+
+    python tools/kvcache_perf.py [--rounds R] [--iters N] [--out FILE]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import statistics
+import sys
+from pathlib import Path
+
+import torch
+
+ROOT = Path(__file__).resolve().parent.parent
+sys.path[:0] = [str(ROOT), str(ROOT / "sparse-videogen_b200"), str(ROOT / "tools")]
+
+from local_attn_perf import card  # noqa: E402
+
+D, FRAME, FRAMES, CHUNK_FRAMES, PAGE = 128, 1560, 21, 3, 256
+L, SQ, SINK, LEFT = FRAMES * FRAME, CHUNK_FRAMES * FRAME, FRAME, 9 * FRAME
+
+
+def timed(fn, iters):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(iters):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / iters
+
+
+def alternate(ways, rounds, iters):
+    for fn in ways.values():
+        fn()  # warm-up
+    torch.cuda.synchronize()
+    ms = {w: [] for w in ways}
+    for _ in range(rounds):
+        for w, fn in ways.items():
+            ms[w].append(timed(fn, iters))
+    return {w: {"median_ms": round(statistics.median(v), 3), "min_ms": round(min(v), 3), "max_ms": round(max(v), 3)}
+            for w, v in ms.items()}
+
+
+def case(H, dev, rounds, iters):
+    from svgb200 import core
+
+    g = torch.Generator(device=dev).manual_seed(H)
+    bf = torch.bfloat16
+    rnd = lambda *s: torch.randn(*s, device=dev, generator=g).to(bf)  # noqa: E731
+    cap = ((L + PAGE - 1) // PAGE) * PAGE
+    kc, vc = rnd(1, cap, H, D), rnd(1, cap, H, D)
+    q, q1 = rnd(1, SQ, H, D), rnd(1, 1, H, D)
+    knew, vnew = rnd(1, SQ, H, D), rnd(1, SQ, H, D)
+    npages = cap // PAGE
+    perm = torch.randperm(npages, generator=torch.Generator().manual_seed(0))
+    kp, vp = torch.empty(npages, PAGE, H, D, device=dev, dtype=bf), torch.empty(npages, PAGE, H, D, device=dev, dtype=bf)
+    kp[perm] = kc[0].view(npages, PAGE, H, D)
+    vp[perm] = vc[0].view(npages, PAGE, H, D)
+    table = perm.to(torch.int32).view(1, npages).to(dev)
+    lens = torch.tensor([L], dtype=torch.int32, device=dev)
+    before = lens - SQ  # the chunk's rows are appended at L - SQ
+    win = dict(causal=True, window_size=(LEFT, 0), sink=SINK)
+
+    def contiguous(qq=q, new_len=0, seq=lens):
+        plan = core.plan_kvcache(seq, q_len=qq.shape[1], num_blocks=1, new_len=new_len, cache_len=cap, **win)
+        return core.attn_fwd(qq, kc, vc, plan)
+
+    def paged(qq=q, new_len=0, seq=lens):
+        plan = core.plan_kvcache(seq, q_len=qq.shape[1], num_blocks=npages, new_len=new_len, block_table=table,
+                                 page_size=PAGE, **win)
+        return core.attn_fwd(qq, kp, vp, plan)
+
+    def append_paged():
+        core.kvcache_append(kp, vp, knew, vnew, before, block_table=table)
+        return paged(new_len=SQ, seq=before)
+
+    def index_contig():
+        kc[:, L - SQ:L] = knew
+        vc[:, L - SQ:L] = vnew
+        return contiguous()
+
+    def roll_contig():
+        n = L - SINK - SQ  # the window part that stays, moved down by one chunk
+        kc[:, SINK:SINK + n] = kc[:, SINK + SQ:L].clone()
+        vc[:, SINK:SINK + n] = vc[:, SINK + SQ:L].clone()
+        kc[:, L - SQ:L] = knew
+        vc[:, L - SQ:L] = vnew
+        return contiguous()
+
+    p = torch.arange(SQ, device=dev)[:, None] + (L - SQ)
+    kv = torch.arange(L, device=dev)[None, :]
+    mask = (kv < SINK) | ((p - kv <= LEFT) & (kv <= p))
+    qt = q.transpose(1, 2)
+
+    def sdpa():
+        k, v = kc[:, :L].transpose(1, 2), vc[:, :L].transpose(1, 2)
+        return torch.nn.functional.scaled_dot_product_attention(qt, k, v, attn_mask=mask)
+
+    # the ways agree before they are timed
+    o_c, o_p = contiguous(), paged()
+    assert torch.equal(o_c, o_p), "paged and contiguous differ"
+    err = (sdpa().transpose(1, 2).float() - o_c.float()).abs().max().item()
+    assert err < 3e-2, f"sdpa differs by {err}"
+    ways = {"contiguous": contiguous, "paged": paged, "append+paged": append_paged, "index+contig": index_contig,
+            "roll+contig": roll_contig, "sdpa": sdpa, "decode": lambda: paged(qq=q1)}
+    return alternate(ways, rounds, iters)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--out")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("kvcache_perf needs a GPU")
+    dev = torch.device("cuda:0")
+    res = {"card": card(), "rounds": a.rounds, "iters": a.iters,
+           "shape": dict(queries=SQ, keys=L, sink=SINK, left=LEFT, page=PAGE, D=D)}
+    for name, H in (("wan1.3b", 12), ("wan14b", 40)):
+        res[name] = case(H, dev, a.rounds, a.iters)
+        print(json.dumps({name: res[name]}), flush=True)
+    print(json.dumps(res))
+    if a.out:
+        Path(a.out).parent.mkdir(parents=True, exist_ok=True)
+        Path(a.out).write_text(json.dumps(res, indent=1))
+
+
+if __name__ == "__main__":
+    main()
