@@ -180,13 +180,27 @@ int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void*
                         int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                         const long long* vc_strides, const long long* k_strides, const long long* v_strides,
                         void* stream);
+/* Append into an e4m3 cache (FP8 KV cache): svgb_kvcache_append's arguments, with dtype the 16-bit (SVGB_BF16 / SVGB_F16)
+ * type of the new rows k, v and the caches e4m3 bytes, plus k_scale, v_scale: device float [Hkv], one dequantisation
+ * scale per key/value head for the cache's lifetime (cache element ~= e4m3 * scale[h]).  Each new element is written as
+ * RN-satfinite(x * (1 / scale[h])), the conversion of svgb_quantize_e4m3, so a value past 448 * scale saturates to
+ * +-448; the scales are not checked on the device.  One launch for K and V; nothing else is written.  The cache strides
+ * (in elements, i.e. bytes) must be multiples of 16, as the attention's TMA maps need; the new rows' strides follow
+ * svgb_kvcache_append.  Rows past a stream's length must be finite here too, and 0x7F / 0xFF are e4m3 NaN: allocate
+ * the cache with zeros. */
+int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
+                             const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew,
+                             int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                             const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                             const float* k_scale, const float* v_scale, void* stream);
 /* Plan: stream b has L_b = min(cache_seqlens[b] + Snew, capacity) keys at logical positions 0 .. L_b - 1 (Snew: rows
  * appended before this attention), and Sq queries, query i at logical position L_b - Sq + i (FlashAttention's
  * bottom-right alignment).  Query p sees key kv when kv < sink, or when p - kv <= left and kv - p <= right (causal:
  * right = 0); all three >= 0.  A row without an allowed key gets o = 0 and lse = -inf.
  * The queries are the packed rows [B * Sq, Hq, D] (query i of stream b is row b Sq + i); k and v are the cache viewed as
  * num_blocks * block_rows rows.  Runs with svgb_attn_fwd_gqa and svgb_attn_fwd_strided (B = 1 at the ABI, Sq = B * Sq
- * rows, Skv = num_blocks * block_rows rows), 16-bit inputs; no backward, e4m3, row vectors or gather.
+ * rows, Skv = num_blocks * block_rows rows), 16-bit inputs, and with svgb_attn_fwd_strided_e4m3 on an e4m3 cache; no
+ * backward, row vectors or gather.
  * One launch, one warp per item: a stream's queries are cut into items of 256 rows from its first row, and each item
  * visits only the chunks of its sinks and of its window (the pages behind a window are not read, so pages evicted from
  * behind a window may be recycled as long as the sink pages are kept).  Chunks are 128 logical keys from position 0,
@@ -280,6 +294,22 @@ int svgb_attn_fwd_strided(const void* q, const void* k, const void* v, void* o, 
                           int Hkv, int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
                           const long long* v_strides, const long long* o_strides, float sm_scale,
                           const svgb_plan* plan, const void* plan_ws, void* stream);
+/* svgb_attn_fwd_strided on e4m3 inputs (the FP8 KV cache, and FP8 with grouped-query heads):
+ *   q, k, v : e4m3 bytes, D = 128, strides (in elements, i.e. bytes) multiples of 16; bases 16-byte aligned.
+ *   q_scale : float [B * Hq], by flat query head b * Hq + hq;  k_scale, v_scale : float [B * Hkv], by flat key/value
+ *           head b * Hkv + hkv (x ~= x8 * scale), all three required.  Query head hq reads the scales of the key/value
+ *           head hq / G it attends with.
+ *   o     : bf16 at its own strides (nonzero multiples of 8 elements);  lse : optional float [B * Hq, Sq].
+ *   plan  : SVGB_PLAN_KVCACHE (the cache as num_blocks * block_rows rows, B = 1 at the ABI), SVGB_PLAN_VARBLOCK (over
+ *           the B * Hkv key/value heads) or SVGB_PLAN_BAND (Sq == Skv).
+ * Refused by name: segment plans, gather plans (row vectors run on svgb_attn_fwd only) and D = 64.  The kernel is
+ * svgb_attn_fwd's e4m3 instantiation: with G = 1 and B = 1 each output row is bit for bit svgb_attn_fwd's, and with
+ * G > 1 the one of G = 1 on K, V and their scales repeated per group. */
+int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, const float* q_scale,
+                               const float* k_scale, const float* v_scale, void* o, float* lse, int B, int Hq, int Hkv,
+                               int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
+                               const long long* v_strides, const long long* o_strides, float sm_scale,
+                               const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
 
 /* Backward of svgb_attn_fwd: dq, dk, dv from q, k, v, the forward's o and natural-log lse, and the output gradient dO.

@@ -353,8 +353,8 @@ struct AttnArgs {
   // KV-cache plans: segs is the plan's {B, Sq, L_b} (kv_origin) and element masks see each chunk's logical position
   int kv_logical = 0;
   int out_f32 = 0;               // 1: o is fp32 (used for split-KV partials)
-  // FP8 (e4m3) inputs: per-head dequantisation scales [BH]; s_q * s_k multiplies the logits, s_v the
-  // output.  NULL for 16-bit inputs.
+  // FP8 (e4m3) inputs: per-head dequantisation scales, q_scale [BH] by query head, k_scale and v_scale [BH / kv_group]
+  // by key/value head; s_q * s_k multiplies the logits, s_v the output.  NULL for 16-bit inputs.
   const float* q_scale = nullptr;
   const float* k_scale = nullptr;
   const float* v_scale = nullptr;

@@ -699,7 +699,6 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
                "a key-major segment plan (svgb_attn_plan_local_varlen_t) is for the backward; the forward takes "
                "svgb_attn_plan_local_varlen");
   const bool kvc = plan->kind == SVGB_PLAN_KVCACHE;
-  SVGB_REQUIRE(!kvc || dtype != SVGB_E4M3, "KV-cache plans (svgb_attn_plan_kvcache) take bf16 or fp16 inputs, not e4m3");
   SVGB_REQUIRE(!kvc || (!q_rows && !kv_rows && !o_rows),
                "KV-cache plans (svgb_attn_plan_kvcache) take no row vectors or gathers (q_rows / kv_rows / o_rows)");
   const bool seg = plan->kind == SVGB_PLAN_SEG;
@@ -858,6 +857,10 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream) {
+  // its scales are [BH] by query head: an e4m3 cache, whose scales are by key/value head, takes the strided e4m3 entry
+  SVGB_REQUIRE(!plan || plan->kind != SVGB_PLAN_KVCACHE || dtype != SVGB_E4M3,
+               "KV-cache plans (svgb_attn_plan_kvcache) take bf16 or fp16 inputs here; an e4m3 cache takes "
+               "svgb_attn_fwd_strided_e4m3");
   const Strides in = flat_strides(row_stride, head_stride, BH);
   return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, 1, BH, 1, S, S, D,
                       in, in, in, flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, stream);
@@ -909,6 +912,36 @@ int svgb_attn_fwd_strided(const void* q, const void* k, const void* v, void* o, 
     return -1;
   if (attn_gqa_check(dtype, B * Hq, B * Hkv, Sq, Skv, plan, "svgb_attn_fwd_strided")) return -1;
   return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, B, B * Hq,
+                      Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, stream);
+}
+
+int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, const float* q_scale,
+                               const float* k_scale, const float* v_scale, void* o, float* lse, int B, int Hq, int Hkv,
+                               int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
+                               const long long* v_strides, const long long* o_strides, float sm_scale,
+                               const svgb_plan* plan, const void* plan_ws, void* stream) {
+  const char* who = "svgb_attn_fwd_strided_e4m3";
+  SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
+               who, D);
+  SVGB_REQUIRE(q_scale && k_scale && v_scale,
+               "%s needs the three scale vectors: q_scale [B*Hq], k_scale and v_scale [B*Hkv]", who);
+  SVGB_REQUIRE(plan, "null pointer");
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG && plan->kind != SVGB_PLAN_SEG_T,
+               "%s: segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs, not e4m3", who);
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_GATHER,
+               "%s: gather plans (svgb_attn_plan_varblock_gather) and row vectors run on svgb_attn_fwd only", who);
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_KVCACHE,
+               "%s takes variable-block, band or KV-cache plans (kind %d)", who, plan->kind);
+  Strides st[4];
+  if (attn_strided_check(B, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st, who)) return -1;
+  for (int i = 0; i < 3; ++i)
+    SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
+                 "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
+                 st[i].b, st[i].h, st[i].r);
+  SVGB_REQUIRE(Hq % Hkv == 0, "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d", who, Hq,
+               Hkv);
+  if (attn_group_plan_check(B * Hkv, Sq, Skv, plan, who)) return -1;
+  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, B, B * Hq,
                       Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, stream);
 }
 

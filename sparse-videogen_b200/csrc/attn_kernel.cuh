@@ -345,8 +345,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   setmaxnreg_inc<kConsumerRegs>();
   const int cw = wg - 1;                    // this consumer's 64 rows of the tile: 64cw .. 64cw+63
   const uint32_t sQw = sQ + 64 * cw * 128;
-  const float c = args.scale_log2 * (args.q_scale ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[bh]) : 1.f);
-  const float vs = args.v_scale ? __ldg(&args.v_scale[bh]) : 1.f;
+  // FP8: q_scale per query head, k_scale and v_scale per key/value head (a group's query heads share its K and V).
+  // 16-bit inputs take no scales; their instantiations keep indexing by bh, so their code does not depend on kvh.
+  const int sh = FP8 ? kvh : bh;
+  const float c = args.scale_log2 * (args.q_scale ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[sh]) : 1.f);
+  const float vs = args.v_scale ? __ldg(&args.v_scale[sh]) : 1.f;
   const int mode = args.mask_mode, m0 = args.m0, m1 = args.m1, m2 = args.m2;
 
   // Turns on the tensor cores: each consumer issues its wgmma groups between turn_wait and turn_pass, so the two

@@ -70,6 +70,15 @@ inline int plan_kv_len(const svgb_plan* p) {
   return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S;
 }
 
+// what a plan of an accepted kind needs to be shared by the groups of query heads: band plans Sq == Skv, per-head
+// plans built over the BHkv key/value heads
+inline int attn_group_plan_check(int BHkv, int Sq, int Skv, const svgb_plan* plan, const char* who) {
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
+  SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
+               "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
+  return 0;
+}
+
 // the checks the grouped-query and strided entries (svgb_attn_{fwd,bwd}_{gqa,strided}) share, before any device
 // work: BHq query heads in groups over BHkv key/value heads, 16-bit inputs, and a variable-block plan over the
 // key/value heads, a band plan (one work list for every head, Sq == Skv) or a segment plan (one work list for every head)
@@ -83,10 +92,7 @@ inline int attn_gqa_check(int dtype, int BHq, int BHkv, int Sq, int Skv, const s
                    plan->kind == SVGB_PLAN_KVCACHE,
                "%s takes variable-block, band, segment or KV-cache plans (kind %d; gather and key-major plans have no "
                "GQA or strided path)", who, plan->kind);
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
-  SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
-               "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
-  return 0;
+  return attn_group_plan_check(BHkv, Sq, Skv, plan, who);
 }
 
 // KV-cache plans (svgb_attn_plan_kvcache) run forward only, as FlashAttention's flash_attn_with_kvcache

@@ -1,7 +1,11 @@
-// KV cache: the in-place append of new key / value rows (svgb_kvcache_append) and the plan of the attention of a batch
+// KV cache: the in-place append of new key / value rows (svgb_kvcache_append, and svgb_kvcache_append_e4m3 into an
+// e4m3 cache) and the plan of the attention of a batch
 // of streams into a contiguous or paged cache (svgb_attn_plan_kvcache), run by the attention forward (attn_kernel.cuh).
 // Both read the per-stream lengths on the device only.
+#include <cuda_fp16.h>
+
 #include <algorithm>
+#include <type_traits>
 
 #include "../../include/svgb200.h"
 #include "attn_common.cuh"
@@ -26,16 +30,41 @@ __device__ __forceinline__ int kv_block(const int* __restrict__ batch_idx, const
   return min(max(blk, 0), nblocks - 1);
 }
 
+// what the append writes from 16-bit new rows: the rows themselves, or e4m3 quantised from bf16 or fp16 rows
+enum KvStore { KV_COPY, KV_E4M3_BF16, KV_E4M3_F16 };
+
+// 8 16-bit elements -> 8 e4m3 bytes, RN-satfinite(x * inv), as quantize_kernel (quant_fp8.cu)
+template <bool BF16>
+__device__ __forceinline__ uint2 kv_to_e4m3(uint4 x, float inv) {
+  const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+  uint32_t out[2];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    uint16_t p[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const uint16_t lo16 = static_cast<uint16_t>(w[2 * j + i] & 0xffff), hi16 = static_cast<uint16_t>(w[2 * j + i] >> 16);
+      const float a = (BF16 ? __uint_as_float(static_cast<uint32_t>(lo16) << 16) : __half2float(__ushort_as_half(lo16))) * inv;
+      const float b = (BF16 ? __uint_as_float(static_cast<uint32_t>(hi16) << 16) : __half2float(__ushort_as_half(hi16))) * inv;
+      asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(p[i]) : "f"(b), "f"(a));
+    }
+    out[j] = static_cast<uint32_t>(p[0]) | (static_cast<uint32_t>(p[1]) << 16);
+  }
+  return make_uint2(out[0], out[1]);
+}
+
 // =============================================================================================
 // Append: new rows k, v [B, Snew, Hkv, D] at logical keys cache_seqlens[b] .. + Snew - 1 of each stream, one 16-byte
-// vector of K and one of V per thread.  Rows whose logical key lies outside [0, capacity) or whose block lies outside
-// the cache are not written.
+// vector of K and one of V per thread (e4m3 caches: 8 elements of each, written as 8 bytes).  Rows whose logical key
+// lies outside [0, capacity) or whose block lies outside the cache are not written.
 // =============================================================================================
+template <int kStore, typename Cache = typename std::conditional<kStore == KV_COPY, uint16_t, uint8_t>::type>
 __global__ void __launch_bounds__(256)
-kv_append_kernel(uint16_t* __restrict__ kc, uint16_t* __restrict__ vc, const uint16_t* __restrict__ k,
+kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t* __restrict__ k,
                  const uint16_t* __restrict__ v, const int* __restrict__ seqlens, const int* __restrict__ batch_idx,
                  const int* __restrict__ table, int B, int Snew, int Hkv, int nvec, int nblocks, int block_rows,
-                 int max_pages, int cap, Strides kcs, Strides vcs, Strides ks, Strides vs) {
+                 int max_pages, int cap, Strides kcs, Strides vcs, Strides ks, Strides vs,
+                 const float* __restrict__ k_scale, const float* __restrict__ v_scale) {
   const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -59,8 +88,16 @@ kv_append_kernel(uint16_t* __restrict__ kc, uint16_t* __restrict__ vc, const uin
     const long long e = 8ll * c;
     const uint4 kx = *reinterpret_cast<const uint4*>(k + b * ks.b + i * ks.r + h * ks.h + e);
     const uint4 vx = *reinterpret_cast<const uint4*>(v + b * vs.b + i * vs.r + h * vs.h + e);
-    *reinterpret_cast<uint4*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) = kx;
-    *reinterpret_cast<uint4*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) = vx;
+    if constexpr (kStore == KV_COPY) {
+      *reinterpret_cast<uint4*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) = kx;
+      *reinterpret_cast<uint4*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) = vx;
+    } else {
+      constexpr bool BF16 = kStore == KV_E4M3_BF16;
+      *reinterpret_cast<uint2*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) =
+          kv_to_e4m3<BF16>(kx, 1.f / __ldg(&k_scale[h]));
+      *reinterpret_cast<uint2*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) =
+          kv_to_e4m3<BF16>(vx, 1.f / __ldg(&v_scale[h]));
+    }
   }
 }
 
@@ -174,6 +211,48 @@ static int kv_geometry(const int32_t* cache_batch_idx, const int32_t* block_tabl
 
 using namespace svgb;
 
+// both appends: 16-bit new rows (dtype) into a 16-bit cache of that dtype, or (k_scale, v_scale given) into an e4m3 cache
+static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
+                         const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew,
+                         int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                         const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                         const float* k_scale, const float* v_scale, void* stream, const char* who) {
+  const bool e4m3 = k_scale != nullptr;
+  SVGB_REQUIRE(cache_seqlens, "null pointer");
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "%s takes bf16 or fp16 %s (dtype %d)", who,
+               e4m3 ? "new rows" : "caches", dtype);
+  SVGB_REQUIRE(D == 64 || D == 128, "%s: head_dim %d unsupported (64 or 128)", who, D);
+  SVGB_REQUIRE(Snew > 0, "%s: no new rows (Snew=%d)", who, Snew);
+  Strides st[4];
+  if (attn_strided_check(B, Hkv, Hkv, {k_cache, v_cache, k, v}, {kc_strides, vc_strides, k_strides, v_strides}, st, who))
+    return -1;
+  if (e4m3)
+    for (int i = 0; i < 2; ++i)
+      SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
+                   "%s: every e4m3 cache (block, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)",
+                   who, st[i].b, st[i].h, st[i].r);
+  int cap = 0;
+  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
+  const int nvec = D / 8;
+  const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
+  const unsigned blocks = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 1 << 20));
+  cudaStream_t cs = static_cast<cudaStream_t>(stream);
+  const uint16_t *kn = static_cast<const uint16_t*>(k), *vn = static_cast<const uint16_t*>(v);
+  if (!e4m3) {
+    kv_append_kernel<KV_COPY><<<blocks, 256, 0, cs>>>(
+        static_cast<uint16_t*>(k_cache), static_cast<uint16_t*>(v_cache), kn, vn, cache_seqlens, cache_batch_idx,
+        block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages, cap, st[0], st[1], st[2], st[3], nullptr,
+        nullptr);
+  } else {
+    auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_BF16> : kv_append_kernel<KV_E4M3_F16>;
+    kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
+                                 cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages,
+                                 cap, st[0], st[1], st[2], st[3], k_scale, v_scale);
+  }
+  SVGB_LAUNCH_OK();
+  return 0;
+}
+
 extern "C" {
 
 int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
@@ -181,25 +260,21 @@ int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void*
                         int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                         const long long* vc_strides, const long long* k_strides, const long long* v_strides,
                         void* stream) {
-  const char* who = "svgb_kvcache_append";
-  SVGB_REQUIRE(cache_seqlens, "null pointer");
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "%s takes bf16 or fp16 caches (dtype %d)", who, dtype);
-  SVGB_REQUIRE(D == 64 || D == 128, "%s: head_dim %d unsupported (64 or 128)", who, D);
-  SVGB_REQUIRE(Snew > 0, "%s: no new rows (Snew=%d)", who, Snew);
-  Strides st[4];
-  if (attn_strided_check(B, Hkv, Hkv, {k_cache, v_cache, k, v}, {kc_strides, vc_strides, k_strides, v_strides}, st, who))
-    return -1;
-  int cap = 0;
-  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
-  const int nvec = D / 8;
-  const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
-  const unsigned blocks = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 1 << 20));
-  kv_append_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<uint16_t*>(k_cache), static_cast<uint16_t*>(v_cache), static_cast<const uint16_t*>(k),
-      static_cast<const uint16_t*>(v), cache_seqlens, cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks,
-      block_rows, max_pages, cap, st[0], st[1], st[2], st[3]);
-  SVGB_LAUNCH_OK();
-  return 0;
+  return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
+                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
+                       nullptr, stream, "svgb_kvcache_append");
+}
+
+int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
+                             const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew,
+                             int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                             const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                             const float* k_scale, const float* v_scale, void* stream) {
+  const char* who = "svgb_kvcache_append_e4m3";
+  SVGB_REQUIRE(k_scale && v_scale, "%s needs both scale vectors k_scale and v_scale (float [Hkv])", who);
+  return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
+                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, k_scale,
+                       v_scale, stream, who);
 }
 
 int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {

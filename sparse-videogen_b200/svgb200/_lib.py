@@ -51,6 +51,8 @@ _PROTOS = {
     "svgb_attn_plan_local_varlen_t": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_kvcache_append": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll, _pll,
                             _vp],
+    "svgb_kvcache_append_e4m3": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll,
+                                 _pll, _vp, _vp, _vp],
     "svgb_attn_plan_kvcache_bytes": [_i, _i, _i, _i, _i, _i, _psz],
     "svgb_attn_plan_kvcache": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
@@ -61,6 +63,8 @@ _PROTOS = {
                           _vp, _vp],
     "svgb_attn_fwd_strided": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll, _pll, _f, _pplan,
                               _vp, _vp],
+    "svgb_attn_fwd_strided_e4m3": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll,
+                                   _pll, _f, _pplan, _vp, _vp],
     "svgb_quantize_e4m3": [_vp, _i, _vp, _vp, _i, _i, _i, _vp],
     "svgb_attn_bwd_bytes": [_i, _i, _psz],
     "svgb_attn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _f, _pplan, _vp, _pplan,

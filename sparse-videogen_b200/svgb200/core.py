@@ -282,20 +282,33 @@ def _cache_layout(B, block_table, cache_batch_idx):
 
 
 def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cache_seqlens, *,
-                   block_table: Optional[torch.Tensor] = None, cache_batch_idx: Optional[torch.Tensor] = None):
+                   block_table: Optional[torch.Tensor] = None, cache_batch_idx: Optional[torch.Tensor] = None,
+                   k_scale: Optional[torch.Tensor] = None, v_scale: Optional[torch.Tensor] = None):
     """Write the new rows k, v [B, Snew, Hkv, D] into the cache in place, at keys cache_seqlens[b] .. + Snew - 1 of each
     stream b, in one launch.  The cache is contiguous, k_cache / v_cache [B_cache, S_cache, Hkv, D] with stream b in
     row cache_batch_idx[b] (default b), or paged, [num_pages, page_size, Hkv, D] with block_table int [B, max_pages]
     (page_size a multiple of 128).  cache_seqlens: int or device int tensor [B], read on the device only.  Rows whose key
-    or block falls outside the cache are not written (include/svgb200.h, svgb_kvcache_append)."""
+    or block falls outside the cache are not written (include/svgb200.h, svgb_kvcache_append).
+    FP8 cache: caches of dtype torch.float8_e4m3fn take 16-bit k, v and k_scale, v_scale, float32 device tensors [Hkv]
+    fixed for the cache's lifetime; each element is stored as RN-satfinite(x * (1 / scale[h])), values past 448 * scale
+    saturating (svgb_kvcache_append_e4m3).  16-bit caches take no scales."""
     _need_cuda(k_cache, v_cache, k, v)
     if k_cache.dim() != 4 or k.dim() != 4 or k_cache.shape != v_cache.shape or k.shape != v.shape:
         raise SvgbError(f"kvcache_append: k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] and "
                         f"k, v {tuple(k.shape)} [B, Snew, Hkv, D], each pair of one shape")
     if k.shape[2:] != k_cache.shape[2:]:
         raise SvgbError(f"kvcache_append: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
-    if not (k_cache.dtype == v_cache.dtype == k.dtype == v.dtype):
-        raise SvgbError("kvcache_append: the caches and the new rows must share one dtype")
+    fp8 = k_cache.dtype == torch.float8_e4m3fn
+    if fp8:
+        if v_cache.dtype != k_cache.dtype or k.dtype != v.dtype:
+            raise SvgbError("kvcache_append: an e4m3 k_cache needs an e4m3 v_cache, and k, v of one 16-bit dtype")
+        scales = _fp8_scales("kvcache_append", k_scale, v_scale, k.shape[2])
+    else:
+        if k_scale is not None or v_scale is not None:
+            raise SvgbError("kvcache_append: k_scale / v_scale are for float8_e4m3fn caches; a "
+                            f"{k_cache.dtype} cache takes none")
+        if not (k_cache.dtype == v_cache.dtype == k.dtype == v.dtype):
+            raise SvgbError("kvcache_append: the caches and the new rows must share one dtype")
     dt = _dt(k)
     B, Snew, Hkv, D = k.shape
     if Snew == 0:
@@ -307,11 +320,30 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     k, v = (_addressed(t.transpose(1, 2), "bhsd") for t in (k, v))
     bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
     lens = _seqlens(cache_seqlens, B, k.device)
-    check(lib().svgb_kvcache_append(k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(), lens.data_ptr(),
-                                    _p(bi), _p(bt), dt, B, Snew, Hkv, D, k_cache.shape[0], k_cache.shape[1], max_pages,
-                                    _st(k_cache.transpose(1, 2), "bhsd"), _st(v_cache.transpose(1, 2), "bhsd"),
-                                    _st(k, "bhsd"), _st(v, "bhsd"), _stream(k)), "svgb_kvcache_append")
+    fill = 16 if fp8 else 8  # e4m3 cache strides are multiples of 16 bytes
+    args = (k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(), lens.data_ptr(), _p(bi), _p(bt), dt, B,
+            Snew, Hkv, D, k_cache.shape[0], k_cache.shape[1], max_pages, _st(k_cache.transpose(1, 2), "bhsd", fill),
+            _st(v_cache.transpose(1, 2), "bhsd", fill), _st(k, "bhsd"), _st(v, "bhsd"))
+    if fp8:
+        check(lib().svgb_kvcache_append_e4m3(*args, *(t.data_ptr() for t in scales), _stream(k)),
+              "svgb_kvcache_append_e4m3")
+    else:
+        check(lib().svgb_kvcache_append(*args, _stream(k)), "svgb_kvcache_append")
     _bump()
+
+
+def _fp8_scales(who, k_scale, v_scale, Hkv):
+    """The per-KV-head dequantisation scales of an e4m3 cache: both float32 device tensors [Hkv]."""
+    if k_scale is None or v_scale is None:
+        raise SvgbError(f"{who}: a float8_e4m3fn cache needs k_scale and v_scale (float32 [Hkv], one scale per key/value "
+                        "head)")
+    for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) != (Hkv,):
+            shown = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise SvgbError(f"{who}: {name} must be a float32 tensor [Hkv={Hkv}] (got {shown}"
+                            f"{', ' + str(t.dtype) if isinstance(t, torch.Tensor) else ''})")
+    _need_cuda(k_scale, v_scale)
+    return k_scale.contiguous(), v_scale.contiguous()
 
 
 def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0, cache_len: Optional[int] = None,
@@ -405,14 +437,15 @@ def _kv_group(q, k):
     return q.shape[1] // k.shape[1]
 
 
-def _strides(t, layout):
+def _strides(t, layout, fill=8):
     """(batch, head, row) element strides of an attention operand, as the strided entries take them; 'shd' is one batch
-    element.  A dimension of extent 1 is never stepped, so a stride there that the ABI would refuse is replaced by 8."""
+    element.  A dimension of extent 1 is never stepped, so a stride there that the ABI would refuse is replaced by fill:
+    8 elements for the 16-bit entries, 16 (bytes) for the e4m3 ones."""
     if layout == "bhsd":
         n, st = t.shape[:3], t.stride()[:3]
     else:
         n, st = (1, t.shape[1], t.shape[0]), (t.shape[1] * t.stride(1), t.stride(1), t.stride(0))
-    return tuple(8 if e == 1 and not (x and x % 8 == 0) else x for e, x in zip(n, st))
+    return tuple(fill if e == 1 and not (x and x % fill == 0) else x for e, x in zip(n, st))
 
 
 def _addressable(t, layout):
@@ -428,8 +461,8 @@ def _addressed(t, layout):
     return t if _addressable(t, layout) else t.clone(memory_format=torch.contiguous_format)
 
 
-def _st(t, layout):
-    return (C.c_longlong * 3)(*_strides(t, layout))
+def _st(t, layout, fill=8):
+    return (C.c_longlong * 3)(*_strides(t, layout, fill))
 
 
 def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
@@ -483,7 +516,8 @@ def _gqa_check(dtype, plan, rows=()):
 
 def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[torch.Tensor] = None,
              q_rows: Optional[torch.Tensor] = None, kv_rows: Optional[torch.Tensor] = None,
-             return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
+             return_lse: bool = False, sm_scale: Optional[float] = None, out: Optional[torch.Tensor] = None,
+             k_scale: Optional[torch.Tensor] = None, v_scale: Optional[torch.Tensor] = None):
     """layout 'bhsd': q,k,v [B,H,S,D];  'shd': [S,H,D] (ops API).  q, k, v may be views ([B, S, H, D] passed as
     x.transpose(1, 2), one of a packed projection's unbind(2), every other head, a batch slice): they are read in place
     when their last stride is 1, their base 16-byte aligned and their other strides nonzero multiples of 8 elements,
@@ -496,12 +530,16 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     variable-block plan (plan_varblock(..., S_kv=)), o has q's shape, and row vectors are not taken.
     k, v may have fewer heads than q, Hq = G * Hkv (grouped-query attention, FlashInfer's mapping: query head h attends
     with key/value head h // G): a variable-block plan is then built over the B * Hkv key/value heads and shared by
-    each group, band plans are shared by every head already; no row vectors, FP8 or gather plans."""
+    each group, band plans are shared by every head already; no row vectors, FP8 or gather plans.
+    k_scale, v_scale: the per-KV-head scales of float8_e4m3fn caches under a KV-cache plan (see _attn_kvcache)."""
     _need_cuda(q, k, v)
     if plan.desc.kind == PLAN_KVCACHE:
         if any(r is not None for r in (q_rows, kv_rows, o_rows)):
             raise SvgbError("a KV-cache plan (plan_kvcache) takes no row vectors (o_rows / q_rows / kv_rows)")
-        return _attn_kvcache(q, k, v, plan, return_lse, sm_scale, out)
+        return _attn_kvcache(q, k, v, plan, return_lse, sm_scale, out, k_scale, v_scale)
+    if k_scale is not None or v_scale is not None:
+        raise SvgbError("k_scale / v_scale are for float8_e4m3fn caches under a KV-cache plan (plan_kvcache); other "
+                        "FP8 attention takes attn_fwd_fp8")
     rows = (q_rows, kv_rows, o_rows)
     if any(r is not None for r in rows) or plan.desc.kind == PLAN_GATHER:
         # the row vectors and the row-gather kernel index one flat [BH, S, D] stride pair
@@ -525,9 +563,11 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     return (out, res[1]) if return_lse else out
 
 
-def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out):
+def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=None, v_scale=None):
     """attn_fwd under a KV-cache plan: q [B, Sq, Hq, D] as B * Sq packed rows, the cache [blocks, rows, Hkv, D] as
-    blocks * rows rows (both views), o [B, Sq, Hq, D] and lse [B, Hq, Sq] (flash_attn_with_kvcache's shapes)."""
+    blocks * rows rows (both views), o [B, Sq, Hq, D] and lse [B, Hq, Sq] (flash_attn_with_kvcache's shapes).
+    float8_e4m3fn caches (FP8 KV cache) take bf16 q, D = 128 and k_scale, v_scale float32 [Hkv]: q is quantised per
+    query head over the call's B * Sq rows (quantize_e4m3 on a transposed [Hq, B * Sq, D] copy) and o is bf16."""
     B, Sq = plan.source
     if q.dim() != 4 or q.shape[:2] != (B, Sq) or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
         raise SvgbError(f"a KV-cache plan for B={B} streams of Sq={Sq} queries takes q [B, Sq, Hq, D] (got "
@@ -536,6 +576,10 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out):
     if k_cache.shape[0] * k_cache.shape[1] != plan.S_kv:
         raise SvgbError(f"the KV-cache plan was built for {plan.S_kv} cache rows, the cache {tuple(k_cache.shape)} has "
                         f"{k_cache.shape[0] * k_cache.shape[1]}")
+    if k_cache.dtype == torch.float8_e4m3fn:
+        return _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale)
+    if k_scale is not None or v_scale is not None:
+        raise SvgbError(f"k_scale / v_scale are for float8_e4m3fn caches; a {k_cache.dtype} cache takes none")
     if not (q.dtype == k_cache.dtype == v_cache.dtype):
         raise SvgbError("q and the caches must share one dtype")
     if out is not None and (out.shape != q.shape or out.dtype != q.dtype):
@@ -552,6 +596,46 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out):
     if not return_lse:
         return o
     return o, res[1].view(Hq, B, Sq).transpose(0, 1)
+
+
+def _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
+    """_attn_kvcache on float8_e4m3fn caches: svgb_attn_fwd_strided_e4m3 with the cache read in place."""
+    B, Sq = plan.source
+    Hq, D = q.shape[2:]
+    Hkv = k_cache.shape[2]
+    if v_cache.dtype != torch.float8_e4m3fn:
+        raise SvgbError("an e4m3 k_cache needs an e4m3 v_cache")
+    if q.dtype != torch.bfloat16:
+        raise SvgbError(f"an FP8 KV cache takes bf16 q (got {q.dtype}); it is quantised per query head here, and the "
+                        "output is bf16")
+    if D != 128 or k_cache.shape[3] != 128:
+        raise SvgbError(f"an FP8 KV cache needs head_dim 128 (got q {D}, cache {k_cache.shape[3]}): 64-byte e4m3 rows "
+                        "have no 128-byte swizzle")
+    if Hq % Hkv:
+        raise SvgbError(f"q's {Hq} heads must be a multiple of the cache's {Hkv} key/value heads")
+    if out is not None and (out.shape != q.shape or out.dtype != torch.bfloat16):
+        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype bf16")
+    ks, vs = _fp8_scales("attn_fwd on an FP8 KV cache", k_scale, v_scale, Hkv)
+    # per query head over the B * Sq rows of this call: the scale kernel takes [heads, rows, D]
+    q8, q_scale = quantize_e4m3(q.reshape(B * Sq, Hq, D).transpose(0, 1).contiguous())
+    kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))  # [rows, Hkv, D] views, read in place
+    o = torch.empty(B * Sq, Hq, D, dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty(Hq, B * Sq, dtype=torch.float32, device=q.device) if return_lse else None
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    # q8 [Hq, B Sq, D] is one batch element; the cache and o are "shd" views, each at its own strides
+    check(lib().svgb_attn_fwd_strided_e4m3(q8.data_ptr(), kf.data_ptr(), vf.data_ptr(), q_scale.data_ptr(),
+                                           ks.data_ptr(), vs.data_ptr(), o.data_ptr(), _p(lse), 1, Hq, Hkv, B * Sq,
+                                           plan.S_kv, D, _st(q8[None], "bhsd", 16), _st(kf, "shd", 16), _st(vf, "shd", 16),
+                                           _st(o, "shd"), scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
+          "svgb_attn_fwd_strided_e4m3")
+    _bump()
+    o = o.view(B, Sq, Hq, D)
+    if out is not None:
+        out.copy_(o)
+        o = out
+    if not return_lse:
+        return o
+    return o, lse.view(Hq, B, Sq).transpose(0, 1)
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,

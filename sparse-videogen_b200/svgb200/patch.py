@@ -120,10 +120,16 @@ def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, m
                              layout="shd", sm_scale=softmax_scale)
 
 
+def _is_fp8(t) -> bool:
+    import torch
+
+    return getattr(t, "dtype", None) in (torch.float8_e4m3fn, torch.float8_e5m2)
+
+
 def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None, rotary_sin=None, cache_seqlens=None,
                             cache_batch_idx=None, cache_leftpad=None, block_table=None, softmax_scale=None, causal=False,
                             window_size=(-1, -1), softcap=0.0, rotary_interleaved=True, alibi_slopes=None,
-                            num_splits=0, return_softmax_lse=False):
+                            num_splits=0, return_softmax_lse=False, *, q_descale=None, k_descale=None, v_descale=None):
     """flash_attn.flash_attn_with_kvcache (FlashAttention 2's signature and return convention), forward only.
     q [B, Sq, Hq, D]; k_cache, v_cache [B_cache, S_cache, Hkv, D] (stream b in row cache_batch_idx[b], default b) or
     paged [num_pages, page_size, Hkv, D] with block_table int32 [B, max_pages] (page_size a multiple of 128).  k, v
@@ -133,7 +139,14 @@ def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None
     cache); nothing is read on the host.  Returns out [B, Sq, Hq, D], and lse [B, Hq, Sq] with return_softmax_lse.
     num_splits is a scheduling hint and is ignored; rotary_cos / rotary_sin, cache_leftpad, softcap and alibi_slopes
     other than their defaults raise SvgbError rather than being ignored (video models apply their own RoPE before
-    caching)."""
+    caching).
+    FP8 KV cache: k_cache, v_cache of dtype torch.float8_e4m3fn with k_descale, v_descale, keyword-only and named as in
+    FlashAttention 3, float32 [Hkv]: one dequantisation scale per key/value head for the whole cache (FlashAttention 3
+    takes [B, Hkv], one per stream, which is refused by shape).  q stays bf16 and is quantised per query head inside the
+    call; k, v stay 16-bit and are quantised by the append; out is bf16, D = 128.  An fp8 q, fp8 k / v and q_descale
+    are refused.  Without k_descale / v_descale the call makes exactly the 16-bit launches."""
+    import torch
+
     from . import core
     from .core import SvgbError
 
@@ -147,6 +160,23 @@ def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None
         raise SvgbError("flash_attn_with_kvcache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
     if (k is None) != (v is None):
         raise SvgbError("flash_attn_with_kvcache: k and v are given together or not at all")
+    if q_descale is not None:
+        raise SvgbError("flash_attn_with_kvcache: q_descale is not supported: q is bf16 and quantised per query head "
+                        "inside the call")
+    for name, t in (("q", q), ("k", k), ("v", v)):
+        if _is_fp8(t):
+            raise SvgbError(f"flash_attn_with_kvcache: {name} is {t.dtype}; q and the new k, v rows are 16-bit (an FP8 "
+                            "cache quantises them itself)")
+    for name, t in (("k_descale", k_descale), ("v_descale", v_descale)):
+        if t is not None and (not isinstance(t, torch.Tensor) or t.dim() != 1):
+            shown = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise SvgbError(f"flash_attn_with_kvcache: {name} must be [Hkv], one scale per key/value head for the whole "
+                            f"cache (got {shown}; FlashAttention 3's per-stream [B, Hkv] is not supported)")
+    given = k_descale is not None or v_descale is not None
+    if _is_fp8(k_cache) != given or (given and (k_descale is None or v_descale is None)):
+        raise SvgbError("flash_attn_with_kvcache: k_descale and v_descale (float32 [Hkv]) go together with a "
+                        "float8_e4m3fn cache, and only with one")
+    scales = dict(k_scale=k_descale, v_scale=v_descale) if given else {}
     B, Sq = q.shape[:2]
     if cache_seqlens is None:
         if block_table is not None:
@@ -154,13 +184,14 @@ def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None
         cache_seqlens = k_cache.shape[1]
     lens = core._seqlens(cache_seqlens, B, q.device)
     if k is not None:
-        core.kvcache_append(k_cache, v_cache, k, v, lens, block_table=block_table, cache_batch_idx=cache_batch_idx)
+        core.kvcache_append(k_cache, v_cache, k, v, lens, block_table=block_table, cache_batch_idx=cache_batch_idx,
+                            **scales)
     paged = block_table is not None
     plan = core.plan_kvcache(lens, q_len=Sq, num_blocks=k_cache.shape[0], new_len=0 if k is None else k.shape[1],
                              cache_len=None if paged else k_cache.shape[1], block_table=block_table,
                              page_size=k_cache.shape[1] if paged else None, cache_batch_idx=cache_batch_idx,
                              causal=causal, window_size=window_size)
-    return core.attn_fwd(q, k_cache, v_cache, plan, return_lse=return_softmax_lse, sm_scale=softmax_scale)
+    return core.attn_fwd(q, k_cache, v_cache, plan, return_lse=return_softmax_lse, sm_scale=softmax_scale, **scales)
 
 
 def _model_of(module):

@@ -11,6 +11,11 @@ Wan 1.3B (12 heads) and Wan 14B (40 heads).  Ways, each one call sequence as a c
                   as rolling caches do), the new rows written at the end, then plan + forward
   sdpa            torch scaled_dot_product_attention on the sliced cache under the same boolean mask (built once)
   decode          Sq = 1: one query against the same cache, plan + forward (one CTA per head: no split-KV)
+  fp8 paged       plan + forward on the same pages in e4m3 (per-KV-head scales), q quantised inside the call
+  fp8 append+paged  kvcache_append quantising the chunk's new rows into the e4m3 pages, then plan + forward
+  fp8 q quant     the q quantisation of the fp8 forward alone (a transposed copy and quantize_e4m3)
+
+Besides the times: the bytes of each cache (K and V, one layer) and mean / max |o_fp8 - o_bf16| of the paged forward.
 
 Each figure is the median of R rounds with the rounds' min and max; every round times N back-to-back calls of each way
 with CUDA events, the ways alternated within every round.  The card name and power limit are read in the same run.
@@ -113,14 +118,36 @@ def case(H, dev, rounds, iters):
         k, v = kc[:, :L].transpose(1, 2), vc[:, :L].transpose(1, 2)
         return torch.nn.functional.scaled_dot_product_attention(qt, k, v, attn_mask=mask)
 
+    # the e4m3 pages: per-KV-head absmax scales, the append's conversion
+    amax = lambda t: (t.float().abs().amax(dim=(0, 1, 3)) / 448).clamp_min(1e-12)  # noqa: E731
+    ks, vs = amax(kp), amax(vp)
+    e4m3 = lambda t, sc: (t.float() * (1 / sc)[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn)  # noqa: E731
+    kp8, vp8 = e4m3(kp, ks), e4m3(vp, vs)
+
+    def paged_fp8(new_len=0, seq=lens):
+        plan = core.plan_kvcache(seq, q_len=SQ, num_blocks=npages, new_len=new_len, block_table=table, page_size=PAGE,
+                                 **win)
+        return core.attn_fwd(q, kp8, vp8, plan, k_scale=ks, v_scale=vs)
+
+    def append_paged_fp8():
+        core.kvcache_append(kp8, vp8, knew, vnew, before, block_table=table, k_scale=ks, v_scale=vs)
+        return paged_fp8(new_len=SQ, seq=before)
+
+    def q_quant():
+        return core.quantize_e4m3(q.reshape(SQ, H, D).transpose(0, 1).contiguous())
+
     # the ways agree before they are timed
     o_c, o_p = contiguous(), paged()
     assert torch.equal(o_c, o_p), "paged and contiguous differ"
     err = (sdpa().transpose(1, 2).float() - o_c.float()).abs().max().item()
     assert err < 3e-2, f"sdpa differs by {err}"
+    d = (paged_fp8().float() - o_p.float()).abs()
+    fp8 = {"cache_bytes": {"bf16": 2 * kp.numel() * 2, "e4m3": 2 * kp8.numel()},
+           "o_abs_diff_vs_bf16": {"mean": d.mean().item(), "max": d.max().item()}}
     ways = {"contiguous": contiguous, "paged": paged, "append+paged": append_paged, "index+contig": index_contig,
-            "roll+contig": roll_contig, "sdpa": sdpa, "decode": lambda: paged(qq=q1)}
-    return alternate(ways, rounds, iters)
+            "roll+contig": roll_contig, "sdpa": sdpa, "decode": lambda: paged(qq=q1), "fp8 paged": paged_fp8,
+            "fp8 append+paged": append_paged_fp8, "fp8 q quant": q_quant}
+    return {**alternate(ways, rounds, iters), "fp8": fp8}
 
 
 def main():
