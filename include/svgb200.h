@@ -193,6 +193,20 @@ int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const 
                              int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                              const long long* vc_strides, const long long* k_strides, const long long* v_strides,
                              const float* k_scale, const float* v_scale, void* stream);
+/* Append into an e4m3 cache with per-row scales (the per-row FP8 KV cache): svgb_kvcache_append_e4m3's arguments with
+ * D = 128, where k_scale, v_scale are device float [num_blocks, Hkv, block_rows], contiguous and 16-byte aligned
+ * (block_rows a multiple of 4): scale [blk, h, row] belongs to cache row `row` of block `blk`, head h, and the append
+ * writes it.  A new row x (one position of one head, 128 values) with a = max|x| gets s = 2^e, e the smallest integer
+ * with a <= 448 * 2^e, clamped to [-126, 127] (a = 0: e = 0), and its elements are stored as RN(x * 2^-e) in e4m3, so
+ * nothing saturates and an overwrite computes a fresh scale.  Only the new rows and their scales are written, under
+ * svgb_kvcache_append's skip rules; a row with a non-finite value is unspecified.  Allocate the scale tensors with
+ * finite values (e.g. ones): rows past a stream's length in its last chunk are loaded and masked, like the cache bytes. */
+int svgb_kvcache_append_e4m3_rows(void* k_cache, void* v_cache, const void* k, const void* v,
+                                  const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                  const int32_t* block_table, int dtype, int B, int Snew, int Hkv, int D,
+                                  int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                                  const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                                  float* k_scale, float* v_scale, void* stream);
 /* Plan: stream b has L_b = min(cache_seqlens[b] + Snew, capacity) keys at logical positions 0 .. L_b - 1 (Snew: rows
  * appended before this attention), and Sq queries, query i at logical position L_b - Sq + i (FlashAttention's
  * bottom-right alignment).  Query p sees key kv when kv < sink, or when p - kv <= left and kv - p <= right (causal:
@@ -311,6 +325,26 @@ int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, cons
                                const long long* v_strides, const long long* o_strides, float sm_scale,
                                const svgb_plan* plan, const void* plan_ws, void* stream);
 int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D, void* stream);
+/* Attention into an e4m3 cache with per-row scales (svgb_kvcache_append_e4m3_rows):
+ *   q     : e4m3 [Sq, Hq, 128] (the packed queries of a KV-cache plan) with q_scale float [Hq, Sq], one scale per query
+ *           row and head (svgb_quantize_e4m3_rows);  k, v : the e4m3 cache as num_blocks * block_rows rows of Hkv heads,
+ *           with k_scale, v_scale float [num_blocks, Hkv, block_rows] (16-byte aligned, block_rows a multiple of 4).
+ *   x_strides : {batch, head, row} strides in elements (bytes for e4m3, multiples of 16; the batch stride is not
+ *           stepped);  o : bf16 [Sq, Hq, 128] at its strides (multiples of 8 elements);  lse : optional float [Hq, Sq].
+ *   s_ij = (q8_i . k8_j) * sq_i * sk_j * sm_scale and o_i = sum_j p_ij (v8_j * sv_j) / l_i, with P and the widened V
+ *   in bf16.  Query head hq attends with key/value head hq / (Hq / Hkv).
+ * SVGB_PLAN_KVCACHE plans only (every other kind is refused by name), D = 128.  Rows past a block's end in a chunk read
+ * zero scales; rows past a stream's length in its last chunk read the tensors and are masked. */
+int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v, const float* q_scale,
+                                    const float* k_scale, const float* v_scale, void* o, float* lse, int Hq, int Hkv,
+                                    int Sq, int num_blocks, int block_rows, int D, const long long* q_strides,
+                                    const long long* k_strides, const long long* v_strides, const long long* o_strides,
+                                    float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream);
+/* Per-row quantisation of 16-bit x [rows, H, 128], read at row_stride / head_stride (elements, multiples of 8; base
+ * 16-byte aligned), into e4m3 x8 [rows, H, 128] contiguous and scale float [H, rows], by the rule of
+ * svgb_kvcache_append_e4m3_rows; one launch.  A row's bytes and scale depend on that row alone. */
+int svgb_quantize_e4m3_rows(const void* x, int dtype, void* x8, float* scale, int rows, int H, int D,
+                            long long row_stride, long long head_stride, void* stream);
 
 /* Backward of svgb_attn_fwd: dq, dk, dv from q, k, v, the forward's o and natural-log lse, and the output gradient dO.
  *   q,k,v,o,dO,dq,dk,dv : [BH, S, D] 16-bit (SVGB_BF16 / SVGB_F16), D in {64,128}, all addressed with the one

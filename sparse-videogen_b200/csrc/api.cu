@@ -71,6 +71,22 @@ int encode_tmap_bhsd(CUtensorMap* map, const void* base, int dtype, int B, int H
   return encode_rows(map, base, dtype, 4, dims, s, 128);
 }
 
+int encode_tmap_scale_rows(CUtensorMap* map, const float* base, int num_blocks, int H, int block_rows) {
+  PFN_encodeTiled enc = get_encode();
+  SVGB_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && block_rows % 4 == 0,
+               "per-row scales must be 16-byte aligned with block_rows a multiple of 4");
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(block_rows), static_cast<cuuint64_t>(H),
+                              static_cast<cuuint64_t>(num_blocks)};
+  const cuuint64_t strides[2] = {static_cast<cuuint64_t>(block_rows) * 4, static_cast<cuuint64_t>(block_rows) * H * 4};
+  const cuuint32_t box[3] = {128, 1, 1}, estr[3] = {1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  SVGB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+  return 0;
+}
+
 }  // namespace svgb
 
 extern "C" {

@@ -366,6 +366,10 @@ struct AttnArgs {
   const void* k_ptr = nullptr;
   const void* v_ptr = nullptr;
   long long in_row_stride = 0, in_head_stride = 0;  // elements
+  // ---- per-row FP8 (attn_fwd_kernel<128, DT_E4M3_ROWS, false>, KV-cache plans): block_rows of the cache, which splits a
+  // chunk's physical row into (block, row) for its scale boxes; q_scale is then [BH, S] like the LSE and the K / V row
+  // scales come through their own tensor maps.  0 otherwise.
+  int scale_block_rows = 0;
 };
 
 }  // namespace svgb

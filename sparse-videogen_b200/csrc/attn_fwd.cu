@@ -504,13 +504,18 @@ selftest_tile_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_cons
       for (int v0 = 0; v0 < 2; ++v0) o_out[(row0 + 8 * v1) * D + 8 * jj + col0 + v0] = o[4 * jj + 2 * v1 + v0];
 }
 
+// ksm, vsm: the row-scale maps of DT_E4M3_ROWS, which has no row-gather instantiation
 template <int D, int DT>
 static int launch_attn(const CUtensorMap& qm, const CUtensorMap& km, const CUtensorMap& vm,
-                       const AttnArgs& args, bool gather, dim3 grid, cudaStream_t stream) {
+                       const AttnArgs& args, bool gather, dim3 grid, cudaStream_t stream,
+                       const CUtensorMap& ksm = CUtensorMap{}, const CUtensorMap& vsm = CUtensorMap{}) {
   using Cfg = AttnCfg<D, DT>;
-  auto kern = gather ? attn_fwd_kernel<D, DT, true> : attn_fwd_kernel<D, DT, false>;
+  auto kern = attn_fwd_kernel<D, DT, false>;
+  if constexpr (DT != DT_E4M3_ROWS) {
+    if (gather) kern = attn_fwd_kernel<D, DT, true>;
+  }
   SVGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args);
+  kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(qm, km, vm, args, ksm, vsm);
   SVGB_LAUNCH_OK();
   return 0;
 }
@@ -541,6 +546,13 @@ int attn_fwd_impl(const void* q, Strides qs, int Sq, const void* k, Strides ks, 
   dim3 grid(grid_x, BH);
   if (dtype == SVGB_E4M3) {
     SVGB_REQUIRE(D == 128, "the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle", D);
+    if (a.scale_block_rows > 0) {  // per-row scales: the cache is Skv / block_rows blocks (svgb_attn_fwd_kvcache_e4m3_rows)
+      CUtensorMap ksm, vsm;
+      const int nblk = Skv / a.scale_block_rows;
+      if (encode_tmap_scale_rows(&ksm, a.k_scale, nblk, Hkv, a.scale_block_rows)) return -1;
+      if (encode_tmap_scale_rows(&vsm, a.v_scale, nblk, Hkv, a.scale_block_rows)) return -1;
+      return launch_attn<128, DT_E4M3_ROWS>(qm, km, vm, args, false, grid, st, ksm, vsm);
+    }
     return launch_attn<128, DT_E4M3>(qm, km, vm, args, gather, grid, st);
   }
   if (D == 128) {
@@ -687,7 +699,7 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
                         const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
                         const int32_t* o_rows, int dtype, int B, int BH, int kv_group, int Sq, int Skv, int D,
                         Strides qs, Strides ks, Strides vs, Strides os, float sm_scale, const svgb_plan* plan,
-                        const void* plan_ws, void* stream) {
+                        const void* plan_ws, void* stream, int scale_block_rows = 0) {
   SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
   SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
                "fp8 attention needs the three per-head scale vectors");
@@ -746,6 +758,7 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.v_ptr = v;
   a.in_row_stride = qs.r;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
   a.in_head_stride = qs.h;
+  a.scale_block_rows = scale_block_rows;
   return attn_fwd_impl(q, qs, Sq, k, ks, v, vs, Skv, dtype, B, BH, D, a, gather, plan->max_items,
                        static_cast<cudaStream_t>(stream));
 }
@@ -943,6 +956,35 @@ int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, cons
   if (attn_group_plan_check(B * Hkv, Sq, Skv, plan, who)) return -1;
   return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, B, B * Hq,
                       Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, stream);
+}
+
+int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v, const float* q_scale,
+                                    const float* k_scale, const float* v_scale, void* o, float* lse, int Hq, int Hkv,
+                                    int Sq, int num_blocks, int block_rows, int D, const long long* q_strides,
+                                    const long long* k_strides, const long long* v_strides, const long long* o_strides,
+                                    float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
+  const char* who = "svgb_attn_fwd_kvcache_e4m3_rows";
+  SVGB_REQUIRE(plan, "null pointer");
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_KVCACHE,
+               "%s takes KV-cache plans (svgb_attn_plan_kvcache) only (kind %d): per-row scales live beside the cache "
+               "rows", who, plan->kind);
+  SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
+               who, D);
+  SVGB_REQUIRE(q_scale, "%s needs the query row scales q_scale (float [Hq, Sq])", who);
+  if (kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
+  SVGB_REQUIRE(num_blocks > 0 && block_rows > 0 && static_cast<long long>(num_blocks) * block_rows < (1ll << 31),
+               "%s: bad cache geometry (num_blocks=%d, block_rows=%d)", who, num_blocks, block_rows);
+  Strides st[4];
+  if (attn_strided_check(1, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st, who)) return -1;
+  for (int i = 0; i < 3; ++i)
+    SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
+                 "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
+                 st[i].b, st[i].h, st[i].r);
+  SVGB_REQUIRE(Hq % Hkv == 0, "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d", who, Hq,
+               Hkv);
+  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, 1, Hq,
+                      Hq / Hkv, Sq, num_blocks * block_rows, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws,
+                      stream, block_rows);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

@@ -20,6 +20,10 @@
 // each V tile to fp16 in shared memory (two buffers, with their own full and empty barriers) and P V runs in fp16.
 // Both loaders serve e4m3: the row gather copies 128-byte e4m3 rows into the same swizzled image TMA writes, and
 // the widening step that follows is shared.
+// Per-row FP8 (DT_E4M3_ROWS, KV-cache plans only): every q, k and v row has its own power-of-two scale (fp8_rows.cuh).
+// The K and V scales of a chunk (128 floats each) land with its K and V tiles, in the same TMA transactions; the
+// consumers multiply each S column by its K scale before the row max, each row's c carries its q scale, and the
+// producer's widening multiplies every V row by its scale and writes bf16, so P V runs in bf16 (DESIGN.md).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -34,8 +38,9 @@
 
 namespace svgb {
 
-// element type of Q/K/V: 0 = bf16, 1 = fp16, 2 = fp8 e4m3 (output bf16)
-constexpr int DT_BF16 = 0, DT_F16 = 1, DT_E4M3 = 2;
+// element type of Q/K/V: 0 = bf16, 1 = fp16, 2 = fp8 e4m3 with per-head scales, 3 = fp8 e4m3 with per-row scales
+// (both output bf16)
+constexpr int DT_BF16 = 0, DT_F16 = 1, DT_E4M3 = 2, DT_E4M3_ROWS = 3;
 // K/V stages: with P V(j) still running when Q K(j+1)^T is issued, V(j) frees late in iteration j, so the load of
 // chunk j+3 into its stage gets about two chunks of lead time
 constexpr int kKvStages = 3;
@@ -43,18 +48,24 @@ constexpr int kKvStages = 3;
 template <int D, int DT = DT_BF16>
 struct AttnCfg {
   static_assert(D == 64 || D == 128, "head_dim must be 64 or 128");
-  static_assert(DT != DT_E4M3 || D == 128, "the e4m3 path is built for head_dim 128 (128-byte rows)");
-  static constexpr int kElemBytes = DT == DT_E4M3 ? 1 : 2;
+  static_assert(DT < DT_E4M3 || D == 128, "the e4m3 path is built for head_dim 128 (128-byte rows)");
+  static constexpr int kElemBytes = DT >= DT_E4M3 ? 1 : 2;
   static constexpr int kRowBytes = D * kElemBytes;
   static constexpr int kHalves = kRowBytes / 128;        // 128-byte swizzle panels per row
   static constexpr int kPanelElems = 128 / kElemBytes;   // elements per panel row (TMA box width)
   static constexpr int kPanelBytes = 128 * 128;          // 128 rows x 128 B
   static constexpr int kTileBytes = kPanelBytes * kHalves;
   static constexpr int kKSteps = kRowBytes / 32;         // wgmma K steps of Q K^T (32 bytes each)
-  static constexpr int kVhBytes = DT == DT_E4M3 ? 2 * kPanelBytes : 0;  // fp16 copy of one e4m3 V tile
+  static constexpr int kVhBytes = DT >= DT_E4M3 ? 2 * kPanelBytes : 0;  // 16-bit copy of one e4m3 V tile
+  // per-row FP8 (KV-cache plans, TMA loader only).  The kernel reads these here rather than from locals of its own:
+  // extra local constants in attn_fwd_kernel change the register allocation of the per-head e4m3 instantiation.
+  static constexpr bool kRows = DT == DT_E4M3_ROWS;
+  static constexpr int kScaleRowBytes = 128 * 4;                             // one chunk's K (or V) row scales
+  static constexpr int kScaleBytes = kRows ? kKvStages * 2 * kScaleRowBytes : 0;  // per stage: K, V row scales
   static constexpr int kBarBytes = 1024;                 // mbarriers + gather row table
   // + 1 KB: the kernel aligns the dynamic window to 1024 bytes itself
-  static constexpr int kSmemBytes = 1024 + kTileBytes + 2 * kKvStages * kTileBytes + 2 * kVhBytes + kBarBytes;
+  static constexpr int kSmemBytes =
+      1024 + kTileBytes + 2 * kKvStages * kTileBytes + 2 * kVhBytes + kScaleBytes + kBarBytes;
   static constexpr int kThreads = 384;  // producer warpgroup + two consumer warpgroups
   static_assert(kSmemBytes <= 227 * 1024, "exceeds the 227 KB per-CTA shared memory of sm_90");
 };
@@ -73,7 +84,7 @@ __device__ __forceinline__ void attn_qk_issue(float (&s)[64], uint32_t sQw, uint
   for (int kk = 0; kk < Cfg::kKSteps; ++kk) {
     const uint32_t off = (kk >> 2) * Cfg::kPanelBytes + (kk & 3) * 32;
     const uint64_t a = wg_desc_kmajor(sQw + off), b = wg_desc_kmajor(sK + off);
-    if constexpr (DT == DT_E4M3) wgmma_m64n128k32_e4m3_ss(s, a, b, kk > 0);
+    if constexpr (DT >= DT_E4M3) wgmma_m64n128k32_e4m3_ss(s, a, b, kk > 0);
     else wgmma_m64n128k16_ss<DT == DT_BF16>(s, a, b, kk > 0);
   }
   wg_commit();
@@ -109,6 +120,19 @@ __device__ __forceinline__ void attn_wait(float (&d)[M]) {
   wg_fence_regs(d);
 }
 
+// Per-row FP8: 16 e4m3 values of one V row -> bf16(v8 * sv), sv = 2^e its scale.  e4m3 -> fp16 -> fp32 are exact, the
+// product is an exponent shift, and the bf16 rounding is exact wherever the result lies in bf16's range (DESIGN.md).
+__device__ __forceinline__ void widen_rows(const uint32_t (&in)[4], uint32_t (&out)[8], float sv) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const __half2_raw h2 =
+        __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>((in[k >> 1] >> (16 * (k & 1))) & 0xffffu), __NV_E4M3);
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h2));
+    const __nv_bfloat162 b2 = __floats2bfloat162_rn(f.x * sv, f.y * sv);
+    out[k] = *reinterpret_cast<const uint32_t*>(&b2);
+  }
+}
+
 // mbarriers of the producer / consumer protocol.  A full barrier completes once its data has landed: one arrival
 // with the transaction bytes from the TMA-issuing thread, or (row gather) one cp.async arrival from each of the
 // producer's 128 threads.  An empty barrier completes once both consumers are done with the buffer: one arrival
@@ -128,15 +152,18 @@ constexpr int kBarProducer = 1, kBarTurn = 2;  // consumer c waits for its turn 
 constexpr int kProducerRegs = 24, kConsumerRegs = 240;
 
 // kGather selects the loader: false = TMA boxes over contiguous key ranges (chunk list), true = cp.async
-// row gathers over a run list.
+// row gathers over a run list.  ksmap, vsmap: DT_E4M3_ROWS only, the K and V row scales [num_blocks, Hkv, block_rows]
+// as (row, head, block), box 128 x 1 x 1 fp32.
 template <int D, int DT, bool kGather>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant__ CUtensorMap kmap,
-                const __grid_constant__ CUtensorMap vmap, const AttnArgs args) {
+                const __grid_constant__ CUtensorMap vmap, const AttnArgs args,
+                const __grid_constant__ CUtensorMap ksmap, const __grid_constant__ CUtensorMap vsmap) {
   using Cfg = AttnCfg<D, DT>;
   constexpr bool BF16 = DT != DT_F16;  // output format (fp8 inputs produce bf16 output)
-  constexpr bool FP8 = DT == DT_E4M3;
-  constexpr bool kPBF16 = DT == DT_BF16;  // format of P and V in the P V product (fp8: fp16)
+  constexpr bool FP8 = DT >= DT_E4M3;
+  // format of P and V in the P V product (fp8: fp16 with per-head scales, bf16 with per-row scales)
+  constexpr bool kPBF16 = DT == DT_BF16 || Cfg::kRows;
   using Elem = typename std::conditional<FP8, uint8_t, uint16_t>::type;  // storage element of Q / K / V
   const int bh = blockIdx.y;  // query head: Q, O, LSE
   // key/value head: K, V and the plan's work list.  Gather plans take no groups (their kv_rows are per query head; the
@@ -153,8 +180,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   const uint32_t sQ = base;
   const uint32_t sK0 = sQ + Cfg::kTileBytes;  // stage s: K at sK0 + 2s*tile, V at sK0 + (2s+1)*tile
   const uint32_t sVh = sK0 + 2 * kKvStages * Cfg::kTileBytes;  // FP8: buffer b at sVh + b*kVhBytes
-  AttnSmemCtl* ctl =
-      reinterpret_cast<AttnSmemCtl*>(smem_al + Cfg::kTileBytes * (1 + 2 * kKvStages) + 2 * Cfg::kVhBytes);
+  // ROWS: stage s's K row scales at sSc + 2s * 512, its V row scales 512 bytes after them
+  const uint32_t sSc = sVh + 2 * Cfg::kVhBytes;
+  AttnSmemCtl* ctl = reinterpret_cast<AttnSmemCtl*>(smem_al + Cfg::kTileBytes * (1 + 2 * kKvStages) +
+                                                    2 * Cfg::kVhBytes + Cfg::kScaleBytes);
 
   const int tid = threadIdx.x;
   // the warpgroup index through a shuffle, so that ptxas sees it is warp-uniform and splits the register allocation
@@ -167,7 +196,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     mbar_init(smem_u32(&ctl->q_empty), 2);
     for (int i = 0; i < kKvStages; ++i) {
       mbar_init(smem_u32(&ctl->k_full[i]), full_count);
-      mbar_init(smem_u32(&ctl->k_empty[i]), 2);
+      // ROWS: the consumers also read the stage's K scales, so each of their 8 warps releases it
+      mbar_init(smem_u32(&ctl->k_empty[i]), Cfg::kRows ? 8 : 2);
       mbar_init(smem_u32(&ctl->v_full[i]), full_count);
       mbar_init(smem_u32(&ctl->v_empty[i]), 2);
     }
@@ -180,6 +210,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       tma_prefetch_desc(&qmap);
       tma_prefetch_desc(&kmap);
       tma_prefetch_desc(&vmap);
+    }
+    if constexpr (Cfg::kRows) {
+      tma_prefetch_desc(&ksmap);
+      tma_prefetch_desc(&vsmap);
     }
   }
   __syncthreads();  // the barriers are initialised; the last block-wide barrier of the kernel
@@ -206,6 +240,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   // streams) lives in K/V stage n % 3, phase (n / 3) & 1 of that stage's barriers; FP8: its fp16 V copy in buffer
   // n & 1, phase (n / 2) & 1.  An empty barrier's wait for round r is on parity (r & 1) ^ 1: round 0 passes at once.
   auto stage_k = [&](int n) { return sK0 + 2 * (n % kKvStages) * Cfg::kTileBytes; };
+  auto stage_ks = [&](int n) { return sSc + 2 * (n % kKvStages) * Cfg::kScaleRowBytes; };  // ROWS: K scales; V: + 512
   auto vh_buf = [&](int n) { return sVh + (n & 1) * Cfg::kVhBytes; };
 
   if (wg == 0) {
@@ -260,12 +295,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         const uint4 w = *reinterpret_cast<const uint4*>(smem_al + (sV - base) + r * 128 + ((pc ^ (r & 7)) << 4));
         const uint32_t in[4] = {w.x, w.y, w.z, w.w};
         uint32_t out[8];
+        if constexpr (Cfg::kRows) widen_rows(in, out, *reinterpret_cast<const float*>(smem_al + (stage_ks(n) - base) +
+                                                                                 Cfg::kScaleRowBytes + 4 * r));
+        else {
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(in[k] & 0xffffu), __NV_E4M3);
           const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(in[k] >> 16), __NV_E4M3);
           out[2 * k] = static_cast<uint32_t>(lo.x) | (static_cast<uint32_t>(lo.y) << 16);
           out[2 * k + 1] = static_cast<uint32_t>(hi.x) | (static_cast<uint32_t>(hi.y) << 16);
+        }
         }
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
@@ -322,12 +361,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
           named_bar_sync(kBarProducer, 128);  // ctl->src is reused by the next resolve
         } else if (leader) {
           const int kv0 = __ldg(&sm.list[j].x);
+          // ROWS: the chunk's scales at (row, head, block) of its physical row kv0; rows past the block's end are
+          // outside the scale map and TMA fills them with zeros
+          int srow = 0, sblk = 0;
+          if constexpr (Cfg::kRows) {
+            sblk = kv0 / args.scale_block_rows;
+            srow = kv0 - sblk * args.scale_block_rows;
+          }
           mbar_wait(smem_u32(&ctl->k_empty[s]), par, 6);
-          mbar_expect_tx(kf, Cfg::kTileBytes);
+          mbar_expect_tx(kf, Cfg::kTileBytes + (Cfg::kRows ? Cfg::kScaleRowBytes : 0));
           for (int x = 0; x < Cfg::kHalves; ++x) tma_load_4d(sK + x * Cfg::kPanelBytes, &kmap, kf, x * Cfg::kPanelElems, kv0, hkv, batch);
+          if constexpr (Cfg::kRows) tma_load_3d(stage_ks(n), &ksmap, kf, srow, hkv, sblk);
           mbar_wait(smem_u32(&ctl->v_empty[s]), par, 7);
-          mbar_expect_tx(vf, Cfg::kTileBytes);
+          mbar_expect_tx(vf, Cfg::kTileBytes + (Cfg::kRows ? Cfg::kScaleRowBytes : 0));
           for (int x = 0; x < Cfg::kHalves; ++x) tma_load_4d(sV + x * Cfg::kPanelBytes, &vmap, vf, x * Cfg::kPanelElems, kv0, hkv, batch);
+          if constexpr (Cfg::kRows) tma_load_3d(stage_ks(n) + Cfg::kScaleRowBytes, &vsmap, vf, srow, hkv, sblk);
         }
         // FP8: widen the previous chunk's V, requested one chunk earlier, rather than wait here for V(j) to land
         if constexpr (FP8) {
@@ -347,9 +395,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   const uint32_t sQw = sQ + 64 * cw * 128;
   // FP8: q_scale per query head, k_scale and v_scale per key/value head (a group's query heads share its K and V).
   // 16-bit inputs take no scales; their instantiations keep indexing by bh, so their code does not depend on kvh.
+  // ROWS: the row scales take their place (c_row below, the K scales on S, the V scales in the widening).
   const int sh = FP8 ? kvh : bh;
-  const float c = args.scale_log2 * (args.q_scale ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[sh]) : 1.f);
-  const float vs = args.v_scale ? __ldg(&args.v_scale[sh]) : 1.f;
+  const float c = args.scale_log2 * ((!Cfg::kRows && args.q_scale) ? __ldg(&args.q_scale[bh]) * __ldg(&args.k_scale[sh]) : 1.f);
+  const float vs = (!Cfg::kRows && args.v_scale) ? __ldg(&args.v_scale[sh]) : 1.f;
   const int mode = args.mask_mode, m0 = args.m0, m1 = args.m1, m2 = args.m2;
 
   // Turns on the tensor cores: each consumer issues its wgmma groups between turn_wait and turn_pass, so the two
@@ -359,6 +408,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
   // thread 0 of the warpgroup arrives for it, after the warpgroup's wgmma reading the buffer has retired
   auto release = [&](uint64_t& bar) {
     if (wt == 0) mbar_arrive(smem_u32(&bar));
+  };
+  // a K stage is free once the warpgroup's Q K^T has retired and (ROWS) each warp has read the stage's K scales
+  auto release_k = [&](int n) {
+    if constexpr (Cfg::kRows) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&ctl->k_empty[n % kKvStages]));
+    } else {
+      release(ctl->k_empty[n % kKvStages]);
+    }
   };
   if (cw == 1) turn_pass();
 
@@ -397,6 +455,19 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       }
       em.init(mode, qm, so.sink_end, m1, m2);
     }
+    // ROWS: c of each of the thread's two rows carries the row's q scale, q_scale [Hq, S] (rows past nr: never stored)
+    float c_row[2] = {0.f, 0.f};
+    if constexpr (Cfg::kRows) {
+#pragma unroll
+      for (int v1 = 0; v1 < 2; ++v1) {
+        const int row = rloc + 8 * v1;
+        c_row[v1] = c * (row < nr ? __ldg(&args.q_scale[static_cast<size_t>(bh) * args.S + q0 + row]) : 1.f);
+      }
+    }
+    auto crow = [&](int v1) {
+      if constexpr (Cfg::kRows) return c_row[v1];
+      else return c;
+    };
     float o[D / 2];
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
@@ -404,6 +475,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     float s[64];        // S of the chunk being scored, then its P
     uint32_t pa[8][4];  // P of the chunk whose P V is next, packed to 16 bit
 
+    // ROWS: S column 8 jj + 2 (lane % 4) + v0 times the K scale of its key row (chunk n's stage)
+    auto scale_k = [&](int n) {
+      if constexpr (Cfg::kRows) {
+        const float* ks = reinterpret_cast<const float*>(smem_al + (stage_ks(n) - base)) + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const float2 k2 = *reinterpret_cast<const float2*>(ks + 8 * jj);
+#pragma unroll
+          for (int v1 = 0; v1 < 2; ++v1) {
+            s[4 * jj + 2 * v1] *= k2.x;
+            s[4 * jj + 2 * v1 + 1] *= k2.y;
+          }
+        }
+      }
+    };
     // mask and online softmax of chunk j (scores in log2 units: x * c): S -> P, running max and sum, alpha = the
     // factor O still has to be scaled by before P(j) V(j) is accumulated
     auto softmax = [&](int j) {
@@ -443,15 +529,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
         const float m_new = fmaxf(m_run[v1], mx);
-        const float mc = m_new == -INFINITY ? 0.f : m_new * c;
-        alpha[v1] = ex2_approx(m_run[v1] == -INFINITY ? -INFINITY : m_run[v1] * c - mc);
+        const float mc = m_new == -INFINITY ? 0.f : m_new * crow(v1);
+        alpha[v1] = ex2_approx(m_run[v1] == -INFINITY ? -INFINITY : m_run[v1] * crow(v1) - mc);
         m_run[v1] = m_new;
         float ls = 0.f;
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
           for (int v0 = 0; v0 < 2; ++v0) {
-            const float p = ex2_approx(fmaf(s[4 * jj + 2 * v1 + v0], c, -mc));
+            const float p = ex2_approx(fmaf(s[4 * jj + 2 * v1 + v0], crow(v1), -mc));
             s[4 * jj + 2 * v1 + v0] = p;
             ls += p;
           }
@@ -478,7 +564,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       attn_qk_issue<D, DT>(s, sQw, stage_k(g));
       turn_pass();
       attn_wait<0>(s);
-      release(ctl->k_empty[g % kKvStages]);
+      scale_k(g);
+      release_k(g);
       if (nch == 1) release(ctl->q_empty);
       softmax(0);
       rescale_pack();
@@ -493,7 +580,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         attn_pv_issue<D, kPBF16>(o, pa, pv_b(n));      // group B: O and pa stay in flight
         turn_pass();
         attn_wait<1>(s);                               // A has retired, B may still be running
-        release(ctl->k_empty[(n + 1) % kKvStages]);
+        scale_k(n + 1);
+        release_k(n + 1);
         if (j + 2 == nch) release(ctl->q_empty);       // the stream's last Q K^T has retired
         softmax(j + 1);                                // runs under P V(j)
         // ptxas schedules wgmma.wait_group ahead of register math that does not depend on it, which would move
@@ -551,7 +639,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       }
       if (args.lse && (lane & 3) == 0) {
         // natural-log LSE of the scaled scores; -inf for rows that saw no key
-        const float lse = l > 0.f ? (m_run[v1] * c + log2f(l)) * 0.6931471805599453f : -INFINITY;
+        const float lse = l > 0.f ? (m_run[v1] * crow(v1) + log2f(l)) * 0.6931471805599453f : -INFINITY;
         args.lse[static_cast<size_t>(bh) * args.S + out_row] = lse;
       }
     }

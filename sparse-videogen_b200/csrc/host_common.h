@@ -63,6 +63,13 @@ inline Strides flat_strides(long long rs, long long hs, int BH) { return {BH * h
 // box = one 128-byte panel x 128 rows x 1 x 1, 128-byte swizzle.  Returns 0 on success.
 int encode_tmap_bhsd(CUtensorMap* map, const void* base, int dtype, int B, int H, int S, int D, Strides st);
 
+// 3-D TMA descriptor over per-row scales, float [num_blocks, H, block_rows] contiguous, addressed as (row, head, block),
+// box = 128 x 1 x 1, no swizzle; rows past block_rows are filled with zeros.  Returns 0 on success.
+int encode_tmap_scale_rows(CUtensorMap* map, const float* base, int num_blocks, int H, int block_rows);
+
+// the per-row scale tensors of an e4m3 cache (kvcache.cu): both given, 16-byte aligned, block_rows a multiple of 4
+int kv_scale_rows_check(const float* k_scale, const float* v_scale, int block_rows, const char* who);
+
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
 // BH (svgb200.h); every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) {

@@ -1,6 +1,7 @@
-// KV cache: the in-place append of new key / value rows (svgb_kvcache_append, and svgb_kvcache_append_e4m3 into an
-// e4m3 cache) and the plan of the attention of a batch
-// of streams into a contiguous or paged cache (svgb_attn_plan_kvcache), run by the attention forward (attn_kernel.cuh).
+// KV cache: the in-place append of new key / value rows (svgb_kvcache_append, and svgb_kvcache_append_e4m3 and
+// svgb_kvcache_append_e4m3_rows into an e4m3 cache with per-head or per-row scales) and the plan of the attention of a
+// batch of streams into a contiguous or paged cache (svgb_attn_plan_kvcache), run by the attention forward
+// (attn_kernel.cuh).
 // Both read the per-stream lengths on the device only.
 #include <cuda_fp16.h>
 
@@ -9,6 +10,7 @@
 
 #include "../../include/svgb200.h"
 #include "attn_common.cuh"
+#include "fp8_rows.cuh"
 #include "host_common.h"
 
 namespace svgb {
@@ -30,8 +32,9 @@ __device__ __forceinline__ int kv_block(const int* __restrict__ batch_idx, const
   return min(max(blk, 0), nblocks - 1);
 }
 
-// what the append writes from 16-bit new rows: the rows themselves, or e4m3 quantised from bf16 or fp16 rows
-enum KvStore { KV_COPY, KV_E4M3_BF16, KV_E4M3_F16 };
+// what the append writes from 16-bit new rows: the rows themselves, e4m3 quantised from bf16 or fp16 rows with the
+// caller's per-head scales, or e4m3 quantised with a power-of-two scale per row, written beside the row (fp8_rows.cuh)
+enum KvStore { KV_COPY, KV_E4M3_BF16, KV_E4M3_F16, KV_E4M3_ROWS_BF16, KV_E4M3_ROWS_F16 };
 
 // 8 16-bit elements -> 8 e4m3 bytes, RN-satfinite(x * inv), as quantize_kernel (quant_fp8.cu)
 template <bool BF16>
@@ -64,7 +67,8 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
                  const uint16_t* __restrict__ v, const int* __restrict__ seqlens, const int* __restrict__ batch_idx,
                  const int* __restrict__ table, int B, int Snew, int Hkv, int nvec, int nblocks, int block_rows,
                  int max_pages, int cap, Strides kcs, Strides vcs, Strides ks, Strides vs,
-                 const float* __restrict__ k_scale, const float* __restrict__ v_scale) {
+                 const float* __restrict__ k_scale, const float* __restrict__ v_scale, float* __restrict__ k_rows,
+                 float* __restrict__ v_rows) {
   const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -91,12 +95,25 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
     if constexpr (kStore == KV_COPY) {
       *reinterpret_cast<uint4*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) = kx;
       *reinterpret_cast<uint4*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) = vx;
-    } else {
+    } else if constexpr (kStore == KV_E4M3_BF16 || kStore == KV_E4M3_F16) {
       constexpr bool BF16 = kStore == KV_E4M3_BF16;
       *reinterpret_cast<uint2*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) =
           kv_to_e4m3<BF16>(kx, 1.f / __ldg(&k_scale[h]));
       *reinterpret_cast<uint2*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) =
           kv_to_e4m3<BF16>(vx, 1.f / __ldg(&v_scale[h]));
+    } else {
+      // per row (D = 128, nvec = 16): the 16 threads of a (row, head) are an aligned half-warp, since the block size
+      // and the grid stride are multiples of 16, and every skip above is uniform over them
+      constexpr bool BF16 = kStore == KV_E4M3_ROWS_BF16;
+      const unsigned half = 0xffffu << (threadIdx.x & 16);
+      int ek, ev;
+      *reinterpret_cast<uint2*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) = e4m3_row_quantise<BF16>(kx, half, &ek);
+      *reinterpret_cast<uint2*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) = e4m3_row_quantise<BF16>(vx, half, &ev);
+      if (c == 0) {
+        const long long si = (static_cast<long long>(blk) * Hkv + h) * block_rows + row;  // [num_blocks, Hkv, block_rows]
+        k_rows[si] = e4m3_row_scale(ek);
+        v_rows[si] = e4m3_row_scale(ev);
+      }
     }
   }
 }
@@ -211,17 +228,34 @@ static int kv_geometry(const int32_t* cache_batch_idx, const int32_t* block_tabl
 
 using namespace svgb;
 
-// both appends: 16-bit new rows (dtype) into a 16-bit cache of that dtype, or (k_scale, v_scale given) into an e4m3 cache
+// the per-row scale tensors of an e4m3 cache, float [num_blocks, Hkv, block_rows] contiguous: one 128-key chunk of one
+// head is 512 contiguous bytes that the attention loads with one TMA box, whose rows need 16-byte alignment
+int svgb::kv_scale_rows_check(const float* k_scale, const float* v_scale, int block_rows, const char* who) {
+  SVGB_REQUIRE(k_scale && v_scale, "%s needs both per-row scale tensors k_scale and v_scale (float [num_blocks, Hkv, "
+               "block_rows])", who);
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(k_scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(v_scale) & 15) == 0,
+               "%s: the per-row scale tensors must be 16-byte aligned", who);
+  SVGB_REQUIRE(block_rows % 4 == 0,
+               "%s: per-row scales need block_rows (%d) a multiple of 4, so that every scale row is 16-byte aligned", who,
+               block_rows);
+  return 0;
+}
+
+// every append: 16-bit new rows (dtype) into a 16-bit cache of that dtype, or into an e4m3 cache with the per-head
+// scales k_scale, v_scale, or (k_rows, v_rows given) with per-row scales the append writes
 static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
                          const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew,
                          int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                          const long long* vc_strides, const long long* k_strides, const long long* v_strides,
-                         const float* k_scale, const float* v_scale, void* stream, const char* who) {
-  const bool e4m3 = k_scale != nullptr;
+                         const float* k_scale, const float* v_scale, float* k_rows, float* v_rows, void* stream,
+                         const char* who) {
+  const bool rows = k_rows != nullptr;
+  const bool e4m3 = k_scale != nullptr || rows;
   SVGB_REQUIRE(cache_seqlens, "null pointer");
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "%s takes bf16 or fp16 %s (dtype %d)", who,
                e4m3 ? "new rows" : "caches", dtype);
   SVGB_REQUIRE(D == 64 || D == 128, "%s: head_dim %d unsupported (64 or 128)", who, D);
+  SVGB_REQUIRE(!rows || D == 128, "%s: per-row scales need head_dim 128 (got %d)", who, D);
   SVGB_REQUIRE(Snew > 0, "%s: no new rows (Snew=%d)", who, Snew);
   Strides st[4];
   if (attn_strided_check(B, Hkv, Hkv, {k_cache, v_cache, k, v}, {kc_strides, vc_strides, k_strides, v_strides}, st, who))
@@ -242,12 +276,17 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
     kv_append_kernel<KV_COPY><<<blocks, 256, 0, cs>>>(
         static_cast<uint16_t*>(k_cache), static_cast<uint16_t*>(v_cache), kn, vn, cache_seqlens, cache_batch_idx,
         block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages, cap, st[0], st[1], st[2], st[3], nullptr,
-        nullptr);
+        nullptr, nullptr, nullptr);
+  } else if (rows) {
+    auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_ROWS_BF16> : kv_append_kernel<KV_E4M3_ROWS_F16>;
+    kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
+                                 cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages,
+                                 cap, st[0], st[1], st[2], st[3], nullptr, nullptr, k_rows, v_rows);
   } else {
     auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_BF16> : kv_append_kernel<KV_E4M3_F16>;
     kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
                                  cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages,
-                                 cap, st[0], st[1], st[2], st[3], k_scale, v_scale);
+                                 cap, st[0], st[1], st[2], st[3], k_scale, v_scale, nullptr, nullptr);
   }
   SVGB_LAUNCH_OK();
   return 0;
@@ -262,7 +301,7 @@ int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void*
                         void* stream) {
   return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
                        num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
-                       nullptr, stream, "svgb_kvcache_append");
+                       nullptr, nullptr, nullptr, stream, "svgb_kvcache_append");
 }
 
 int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
@@ -274,7 +313,20 @@ int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const 
   SVGB_REQUIRE(k_scale && v_scale, "%s needs both scale vectors k_scale and v_scale (float [Hkv])", who);
   return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
                        num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, k_scale,
-                       v_scale, stream, who);
+                       v_scale, nullptr, nullptr, stream, who);
+}
+
+int svgb_kvcache_append_e4m3_rows(void* k_cache, void* v_cache, const void* k, const void* v,
+                                  const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                  const int32_t* block_table, int dtype, int B, int Snew, int Hkv, int D,
+                                  int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                                  const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                                  float* k_scale, float* v_scale, void* stream) {
+  const char* who = "svgb_kvcache_append_e4m3_rows";
+  if (kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
+  return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
+                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
+                       nullptr, k_scale, v_scale, stream, who);
 }
 
 int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {

@@ -1,9 +1,13 @@
 // Per-head absmax quantisation of a 16-bit [BH, S, D] tensor to fp8 e4m3 (bytes) for the FP8 attention
-// path: scale[h] = absmax_h / 448, x8 = round_to_nearest_sat(x / scale[h]).  Two HBM-bound passes.
+// path: scale[h] = absmax_h / 448, x8 = round_to_nearest_sat(x / scale[h]).  Two HBM-bound passes.  And the per-row
+// quantisation of the queries of the per-row FP8 KV cache (svgb_quantize_e4m3_rows): one pass.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <algorithm>
+
 #include "../../include/svgb200.h"
+#include "fp8_rows.cuh"
 #include "host_common.h"
 
 namespace svgb {
@@ -70,9 +74,50 @@ quantize_kernel(const uint4* __restrict__ x, const float* __restrict__ scale, ui
   }
 }
 
+// Per-row quantisation of a 16-bit [rows, H, 128] tensor read at its strides: x8 [rows, H, 128] contiguous e4m3 and
+// scale [H, rows] (fp8_rows.cuh), one 16-byte vector per thread, 16 threads per (row, head)
+template <bool BF16>
+__global__ void __launch_bounds__(256)
+quantize_rows_kernel(const uint16_t* __restrict__ x, long long row_stride, long long head_stride, int rows, int H,
+                     uint2* __restrict__ x8, float* __restrict__ scale) {
+  const long long total = static_cast<long long>(rows) * H * 16;
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(idx & 15);
+    const long long rh = idx >> 4;
+    const int h = static_cast<int>(rh % H), r = static_cast<int>(rh / H);
+    const uint4 v = *reinterpret_cast<const uint4*>(x + r * row_stride + h * head_stride + 8 * c);
+    int e;
+    x8[idx] = e4m3_row_quantise<BF16>(v, 0xffffu << (threadIdx.x & 16), &e);  // a (row, head) is an aligned half-warp
+    if (c == 0) scale[static_cast<long long>(h) * rows + r] = e4m3_row_scale(e);
+  }
+}
+
 }  // namespace svgb
 
 using namespace svgb;
+
+extern "C" int svgb_quantize_e4m3_rows(const void* x, int dtype, void* x8, float* scale, int rows, int H, int D,
+                                       long long row_stride, long long head_stride, void* stream) {
+  const char* who = "svgb_quantize_e4m3_rows";
+  SVGB_REQUIRE(x && x8 && scale, "null pointer");
+  SVGB_REQUIRE(rows > 0 && H > 0, "%s: bad sizes (rows=%d, H=%d)", who, rows, H);
+  SVGB_REQUIRE(D == 128, "%s: per-row scales need head_dim 128 (got %d)", who, D);
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "%s takes bf16 or fp16 input (dtype %d)", who, dtype);
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(x8) & 7) == 0,
+               "%s: x must be 16-byte and x8 8-byte aligned", who);
+  SVGB_REQUIRE(row_stride % 8 == 0 && head_stride % 8 == 0,
+               "%s: the row and head strides must be multiples of 8 elements (got %lld, %lld)", who, row_stride,
+               head_stride);
+  const long long total = static_cast<long long>(rows) * H * 16;
+  const unsigned blocks = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 1 << 20));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  auto kern = dtype == SVGB_BF16 ? quantize_rows_kernel<true> : quantize_rows_kernel<false>;
+  kern<<<blocks, 256, 0, st>>>(static_cast<const uint16_t*>(x), row_stride, head_stride, rows, H,
+                               static_cast<uint2*>(x8), scale);
+  SVGB_LAUNCH_OK();
+  return 0;
+}
 
 extern "C" int svgb_quantize_e4m3(const void* x, int dtype, void* x8, float* scale, int BH, int S, int D,
                                   void* stream) {

@@ -53,6 +53,8 @@ _PROTOS = {
                             _vp],
     "svgb_kvcache_append_e4m3": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll,
                                  _pll, _vp, _vp, _vp],
+    "svgb_kvcache_append_e4m3_rows": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll,
+                                      _pll, _pll, _vp, _vp, _vp],
     "svgb_attn_plan_kvcache_bytes": [_i, _i, _i, _i, _i, _i, _psz],
     "svgb_attn_plan_kvcache": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
@@ -66,6 +68,9 @@ _PROTOS = {
     "svgb_attn_fwd_strided_e4m3": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll,
                                    _pll, _f, _pplan, _vp, _vp],
     "svgb_quantize_e4m3": [_vp, _i, _vp, _vp, _i, _i, _i, _vp],
+    "svgb_attn_fwd_kvcache_e4m3_rows": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _pll, _pll,
+                                        _pll, _pll, _f, _pplan, _vp, _vp],
+    "svgb_quantize_e4m3_rows": [_vp, _i, _vp, _vp, _i, _i, _i, _ll, _ll, _vp],
     "svgb_attn_bwd_bytes": [_i, _i, _psz],
     "svgb_attn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _f, _pplan, _vp, _pplan,
                       _vp, _vp, _sz, _vp],

@@ -289,9 +289,12 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     row cache_batch_idx[b] (default b), or paged, [num_pages, page_size, Hkv, D] with block_table int [B, max_pages]
     (page_size a multiple of 128).  cache_seqlens: int or device int tensor [B], read on the device only.  Rows whose key
     or block falls outside the cache are not written (include/svgb200.h, svgb_kvcache_append).
-    FP8 cache: caches of dtype torch.float8_e4m3fn take 16-bit k, v and k_scale, v_scale, float32 device tensors [Hkv]
-    fixed for the cache's lifetime; each element is stored as RN-satfinite(x * (1 / scale[h])), values past 448 * scale
-    saturating (svgb_kvcache_append_e4m3).  16-bit caches take no scales."""
+    FP8 cache: caches of dtype torch.float8_e4m3fn take 16-bit k, v and k_scale, v_scale, float32 device tensors whose
+    shape picks the format.  [Hkv]: one scale per head fixed for the cache's lifetime; each element is stored as
+    RN-satfinite(x * (1 / scale[h])), values past 448 * scale saturating (svgb_kvcache_append_e4m3).  [num_blocks, Hkv,
+    block_rows] (contiguous, block_rows a multiple of 4, D = 128): one power-of-two scale per cache row, which the append
+    computes from the row's absmax and writes there, so nothing saturates (svgb_kvcache_append_e4m3_rows).  16-bit
+    caches take no scales."""
     _need_cuda(k_cache, v_cache, k, v)
     if k_cache.dim() != 4 or k.dim() != 4 or k_cache.shape != v_cache.shape or k.shape != v.shape:
         raise SvgbError(f"kvcache_append: k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] and "
@@ -299,10 +302,12 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     if k.shape[2:] != k_cache.shape[2:]:
         raise SvgbError(f"kvcache_append: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
     fp8 = k_cache.dtype == torch.float8_e4m3fn
+    rows = None
     if fp8:
         if v_cache.dtype != k_cache.dtype or k.dtype != v.dtype:
             raise SvgbError("kvcache_append: an e4m3 k_cache needs an e4m3 v_cache, and k, v of one 16-bit dtype")
-        scales = _fp8_scales("kvcache_append", k_scale, v_scale, k.shape[2])
+        rows = _row_scales("kvcache_append", k_scale, v_scale, k_cache)
+        scales = rows or _fp8_scales("kvcache_append", k_scale, v_scale, k.shape[2])
     else:
         if k_scale is not None or v_scale is not None:
             raise SvgbError("kvcache_append: k_scale / v_scale are for float8_e4m3fn caches; a "
@@ -324,7 +329,10 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     args = (k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(), lens.data_ptr(), _p(bi), _p(bt), dt, B,
             Snew, Hkv, D, k_cache.shape[0], k_cache.shape[1], max_pages, _st(k_cache.transpose(1, 2), "bhsd", fill),
             _st(v_cache.transpose(1, 2), "bhsd", fill), _st(k, "bhsd"), _st(v, "bhsd"))
-    if fp8:
+    if fp8 and rows:
+        check(lib().svgb_kvcache_append_e4m3_rows(*args, *(t.data_ptr() for t in scales), _stream(k)),
+              "svgb_kvcache_append_e4m3_rows")
+    elif fp8:
         check(lib().svgb_kvcache_append_e4m3(*args, *(t.data_ptr() for t in scales), _stream(k)),
               "svgb_kvcache_append_e4m3")
     else:
@@ -340,10 +348,31 @@ def _fp8_scales(who, k_scale, v_scale, Hkv):
     for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
         if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) != (Hkv,):
             shown = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
-            raise SvgbError(f"{who}: {name} must be a float32 tensor [Hkv={Hkv}] (got {shown}"
-                            f"{', ' + str(t.dtype) if isinstance(t, torch.Tensor) else ''})")
+            raise SvgbError(f"{who}: {name} must be a float32 tensor [Hkv={Hkv}] per head, or [num_blocks, Hkv, "
+                            f"block_rows] per row (got {shown}{', ' + str(t.dtype) if isinstance(t, torch.Tensor) else ''})")
     _need_cuda(k_scale, v_scale)
     return k_scale.contiguous(), v_scale.contiguous()
+
+
+def _row_scales(who, k_scale, v_scale, cache):
+    """The per-row scales of an e4m3 cache [num_blocks, block_rows, Hkv, D]: (k_scale, v_scale) when either is 3-D, both
+    then float32 device tensors [num_blocks, Hkv, block_rows], contiguous (written in place), with D = 128 and block_rows
+    a multiple of 4; None for the per-head format ([Hkv], checked by _fp8_scales)."""
+    if not any(isinstance(t, torch.Tensor) and t.dim() == 3 for t in (k_scale, v_scale)):
+        return None
+    nb, rows, Hkv, D = cache.shape
+    want = (nb, Hkv, rows)
+    for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
+        if not isinstance(t, torch.Tensor) or t.dim() != 3:
+            raise SvgbError(f"{who}: k_scale and v_scale mix formats: per-row scales [num_blocks, Hkv, block_rows] go "
+                            f"with per-row scales, not {tuple(t.shape) if isinstance(t, torch.Tensor) else t!r}")
+        if t.dtype != torch.float32 or tuple(t.shape) != want or not t.is_contiguous():
+            raise SvgbError(f"{who}: per-row {name} must be a contiguous float32 tensor [num_blocks, Hkv, block_rows]="
+                            f"{list(want)} (got {tuple(t.shape)}, {t.dtype})")
+    if D != 128 or rows % 4:
+        raise SvgbError(f"{who}: per-row scales need head_dim 128 (got {D}) and block_rows a multiple of 4 (got {rows})")
+    _need_cuda(k_scale, v_scale)
+    return k_scale, v_scale
 
 
 def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0, cache_len: Optional[int] = None,
@@ -531,7 +560,8 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     k, v may have fewer heads than q, Hq = G * Hkv (grouped-query attention, FlashInfer's mapping: query head h attends
     with key/value head h // G): a variable-block plan is then built over the B * Hkv key/value heads and shared by
     each group, band plans are shared by every head already; no row vectors, FP8 or gather plans.
-    k_scale, v_scale: the per-KV-head scales of float8_e4m3fn caches under a KV-cache plan (see _attn_kvcache)."""
+    k_scale, v_scale: the scales of float8_e4m3fn caches under a KV-cache plan, per key/value head [Hkv] or per cache row
+    [num_blocks, Hkv, block_rows] (see _attn_kvcache)."""
     _need_cuda(q, k, v)
     if plan.desc.kind == PLAN_KVCACHE:
         if any(r is not None for r in (q_rows, kv_rows, o_rows)):
@@ -567,7 +597,8 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=
     """attn_fwd under a KV-cache plan: q [B, Sq, Hq, D] as B * Sq packed rows, the cache [blocks, rows, Hkv, D] as
     blocks * rows rows (both views), o [B, Sq, Hq, D] and lse [B, Hq, Sq] (flash_attn_with_kvcache's shapes).
     float8_e4m3fn caches (FP8 KV cache) take bf16 q, D = 128 and k_scale, v_scale float32 [Hkv]: q is quantised per
-    query head over the call's B * Sq rows (quantize_e4m3 on a transposed [Hq, B * Sq, D] copy) and o is bf16."""
+    query head over the call's B * Sq rows (quantize_e4m3 on a transposed [Hq, B * Sq, D] copy) and o is bf16.  With
+    per-row scales [num_blocks, Hkv, block_rows] each q row is quantised on its own (_attn_kvcache_fp8_rows)."""
     B, Sq = plan.source
     if q.dim() != 4 or q.shape[:2] != (B, Sq) or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
         raise SvgbError(f"a KV-cache plan for B={B} streams of Sq={Sq} queries takes q [B, Sq, Hq, D] (got "
@@ -577,6 +608,9 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=
         raise SvgbError(f"the KV-cache plan was built for {plan.S_kv} cache rows, the cache {tuple(k_cache.shape)} has "
                         f"{k_cache.shape[0] * k_cache.shape[1]}")
     if k_cache.dtype == torch.float8_e4m3fn:
+        rows = _row_scales("attn_fwd on an FP8 KV cache", k_scale, v_scale, k_cache)
+        if rows:
+            return _attn_kvcache_fp8_rows(q, k_cache, v_cache, plan, return_lse, sm_scale, out, *rows)
         return _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale)
     if k_scale is not None or v_scale is not None:
         raise SvgbError(f"k_scale / v_scale are for float8_e4m3fn caches; a {k_cache.dtype} cache takes none")
@@ -788,6 +822,65 @@ class _Permute(torch.autograd.Function):
     def backward(ctx, g):
         perm, = ctx.saved_tensors
         return (permute_gather if ctx.scatter else permute_scatter)(g, perm), None, None
+
+
+def _attn_kvcache_fp8_rows(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
+    """_attn_kvcache on an e4m3 cache with per-row scales: q quantised per row (quantize_e4m3_rows, read in place), then
+    svgb_attn_fwd_kvcache_e4m3_rows on the cache in place.  Each stream's o and lse depend on that stream alone."""
+    B, Sq = plan.source
+    Hq, D = q.shape[2:]
+    nb, rows, Hkv, _ = k_cache.shape
+    if v_cache.dtype != torch.float8_e4m3fn:
+        raise SvgbError("an e4m3 k_cache needs an e4m3 v_cache")
+    if q.dtype != torch.bfloat16:
+        raise SvgbError(f"an FP8 KV cache takes bf16 q (got {q.dtype}); it is quantised per row here, and the output is "
+                        "bf16")
+    if D != 128:
+        raise SvgbError(f"an FP8 KV cache needs head_dim 128 (got q {D})")
+    if Hq % Hkv:
+        raise SvgbError(f"q's {Hq} heads must be a multiple of the cache's {Hkv} key/value heads")
+    if out is not None and (out.shape != q.shape or out.dtype != torch.bfloat16):
+        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype bf16")
+    if needs_grad(q, k_cache, v_cache):
+        raise SvgbError("attention into a KV cache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
+    q8, q_scale = quantize_e4m3_rows(q.reshape(B * Sq, Hq, D))
+    kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))  # [rows, Hkv, D] views, read in place
+    o = torch.empty(B * Sq, Hq, D, dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty(Hq, B * Sq, dtype=torch.float32, device=q.device) if return_lse else None
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    check(lib().svgb_attn_fwd_kvcache_e4m3_rows(q8.data_ptr(), kf.data_ptr(), vf.data_ptr(), q_scale.data_ptr(),
+                                                k_scale.data_ptr(), v_scale.data_ptr(), o.data_ptr(), _p(lse), Hq, Hkv,
+                                                B * Sq, nb, rows, D, _st(q8, "shd", 16), _st(kf, "shd", 16),
+                                                _st(vf, "shd", 16), _st(o, "shd"), scale, C.byref(plan.desc),
+                                                plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd_kvcache_e4m3_rows")
+    _bump()
+    o = o.view(B, Sq, Hq, D)
+    if out is not None:
+        out.copy_(o)
+        o = out
+    if not return_lse:
+        return o
+    return o, lse.view(Hq, B, Sq).transpose(0, 1)
+
+
+def quantize_e4m3_rows(x: torch.Tensor):
+    """Per-row quantisation of a 16-bit [rows, H, 128] tensor, read in place at its row and head strides (a view is
+    copied only when they are not multiples of 8 elements): returns (x8 uint8 [rows, H, 128], scale fp32 [H, rows]) with
+    x ~= x8.view(float8_e4m3fn) * scale[h, r], scale a power of two from the row's own absmax (include/svgb200.h,
+    svgb_kvcache_append_e4m3_rows).  One launch."""
+    _need_cuda(x)
+    if x.dim() != 3 or x.shape[2] != 128 or x.dtype not in (torch.bfloat16, torch.float16):
+        raise SvgbError(f"quantize_e4m3_rows takes a bf16 or fp16 [rows, H, 128] tensor (got {tuple(x.shape)}, {x.dtype})")
+    if not _addressable(x, "shd"):
+        x = x.clone(memory_format=torch.contiguous_format)
+    R, H, D = x.shape
+    x8 = torch.empty(R, H, D, dtype=torch.uint8, device=x.device)
+    scale = torch.empty(H, R, dtype=torch.float32, device=x.device)
+    _, hs, rs = _strides(x, "shd")
+    check(lib().svgb_quantize_e4m3_rows(x.data_ptr(), _dt(x), x8.data_ptr(), scale.data_ptr(), R, H, D, rs, hs,
+                                        _stream(x)), "svgb_quantize_e4m3_rows")
+    _bump()
+    return x8, scale
 
 
 def quantize_e4m3(x: torch.Tensor):

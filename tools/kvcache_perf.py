@@ -14,8 +14,12 @@ Wan 1.3B (12 heads) and Wan 14B (40 heads).  Ways, each one call sequence as a c
   fp8 paged       plan + forward on the same pages in e4m3 (per-KV-head scales), q quantised inside the call
   fp8 append+paged  kvcache_append quantising the chunk's new rows into the e4m3 pages, then plan + forward
   fp8 q quant     the q quantisation of the fp8 forward alone (a transposed copy and quantize_e4m3)
+  rows paged      plan + forward on the same pages in e4m3 with per-row scales, q quantised per row inside the call
+  rows append+paged  kvcache_append quantising the chunk's new rows per row into those pages, then plan + forward
+  rows q quant    the per-row q quantisation alone (quantize_e4m3_rows on q in place)
 
-Besides the times: the bytes of each cache (K and V, one layer) and mean / max |o_fp8 - o_bf16| of the paged forward.
+Besides the times: the bytes of each cache (K and V, one layer, and the per-row scales) and mean / max
+|o_fp8 - o_bf16| of the paged forward in both formats.
 
 Each figure is the median of R rounds with the rounds' min and max; every round times N back-to-back calls of each way
 with CUDA events, the ways alternated within every round.  The card name and power limit are read in the same run.
@@ -136,17 +140,39 @@ def case(H, dev, rounds, iters):
     def q_quant():
         return core.quantize_e4m3(q.reshape(SQ, H, D).transpose(0, 1).contiguous())
 
+    # the e4m3 pages with per-row scales [pages, H, PAGE]: the rows of the per-row append
+    e = lambda t: (lambda m, k: torch.where(m <= 0.875, k - 9, k - 8))(*torch.frexp(t.float().abs().amax(-1)))  # noqa: E731
+    ke, ve = e(kp).clamp(-126, 127), e(vp).clamp(-126, 127)
+    kpr, vpr = ((t.float() * torch.exp2(-x.float())[..., None]).to(torch.float8_e4m3fn) for t, x in ((kp, ke), (vp, ve)))
+    ksr, vsr = (torch.exp2(x.float()).transpose(1, 2).contiguous() for x in (ke, ve))
+
+    def paged_rows(new_len=0, seq=lens):
+        plan = core.plan_kvcache(seq, q_len=SQ, num_blocks=npages, new_len=new_len, block_table=table, page_size=PAGE,
+                                 **win)
+        return core.attn_fwd(q, kpr, vpr, plan, k_scale=ksr, v_scale=vsr)
+
+    def append_paged_rows():
+        core.kvcache_append(kpr, vpr, knew, vnew, before, block_table=table, k_scale=ksr, v_scale=vsr)
+        return paged_rows(new_len=SQ, seq=before)
+
+    def q_quant_rows():
+        return core.quantize_e4m3_rows(q.reshape(SQ, H, D))
+
     # the ways agree before they are timed
     o_c, o_p = contiguous(), paged()
     assert torch.equal(o_c, o_p), "paged and contiguous differ"
     err = (sdpa().transpose(1, 2).float() - o_c.float()).abs().max().item()
     assert err < 3e-2, f"sdpa differs by {err}"
     d = (paged_fp8().float() - o_p.float()).abs()
-    fp8 = {"cache_bytes": {"bf16": 2 * kp.numel() * 2, "e4m3": 2 * kp8.numel()},
-           "o_abs_diff_vs_bf16": {"mean": d.mean().item(), "max": d.max().item()}}
+    dr = (paged_rows().float() - o_p.float()).abs()
+    fp8 = {"cache_bytes": {"bf16": 2 * kp.numel() * 2, "e4m3": 2 * kp8.numel(),
+                           "e4m3 rows": 2 * kpr.numel() + 2 * 4 * ksr.numel()},
+           "o_abs_diff_vs_bf16": {"mean": d.mean().item(), "max": d.max().item()},
+           "rows_o_abs_diff_vs_bf16": {"mean": dr.mean().item(), "max": dr.max().item()}}
     ways = {"contiguous": contiguous, "paged": paged, "append+paged": append_paged, "index+contig": index_contig,
             "roll+contig": roll_contig, "sdpa": sdpa, "decode": lambda: paged(qq=q1), "fp8 paged": paged_fp8,
-            "fp8 append+paged": append_paged_fp8, "fp8 q quant": q_quant}
+            "fp8 append+paged": append_paged_fp8, "fp8 q quant": q_quant, "rows paged": paged_rows,
+            "rows append+paged": append_paged_rows, "rows q quant": q_quant_rows}
     return {**alternate(ways, rounds, iters), "fp8": fp8}
 
 
