@@ -486,7 +486,12 @@ int svgb_dynamic_map(const void* qc, const void* kc, const int32_t* k_sizes, int
  * layout: 0 = HY (text last, band 1.5*P; hyvideo/utils.py:47-93), 1 = WAN (first-frame sink, band 2*P;
  * wan/utils.py:63-110), 2 = COG (text first, band 1.5*P; cog/utils.py:61-88 -- its temporal mask leaves text rows
  * empty: a sampled text row contributes 0 output here where the reference's softmax yields NaN; the Python mirror
- * CogSVG1Core.sample_mse restores the NaN so argmin picks the same head type). */
+ * CogSVG1Core.sample_mse restores the NaN so argmin picks the same head type).
+ * q, k, v: 16-bit only (SVGB_BF16 or SVGB_F16), [BH, S, D] contiguous, D in {64, 128}; 1 <= n_rows <= 128;
+ * S == ctx + F * P with F, P > 0, ctx == 0 for WAN and ctx < 2^19 for COG; the band threshold (1.5 * P or 2 * P) / 128
+ * below 4096.  Each of these errors returns before the device is queried; only the workspace size depends on the
+ * device (its SM count sets the split count).  Precondition, not checked (rows is device data):
+ * every rows[i] lies in [0, S). */
 int svgb_sample_mse_bytes(int BH, int S, int D, int n_rows, size_t* bytes);
 int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* rows, int n_rows,
                     int BH, int S, int D, int dtype, int layout, int ctx, int F, int P, float* mse,

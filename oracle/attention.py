@@ -192,7 +192,7 @@ def generic_mask_fn(mode, m0, m1, m2):
 # --------------------------------------------------------------------------------------------
 # SVG1 profiling masks + sample_mse
 # --------------------------------------------------------------------------------------------
-def profiling_mask_rows(mask_name, rows, layout, context_length, num_frame, frame_size):
+def profiling_mask_rows(mask_name, rows, layout, context_length, num_frame, frame_size, thres=None):
     """Rows `rows` of get_attention_mask(...) evaluated analytically -> bool [len(rows), S].
 
     hyvideo/utils.py:47-93 (layout 'hy': text last, band threshold (1.5*P)//128 blocks),
@@ -201,11 +201,12 @@ def profiling_mask_rows(mask_name, rows, layout, context_length, num_frame, fram
     mask is the same picture pushed through reshape(P,F,P,F).permute(1,0,3,2), i.e.
         temporal[f*P+p, f2*P+p2] = picture[p*F+f, p2*F+f2].
     For 'wan' the first-frame sink columns are painted BEFORE that permutation (wan/utils.py:95-108)
-    so they are permuted too."""
+    so they are permuted too.  `thres` overrides the band threshold (blocks)."""
     F_, P_ = num_frame, frame_size
     V = F_ * P_
     S = context_length + V
-    thres = (frame_size * (1.5 if layout == "hy" else 2)) // 128
+    if thres is None:
+        thres = (frame_size * (1.5 if layout == "hy" else 2)) // 128
     kv = torch.arange(V)
     ki = kv if mask_name == "spatial" else (kv % P_) * F_ + kv // P_
     out = torch.zeros(len(rows), S, dtype=torch.bool)
@@ -223,17 +224,19 @@ def profiling_mask_rows(mask_name, rows, layout, context_length, num_frame, fram
     return out
 
 
-def profiling_mask_rows_cog(mask_name, rows, context_length, num_frame, frame_size):
+def profiling_mask_rows_cog(mask_name, rows, context_length, num_frame, frame_size, thres=None):
     """Rows of the CogVideoX profiling masks (text FIRST), svg/models/cog/utils.py:61-88, analytically.
 
     spatial : text rows / columns all-ones (:66-67); the 128-token block band |bi-bj| < (1.5*P)//128 is painted in
               ABSOLUTE coordinates from row / column 0 for blocks 0..ceil(F*P/128)-1 (:68-74, not offset by the text);
     temporal: the same band picture pushed through reshape(P,F,P,F).permute(1,0,3,2) on the video x video part only
-              (:76-86); text rows and text columns stay ZERO (a sampled text row is fully masked)."""
+              (:76-86); text rows and text columns stay ZERO (a sampled text row is fully masked).
+    `thres` overrides the band threshold (blocks)."""
     F_, P_, ctx = num_frame, frame_size, context_length
     V = F_ * P_
     S = ctx + V
-    thres = (frame_size * 1.5) // 128
+    if thres is None:
+        thres = (frame_size * 1.5) // 128
     lim = math.ceil(V / 128) * 128
     kv = torch.arange(S)
     out = torch.zeros(len(rows), S, dtype=torch.bool)

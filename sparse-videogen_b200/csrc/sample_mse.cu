@@ -170,14 +170,23 @@ int svgb_sample_mse_bytes(int BH, int S, int D, int n_rows, size_t* bytes) {
 int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* rows, int n_rows,
                     int BH, int S, int D, int dtype, int layout, int ctx, int F, int P, float* mse,
                     void* ws, size_t ws_bytes, void* stream) {
+  // every check on the arguments alone comes before the device query and the first launch
   SVGB_REQUIRE(q && k && v && rows && mse && ws, "null pointer");
+  // the gather moves 2-byte elements and the attention passes run without fp8 scales
+  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
+               "sample_mse takes 16-bit q/k/v only: SVGB_BF16 or SVGB_F16, not dtype %d", dtype);
+  SVGB_REQUIRE(layout >= 0 && layout <= 2, "layout %d unsupported (0 = HY text-last, 1 = WAN, 2 = COG text-first)", layout);
+  SVGB_REQUIRE(ctx >= 0 && F > 0 && P > 0, "bad sequence layout ctx %d, F %d, P %d", ctx, F, P);
+  SVGB_REQUIRE(static_cast<long long>(S) == ctx + static_cast<long long>(F) * P, "seq_len %d != ctx %d + F %d * P %d",
+               S, ctx, F, P);
+  SVGB_REQUIRE(layout != 1 || ctx == 0, "WAN layout has no text tokens");
+  SVGB_REQUIRE(layout != 2 || ctx < (1 << 19), "COG layout: context length %d too large", ctx);
+  // reference thresholds: block_thres // block_size with block_thres = 1.5*P (HY, COG) or 2*P (WAN)
+  const int thres = layout == 1 ? static_cast<int>((2LL * P) / 128) : static_cast<int>((1.5 * P) / 128.0);
+  SVGB_REQUIRE(thres < (1 << 12), "profiling band threshold %d too large", thres);
   size_t need = 0;
   if (svgb_sample_mse_bytes(BH, S, D, n_rows, &need)) return -1;
   SVGB_REQUIRE(ws_bytes >= need, "workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(layout >= 0 && layout <= 2, "layout %d unsupported (0 = HY text-last, 1 = WAN, 2 = COG text-first)", layout);
-  SVGB_REQUIRE(S == ctx + F * P, "seq_len %d != ctx %d + F %d * P %d", S, ctx, F, P);
-  SVGB_REQUIRE(layout != 1 || ctx == 0, "WAN layout has no text tokens");
-  SVGB_REQUIRE(layout != 2 || ctx < (1 << 19), "COG layout: context length %d too large", ctx);
   int n_sms = 0;
   if (device_sms(&n_sms)) return -1;
   const SmseLayout L = smse_layout(BH, S, D, n_sms);  // the same device, so the same layout as the byte count
@@ -194,9 +203,6 @@ int svgb_sample_mse(const void* q, const void* k, const void* v, const int32_t* 
                                       reinterpret_cast<int2*>(w + L.chunks_plain),
                                       reinterpret_cast<int2*>(w + L.chunks_elem));
   SVGB_LAUNCH_OK();
-  // reference thresholds: block_thres // block_size with block_thres = 1.5*P (HY, COG) or 2*P (WAN)
-  const int thres = layout == 1 ? (2 * P) / 128 : static_cast<int>((1.5 * P) / 128.0);
-  SVGB_REQUIRE(thres < (1 << 12), "profiling band threshold %d too large", thres);
   static const int kModes[3][2] = {{MASK_PROF_HY_S, MASK_PROF_HY_T}, {MASK_PROF_WAN_S, MASK_PROF_WAN_T},
                                    {MASK_PROF_COG_S, MASK_PROF_COG_T}};
   for (int var = 0; var < 3; ++var) {
