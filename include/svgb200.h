@@ -65,6 +65,7 @@ int svgb_device_check(int* sm_major, int* sm_minor, int* num_sms);
 #define SVGB_PLAN_SEG 5      /* local mask inside packed variable-length segments (svgb_attn_plan_local_varlen) */
 #define SVGB_PLAN_SEG_T 6    /* its key-major companion for the backward (svgb_attn_plan_local_varlen_t) */
 #define SVGB_PLAN_KVCACHE 7  /* local mask into a contiguous or paged KV cache, forward only (svgb_attn_plan_kvcache) */
+#define SVGB_PLAN_KVCACHE_SPLIT 8 /* the same, split across the keys (svgb_attn_plan_kvcache_split) */
 typedef struct svgb_plan {
   int32_t kind;          /* SVGB_PLAN_* */
   int32_t BH, S;
@@ -232,6 +233,21 @@ int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int
 int svgb_attn_plan_kvcache(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table,
                            int B, int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left,
                            int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
+/* Split across the keys (split-KV, for decode and short chunks, where B ceil(Sq / 256) Hq CTAs leave SMs idle):
+ * svgb_attn_plan_kvcache's arguments plus num_splits = n >= 1.  The plan has n B ceil(Sq / 256) items, split-major: item
+ * s B I + i is split s of the single plan's item i, and visits the s-th piece of ceil(nvis / n) of that item's nvis
+ * visited chunks (sinks first, then the window), classified and compacted as the single plan's, so the split lists of
+ * an item concatenated in split order are its single-pass list chunk for chunk; splits past the last piece are empty.
+ * plan->kind = SVGB_PLAN_KVCACHE_SPLIT, max_items = n B ceil(Sq / 256), every other field and the {B, Sq, L_b} header as
+ * svgb_attn_plan_kvcache.  Workspace: svgb_attn_plan_kvcache_bytes's with I' = n I items of ceil(slots / n) slots:
+ *   bytes = 16 + align16(4 (B + 2)) + 32 I' + 8 I' ceil(slots / n).
+ * Runs on svgb_attn_fwd_kvcache_split only; every other attention entry and the backward refuse it by name. */
+int svgb_attn_plan_kvcache_split_bytes(int B, int Sq, int cap, int sink, int left, int right, int num_splits,
+                                       size_t* bytes);
+int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
+                                 int max_pages, int sink, int left, int right, int num_splits, void* plan_ws,
+                                 size_t ws_bytes, svgb_plan* plan, void* stream);
 
 /* ---- attention -------------------------------------------------------------------------- */
 /* o = softmax(q k^T * sm_scale  [masked by plan]) v, per head.  Stands behind
@@ -340,6 +356,28 @@ int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v,
                                     int Sq, int num_blocks, int block_rows, int D, const long long* q_strides,
                                     const long long* k_strides, const long long* v_strides, const long long* o_strides,
                                     float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream);
+/* Attention under a split KV-cache plan (svgb_attn_plan_kvcache_split), for every cache format, in two launches: the
+ * attention writes each split's fp32 partial o and natural-log lse into ws, then a merge combines the n splits of each
+ * (row, query head) in order s = 0 .. n-1: m = max lse_s, w_s = exp(lse_s - m) (0 when lse_s = -inf),
+ * o = sum w_s o_s / sum w_s, lse = m + log sum w_s; a row no split saw gets o = 0, lse = -inf.  With one live split the
+ * result is the single pass's bit for bit.
+ *   q     : the packed queries [B * Sq, Hq, D] at q_strides;  k, v : the cache as num_blocks * block_rows rows of Hkv
+ *           heads;  o : [B * Sq, Hq, D] at o_strides;  lse : optional float [Hq, B * Sq].  Strides {batch, head, row}
+ *           in elements (the batch stride is not stepped), as svgb_attn_fwd_strided.  Hq = G * Hkv.
+ *   dtype : SVGB_BF16 / SVGB_F16 -- 16-bit q, k, v and o, no scales (NULL, row_scales = 0); or SVGB_E4M3 -- an e4m3
+ *           cache, D = 128, strides multiples of 16 bytes, bf16 o, and all three scales: row_scales = 0 per head as
+ *           svgb_attn_fwd_strided_e4m3 with B = 1 (q_scale [Hq], k_scale, v_scale [Hkv]), row_scales = 1 per row as
+ *           svgb_attn_fwd_kvcache_e4m3_rows (q_scale [Hq, B * Sq], k_scale, v_scale [num_blocks, Hkv, block_rows]).
+ *   ws    : device, 16-byte aligned, svgb_attn_fwd_kvcache_split_bytes(n, B * Sq, Hq, D) bytes:
+ *           n (B Sq) Hq D 4 (partial o [n, B Sq, Hq, D]) + n Hq (B Sq) 4 (partial lse [n, Hq, B Sq]).
+ * The split count n comes from the plan (max_items / (B ceil(Sq / 256))).  Deterministic, no atomics. */
+int svgb_attn_fwd_kvcache_split_bytes(int num_splits, int rows, int Hq, int D, size_t* bytes);
+int svgb_attn_fwd_kvcache_split(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
+                                const float* v_scale, void* o, float* lse, int dtype, int row_scales, int B, int Hq,
+                                int Hkv, int Sq, int num_blocks, int block_rows, int D, const long long* q_strides,
+                                const long long* k_strides, const long long* v_strides, const long long* o_strides,
+                                float sm_scale, const svgb_plan* plan, const void* plan_ws, void* ws, size_t ws_bytes,
+                                void* stream);
 /* Per-row quantisation of 16-bit x [rows, H, 128], read at row_stride / head_stride (elements, multiples of 8; base
  * 16-byte aligned), into e4m3 x8 [rows, H, 128] contiguous and scale float [H, rows], by the rule of
  * svgb_kvcache_append_e4m3_rows; one launch.  A row's bytes and scale depend on that row alone. */

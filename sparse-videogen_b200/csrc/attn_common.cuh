@@ -156,7 +156,7 @@ __host__ __device__ inline SegOrigin seg_origin(const int* seg, int row, bool ke
   return o;
 }
 
-// KV-cache plans (SVGB_PLAN_KVCACHE).  The plan keeps at byte SVGB_PLAN_SEG_BOUNDS_OFF of its workspace
+// KV-cache plans (SVGB_PLAN_KVCACHE, and SVGB_PLAN_KVCACHE_SPLIT with the same header).  The plan keeps at byte SVGB_PLAN_SEG_BOUNDS_OFF of its workspace
 // kv = {B, Sq, L_0 .. L_B-1}: stream b has its queries at packed rows [b Sq, (b+1) Sq) and L_b keys at logical positions
 // 0 .. L_b - 1 (clamped to its capacity).  Query row q of stream b sits at logical position L_b - Sq + (q - b Sq), so the
 // mask is MASK_LOCAL(sink, left, right) on logical positions with shift (b+1) Sq - L_b and the sink bound `sink`; the
@@ -353,6 +353,11 @@ struct AttnArgs {
   // KV-cache plans: segs is the plan's {B, Sq, L_b} (kv_origin) and element masks see each chunk's logical position
   int kv_logical = 0;
   int out_f32 = 0;               // 1: o is fp32 (used for split-KV partials)
+  // split KV-cache plans (SVGB_PLAN_KVCACHE_SPLIT): the plan's items per split, so that CTA x runs split
+  // x / split_items, whose fp32 partial o starts o_split_stride elements and whose partial LSE gridDim.y * S floats
+  // after the previous split's.  0: no split
+  int split_items = 0;
+  long long o_split_stride = 0;
   // FP8 (e4m3) inputs: per-head dequantisation scales, q_scale [BH] by query head, k_scale and v_scale [BH / kv_group]
   // by key/value head; s_q * s_k multiplies the logits, s_v the output.  NULL for 16-bit inputs.
   const float* q_scale = nullptr;

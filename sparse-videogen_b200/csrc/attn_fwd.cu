@@ -445,6 +445,55 @@ __global__ void density_kernel(const uint8_t* __restrict__ map, const int* __res
 }
 
 // =============================================================================================
+// Merge of a split KV-cache forward (svgb_attn_fwd_kvcache_split): one warp per (query row, query head), D / 32 columns
+// per lane.  Over the splits s = 0 .. n-1 in order: m = max lse_s, w_s = exp(lse_s - m) (0 for lse_s = -inf), o = sum w_s
+// o_s / sum w_s and lse = m + log sum w_s; every split -inf gives o = 0, lse = -inf.  With one live split w = 1, so o and
+// lse are that split's bits.  o_part [n, R, Hq, D] and lse_part [n, Hq, R] fp32; o 16-bit at its strides, lse [Hq, R].
+// =============================================================================================
+template <int D, bool BF16>
+__global__ void __launch_bounds__(256)
+kv_split_merge_kernel(const float* __restrict__ o_part, const float* __restrict__ lse_part, int nsplit, int R, int Hq,
+                      uint16_t* __restrict__ o, long long o_row_stride, long long o_head_stride, float* __restrict__ lse) {
+  constexpr int kPer = D / 32;
+  const long long w = blockIdx.x * 8ll + (threadIdx.x >> 5);
+  if (w >= static_cast<long long>(R) * Hq) return;
+  const int lane = threadIdx.x & 31;
+  const int r = static_cast<int>(w / Hq), h = static_cast<int>(w - static_cast<long long>(r) * Hq);
+  const size_t split_o = static_cast<size_t>(R) * Hq * D, split_l = static_cast<size_t>(Hq) * R;
+  const float* lp = lse_part + static_cast<size_t>(h) * R + r;
+  const float* op = o_part + static_cast<size_t>(w) * D + lane * kPer;
+  float m = -INFINITY;
+  for (int s = 0; s < nsplit; ++s) m = fmaxf(m, __ldg(lp + s * split_l));
+  float acc[kPer], den = 0.f;
+#pragma unroll
+  for (int i = 0; i < kPer; ++i) acc[i] = 0.f;
+  for (int s = 0; s < nsplit; ++s) {
+    const float l = __ldg(lp + s * split_l);
+    if (l == -INFINITY) continue;  // weight 0: the split saw no key of this row
+    const float ws = expf(l - m);
+    float x[kPer];
+    if constexpr (kPer == 4) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(op + s * split_o));
+      x[0] = v.x, x[1] = v.y, x[2] = v.z, x[3] = v.w;
+    } else {
+      const float2 v = __ldg(reinterpret_cast<const float2*>(op + s * split_o));
+      x[0] = v.x, x[1] = v.y;
+    }
+#pragma unroll
+    for (int i = 0; i < kPer; ++i) acc[i] = fmaf(ws, x[i], acc[i]);
+    den += ws;
+  }
+  const float inv = den > 0.f ? 1.f / den : 0.f;
+  uint32_t packed[kPer / 2];
+#pragma unroll
+  for (int i = 0; i < kPer / 2; ++i) packed[i] = pack2<BF16>(acc[2 * i] * inv, acc[2 * i + 1] * inv);
+  uint16_t* dst = o + r * o_row_stride + h * o_head_stride + lane * kPer;
+  if constexpr (kPer == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(packed[0], packed[1]);
+  else *reinterpret_cast<uint32_t*>(dst) = packed[0];
+  if (lse && lane == 0) lse[static_cast<size_t>(h) * R + r] = den > 0.f ? m + logf(den) : -INFINITY;
+}
+
+// =============================================================================================
 // Tile self-test: the exact descriptor paths of the attention kernel on one 128x128xD tile.
 // =============================================================================================
 template <int D, bool BF16>
@@ -699,8 +748,10 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
                         const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
                         const int32_t* o_rows, int dtype, int B, int BH, int kv_group, int Sq, int Skv, int D,
                         Strides qs, Strides ks, Strides vs, Strides os, float sm_scale, const svgb_plan* plan,
-                        const void* plan_ws, void* stream, int scale_block_rows = 0) {
+                        const void* plan_ws, void* stream, int scale_block_rows = 0, int split_items = 0) {
   SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
+  SVGB_REQUIRE((plan->kind == SVGB_PLAN_KVCACHE_SPLIT) == (split_items > 0),
+               "internal: a split KV-cache plan runs with its split count, and only it");
   SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
                "fp8 attention needs the three per-head scale vectors");
   SVGB_REQUIRE(dtype == SVGB_E4M3 || (!q_scale && !k_scale && !v_scale),
@@ -710,7 +761,7 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG_T,
                "a key-major segment plan (svgb_attn_plan_local_varlen_t) is for the backward; the forward takes "
                "svgb_attn_plan_local_varlen");
-  const bool kvc = plan->kind == SVGB_PLAN_KVCACHE;
+  const bool kvc = plan->kind == SVGB_PLAN_KVCACHE || plan->kind == SVGB_PLAN_KVCACHE_SPLIT;
   SVGB_REQUIRE(!kvc || (!q_rows && !kv_rows && !o_rows),
                "KV-cache plans (svgb_attn_plan_kvcache) take no row vectors or gathers (q_rows / kv_rows / o_rows)");
   const bool seg = plan->kind == SVGB_PLAN_SEG;
@@ -759,6 +810,11 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   a.in_row_stride = qs.r;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
   a.in_head_stride = qs.h;
   a.scale_block_rows = scale_block_rows;
+  if (split_items > 0) {  // o: the fp32 partials, one batch-stride apart per split (svgb_attn_fwd_kvcache_split)
+    a.out_f32 = 1;
+    a.split_items = split_items;
+    a.o_split_stride = os.b;
+  }
   return attn_fwd_impl(q, qs, Sq, k, ks, v, vs, Skv, dtype, B, BH, D, a, gather, plan->max_items,
                        static_cast<cudaStream_t>(stream));
 }
@@ -870,6 +926,7 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream) {
+  if (no_split_plan(plan, "svgb_attn_fwd")) return -1;
   // its scales are [BH] by query head: an e4m3 cache, whose scales are by key/value head, takes the strided e4m3 entry
   SVGB_REQUIRE(!plan || plan->kind != SVGB_PLAN_KVCACHE || dtype != SVGB_E4M3,
                "KV-cache plans (svgb_attn_plan_kvcache) take bf16 or fp16 inputs here; an e4m3 cache takes "
@@ -884,6 +941,7 @@ int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float
                      long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                      const svgb_plan* plan, const void* plan_ws, void* stream) {
   SVGB_REQUIRE(plan, "null pointer");
+  if (no_split_plan(plan, "svgb_attn_fwd_kv")) return -1;
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
                "svgb_attn_fwd_kv takes bf16 or fp16 inputs (dtype %d; e4m3 attention needs Sq == Skv, svgb_attn_fwd)",
                dtype);
@@ -904,6 +962,7 @@ int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, floa
                       int Sq, int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                       long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                       const svgb_plan* plan, const void* plan_ws, void* stream) {
+  if (no_split_plan(plan, "svgb_attn_fwd_gqa")) return -1;
   if (attn_gqa_check(dtype, BHq, BHkv, Sq, Skv, plan, "svgb_attn_fwd_gqa")) return -1;
   SVGB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
@@ -919,6 +978,7 @@ int svgb_attn_fwd_strided(const void* q, const void* k, const void* v, void* o, 
                           int Hkv, int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
                           const long long* v_strides, const long long* o_strides, float sm_scale,
                           const svgb_plan* plan, const void* plan_ws, void* stream) {
+  if (no_split_plan(plan, "svgb_attn_fwd_strided")) return -1;
   Strides st[4];
   if (attn_strided_check(B, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st,
                          "svgb_attn_fwd_strided"))
@@ -934,6 +994,7 @@ int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, cons
                                const long long* v_strides, const long long* o_strides, float sm_scale,
                                const svgb_plan* plan, const void* plan_ws, void* stream) {
   const char* who = "svgb_attn_fwd_strided_e4m3";
+  if (no_split_plan(plan, who)) return -1;
   SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
                who, D);
   SVGB_REQUIRE(q_scale && k_scale && v_scale,
@@ -965,6 +1026,7 @@ int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v,
                                     float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
   const char* who = "svgb_attn_fwd_kvcache_e4m3_rows";
   SVGB_REQUIRE(plan, "null pointer");
+  if (no_split_plan(plan, who)) return -1;
   SVGB_REQUIRE(plan->kind == SVGB_PLAN_KVCACHE,
                "%s takes KV-cache plans (svgb_attn_plan_kvcache) only (kind %d): per-row scales live beside the cache "
                "rows", who, plan->kind);
@@ -985,6 +1047,77 @@ int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v,
   return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, 1, Hq,
                       Hq / Hkv, Sq, num_blocks * block_rows, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws,
                       stream, block_rows);
+}
+
+int svgb_attn_fwd_kvcache_split_bytes(int num_splits, int rows, int Hq, int D, size_t* bytes) {
+  SVGB_REQUIRE(num_splits >= 1 && rows > 0 && Hq > 0 && (D == 64 || D == 128) && bytes,
+               "bad arguments (num_splits=%d, rows=%d, Hq=%d, D=%d)", num_splits, rows, Hq, D);
+  const size_t n = static_cast<size_t>(num_splits) * rows * Hq;
+  *bytes = n * D * sizeof(float) + n * sizeof(float);
+  return 0;
+}
+
+int svgb_attn_fwd_kvcache_split(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
+                                const float* v_scale, void* o, float* lse, int dtype, int row_scales, int B, int Hq,
+                                int Hkv, int Sq, int num_blocks, int block_rows, int D, const long long* q_strides,
+                                const long long* k_strides, const long long* v_strides, const long long* o_strides,
+                                float sm_scale, const svgb_plan* plan, const void* plan_ws, void* ws, size_t ws_bytes,
+                                void* stream) {
+  const char* who = "svgb_attn_fwd_kvcache_split";
+  SVGB_REQUIRE(plan && ws, "null pointer");
+  SVGB_REQUIRE(plan->kind == SVGB_PLAN_KVCACHE_SPLIT,
+               "%s takes split KV-cache plans (svgb_attn_plan_kvcache_split) only (kind %d)", who, plan->kind);
+  SVGB_REQUIRE(B > 0 && Sq > 0 && static_cast<long long>(B) * Sq == plan->S,
+               "%s: the plan was built for %d query rows, called with B=%d streams of Sq=%d", who, plan->S, B, Sq);
+  const int items = B * ((Sq + kItemRows - 1) / kItemRows);  // items per split
+  SVGB_REQUIRE(plan->max_items > 0 && plan->max_items % items == 0,
+               "%s: the plan's %d items are no whole number of splits of %d items (B=%d, Sq=%d)", who, plan->max_items,
+               items, B, Sq);
+  const int nsplit = plan->max_items / items;
+  const bool e4m3 = dtype == SVGB_E4M3;
+  SVGB_REQUIRE(e4m3 || dtype == SVGB_BF16 || dtype == SVGB_F16, "%s: dtype %d unsupported", who, dtype);
+  if (e4m3) {
+    SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
+                 who, D);
+    SVGB_REQUIRE(q_scale && k_scale && v_scale, "%s: an e4m3 cache needs the three scale tensors q_scale, k_scale and "
+                 "v_scale", who);
+    if (row_scales && kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
+  } else {
+    SVGB_REQUIRE(!q_scale && !k_scale && !v_scale && !row_scales,
+                 "%s: 16-bit inputs (dtype %d) take no scales; scales are for e4m3 caches", who, dtype);
+  }
+  SVGB_REQUIRE(num_blocks > 0 && block_rows > 0 && static_cast<long long>(num_blocks) * block_rows < (1ll << 31),
+               "%s: bad cache geometry (num_blocks=%d, block_rows=%d)", who, num_blocks, block_rows);
+  Strides st[4];
+  if (attn_strided_check(1, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st, who)) return -1;
+  if (e4m3)
+    for (int i = 0; i < 3; ++i)
+      SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
+                   "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
+                   st[i].b, st[i].h, st[i].r);
+  SVGB_REQUIRE(Hq % Hkv == 0, "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d", who, Hq,
+               Hkv);
+  const int R = plan->S;
+  size_t need = 0;
+  if (svgb_attn_fwd_kvcache_split_bytes(nsplit, R, Hq, D, &need)) return -1;
+  SVGB_REQUIRE(ws_bytes >= need, "%s: workspace too small: %zu < %zu", who, ws_bytes, need);
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "%s: the workspace must be 16-byte aligned", who);
+  // partials: o [n, R, Hq, D] (the split as its batch dimension), then lse [n, Hq, R]
+  float* o_part = static_cast<float*>(ws);
+  float* lse_part = o_part + static_cast<size_t>(nsplit) * R * Hq * D;
+  const Strides ps{static_cast<long long>(R) * Hq * D, D, static_cast<long long>(Hq) * D};
+  if (attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o_part, lse_part, nullptr, nullptr, nullptr,
+                   e4m3 ? SVGB_E4M3 : dtype, 1, Hq, Hq / Hkv, R, num_blocks * block_rows, D, st[0], st[1], st[2], ps,
+                   sm_scale, plan, plan_ws, stream, e4m3 && row_scales ? block_rows : 0, items))
+    return -1;
+  const bool bf16 = dtype != SVGB_F16;  // e4m3 caches give bf16 o
+  auto merge = D == 128 ? (bf16 ? kv_split_merge_kernel<128, true> : kv_split_merge_kernel<128, false>)
+                        : (bf16 ? kv_split_merge_kernel<64, true> : kv_split_merge_kernel<64, false>);
+  const long long warps = static_cast<long long>(R) * Hq;
+  merge<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      o_part, lse_part, nsplit, R, Hq, static_cast<uint16_t*>(o), st[3].r, st[3].h, lse);
+  SVGB_LAUNCH_OK();
+  return 0;
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

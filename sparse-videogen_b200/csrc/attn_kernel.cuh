@@ -608,9 +608,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     // batch element and head of the o store (the row gather: its one batch element), derived per stream rather than
     // kept live through the chunk loop, since the consumers are register-bound
     long long o_base = bh * args.o_head_stride;
+    float* lse_out = args.lse;
     if constexpr (!kGather) {
       const int bhe = ctaid_y_here(), batch = bhe / args.Hq;
       o_base = batch * args.o_batch_stride + (bhe - batch * args.Hq) * args.o_head_stride;
+      if (args.split_items) {  // split KV-cache plans: the fp32 partial o and LSE of this CTA's split
+        const int sp = static_cast<int>(blockIdx.x) / args.split_items;
+        o_base += sp * args.o_split_stride;
+        lse_out += static_cast<size_t>(sp) * gridDim.y * args.S;
+      }
     }
 #pragma unroll
     for (int v1 = 0; v1 < 2; ++v1) {
@@ -640,7 +646,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       if (args.lse && (lane & 3) == 0) {
         // natural-log LSE of the scaled scores; -inf for rows that saw no key
         const float lse = l > 0.f ? (m_run[v1] * crow(v1) + log2f(l)) * 0.6931471805599453f : -INFINITY;
-        args.lse[static_cast<size_t>(bh) * args.S + out_row] = lse;
+        lse_out[static_cast<size_t>(bh) * args.S + out_row] = lse;
       }
     }
   }

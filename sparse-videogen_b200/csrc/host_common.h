@@ -73,7 +73,9 @@ int kv_scale_rows_check(const float* k_scale, const float* v_scale, int block_ro
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
 // BH (svgb200.h); every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) {
-  if (p->kind == SVGB_PLAN_SEG || p->kind == SVGB_PLAN_SEG_T || p->kind == SVGB_PLAN_KVCACHE) return p->BH;
+  if (p->kind == SVGB_PLAN_SEG || p->kind == SVGB_PLAN_SEG_T || p->kind == SVGB_PLAN_KVCACHE ||
+      p->kind == SVGB_PLAN_KVCACHE_SPLIT)
+    return p->BH;
   return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S;
 }
 
@@ -107,6 +109,16 @@ inline int no_kvcache_backward(const svgb_plan* plan, const char* who) {
   SVGB_REQUIRE(plan, "null pointer");
   SVGB_REQUIRE(plan->kind != SVGB_PLAN_KVCACHE,
                "%s: a KV-cache plan (svgb_attn_plan_kvcache) has no backward; it runs forward only", who);
+  SVGB_REQUIRE(plan->kind != SVGB_PLAN_KVCACHE_SPLIT,
+               "%s: a split KV-cache plan (svgb_attn_plan_kvcache_split) has no backward; it runs forward only, on "
+               "svgb_attn_fwd_kvcache_split", who);
+  return 0;
+}
+
+// a split KV-cache plan writes fp32 partials that a merge combines: only svgb_attn_fwd_kvcache_split runs it
+inline int no_split_plan(const svgb_plan* plan, const char* who) {
+  SVGB_REQUIRE(!plan || plan->kind != SVGB_PLAN_KVCACHE_SPLIT,
+               "%s: a split KV-cache plan (svgb_attn_plan_kvcache_split) runs on svgb_attn_fwd_kvcache_split only", who);
   return 0;
 }
 

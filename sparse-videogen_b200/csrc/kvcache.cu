@@ -124,24 +124,28 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
 // sinks and those of the item's window, so the pages behind a window are never read -- classifies each from the band's
 // interval form on logical positions (seg_chunk_kind) and writes the kept ones, compacted with a ballot, with the
 // physical row its TMA box loads from and its logical index in the meta's high bits.
+// Split plans (nsplit > 1) repeat the B I items once per split, split-major: item s B I + i is split s of item i, and
+// visits the s-th piece of ceil(nvis / nsplit) of the item's nvis visited chunks (sinks first, then the window), so the
+// item's split lists, concatenated in split order, are its single-pass list.
 // =============================================================================================
 __global__ void __launch_bounds__(256)
 kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_idx, const int* __restrict__ table, int B,
-                int Sq, int Snew, int nblocks, int block_rows, int max_pages, int cap, int slots, int sink, int left,
-                int right, int* __restrict__ counts, int* __restrict__ kv, int2* __restrict__ chunks,
+                int Sq, int Snew, int nblocks, int block_rows, int max_pages, int cap, int slots, int nsplit, int sink,
+                int left, int right, int* __restrict__ counts, int* __restrict__ kv, int2* __restrict__ chunks,
                 int4* __restrict__ items) {
   const int lane = threadIdx.x & 31;
   const int per = (Sq + kItemRows - 1) / kItemRows;  // items per stream
   const int it = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (it == 0 && lane == 0) {
-    counts[0] = B * per;
+    counts[0] = nsplit * B * per;
     kv[0] = B;
     kv[1] = Sq;
   }
-  if (it >= B * per) return;
-  const int b = it / per, k = it - b * per;
+  if (it >= nsplit * B * per) return;
+  const int sp = it / (B * per), bi = it - sp * (B * per);
+  const int b = bi / per, k = bi - b * per;
   const int L = kv_len(__ldg(&seqlens[b]), Snew, cap);
-  if (k == 0 && lane == 0) kv[2 + b] = L;
+  if (sp == 0 && k == 0 && lane == 0) kv[2 + b] = L;
   const int r0 = b * Sq + k * kItemRows, nr = min(kItemRows, Sq - k * kItemRows);
   SegOrigin o;
   o.shift = (b + 1) * Sq - L;
@@ -154,13 +158,15 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
   const int jlo = max(ns, static_cast<int>(lo / kChunkCols));
   const int jhi = hi < lo ? -1 : min(nch - 1, static_cast<int>(hi / kChunkCols));
   const int nvis = ns + max(0, jhi - jlo + 1);
+  const int piece = (nvis + nsplit - 1) / nsplit;  // this split's visited chunks: [v_lo, v_hi)
+  const int v_lo = min(nvis, sp * piece), v_hi = min(nvis, v_lo + piece);
   const int list = it * slots;
   int n = 0;
-  for (int v0 = 0; v0 < nvis; v0 += 32) {
+  for (int v0 = v_lo; v0 < v_hi; v0 += 32) {
     const int vi = v0 + lane;
     const int j = vi < ns ? vi : jlo + (vi - ns);
     const int c0 = j * kChunkCols, valid = min(kChunkCols, L - c0);
-    const int kind = vi < nvis ? seg_chunk_kind(false, r0, r0 + nr - 1, c0, c0 + valid - 1, o, left, right) : 0;
+    const int kind = vi < v_hi ? seg_chunk_kind(false, r0, r0 + nr - 1, c0, c0 + valid - 1, o, left, right) : 0;
     const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
     const int at = n + __popc(m & ((1u << lane) - 1u));
     if (kind != 0 && at < slots) {
@@ -174,30 +180,33 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
 }
 
 // Workspace of a KV-cache plan, 16-byte aligned pieces:
-//   counts (16 B) | {B, Sq, L_0 .. L_B-1} | items 2 int4 [B I] | chunks [B I slots]
+//   counts (16 B) | {B, Sq, L_0 .. L_B-1} | items 2 int4 [nsplit B I] | chunks [nsplit B I slots]
 // with I = ceil(Sq / 256) items per stream and slots = min(ceil(cap / 128), ceil(sink / 128) + (255 + left + right) / 128
-// + 2), the chunks an item can visit: its sinks and the window of its 256 rows
+// + 2), the chunks an item can visit: its sinks and the window of its 256 rows; a split plan's items have
+// ceil(slots / nsplit) slots each, the most a split's piece can hold
 struct KvLayout {
   long long items, slots;
   size_t items_off, chunks_off, bytes;
 };
-static KvLayout kv_layout(int B, int Sq, int cap, int sink, int left, int right) {
+static KvLayout kv_layout(int B, int Sq, int cap, int sink, int left, int right, int nsplit = 1) {
   KvLayout L;
-  L.items = static_cast<long long>(B) * ((Sq + kItemRows - 1) / kItemRows);
+  L.items = static_cast<long long>(nsplit) * B * ((Sq + kItemRows - 1) / kItemRows);
   const long long win = (static_cast<long long>(sink) + kChunkCols - 1) / kChunkCols +
                         (kItemRows - 1 + static_cast<long long>(left) + right) / kChunkCols + 2;
-  L.slots = std::min<long long>((static_cast<long long>(cap) + kChunkCols - 1) / kChunkCols, win);
+  const long long slots = std::min<long long>((static_cast<long long>(cap) + kChunkCols - 1) / kChunkCols, win);
+  L.slots = (slots + nsplit - 1) / nsplit;
   L.items_off = SVGB_PLAN_SEG_BOUNDS_OFF + align_up(sizeof(int) * (2 + static_cast<size_t>(B)), 16);
   L.chunks_off = L.items_off + 2 * sizeof(int4) * L.items;
   L.bytes = L.chunks_off + sizeof(int2) * L.items * L.slots;
   return L;
 }
 
-static int kv_plan_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {
+static int kv_plan_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes, int nsplit = 1) {
   SVGB_REQUIRE(B > 0 && Sq > 0 && cap > 0 && bytes, "bad arguments (B=%d, Sq=%d, capacity=%d)", B, Sq, cap);
   SVGB_REQUIRE(sink >= 0 && left >= 0 && right >= 0,
                "KV-cache plan: sink (%d), left (%d) and right (%d) must be >= 0", sink, left, right);
-  *bytes = kv_layout(B, Sq, cap, sink, left, right).bytes;
+  SVGB_REQUIRE(nsplit >= 1, "split KV-cache plan: num_splits (%d) must be >= 1", nsplit);
+  *bytes = kv_layout(B, Sq, cap, sink, left, right, nsplit).bytes;
   return 0;
 }
 
@@ -292,6 +301,46 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
   return 0;
 }
 
+// both planners: svgb_attn_plan_kvcache's plan (nsplit = 1, split = false: SVGB_PLAN_KVCACHE) and the split plan of
+// svgb_attn_plan_kvcache_split (SVGB_PLAN_KVCACHE_SPLIT)
+static int kv_plan_run(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table, int B,
+                       int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left, int right,
+                       int nsplit, bool split, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
+                       const char* who) {
+  SVGB_REQUIRE(cache_seqlens && plan_ws && plan, "null pointer");
+  SVGB_REQUIRE(Snew >= 0, "%s: Snew=%d < 0", who, Snew);
+  int cap = 0;
+  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
+  size_t need = 0;
+  if (kv_plan_bytes(B, Sq, cap, sink, left, right, &need, nsplit)) return -1;
+  SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
+  SVGB_REQUIRE(static_cast<long long>(B) * Sq < (1ll << 30), "%s: B * Sq = %lld query rows too many", who,
+               static_cast<long long>(B) * Sq);
+  const KvLayout L = kv_layout(B, Sq, cap, sink, left, right, nsplit);
+  SVGB_REQUIRE(L.items * L.slots < (1ll << 31) && L.items < (1ll << 31), "plan too large for 32-bit chunk offsets");
+  plan->kind = split ? SVGB_PLAN_KVCACHE_SPLIT : SVGB_PLAN_KVCACHE;
+  plan->BH = num_blocks * block_rows;  // a KV-cache plan serves every head: BH holds the cache rows (svgb200.h)
+  plan->S = B * Sq;
+  plan->max_items = static_cast<int>(L.items);
+  plan->items_stride = 0;
+  plan->mask_mode = MASK_LOCAL;
+  plan->m0 = sink;
+  plan->m1 = left;
+  plan->m2 = right;
+  plan->counts_off = 0;
+  plan->items_off = static_cast<int64_t>(L.items_off);
+  plan->chunks_off = static_cast<int64_t>(L.chunks_off);
+  plan->bytes = static_cast<int64_t>(need);
+  char* ws = static_cast<char*>(plan_ws);
+  kv_lists_kernel<<<static_cast<unsigned>((L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, cap,
+      static_cast<int>(L.slots), nsplit, sink, left, right, reinterpret_cast<int*>(ws),
+      reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF), reinterpret_cast<int2*>(ws + L.chunks_off),
+      reinterpret_cast<int4*>(ws + L.items_off));
+  SVGB_LAUNCH_OK();
+  return 0;
+}
+
 extern "C" {
 
 int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
@@ -336,38 +385,23 @@ int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int
 int svgb_attn_plan_kvcache(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table,
                            int B, int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left,
                            int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
-  const char* who = "svgb_attn_plan_kvcache";
-  SVGB_REQUIRE(cache_seqlens && plan_ws && plan, "null pointer");
-  SVGB_REQUIRE(Snew >= 0, "%s: Snew=%d < 0", who, Snew);
-  int cap = 0;
-  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
-  size_t need = 0;
-  if (kv_plan_bytes(B, Sq, cap, sink, left, right, &need)) return -1;
-  SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(static_cast<long long>(B) * Sq < (1ll << 30), "%s: B * Sq = %lld query rows too many", who,
-               static_cast<long long>(B) * Sq);
-  const KvLayout L = kv_layout(B, Sq, cap, sink, left, right);
-  SVGB_REQUIRE(L.items * L.slots < (1ll << 31), "plan too large for 32-bit chunk offsets");
-  plan->kind = SVGB_PLAN_KVCACHE;
-  plan->BH = num_blocks * block_rows;  // a KV-cache plan serves every head: BH holds the cache rows (svgb200.h)
-  plan->S = B * Sq;
-  plan->max_items = static_cast<int>(L.items);
-  plan->items_stride = 0;
-  plan->mask_mode = MASK_LOCAL;
-  plan->m0 = sink;
-  plan->m1 = left;
-  plan->m2 = right;
-  plan->counts_off = 0;
-  plan->items_off = static_cast<int64_t>(L.items_off);
-  plan->chunks_off = static_cast<int64_t>(L.chunks_off);
-  plan->bytes = static_cast<int64_t>(need);
-  char* ws = static_cast<char*>(plan_ws);
-  kv_lists_kernel<<<static_cast<unsigned>((L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, cap,
-      static_cast<int>(L.slots), sink, left, right, reinterpret_cast<int*>(ws), reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF),
-      reinterpret_cast<int2*>(ws + L.chunks_off), reinterpret_cast<int4*>(ws + L.items_off));
-  SVGB_LAUNCH_OK();
-  return 0;
+  return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
+                     left, right, 1, false, plan_ws, ws_bytes, plan, stream, "svgb_attn_plan_kvcache");
+}
+
+int svgb_attn_plan_kvcache_split_bytes(int B, int Sq, int cap, int sink, int left, int right, int num_splits,
+                                       size_t* bytes) {
+  return kv_plan_bytes(B, Sq, cap, sink, left, right, bytes, num_splits);
+}
+
+int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
+                                 int max_pages, int sink, int left, int right, int num_splits, void* plan_ws,
+                                 size_t ws_bytes, svgb_plan* plan, void* stream) {
+  const char* who = "svgb_attn_plan_kvcache_split";
+  SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
+  return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
+                     left, right, num_splits, true, plan_ws, ws_bytes, plan, stream, who);
 }
 
 }  // extern "C"

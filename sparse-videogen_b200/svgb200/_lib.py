@@ -57,6 +57,8 @@ _PROTOS = {
                                       _pll, _pll, _vp, _vp, _vp],
     "svgb_attn_plan_kvcache_bytes": [_i, _i, _i, _i, _i, _i, _psz],
     "svgb_attn_plan_kvcache": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_kvcache_split_bytes": [_i, _i, _i, _i, _i, _i, _i, _psz],
+    "svgb_attn_plan_kvcache_split": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                       _pplan, _vp, _vp],
     "svgb_attn_fwd_kv": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan, _vp,
@@ -70,6 +72,9 @@ _PROTOS = {
     "svgb_quantize_e4m3": [_vp, _i, _vp, _vp, _i, _i, _i, _vp],
     "svgb_attn_fwd_kvcache_e4m3_rows": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _pll, _pll,
                                         _pll, _pll, _f, _pplan, _vp, _vp],
+    "svgb_attn_fwd_kvcache_split_bytes": [_i, _i, _i, _i, _psz],
+    "svgb_attn_fwd_kvcache_split": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _pll,
+                                    _pll, _pll, _pll, _f, _pplan, _vp, _vp, _sz, _vp],
     "svgb_quantize_e4m3_rows": [_vp, _i, _vp, _vp, _i, _i, _i, _ll, _ll, _vp],
     "svgb_attn_bwd_bytes": [_i, _i, _psz],
     "svgb_attn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _f, _pplan, _vp, _pplan,

@@ -18,6 +18,7 @@ MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_
 MASK_LOCAL = 10
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
 PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T, PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE = 1, 2, 3, 4, 5, 6, 7
+PLAN_KVCACHE_SPLIT = 8
 # SVGB_PLAN_SEG_BOUNDS_OFF: a segment plan's {nseg, cu_q, cu_k} in its workspace, a KV-cache plan's {B, Sq, L_b}
 SEG_BOUNDS_OFF = 16
 _E4M3 = 2  # SVGB_E4M3 (the 16-bit dtype ids come from _dt)
@@ -94,7 +95,7 @@ class AttnPlan:
         """Key/value length: a rectangular variable-block plan records it in m0, a segment plan (which serves every
         head) in BH, and so does a KV-cache plan (the cache's rows) (include/svgb200.h, svgb_plan)."""
         d = self.desc
-        if d.kind in (PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE):
+        if d.kind in (PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE, PLAN_KVCACHE_SPLIT):
             return d.BH
         return d.m0 if d.kind == PLAN_VARBLOCK and d.m0 > 0 else d.S
 
@@ -132,6 +133,9 @@ class AttnPlan:
             elif d.kind == PLAN_KVCACHE:
                 raise SvgbError("attention backward: a KV-cache plan (plan_kvcache) has no backward; it runs forward "
                                 "only, as flash_attn_with_kvcache does")
+            elif d.kind == PLAN_KVCACHE_SPLIT:
+                raise SvgbError("attention backward: a split KV-cache plan (plan_kvcache(num_splits=)) has no "
+                                "backward; it runs forward only")
             else:
                 raise SvgbError(f"attention backward: plan kind {d.kind} has no key-major form")
         return self._key_major
@@ -378,7 +382,7 @@ def _row_scales(who, k_scale, v_scale, cache):
 def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0, cache_len: Optional[int] = None,
                  block_table: Optional[torch.Tensor] = None, page_size: Optional[int] = None,
                  cache_batch_idx: Optional[torch.Tensor] = None, causal: bool = False, window_size=(-1, -1),
-                 sink: int = 0) -> AttnPlan:
+                 sink: int = 0, num_splits: int = 1, num_heads: Optional[int] = None) -> AttnPlan:
     """Attention of B streams of q_len queries into a KV cache, in FlashAttention's conventions
     (flash_attn_with_kvcache): stream b holds L_b = cache_seqlens[b] + new_len keys (new_len rows appended before this
     attention, e.g. by kvcache_append) and its query i sits at logical position L_b - q_len + i.  Query p sees key kv
@@ -387,7 +391,11 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
     The cache is k_cache.shape[0] = num_blocks blocks: contiguous, cache_len = S_cache rows each (stream b in block
     cache_batch_idx[b], default b), or paged, page_size rows each (a multiple of 128) with block_table int [B, max_pages].
     cache_seqlens: int or device int tensor [B]; nothing is read on the host.  attn_fwd runs the plan on q [B, q_len, Hq,
-    D] and the cache, any Hq = G * Hkv; it has no backward (attention() under grad and key_major() raise)."""
+    D] and the cache, any Hq = G * Hkv; it has no backward (attention() under grad and key_major() raise).
+    num_splits: 1 is the single pass, one CTA per 256-query item and head.  n > 1 splits every item's keys into n pieces
+    (svgb_attn_plan_kvcache_split), which attn_fwd runs as n times the CTAs writing fp32 partials and a merge, so that
+    decode and short chunks fill the GPU.  0 picks n on the host from the SM count, the CTAs B ceil(q_len / 256)
+    num_heads (num_heads = q's heads, required then) and the chunk slots per item (kvcache_num_splits)."""
     if block_table is not None:
         B = block_table.shape[0]
         if page_size is None:
@@ -415,16 +423,69 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
         right = 0
     # -1: no query position lies further than cap + Sq from a key
     left, right = (min(cap + Sq, 2**31 - 1) if w == -1 else w for w in (left, right))
+    n = int(num_splits)
+    if n < 0:
+        raise SvgbError(f"plan_kvcache: num_splits={n} must be >= 0 (0: automatic, 1: no split)")
+    if n == 0:
+        if num_heads is None:
+            raise SvgbError("plan_kvcache: num_splits=0 picks the split count from the grid, so it needs num_heads (q's "
+                            "query heads)")
+        n = kvcache_num_splits(B * -(-Sq // 256) * int(num_heads), _kvcache_slots(cap, int(sink), left, right),
+                               _sm_count())
     nbytes = C.c_size_t()
-    check(lib().svgb_attn_plan_kvcache_bytes(B, Sq, cap, int(sink), left, right, C.byref(nbytes)),
-          "svgb_attn_plan_kvcache_bytes")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the lengths
     desc = Plan()
-    check(lib().svgb_attn_plan_kvcache(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks), rows,
-                                       max_pages, int(sink), left, right, ws.data_ptr(), ws.numel(), C.byref(desc),
-                                       torch.cuda.current_stream(device).cuda_stream), "svgb_attn_plan_kvcache")
+    stream = torch.cuda.current_stream(device).cuda_stream
+    if n == 1:
+        check(lib().svgb_attn_plan_kvcache_bytes(B, Sq, cap, int(sink), left, right, C.byref(nbytes)),
+              "svgb_attn_plan_kvcache_bytes")
+        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the lengths
+        check(lib().svgb_attn_plan_kvcache(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks), rows,
+                                           max_pages, int(sink), left, right, ws.data_ptr(), ws.numel(), C.byref(desc),
+                                           stream), "svgb_attn_plan_kvcache")
+    else:
+        check(lib().svgb_attn_plan_kvcache_split_bytes(B, Sq, cap, int(sink), left, right, n, C.byref(nbytes)),
+              "svgb_attn_plan_kvcache_split_bytes")
+        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
+        check(lib().svgb_attn_plan_kvcache_split(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks),
+                                                 rows, max_pages, int(sink), left, right, n, ws.data_ptr(), ws.numel(),
+                                                 C.byref(desc), stream), "svgb_attn_plan_kvcache_split")
     _bump()
     return AttnPlan(desc, ws, (B, Sq))
+
+
+# The automatic split count of plan_kvcache(num_splits=0), from tools/kvcache_perf.py on the H100 (DESIGN.md): split only
+# while the single pass leaves SMs idle, into the fewest splits whose grid fills its last wave to _SPLIT_WAVE_FILL (or,
+# when no count does, the most that fit in one wave), with at least _SPLIT_MIN_SLOTS chunk slots per split and at most
+# _SPLIT_MAX splits (the merge reads every split).
+_SPLIT_WAVE_FILL, _SPLIT_MIN_SLOTS, _SPLIT_MAX = 0.85, 4, 32
+
+
+def kvcache_num_splits(ctas: int, slots: int, num_sms: int) -> int:
+    """Split count for a KV-cache attention of `ctas` single-pass CTAs (B ceil(Sq / 256) Hq) whose items have `slots`
+    chunk slots, on `num_sms` SMs (the kernel fits one CTA per SM): 1 once the single pass fills the machine."""
+    if ctas >= num_sms:
+        return 1
+    top = min(_SPLIT_MAX, slots // _SPLIT_MIN_SLOTS)
+    for n in range(2, top + 1):
+        waves = -(-n * ctas // num_sms)
+        if n * ctas >= _SPLIT_WAVE_FILL * waves * num_sms:
+            return n
+    return max(1, min(top, num_sms // ctas))
+
+
+def _kvcache_slots(cap, sink, left, right):
+    """Chunk slots per item of a KV-cache plan (include/svgb200.h, svgb_attn_plan_kvcache_bytes)."""
+    return min(-(-cap // 128), -(-sink // 128) + (255 + left + right) // 128 + 2)
+
+
+_sms: Optional[int] = None
+
+
+def _sm_count() -> int:
+    global _sms
+    if _sms is None:
+        _sms = device_check()[2]
+    return _sms
 
 
 def _is_profiling(mask_mode: int) -> bool:
@@ -563,7 +624,7 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     k_scale, v_scale: the scales of float8_e4m3fn caches under a KV-cache plan, per key/value head [Hkv] or per cache row
     [num_blocks, Hkv, block_rows] (see _attn_kvcache)."""
     _need_cuda(q, k, v)
-    if plan.desc.kind == PLAN_KVCACHE:
+    if plan.desc.kind in (PLAN_KVCACHE, PLAN_KVCACHE_SPLIT):
         if any(r is not None for r in (q_rows, kv_rows, o_rows)):
             raise SvgbError("a KV-cache plan (plan_kvcache) takes no row vectors (o_rows / q_rows / kv_rows)")
         return _attn_kvcache(q, k, v, plan, return_lse, sm_scale, out, k_scale, v_scale)
@@ -621,6 +682,13 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=
     Hq, D = q.shape[2:]
     qf = _addressed(q.reshape(B * Sq, Hq, D), "shd")
     kf, vf = (_addressed(c.flatten(0, 1), "shd") for c in (k_cache, v_cache))
+    if plan.desc.kind == PLAN_KVCACHE_SPLIT:
+        if q.shape[3] != k_cache.shape[3] or Hq % k_cache.shape[2]:
+            raise SvgbError(f"q {tuple(q.shape)} and the cache {tuple(k_cache.shape)} differ in D, or q's heads are no "
+                            "multiple of the cache's")
+        o = _split_out(out, B * Sq, Hq, D, q.dtype, q.device)
+        lse = _split_fwd(qf, _st(qf, "shd"), kf, vf, None, o, plan, _dt(q), 0, k_cache.shape, return_lse, sm_scale)
+        return _split_result(o, lse, out, B, Sq, return_lse)
     of = torch.empty_like(qf)
     res = _attn(qf, kf, vf, of, plan, "shd", _dt(q), (None, None, None), (None, None, None), return_lse, sm_scale)
     o = of.view(B, Sq, Hq, D)
@@ -630,6 +698,50 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=
     if not return_lse:
         return o
     return o, res[1].view(Hq, B, Sq).transpose(0, 1)
+
+
+def _split_out(out, rows, Hq, D, dtype, device):
+    """o [rows, Hq, D] of a split forward: out itself when it is contiguous (the merge writes it in place), else new."""
+    if out is not None and out.is_contiguous():
+        return out.view(rows, Hq, D)
+    return torch.empty(rows, Hq, D, dtype=dtype, device=device)
+
+
+def _split_fwd(qf, q_strides, kf, vf, scales, o, plan, dtype, row_scales, cache_shape, return_lse, sm_scale):
+    """svgb_attn_fwd_kvcache_split under a split KV-cache plan: the attention into fp32 partials in a cached workspace,
+    then the merge into o [B Sq, Hq, D]; returns the lse [Hq, B Sq] or None.  Two launches.  scales: None (16-bit) or
+    (q_scale, k_scale, v_scale) of an e4m3 cache, per head (row_scales = 0) or per row (1)."""
+    B, Sq = plan.source
+    R, Hq, D = o.shape
+    nb, rows, Hkv = cache_shape[:3]
+    n = plan.desc.max_items // (B * -(-Sq // 256))
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_fwd_kvcache_split_bytes(n, R, Hq, D, C.byref(nbytes)), "svgb_attn_fwd_kvcache_split_bytes")
+    ws = workspace("kvcache_split", nbytes.value, o.device)
+    lse = torch.empty(Hq, R, dtype=torch.float32, device=o.device) if return_lse else None
+    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
+    fill = 16 if dtype == _E4M3 else 8
+    check(lib().svgb_attn_fwd_kvcache_split(qf.data_ptr(), kf.data_ptr(), vf.data_ptr(), *map(_p, scales or (None,) * 3),
+                                            o.data_ptr(), _p(lse), dtype, row_scales, B, Hq, Hkv, Sq, nb, rows, D,
+                                            q_strides, _st(kf, "shd", fill), _st(vf, "shd", fill), _st(o, "shd"), scale,
+                                            C.byref(plan.desc), plan.ws.data_ptr(), ws.data_ptr(), ws.numel(),
+                                            _stream(o)), "svgb_attn_fwd_kvcache_split")
+    _bump(2)
+    return lse
+
+
+def _split_result(o, lse, out, B, Sq, return_lse):
+    """o [B, Sq, Hq, D] (copied into an out= the merge could not write) and lse [B, Hq, Sq], as _attn_kvcache returns
+    them."""
+    Hq, D = o.shape[1:]
+    o = o.view(B, Sq, Hq, D)
+    if out is not None:
+        if o.data_ptr() != out.data_ptr():
+            out.copy_(o)
+        o = out
+    if not return_lse:
+        return o
+    return o, lse.view(Hq, B, Sq).transpose(0, 1)
 
 
 def _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
@@ -653,6 +765,11 @@ def _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_sc
     # per query head over the B * Sq rows of this call: the scale kernel takes [heads, rows, D]
     q8, q_scale = quantize_e4m3(q.reshape(B * Sq, Hq, D).transpose(0, 1).contiguous())
     kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))  # [rows, Hkv, D] views, read in place
+    if plan.desc.kind == PLAN_KVCACHE_SPLIT:
+        o = _split_out(out, B * Sq, Hq, D, torch.bfloat16, q.device)
+        lse = _split_fwd(q8, _st(q8[None], "bhsd", 16), kf, vf, (q_scale, ks, vs), o, plan, _E4M3, 0, k_cache.shape,
+                         return_lse, sm_scale)
+        return _split_result(o, lse, out, B, Sq, return_lse)
     o = torch.empty(B * Sq, Hq, D, dtype=torch.bfloat16, device=q.device)
     lse = torch.empty(Hq, B * Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
@@ -766,8 +883,8 @@ def attention(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Option
     LSE, and the plan is not read here."""
     if not needs_grad(q, k, v):
         return attn_fwd(q, k, v, plan, layout=layout, sm_scale=sm_scale)
-    if plan.desc.kind in (PLAN_GATHER, PLAN_KVCACHE) or (plan.desc.kind == PLAN_BAND and
-                                                          _is_profiling(plan.desc.mask_mode)):
+    if plan.desc.kind in (PLAN_GATHER, PLAN_KVCACHE, PLAN_KVCACHE_SPLIT) or (plan.desc.kind == PLAN_BAND and
+                                                                              _is_profiling(plan.desc.mask_mode)):
         plan.key_major()  # raises, naming what has no backward
     return _Attention.apply(q, k, v, plan, layout, sm_scale)
 
@@ -845,6 +962,11 @@ def _attn_kvcache_fp8_rows(q, k_cache, v_cache, plan, return_lse, sm_scale, out,
         raise SvgbError("attention into a KV cache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
     q8, q_scale = quantize_e4m3_rows(q.reshape(B * Sq, Hq, D))
     kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))  # [rows, Hkv, D] views, read in place
+    if plan.desc.kind == PLAN_KVCACHE_SPLIT:
+        o = _split_out(out, B * Sq, Hq, D, torch.bfloat16, q.device)
+        lse = _split_fwd(q8, _st(q8, "shd", 16), kf, vf, (q_scale, k_scale, v_scale), o, plan, _E4M3, 1, k_cache.shape,
+                         return_lse, sm_scale)
+        return _split_result(o, lse, out, B, Sq, return_lse)
     o = torch.empty(B * Sq, Hq, D, dtype=torch.bfloat16, device=q.device)
     lse = torch.empty(Hq, B * Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)

@@ -18,13 +18,18 @@ Wan 1.3B (12 heads) and Wan 14B (40 heads).  Ways, each one call sequence as a c
   rows append+paged  kvcache_append quantising the chunk's new rows per row into those pages, then plan + forward
   rows q quant    the per-row q quantisation alone (quantize_e4m3_rows on q in place)
 
+With --split, the split-KV table instead (plan_kvcache(num_splits=)): decode (Sq = 1) at 12 and 40 heads, the one-frame
+chunk (1 560 queries) at 12 heads and the three-frame chunk at 12 and 40 heads, against the same pages in bf16, in e4m3
+with per-head scales and in e4m3 with per-row scales, each as the single pass (n = 1), n = 2, 4, 8 and the automatic
+choice (n = 0, reported with the n it picked): plan + forward (+ merge) as a caller issues them.
+
 Besides the times: the bytes of each cache (K and V, one layer, and the per-row scales) and mean / max
 |o_fp8 - o_bf16| of the paged forward in both formats.
 
 Each figure is the median of R rounds with the rounds' min and max; every round times N back-to-back calls of each way
 with CUDA events, the ways alternated within every round.  The card name and power limit are read in the same run.
 
-    python tools/kvcache_perf.py [--rounds R] [--iters N] [--out FILE]
+    python tools/kvcache_perf.py [--rounds R] [--iters N] [--split] [--out FILE]
 """
 from __future__ import annotations
 
@@ -176,10 +181,62 @@ def case(H, dev, rounds, iters):
     return {**alternate(ways, rounds, iters), "fp8": fp8}
 
 
+SPLIT_ROWS = [("decode", 1, 12), ("decode", 1, 40), ("one frame", FRAME, 12), ("three frames", SQ, 12),
+              ("three frames", SQ, 40)]
+SPLITS = [1, 2, 4, 8, 0]
+
+
+def split_case(H, queries, dev, rounds, iters):
+    """One row of the split table: the ways of SPLITS in the three cache formats on the same 256-row pages."""
+    from svgb200 import core
+
+    g = torch.Generator(device=dev).manual_seed(H)
+    bf = torch.bfloat16
+    cap = ((L + PAGE - 1) // PAGE) * PAGE
+    npages = cap // PAGE
+    kp, vp = (torch.randn(npages, PAGE, H, D, device=dev, generator=g).to(bf) for _ in range(2))
+    q = torch.randn(1, queries, H, D, device=dev, generator=g).to(bf)
+    table = torch.randperm(npages, generator=torch.Generator().manual_seed(0)).to(torch.int32).view(1, npages).to(dev)
+    lens = torch.tensor([L], dtype=torch.int32, device=dev)
+    amax = lambda t: (t.float().abs().amax(dim=(0, 1, 3)) / 448).clamp_min(1e-12)  # noqa: E731
+    ks, vs = amax(kp), amax(vp)
+    e4m3 = lambda t, sc: (t.float() * (1 / sc)[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn)  # noqa: E731
+    e = lambda t: (lambda m, k: torch.where(m <= 0.875, k - 9, k - 8))(*torch.frexp(t.float().abs().amax(-1)))  # noqa: E731
+    ke, ve = e(kp).clamp(-126, 127), e(vp).clamp(-126, 127)
+    fmts = {"bf16": (kp, vp, {}),
+            "e4m3": (e4m3(kp, ks), e4m3(vp, vs), dict(k_scale=ks, v_scale=vs)),
+            "e4m3 rows": (*((t.float() * torch.exp2(-x.float())[..., None]).to(torch.float8_e4m3fn)
+                            for t, x in ((kp, ke), (vp, ve))),
+                          dict(zip(("k_scale", "v_scale"), (torch.exp2(x.float()).transpose(1, 2).contiguous()
+                                                            for x in (ke, ve)))))}
+
+    def way(k, v, kw, n):
+        def run():
+            plan = core.plan_kvcache(lens, q_len=queries, num_blocks=npages, block_table=table, page_size=PAGE,
+                                     causal=True, window_size=(LEFT, 0), sink=SINK, num_splits=n, num_heads=H)
+            return core.attn_fwd(q, k, v, plan, **kw)
+        return run
+
+    auto = core.plan_kvcache(lens, q_len=queries, num_blocks=npages, block_table=table, page_size=PAGE, causal=True,
+                             window_size=(LEFT, 0), sink=SINK, num_splits=0, num_heads=H)
+    n_auto = auto.desc.max_items // -(-queries // 256)
+    ways, diff = {}, {}
+    for f, (k, v, kw) in fmts.items():
+        ref = way(k, v, kw, 1)().float()
+        for n in SPLITS:
+            name = f"{f} n={n if n else 'auto'}"
+            ways[name] = way(k, v, kw, n)
+            diff[name] = (ways[name]().float() - ref).abs().max().item()  # the ways agree before they are timed
+            assert diff[name] < (3e-2 if f == "bf16" else 8e-2), (name, diff[name])
+    return {"auto_num_splits": n_auto, "ctas_single": -(-queries // 256) * H, **alternate(ways, rounds, iters),
+            "max_abs_diff_vs_single": diff}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--split", action="store_true", help="the split-KV table instead")
     ap.add_argument("--out")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -187,7 +244,12 @@ def main():
     dev = torch.device("cuda:0")
     res = {"card": card(), "rounds": a.rounds, "iters": a.iters,
            "shape": dict(queries=SQ, keys=L, sink=SINK, left=LEFT, page=PAGE, D=D)}
-    for name, H in (("wan1.3b", 12), ("wan14b", 40)):
+    if a.split:
+        for label, queries, H in SPLIT_ROWS:
+            name = f"{label}, {H} heads"
+            res[name] = split_case(H, queries, dev, a.rounds, a.iters)
+            print(json.dumps({name: res[name]}), flush=True)
+    for name, H in (() if a.split else (("wan1.3b", 12), ("wan14b", 40))):
         res[name] = case(H, dev, a.rounds, a.iters)
         print(json.dumps({name: res[name]}), flush=True)
     print(json.dumps(res))
