@@ -48,6 +48,15 @@ extern "C" {
  * Causal attention is (0, S, 0); FlashAttention's window_size = (l, r) is (0, l, r) with -1 taken as S; a streaming
  * sink-plus-window is (sink, l, 0).  SVGB_MASK_WAN(P, W) is SVGB_MASK_LOCAL(P, W, W).  Forward and backward. */
 #define SVGB_MASK_LOCAL 10
+/* Block-causal mask of autoregressive video (chunk-wise causal attention, CausVid / Self-Forcing).  Positions form blocks
+ * of C >= 1 whose ends lie at F, F + C, F + 2C, ... with 1 <= F <= C (a shorter first block: F < C); e(p) is the first
+ * block end greater than p.  With a window W >= C (W >= S: unbounded) and a sink >= 0:
+ *   allowed(q, kv) = (kv < sink) | (e(q) - W <= kv < e(q))
+ * m0 = sink, m1 = SVGB_BLOCK_M1(C, F) (C < 2^16), m2 = W.  Every row sees its whole block and all earlier ones (within
+ * the window); C = 1 is SVGB_MASK_LOCAL(sink, W - 1, 0).  The band planners refuse C < 1, F outside [1, C], W < C and a
+ * negative sink by name.  Forward and backward.  Mode 11 is unassigned. */
+#define SVGB_MASK_BLOCK_CAUSAL 12
+#define SVGB_BLOCK_M1(C, F) ((C) | ((C) - (F)) << 16)
 
 /* ---- library ---------------------------------------------------------------------------- */
 int svgb_version(void);
@@ -115,7 +124,7 @@ int svgb_attn_plan_varblock_gather(const uint8_t* map, const int32_t* row_sz, co
  * create_block_mask (svg/models/hyvideo/attention.py:527-551), and, with SVGB_MASK_LOCAL, behind causal and
  * sliding-window attention (a negative sink, left or right is an error).  Items are issued heaviest first: under
  * SVGB_MASK_LOCAL with left > right the query-major plan lists its items from the last rows back, and with right > left
- * the key-major plan does. */
+ * the key-major plan does; SVGB_MASK_BLOCK_CAUSAL is issued as its local band (sink, W - 1, 0). */
 int svgb_attn_plan_band_bytes(int S, size_t* bytes);
 int svgb_attn_plan_band(int mask_mode, int m0, int m1, int m2, int BH, int S, void* plan_ws,
                         size_t ws_bytes, svgb_plan* plan, void* stream);
@@ -248,6 +257,21 @@ int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* ca
                                  const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
                                  int max_pages, int sink, int left, int right, int num_splits, void* plan_ws,
                                  size_t ws_bytes, svgb_plan* plan, void* stream);
+/* Block-causal KV-cache plan (SVGB_MASK_BLOCK_CAUSAL on logical positions, query i of stream b at L_b - Sq + i): the
+ * arguments of svgb_attn_plan_kvcache_split with (window, block, first_block) = (W, C, F) in place of (left, right).
+ * When the Sq queries of a call form one block (F chosen so that a block ends at L_b), they all attend
+ * [L_b - W, L_b) plus the sinks.  Refuses C outside [1, 2^16), F outside [1, C], W < C, a negative sink and
+ * num_splits < 1 by name.  num_splits = 1 is a single plan (plan->kind = SVGB_PLAN_KVCACHE, run as
+ * svgb_attn_plan_kvcache's), n > 1 a split plan (SVGB_PLAN_KVCACHE_SPLIT, run as svgb_attn_plan_kvcache_split's);
+ * mask_mode = SVGB_MASK_BLOCK_CAUSAL, m0..m2 = sink, SVGB_BLOCK_M1(C, F), W.  Each item visits the chunks of its sinks
+ * and of [e(p0) - W, e(p1) - 1] for its first and last positions p0, p1.  Workspace: the _bytes of
+ * svgb_attn_plan_kvcache_split (of svgb_attn_plan_kvcache at n = 1) with left = W - 1 and right = C - 1. */
+int svgb_attn_plan_kvcache_block_bytes(int B, int Sq, int cap, int sink, int window, int block, int first_block,
+                                       int num_splits, size_t* bytes);
+int svgb_attn_plan_kvcache_block(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
+                                 int max_pages, int sink, int window, int block, int first_block, int num_splits,
+                                 void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
 
 /* ---- attention -------------------------------------------------------------------------- */
 /* o = softmax(q k^T * sm_scale  [masked by plan]) v, per head.  Stands behind

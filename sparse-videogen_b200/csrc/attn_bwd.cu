@@ -63,9 +63,10 @@ static int attn_bwd_run(const void* q, const void* k, const void* v, const void*
                                                    : SVGB_PLAN_VARBLOCK;
   SVGB_REQUIRE(plan_t->kind == kind_t, "plan_t (kind %d) is not the key-major companion of a kind-%d plan",
                plan_t->kind, plan->kind);
-  SVGB_REQUIRE((plan->mask_mode >= MASK_NONE && plan->mask_mode <= MASK_COG) || plan->mask_mode == MASK_LOCAL,
-               "attention backward supports the executed band masks NONE / HY / WAN / COG / LOCAL (mask mode %d)",
-               plan->mask_mode);
+  SVGB_REQUIRE((plan->mask_mode >= MASK_NONE && plan->mask_mode <= MASK_COG) || plan->mask_mode == MASK_LOCAL ||
+                   plan->mask_mode == MASK_BLOCK_CAUSAL,
+               "attention backward supports the executed band masks NONE / HY / WAN / COG / LOCAL / BLOCK_CAUSAL (mask "
+               "mode %d)", plan->mask_mode);
   // a variable-block plan's m0 is its Skv (svgb200.h), checked with the lengths below
   SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK ||
                    (plan_t->mask_mode == plan->mask_mode && plan_t->m0 == plan->m0 && plan_t->m1 == plan->m1 &&

@@ -72,7 +72,20 @@ enum MaskMode : int {
   //   m0 = sink, m1 = left, m2 = right (all >= 0)   : kv < sink | (q - kv <= left & kv - q <= right)
   // MASK_WAN(P, W) is MASK_LOCAL(P, W, W).
   MASK_LOCAL = 10,
+  // Block-causal mask of autoregressive video (chunk-wise causal, CausVid / Self-Forcing): positions form blocks of C
+  // with ends at F, F + C, F + 2C, ... (1 <= F <= C), e(q) the first end past q, and
+  //   m0 = sink, m1 = C | (C - F) << 16, m2 = W >= C   : kv < sink | (e(q) - W <= kv < e(q))
+  // With q rounded to its block's last position e(q) - 1 (block_last) it is MASK_LOCAL(sink, W - 1, 0); W >= C keeps
+  // every row's own block.  Mode 11 is unassigned.
+  MASK_BLOCK_CAUSAL = 12,
 };
+
+// MASK_BLOCK_CAUSAL: the last position e(p) - 1 of p's block, m1 = C | (C - F) << 16.  Positions before the first
+// block end (negative ones too: KV-cache queries ahead of their keys) belong to the first block.
+__host__ __device__ inline int block_last(int p, int m1) {
+  const int C = m1 & 0xffff, F = C - (m1 >> 16);
+  return p < F ? F - 1 : p + (C - 1) - (p - F) % C;
+}
 
 __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, int m1, int m2) {
   // reference semantics, written branch-free (bitwise) so warps do not diverge on it
@@ -89,6 +102,10 @@ __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, in
       return (kv < m0) | (d <= m2);
     case MASK_LOCAL:
       return (kv < m0) | ((q - kv <= m1) & (kv - q <= m2));
+    case MASK_BLOCK_CAUSAL: {
+      const int e = block_last(q, m1);
+      return (kv < m0) | ((kv <= e) & (e - kv <= m2 - 1));
+    }
     case MASK_COG:
       return (kv < m0) | (q < m1) | (d < m2);
     case MASK_PROF_COG_S: {
@@ -202,7 +219,7 @@ __host__ __device__ inline int seg_chunk_kind(bool key_major, int r0, int r1, in
 struct ElemMask {
   int mode, m0, m1, m2;
   // per query row, one register (the kernel is register-bound):
-  //   direct families: the query position
+  //   direct families: the query position (block-causal: its block's last position, evaluated as MASK_LOCAL)
   //   banded profiling masks: band_lo = qblk - thres + 1, the first key block of the row's band, so that
   //   |qblk - kblk| < thres <=> (unsigned)(kblk - band_lo) < 2*thres - 1; or kRowOut when the query lies outside
   //   the banded part (every key then gives Prof::outside_val)
@@ -235,8 +252,14 @@ struct ElemMask {
 
   __device__ __forceinline__ void init(int mode_, const int (&qm)[2], int m0_, int m1_, int m2_) {
     mode = mode_; m0 = m0_; m1 = m1_; m2 = m2_;
+    const bool block = mode == MASK_BLOCK_CAUSAL;
 #pragma unroll
-    for (int v1 = 0; v1 < 2; ++v1) row[v1] = qm[v1];
+    for (int v1 = 0; v1 < 2; ++v1) row[v1] = block ? block_last(qm[v1], m1_) : qm[v1];
+    if (block) {  // rows rounded to their block ends: the local band (sink, W - 1, 0), no division per element
+      mode = MASK_LOCAL;
+      m1 = m2_ - 1;
+      m2 = 0;
+    }
     if (!banded(mode)) return;
     const Prof p = prof();
 #pragma unroll

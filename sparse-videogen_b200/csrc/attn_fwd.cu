@@ -214,8 +214,14 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
   const int k = item - segs.item_base[seg];
   const int q_row0 = segs.bound[seg] + (segs.reversed[seg] ? segs.item_cnt[seg] - 1 - k : k) * kItemRows;
   const int nrows = min(kItemRows, segs.bound[seg + 1] - q_row0);
-  const int q = q_row0 + threadIdx.x;
+  int q = q_row0 + threadIdx.x;
   const bool row_live = static_cast<int>(threadIdx.x) < nrows;
+  if (mode == MASK_BLOCK_CAUSAL && !transposed) {  // the row's block end, once: then the local band, as the kernel does
+    q = block_last(q, m1);
+    mode = MASK_LOCAL;
+    m1 = m2 - 1;
+    m2 = 0;
+  }
   int2* out = chunks + static_cast<size_t>(item) * n_chunks_total;
   int n = 0;
   for (int c = 0; c < n_chunks_total; ++c) {
@@ -247,7 +253,14 @@ __global__ void plan_band_kernel(int mode, int m0, int m1, int m2, int S, int n_
 // are seen by every query and form the heavy first segment.  A one-sided local band (left != right) makes list length
 // grow along the rows: query-major with left > right the last rows see the most keys, key-major with right > left the
 // last keys are reached by the most queries, and that segment's items are then issued from its end (LPT).
+// The block-causal mask segments as its local band (sink, W - 1, 0): its query-major items run from the last rows back
+// when W > 1 (an unbounded window gives the last blocks the longest lists), key-major the sink keys come first.
 static BandSegs band_segments(int mode, int m0, int m1, int m2, int S, bool transposed = false) {
+  if (mode == MASK_BLOCK_CAUSAL) {
+    mode = MASK_LOCAL;
+    m1 = m2 - 1;
+    m2 = 0;
+  }
   int cuts[4], nc = 0;
   auto add = [&](int c) {
     if (c > 0 && c < S && (nc == 0 || cuts[nc - 1] < c)) cuts[nc++] = c;
@@ -865,9 +878,13 @@ static int plan_band_impl(int mask_mode, int m0, int m1, int m2, int BH, int S, 
   if (svgb_attn_plan_band_bytes(S, &need)) return -1;
   SVGB_REQUIRE(plan_ws && plan, "null pointer");
   SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(mask_mode >= MASK_NONE && mask_mode <= MASK_LOCAL, "unknown mask mode %d", mask_mode);
+  SVGB_REQUIRE((mask_mode >= MASK_NONE && mask_mode <= MASK_LOCAL) || mask_mode == MASK_BLOCK_CAUSAL,
+               "unknown mask mode %d", mask_mode);
   SVGB_REQUIRE(mask_mode != MASK_LOCAL || (m0 >= 0 && m1 >= 0 && m2 >= 0),
                "local mask: sink (m0 = %d), left (m1 = %d) and right (m2 = %d) must be >= 0", m0, m1, m2);
+  if (mask_mode == MASK_BLOCK_CAUSAL &&
+      block_causal_check(m0, m1, m2, transposed ? "svgb_attn_plan_band_t" : "svgb_attn_plan_band"))
+    return -1;
   const BandSegs sg = band_segments(mask_mode, m0, m1, m2, S, transposed);
   const int n_items = band_total_items(sg);
   const int n_items_cap = (S + kItemRows - 1) / kItemRows + 4;

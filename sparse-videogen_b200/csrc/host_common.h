@@ -70,6 +70,19 @@ int encode_tmap_scale_rows(CUtensorMap* map, const float* base, int num_blocks, 
 // the per-row scale tensors of an e4m3 cache (kvcache.cu): both given, 16-byte aligned, block_rows a multiple of 4
 int kv_scale_rows_check(const float* k_scale, const float* v_scale, int block_rows, const char* who);
 
+// the parameters of SVGB_MASK_BLOCK_CAUSAL: sink >= 0, m1 = C | (C - F) << 16 with 1 <= C < 2^16 and 1 <= F <= C, and
+// a window W >= C
+inline int block_causal_check(int sink, int m1, int W, const char* who) {
+  const int C = m1 & 0xffff, F = C - ((m1 >> 16) & 0xffff);
+  SVGB_REQUIRE(m1 >= 0, "%s: block-causal m1 = %d is not C | (C - F) << 16 with C, C - F < 2^16", who, m1);
+  SVGB_REQUIRE(C >= 1, "%s: block-causal block C = %d must be >= 1", who, C);
+  SVGB_REQUIRE(F >= 1, "%s: block-causal first_block F = %d must lie in [1, C = %d]", who, F, C);
+  SVGB_REQUIRE(W >= C, "%s: block-causal window W = %d must be >= the block C = %d (every row keeps its own block)", who,
+               W, C);
+  SVGB_REQUIRE(sink >= 0, "%s: block-causal sink = %d must be >= 0", who, sink);
+  return 0;
+}
+
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
 // BH (svgb200.h); every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) {

@@ -127,12 +127,14 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
 // Split plans (nsplit > 1) repeat the B I items once per split, split-major: item s B I + i is split s of item i, and
 // visits the s-th piece of ceil(nvis / nsplit) of the item's nvis visited chunks (sinks first, then the window), so the
 // item's split lists, concatenated in split order, are its single-pass list.
+// Block-causal plans (block = m1 of SVGB_MASK_BLOCK_CAUSAL, left = W - 1, right = 0) round the item's first and last
+// positions to their block ends first: the visited window is [e(p0) - W, e(p1) - 1], and block = 0 is the token rule.
 // =============================================================================================
 __global__ void __launch_bounds__(256)
 kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_idx, const int* __restrict__ table, int B,
                 int Sq, int Snew, int nblocks, int block_rows, int max_pages, int cap, int slots, int nsplit, int sink,
-                int left, int right, int* __restrict__ counts, int* __restrict__ kv, int2* __restrict__ chunks,
-                int4* __restrict__ items) {
+                int left, int right, int block, int* __restrict__ counts, int* __restrict__ kv,
+                int2* __restrict__ chunks, int4* __restrict__ items) {
   const int lane = threadIdx.x & 31;
   const int per = (Sq + kItemRows - 1) / kItemRows;  // items per stream
   const int it = blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -153,8 +155,12 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
   // chunks that can hold an allowed key: [0, ns) with sinks, [jlo, jhi] inside the window of positions p0 .. p1
   const int nch = (L + kChunkCols - 1) / kChunkCols;
   const int ns = (min(sink, L) + kChunkCols - 1) / kChunkCols;
-  const long long p0 = static_cast<long long>(r0) - o.shift, p1 = p0 + nr - 1;
-  const long long lo = std::max(p0 - left, 0ll), hi = std::min(p1 + right, static_cast<long long>(L) - 1);
+  // block-causal (block != 0): the rows' positions rounded to their block ends, where the mask is the local band
+  // (sink, W - 1, 0); rounding is monotone, so rows e0 .. e1 give the chunk kinds of the item's rows exactly
+  const int p0 = r0 - o.shift, p1 = p0 + nr - 1;
+  const int e0 = block ? block_last(p0, block) : p0, e1 = block ? block_last(p1, block) : p1;
+  const long long lo = std::max(static_cast<long long>(e0) - left, 0ll),
+                  hi = std::min(static_cast<long long>(e1) + right, static_cast<long long>(L) - 1);
   const int jlo = max(ns, static_cast<int>(lo / kChunkCols));
   const int jhi = hi < lo ? -1 : min(nch - 1, static_cast<int>(hi / kChunkCols));
   const int nvis = ns + max(0, jhi - jlo + 1);
@@ -166,7 +172,7 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
     const int vi = v0 + lane;
     const int j = vi < ns ? vi : jlo + (vi - ns);
     const int c0 = j * kChunkCols, valid = min(kChunkCols, L - c0);
-    const int kind = vi < v_hi ? seg_chunk_kind(false, r0, r0 + nr - 1, c0, c0 + valid - 1, o, left, right) : 0;
+    const int kind = vi < v_hi ? seg_chunk_kind(false, e0 + o.shift, e1 + o.shift, c0, c0 + valid - 1, o, left, right) : 0;
     const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
     const int at = n + __popc(m & ((1u << lane) - 1u));
     if (kind != 0 && at < slots) {
@@ -183,7 +189,9 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
 //   counts (16 B) | {B, Sq, L_0 .. L_B-1} | items 2 int4 [nsplit B I] | chunks [nsplit B I slots]
 // with I = ceil(Sq / 256) items per stream and slots = min(ceil(cap / 128), ceil(sink / 128) + (255 + left + right) / 128
 // + 2), the chunks an item can visit: its sinks and the window of its 256 rows; a split plan's items have
-// ceil(slots / nsplit) slots each, the most a split's piece can hold
+// ceil(slots / nsplit) slots each, the most a split's piece can hold.  A block-causal plan passes right = C - 1 here: its
+// rows' block ends lie up to C - 1 past them, so an item's window [e(p0) - W, e(p1) - 1] spans at most 255 + (W - 1) +
+// (C - 1) + 1 keys.
 struct KvLayout {
   long long items, slots;
   size_t items_off, chunks_off, bytes;
@@ -303,30 +311,32 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
 
 // both planners: svgb_attn_plan_kvcache's plan (nsplit = 1, split = false: SVGB_PLAN_KVCACHE) and the split plan of
 // svgb_attn_plan_kvcache_split (SVGB_PLAN_KVCACHE_SPLIT)
+// the block-causal planner (block = m1 != 0, left = W - 1, right = 0) of svgb_attn_plan_kvcache_block
 static int kv_plan_run(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table, int B,
                        int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left, int right,
                        int nsplit, bool split, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
-                       const char* who) {
+                       const char* who, int block = 0) {
+  const int widen = block ? (block & 0xffff) - 1 : 0;  // kv_layout's right for a block-causal plan
   SVGB_REQUIRE(cache_seqlens && plan_ws && plan, "null pointer");
   SVGB_REQUIRE(Snew >= 0, "%s: Snew=%d < 0", who, Snew);
   int cap = 0;
   if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
   size_t need = 0;
-  if (kv_plan_bytes(B, Sq, cap, sink, left, right, &need, nsplit)) return -1;
+  if (kv_plan_bytes(B, Sq, cap, sink, left, right + widen, &need, nsplit)) return -1;
   SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
   SVGB_REQUIRE(static_cast<long long>(B) * Sq < (1ll << 30), "%s: B * Sq = %lld query rows too many", who,
                static_cast<long long>(B) * Sq);
-  const KvLayout L = kv_layout(B, Sq, cap, sink, left, right, nsplit);
+  const KvLayout L = kv_layout(B, Sq, cap, sink, left, right + widen, nsplit);
   SVGB_REQUIRE(L.items * L.slots < (1ll << 31) && L.items < (1ll << 31), "plan too large for 32-bit chunk offsets");
   plan->kind = split ? SVGB_PLAN_KVCACHE_SPLIT : SVGB_PLAN_KVCACHE;
   plan->BH = num_blocks * block_rows;  // a KV-cache plan serves every head: BH holds the cache rows (svgb200.h)
   plan->S = B * Sq;
   plan->max_items = static_cast<int>(L.items);
   plan->items_stride = 0;
-  plan->mask_mode = MASK_LOCAL;
+  plan->mask_mode = block ? MASK_BLOCK_CAUSAL : MASK_LOCAL;
   plan->m0 = sink;
-  plan->m1 = left;
-  plan->m2 = right;
+  plan->m1 = block ? block : left;
+  plan->m2 = block ? left + 1 : right;
   plan->counts_off = 0;
   plan->items_off = static_cast<int64_t>(L.items_off);
   plan->chunks_off = static_cast<int64_t>(L.chunks_off);
@@ -334,7 +344,7 @@ static int kv_plan_run(const int32_t* cache_seqlens, const int32_t* cache_batch_
   char* ws = static_cast<char*>(plan_ws);
   kv_lists_kernel<<<static_cast<unsigned>((L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, cap,
-      static_cast<int>(L.slots), nsplit, sink, left, right, reinterpret_cast<int*>(ws),
+      static_cast<int>(L.slots), nsplit, sink, left, right, block, reinterpret_cast<int*>(ws),
       reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF), reinterpret_cast<int2*>(ws + L.chunks_off),
       reinterpret_cast<int4*>(ws + L.items_off));
   SVGB_LAUNCH_OK();
@@ -402,6 +412,35 @@ int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* ca
   SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
   return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
                      left, right, num_splits, true, plan_ws, ws_bytes, plan, stream, who);
+}
+
+// m1 of SVGB_MASK_BLOCK_CAUSAL from (block, first_block), and every parameter checked
+static int kv_block_m1(int sink, int window, int block, int first_block, int num_splits, int* m1, const char* who) {
+  SVGB_REQUIRE(block >= 1 && block < (1 << 16), "%s: block C = %d must lie in [1, 2^16) (it is packed in 16 bits)", who,
+               block);
+  SVGB_REQUIRE(first_block >= 1 && first_block <= block, "%s: first_block F = %d must lie in [1, C = %d]", who,
+               first_block, block);
+  SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
+  *m1 = block | (block - first_block) << 16;
+  return block_causal_check(sink, *m1, window, who);
+}
+
+int svgb_attn_plan_kvcache_block_bytes(int B, int Sq, int cap, int sink, int window, int block, int first_block,
+                                       int num_splits, size_t* bytes) {
+  int m1 = 0;
+  if (kv_block_m1(sink, window, block, first_block, num_splits, &m1, "svgb_attn_plan_kvcache_block_bytes")) return -1;
+  return kv_plan_bytes(B, Sq, cap, sink, window - 1, block - 1, bytes, num_splits);
+}
+
+int svgb_attn_plan_kvcache_block(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
+                                 int max_pages, int sink, int window, int block, int first_block, int num_splits,
+                                 void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
+  const char* who = "svgb_attn_plan_kvcache_block";
+  int m1 = 0;
+  if (kv_block_m1(sink, window, block, first_block, num_splits, &m1, who)) return -1;
+  return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
+                     window - 1, 0, num_splits, num_splits > 1, plan_ws, ws_bytes, plan, stream, who, m1);
 }
 
 }  // extern "C"

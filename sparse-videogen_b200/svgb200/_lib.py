@@ -59,6 +59,8 @@ _PROTOS = {
     "svgb_attn_plan_kvcache": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_plan_kvcache_split_bytes": [_i, _i, _i, _i, _i, _i, _i, _psz],
     "svgb_attn_plan_kvcache_split": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_kvcache_block_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _psz],
+    "svgb_attn_plan_kvcache_block": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                       _pplan, _vp, _vp],
     "svgb_attn_fwd_kv": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan, _vp,

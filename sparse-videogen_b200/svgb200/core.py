@@ -16,6 +16,9 @@ MASK_NONE, MASK_HY, MASK_WAN, MASK_COG = 0, 1, 2, 3
 MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_S, MASK_PROF_COG_T = 4, 5, 6, 7, 8, 9
 # local band with attention sinks (SVGB_MASK_LOCAL): m0 = sink, m1 = left, m2 = right; plan_local builds it
 MASK_LOCAL = 10
+# block-causal mask (SVGB_MASK_BLOCK_CAUSAL): m0 = sink, m1 = block | (block - first_block) << 16, m2 = window;
+# plan_block_causal and plan_kvcache(block=) build it
+MASK_BLOCK_CAUSAL = 12
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
 PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T, PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE = 1, 2, 3, 4, 5, 6, 7
 PLAN_KVCACHE_SPLIT = 8
@@ -211,6 +214,39 @@ def plan_local(BH: int, S: int, device, *, causal: bool = False, window_size=(-1
     return plan_band(MASK_LOCAL, int(sink), left, right, BH, S, device)
 
 
+def _block_m1(who, block, first_block, window, sink):
+    """(m1, W) of MASK_BLOCK_CAUSAL from block C, first_block F (None: C) and window W (-1: unbounded, returned as -1),
+    refused by name before any launch when C, F, W or sink is out of range or C does not fit its 16 bits."""
+    C_ = int(block)
+    F = C_ if first_block is None else int(first_block)
+    W, sink = int(window), int(sink)
+    if not 1 <= C_ < 1 << 16:
+        raise SvgbError(f"{who}: block={C_} must lie in [1, 65536) (it is packed in 16 bits)")
+    if not 1 <= F <= C_:
+        raise SvgbError(f"{who}: first_block={F} must lie in [1, block={C_}]")
+    if W != -1 and W < C_:
+        raise SvgbError(f"{who}: window={W} must be -1 (unbounded) or >= block={C_}, so that every query keeps its own "
+                        "block")
+    if sink < 0:
+        raise SvgbError(f"{who}: sink={sink} must be >= 0")
+    return C_ | (C_ - F) << 16, W
+
+
+def plan_block_causal(BH: int, S: int, device, *, block: int, first_block: Optional[int] = None, window: int = -1,
+                      sink: int = 0) -> AttnPlan:
+    """Block-causal attention of autoregressive video (chunk-wise causal, as CausVid and Self-Forcing train): positions
+    0 .. S-1 form blocks of `block` = C positions, the first one `first_block` = F long (1 <= F <= C, default C), so block
+    ends lie at F, F + C, F + 2C, ...  Query p sees key kv when kv < sink, or when kv lies before the end e(p) of p's block
+    and at most `window` = W keys back from it: e(p) - W <= kv < e(p) (W >= C, -1: unbounded).  Every query sees its whole
+    block and all earlier ones.  A band plan of MASK_BLOCK_CAUSAL, so every entry that runs band plans runs it, forward
+    and backward (attention(), attn_fwd, attn_bwd, key_major()); block=1 is plan_local(causal=True, window_size=(W - 1,
+    0), sink=sink)."""
+    m1, W = _block_m1("plan_block_causal", block, first_block, window, sink)
+    if W == -1:
+        W = min(int(S) + int(block), 2**31 - 1)  # a block end lies at most S + C - 1 past key 0
+    return plan_band(MASK_BLOCK_CAUSAL, int(sink), m1, W, BH, S, device)
+
+
 def _plan_local_varlen(name, cu_q, cu_k, nseg, Sq, Skv, sink, left, right, device) -> AttnPlan:
     nbytes = C.c_size_t()
     check(lib().svgb_attn_plan_local_varlen_bytes(nseg, Sq, Skv, C.byref(nbytes)), "svgb_attn_plan_local_varlen_bytes")
@@ -224,7 +260,7 @@ def _plan_local_varlen(name, cu_q, cu_k, nseg, Sq, Skv, sink, left, right, devic
 
 def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.Tensor] = None, *, total_q: int,
                       total_k: Optional[int] = None, causal: bool = False, window_size=(-1, -1),
-                      sink: int = 0) -> AttnPlan:
+                      sink: int = 0, block: int = 0) -> AttnPlan:
     """Causal or sliding-window attention with attention sinks inside packed variable-length segments, in
     FlashAttention's conventions (flash_attn_varlen_func): cu_seqlens_q / cu_seqlens_k are device int [nseg + 1]
     (cu_seqlens_k None: the same segments), query segment i attends key segment i only, and its queries are aligned to
@@ -234,7 +270,11 @@ def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.T
     window_size[1].  total_q / total_k (default total_q) are the packed lengths, q.shape[0] and k.shape[0] of a
     [total, H, D] call: they are passed rather than read from cu_seqlens so that planning never waits on the device.
     One plan for every head (any H, batch, GQA group or view); attention() runs it forward and backward, in 'shd' and in
-    'bhsd' (every batch element segmented alike).  Rows without an allowed key get o = 0 and lse = -inf."""
+    'bhsd' (every batch element segmented alike).  Rows without an allowed key get o = 0 and lse = -inf.
+    block: only 0; block-causal masks inside packed segments are not supported (plan_block_causal is the square form)."""
+    if block:
+        raise SvgbError(f"plan_local_varlen: block={block}: block-causal masks inside packed segments are not "
+                        "supported; use plan_block_causal on a square sequence or plan_kvcache(block=) into a cache")
     _need_cuda(cu_seqlens_q, cu_seqlens_k)
     cu_q = cu_seqlens_q.to(torch.int32).contiguous()
     cu_k = cu_q if cu_seqlens_k is None else cu_seqlens_k.to(torch.int32).contiguous()
@@ -382,7 +422,8 @@ def _row_scales(who, k_scale, v_scale, cache):
 def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0, cache_len: Optional[int] = None,
                  block_table: Optional[torch.Tensor] = None, page_size: Optional[int] = None,
                  cache_batch_idx: Optional[torch.Tensor] = None, causal: bool = False, window_size=(-1, -1),
-                 sink: int = 0, num_splits: int = 1, num_heads: Optional[int] = None) -> AttnPlan:
+                 sink: int = 0, num_splits: int = 1, num_heads: Optional[int] = None, block: int = 0,
+                 first_block: Optional[int] = None) -> AttnPlan:
     """Attention of B streams of q_len queries into a KV cache, in FlashAttention's conventions
     (flash_attn_with_kvcache): stream b holds L_b = cache_seqlens[b] + new_len keys (new_len rows appended before this
     attention, e.g. by kvcache_append) and its query i sits at logical position L_b - q_len + i.  Query p sees key kv
@@ -395,7 +436,13 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
     num_splits: 1 is the single pass, one CTA per 256-query item and head.  n > 1 splits every item's keys into n pieces
     (svgb_attn_plan_kvcache_split), which attn_fwd runs as n times the CTAs writing fp32 partials and a merge, so that
     decode and short chunks fill the GPU.  0 picks n on the host from the SM count, the CTAs B ceil(q_len / 256)
-    num_heads (num_heads = q's heads, required then) and the chunk slots per item (kvcache_num_splits)."""
+    num_heads (num_heads = q's heads, required then) and the chunk slots per item (kvcache_num_splits).
+    block > 0: the block-causal rule of plan_block_causal on logical positions (blocks of `block` keys, the first ends at
+    `first_block`, default block): query p sees kv < sink and e(p) - W <= kv < e(p), with W = window_size[0] counted
+    back from the block end (-1: unbounded) and window_size[1] = -1; causal=True is refused (the rule is causal).  When
+    the q_len queries form one block, they all attend [L_b - W, L_b) plus the sinks.  A rolling cache that renumbers its
+    positions down by d keys keeps its blocks with first_block = ((F - d - 1) mod block) + 1 (INTEGRATION.md)."""
+    blk = _kvcache_block_args(causal, window_size, sink, block, first_block) if block else None
     if block_table is not None:
         B = block_table.shape[0]
         if page_size is None:
@@ -416,6 +463,9 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
     bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
     lens = _seqlens(cache_seqlens, B, device)
     Sq = int(q_len)
+    if blk:
+        return _plan_kvcache_block(lens, bi, bt, B, Sq, int(new_len), int(num_blocks), rows, max_pages, cap, device,
+                                   sink, num_splits, num_heads, *blk)
     left, right = (int(w) for w in window_size)
     if causal:
         if right > 0:
@@ -423,15 +473,7 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
         right = 0
     # -1: no query position lies further than cap + Sq from a key
     left, right = (min(cap + Sq, 2**31 - 1) if w == -1 else w for w in (left, right))
-    n = int(num_splits)
-    if n < 0:
-        raise SvgbError(f"plan_kvcache: num_splits={n} must be >= 0 (0: automatic, 1: no split)")
-    if n == 0:
-        if num_heads is None:
-            raise SvgbError("plan_kvcache: num_splits=0 picks the split count from the grid, so it needs num_heads (q's "
-                            "query heads)")
-        n = kvcache_num_splits(B * -(-Sq // 256) * int(num_heads), _kvcache_slots(cap, int(sink), left, right),
-                               _sm_count())
+    n = _num_splits(num_splits, num_heads, B, Sq, cap, sink, left, right)
     nbytes = C.c_size_t()
     desc = Plan()
     stream = torch.cuda.current_stream(device).cuda_stream
@@ -449,6 +491,51 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
         check(lib().svgb_attn_plan_kvcache_split(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks),
                                                  rows, max_pages, int(sink), left, right, n, ws.data_ptr(), ws.numel(),
                                                  C.byref(desc), stream), "svgb_attn_plan_kvcache_split")
+    _bump()
+    return AttnPlan(desc, ws, (B, Sq))
+
+
+def _num_splits(num_splits, num_heads, B, Sq, cap, sink, left, right):
+    n = int(num_splits)
+    if n < 0:
+        raise SvgbError(f"plan_kvcache: num_splits={n} must be >= 0 (0: automatic, 1: no split)")
+    if n == 0:
+        if num_heads is None:
+            raise SvgbError("plan_kvcache: num_splits=0 picks the split count from the grid, so it needs num_heads (q's "
+                            "query heads)")
+        n = kvcache_num_splits(B * -(-Sq // 256) * int(num_heads), _kvcache_slots(cap, int(sink), left, right),
+                               _sm_count())
+    return n
+
+
+def _kvcache_block_args(causal, window_size, sink, block, first_block):
+    """(block C, first_block F, window W or -1) of plan_kvcache(block=), checked before any device work."""
+    if causal:
+        raise SvgbError("plan_kvcache: causal=True is redundant with block= (the block rule is causal); pass "
+                        "window_size=(W, -1)")
+    W, right = (int(w) for w in window_size)
+    if right != -1:
+        raise SvgbError(f"plan_kvcache: with block=, window_size[1] = {right} must be -1 (no key past the block end)")
+    m1, W = _block_m1("plan_kvcache", block, first_block, W, sink)
+    return m1 & 0xffff, (m1 & 0xffff) - (m1 >> 16), W
+
+
+def _plan_kvcache_block(lens, bi, bt, B, Sq, new_len, num_blocks, rows, max_pages, cap, device, sink, num_splits,
+                        num_heads, C_, F, W):
+    """plan_kvcache(block=): svgb_attn_plan_kvcache_block, single (n = 1) or split."""
+    if W == -1:  # no query's block end lies further than cap + Sq + C from key 0
+        W = min(cap + Sq + C_, 2**31 - 1)
+    # the slot bound of a block plan: left = W - 1, right = C - 1 (svgb_attn_plan_kvcache_block)
+    n = _num_splits(num_splits, num_heads, B, Sq, cap, sink, W - 1, C_ - 1)
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_plan_kvcache_block_bytes(B, Sq, cap, int(sink), W, C_, F, n, C.byref(nbytes)),
+          "svgb_attn_plan_kvcache_block_bytes")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
+    desc = Plan()
+    check(lib().svgb_attn_plan_kvcache_block(lens.data_ptr(), _p(bi), _p(bt), B, Sq, new_len, num_blocks, rows,
+                                             max_pages, int(sink), W, C_, F, n, ws.data_ptr(), ws.numel(),
+                                             C.byref(desc), torch.cuda.current_stream(device).cuda_stream),
+          "svgb_attn_plan_kvcache_block")
     _bump()
     return AttnPlan(desc, ws, (B, Sq))
 
