@@ -168,6 +168,26 @@ int svgb_attn_plan_local_varlen(const int32_t* cu_q, const int32_t* cu_k, int ns
  * same parameters and the same workspace layout (which is a function of nseg, Sq and Skv). */
 int svgb_attn_plan_local_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
                                   int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
+/* Block-causal mask inside packed variable-length segments (chunk-wise causal video training on a batch of clips of
+ * different lengths): the segments, bounds, alignment and plans of svgb_attn_plan_local_varlen, with SVGB_MASK_BLOCK_CAUSAL
+ * inside every segment and its block grid anchored at the segment's key 0.  With kj the key's and p = qi + Lk_i - Lq_i
+ * the query's position in segment i, and e(p) the first block end (F, F + C, F + 2C, ...) past p (p < F, negative p
+ * too: F):
+ *   allowed(q, kv) = same segment & (kj < sink | e(p) - W <= kj < e(p))
+ * window = W >= C (W >= the longest segment + C: unbounded), block = C in [1, 2^16), first_block = F in [1, C],
+ * sink >= 0, each refused by name before any launch.  A pair of entries of their own, so the _local_varlen signatures
+ * stay as they are.  plan->kind = SVGB_PLAN_SEG (SVGB_PLAN_SEG_T for the key-major companion), mask_mode =
+ * SVGB_MASK_BLOCK_CAUSAL, m0..m2 = sink, SVGB_BLOCK_M1(C, F), W; they run wherever the _local_varlen plans run, forward
+ * and backward.  Query-major items round their first and last positions to their block ends inside the segment and
+ * classify chunks as the local band (sink, W - 1, 0); key-major items classify them from the interval of positions that
+ * reach each key.  Workspace: svgb_attn_plan_local_varlen_bytes (an item has one slot per chunk of its segment whatever
+ * the mask). */
+int svgb_attn_plan_block_varlen(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                int window, int block, int first_block, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
+                                void* stream);
+int svgb_attn_plan_block_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                  int window, int block, int first_block, void* plan_ws, size_t ws_bytes,
+                                  svgb_plan* plan, void* stream);
 
 /* ---- KV cache (FlashAttention's flash_attn_with_kvcache) ----------------------------------
  * A batch of B streams attends into a cache of num_blocks blocks of block_rows rows, Hkv heads, D in {64, 128}:

@@ -17,7 +17,7 @@
 //   dS = P * (dP - delta)                       delta = rowsum(dO * O) of the query
 //   A1 += dS U  (dQ or dK),  A2 += P W (dV)     wgmma m64nDk16, RS (dS, P from registers, U / W MN-major)
 // Masked entries and columns past the chunk's valid count get P = dS = 0.  ELEM chunks evaluate mask_allowed with the
-// query position first in both directions (segment plans: shifted to the stream's segment, seg_origin).  A row without
+// query position first in both directions (segment plans: relative to the stream's segment, seg_origin).  A row without
 // any allowed key has lse = -inf and gets P = 0 on every column, so its dQ is exactly 0; a key that no query reaches
 // gets an empty list and dK = dV = 0.
 //
@@ -167,10 +167,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
     const int4 d = __ldg(&desc[st]);
     const int r0 = d.x, nr = d.y, nch = d.w;
     const int2* __restrict__ chunks = args.chunks + d.z;
-    // segment plans: the stream's segment shifts the query positions (the rows, key-major the columns) and moves the
-    // sink bound (seg_origin)
+    // segment plans: the stream's segment shifts the query positions (the rows, key-major the columns), and the mask
+    // sees both positions relative to the segment's first key, where its block grid is anchored (seg_origin)
     SegOrigin so{0, m0};
     if (args.segs) so = seg_origin(args.segs, r0, kKeyMajor, m0);
+    const int q_off = so.shift + so.key0, sink_rel = so.sink_end - so.key0;
     // step t of the stream takes chunk t % nch of the streamed tiles' head uhead(t): the query-major kernel walks the
     // list once (K / V of head bh / G), the key-major kernel once per query head of the group, g = t / nch in order
     const int steps = kKeyMajor ? G * nch : nch;
@@ -237,8 +238,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
               bool ok = in;
               if (elem && ok) {
                 const int rp = r0 + rloc + 8 * v1, cp = c0 + col;
-                ok = kKeyMajor ? mask_allowed(mode, cp - so.shift, rp, so.sink_end, m1, m2)
-                               : mask_allowed(mode, rp - so.shift, cp, so.sink_end, m1, m2);
+                ok = kKeyMajor ? mask_allowed(mode, cp - q_off, rp - so.key0, sink_rel, m1, m2)
+                               : mask_allowed(mode, rp - q_off, cp - so.key0, sink_rel, m1, m2);
               }
               const float l2 = kKeyMajor ? lse_c : lse_r[v1];
               const float dl = kKeyMajor ? dl_c : dl_r[v1];

@@ -87,6 +87,9 @@ __host__ __device__ inline int block_last(int p, int m1) {
   return p < F ? F - 1 : p + (C - 1) - (p - F) % C;
 }
 
+// the same inside a segment whose block grid is anchored at key position key0 (SegOrigin::key0; 0 for other plans)
+__host__ __device__ inline int seg_block_last(int p, int key0, int m1) { return key0 + block_last(p - key0, m1); }
+
 __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, int m1, int m2) {
   // reference semantics, written branch-free (bitwise) so warps do not diverge on it
   int d = q - kv;
@@ -153,6 +156,7 @@ __host__ __device__ inline bool mask_allowed(int mode, int q, int kv, int m0, in
 struct SegOrigin {
   int shift;     // subtract from a query position
   int sink_end;  // m0 of the stream: keys below it are sinks
+  int key0 = 0;  // the segment's first key ck_i, where its block grid is anchored; 0 for every other plan
 };
 // origin of the stream whose first row is `row`: a query row (key_major = false) or a key row (true).  Its segment is
 // the last one that starts at or before it, so empty segments are skipped.
@@ -170,6 +174,7 @@ __host__ __device__ inline SegOrigin seg_origin(const int* seg, int row, bool ke
   SegOrigin o;
   o.shift = segs[lo + 1] - ck[lo + 1];
   o.sink_end = ck[lo] + sink;
+  o.key0 = ck[lo];
   return o;
 }
 
@@ -204,6 +209,35 @@ __host__ __device__ inline int seg_chunk_kind(bool key_major, int r0, int r1, in
   const long long k0 = r0 > o.sink_end ? r0 : o.sink_end;  // first key of the item past the sinks
   const bool any = r0 < o.sink_end || (c0 <= r1 + o.shift + L && c1 >= r0 + o.shift - R);
   const bool all = k0 > r1 || (c0 >= r1 + o.shift - R && c1 <= k0 + o.shift + L);
+  return any ? (all ? 1 : 2) : 0;
+}
+
+// MASK_BLOCK_CAUSAL, key-major: the positions p that reach key k >= 0 (both relative to the segment's first key, k not
+// a sink) are those with k + 1 <= e(p) <= k + W, the interval [lo, hi]: lo is the first position of k's block (none
+// for k < F, where negative positions share the first block) and hi is one less than the last block end <= k + W
+// (k + W >= W >= C >= F, so there is one).  Both bounds are nondecreasing in k.
+struct PosSpan {
+  long long lo, hi;
+};
+__host__ __device__ inline PosSpan block_reach(int k, int m1, int W) {
+  const int C = m1 & 0xffff, F = C - (m1 >> 16);
+  const long long x = static_cast<long long>(k) + W;
+  PosSpan s;
+  s.lo = k < F ? LLONG_MIN / 2 : k - (k - F) % C;
+  s.hi = x - (x - F) % C - 1;
+  return s;
+}
+
+// Kind of a chunk of a key-major block-causal segment plan (0 / 1 / 2 as seg_chunk_kind): rows r0..r1 are keys, columns
+// c0..c1 queries at positions c - shift, of the segment of o.  The keys past the sinks, k0..r1, are reached by the union
+// [lo(k0), hi(r1)] of their intervals (consecutive ones touch: hi(k) >= k + W - C >= k) and, all of them, by the
+// intersection [lo(r1), hi(k0)]; the sink keys by every query of the segment.
+__host__ __device__ inline int seg_block_chunk_kind_t(int r0, int r1, int c0, int c1, SegOrigin o, int m1, int W) {
+  const int k0 = r0 > o.sink_end ? r0 : o.sink_end;  // first key of the item past the sinks
+  const long long p0 = static_cast<long long>(c0) - o.shift - o.key0, p1 = static_cast<long long>(c1) - o.shift - o.key0;
+  const PosSpan a = block_reach(k0 - o.key0, m1, W), b = block_reach(r1 - o.key0, m1, W);
+  const bool any = r0 < o.sink_end || (k0 <= r1 && p0 <= b.hi && p1 >= a.lo);
+  const bool all = k0 > r1 || (p0 >= b.lo && p1 <= a.hi);
   return any ? (all ? 1 : 2) : 0;
 }
 
@@ -250,11 +284,12 @@ struct ElemMask {
     return p;
   }
 
-  __device__ __forceinline__ void init(int mode_, const int (&qm)[2], int m0_, int m1_, int m2_) {
+  // key0: where the block grid is anchored (SegOrigin::key0), so a block-causal row rounds inside its segment
+  __device__ __forceinline__ void init(int mode_, const int (&qm)[2], int m0_, int m1_, int m2_, int key0) {
     mode = mode_; m0 = m0_; m1 = m1_; m2 = m2_;
     const bool block = mode == MASK_BLOCK_CAUSAL;
 #pragma unroll
-    for (int v1 = 0; v1 < 2; ++v1) row[v1] = block ? block_last(qm[v1], m1_) : qm[v1];
+    for (int v1 = 0; v1 < 2; ++v1) row[v1] = block ? seg_block_last(qm[v1], key0, m1_) : qm[v1];
     if (block) {  // rows rounded to their block ends: the local band (sink, W - 1, 0), no division per element
       mode = MASK_LOCAL;
       m1 = m2_ - 1;

@@ -385,7 +385,8 @@ seg_bounds_kernel(const int* __restrict__ cu_q, const int* __restrict__ cu_k, in
 // One warp per item it < counts[0]: its chunk list and its two stream descriptors, items[2 it], items[2 it + 1].
 __global__ void __launch_bounds__(256)
 seg_lists_kernel(const int* __restrict__ seg, const int* __restrict__ base, const int* __restrict__ counts, int nseg,
-                 int sink, int left, int right, int transposed, int2* __restrict__ chunks, int4* __restrict__ items) {
+                 int sink, int left, int right, int block, int transposed, int2* __restrict__ chunks,
+                 int4* __restrict__ items) {
   const int* segs = seg + 1;
   const int lane = threadIdx.x & 31;
   const int it = blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -409,11 +410,22 @@ seg_lists_kernel(const int* __restrict__ seg, const int* __restrict__ base, cons
   const int per = (ce - cs + kChunkCols - 1) / kChunkCols;
   const int list = cb[si] + k * per;
   const SegOrigin o = seg_origin(seg, r0, transposed != 0, sink);
+  // block-causal (block = m1 != 0, left = W - 1, right = 0), query-major: the item's first and last rows rounded to their
+  // block ends inside the segment, where the mask is the local band; rounding is monotone, so rows a0 .. a1 give the
+  // chunk kinds of the item's rows exactly.  Key-major: the interval form of seg_block_chunk_kind_t
+  int a0 = r0, a1 = r0 + nr - 1;
+  if (block && !transposed) {
+    a0 = seg_block_last(a0 - o.shift, o.key0, block) + o.shift;
+    a1 = seg_block_last(a1 - o.shift, o.key0, block) + o.shift;
+  }
   int n = 0;
   for (int j0 = 0; j0 < per; j0 += 32) {
     const int j = j0 + lane;
     const int c0 = cs + j * kChunkCols, valid = min(kChunkCols, ce - c0);
-    const int kind = j < per ? seg_chunk_kind(transposed != 0, r0, r0 + nr - 1, c0, c0 + valid - 1, o, left, right) : 0;
+    int kind = 0;
+    if (j < per)
+      kind = block && transposed ? seg_block_chunk_kind_t(r0, r0 + nr - 1, c0, c0 + valid - 1, o, block, left + 1)
+                                 : seg_chunk_kind(transposed != 0, a0, a1, c0, c0 + valid - 1, o, left, right);
     const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
     if (kind != 0) chunks[list + n + __popc(m & ((1u << lane) - 1u))] = make_int2(c0, chunk_meta(valid, kind == 2));
     n += __popc(m);
@@ -715,9 +727,11 @@ static int plan_local_varlen_bytes(int nseg, int Sq, int Skv, size_t* bytes) {
   return 0;
 }
 
+// block = 0: MASK_LOCAL(sink, left, right); block = m1 of MASK_BLOCK_CAUSAL (checked by the caller): the block rule with
+// the window W = left + 1 and right = 0
 static int plan_local_varlen_impl(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
                                   int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
-                                  bool transposed) {
+                                  bool transposed, int block = 0) {
   size_t need = 0;
   if (plan_local_varlen_bytes(nseg, Sq, Skv, &need)) return -1;
   SVGB_REQUIRE(cu_q && cu_k && plan_ws && plan, "null pointer");
@@ -733,10 +747,10 @@ static int plan_local_varlen_impl(const int32_t* cu_q, const int32_t* cu_k, int 
   plan->S = rows;
   plan->max_items = max_items;
   plan->items_stride = 0;
-  plan->mask_mode = MASK_LOCAL;
+  plan->mask_mode = block ? MASK_BLOCK_CAUSAL : MASK_LOCAL;
   plan->m0 = sink;
-  plan->m1 = left;
-  plan->m2 = right;
+  plan->m1 = block ? block : left;
+  plan->m2 = block ? left + 1 : right;
   plan->counts_off = 0;
   plan->items_off = static_cast<int64_t>(L.items_off);
   plan->chunks_off = static_cast<int64_t>(L.chunks_off);
@@ -748,8 +762,8 @@ static int plan_local_varlen_impl(const int32_t* cu_q, const int32_t* cu_k, int 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   seg_bounds_kernel<<<1, kSegThreads, 0, st>>>(cu_q, cu_k, nseg, Sq, Skv, sink, transposed ? 1 : 0, segs, base, counts);
   SVGB_LAUNCH_OK();
-  seg_lists_kernel<<<(max_items + 7) / 8, 256, 0, st>>>(segs, base, counts, nseg, sink, left, right, transposed ? 1 : 0,
-                                                        reinterpret_cast<int2*>(ws + L.chunks_off),
+  seg_lists_kernel<<<(max_items + 7) / 8, 256, 0, st>>>(segs, base, counts, nseg, sink, left, right, block,
+                                                        transposed ? 1 : 0, reinterpret_cast<int2*>(ws + L.chunks_off),
                                                         reinterpret_cast<int4*>(ws + L.items_off));
   SVGB_LAUNCH_OK();
   return 0;
@@ -936,6 +950,30 @@ int svgb_attn_plan_local_varlen(const int32_t* cu_q, const int32_t* cu_k, int ns
 int svgb_attn_plan_local_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
                                   int left, int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
   return plan_local_varlen_impl(cu_q, cu_k, nseg, Sq, Skv, sink, left, right, plan_ws, ws_bytes, plan, stream, true);
+}
+
+static int plan_block_varlen(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink, int window,
+                             int block, int first_block, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
+                             bool transposed) {
+  const char* who = transposed ? "svgb_attn_plan_block_varlen_t" : "svgb_attn_plan_block_varlen";
+  int m1 = 0;
+  if (block_causal_m1(block, first_block, &m1, who) || block_causal_check(sink, m1, window, who)) return -1;
+  return plan_local_varlen_impl(cu_q, cu_k, nseg, Sq, Skv, sink, window - 1, 0, plan_ws, ws_bytes, plan, stream,
+                                transposed, m1);
+}
+
+int svgb_attn_plan_block_varlen(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                int window, int block, int first_block, void* plan_ws, size_t ws_bytes, svgb_plan* plan,
+                                void* stream) {
+  return plan_block_varlen(cu_q, cu_k, nseg, Sq, Skv, sink, window, block, first_block, plan_ws, ws_bytes, plan, stream,
+                           false);
+}
+
+int svgb_attn_plan_block_varlen_t(const int32_t* cu_q, const int32_t* cu_k, int nseg, int Sq, int Skv, int sink,
+                                  int window, int block, int first_block, void* plan_ws, size_t ws_bytes,
+                                  svgb_plan* plan, void* stream) {
+  return plan_block_varlen(cu_q, cu_k, nseg, Sq, Skv, sink, window, block, first_block, plan_ws, ws_bytes, plan, stream,
+                           true);
 }
 
 int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,

@@ -443,8 +443,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
     const int rloc = 64 * cw + 16 * wq + (lane >> 2);
     ElemMask em;
     if constexpr (!kGather) {  // gather plans carry no element masks
-      // segment plans: the stream's segment shifts the query positions and moves the sink bound (seg_origin); KV-cache
-      // plans: the stream's length shifts them to logical positions (kv_origin)
+      // segment plans: the stream's segment shifts the query positions, moves the sink bound and anchors the block grid
+      // (seg_origin); KV-cache plans: the stream's length shifts them to logical positions (kv_origin)
       SegOrigin so{0, m0};
       if (args.segs) so = args.kv_logical ? kv_origin(args.segs, q0, m0) : seg_origin(args.segs, q0, false, m0);
       int qm[2];
@@ -453,7 +453,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
         const int q = q0 + rloc + 8 * v1;
         qm[v1] = ((args.q_index && q < args.S) ? __ldg(&args.q_index[q]) : q) - so.shift;  // position seen by the mask
       }
-      em.init(mode, qm, so.sink_end, m1, m2);
+      em.init(mode, qm, so.sink_end, m1, m2, so.key0);
     }
     // ROWS: c of each of the thread's two rows carries the row's q scale, q_scale [Hq, S] (rows past nr: never stored)
     float c_row[2] = {0.f, 0.f};

@@ -83,6 +83,16 @@ inline int block_causal_check(int sink, int m1, int W, const char* who) {
   return 0;
 }
 
+// m1 of SVGB_MASK_BLOCK_CAUSAL from block C and first_block F, each checked by name
+inline int block_causal_m1(int block, int first_block, int* m1, const char* who) {
+  SVGB_REQUIRE(block >= 1 && block < (1 << 16), "%s: block C = %d must lie in [1, 2^16) (it is packed in 16 bits)", who,
+               block);
+  SVGB_REQUIRE(first_block >= 1 && first_block <= block, "%s: first_block F = %d must lie in [1, C = %d]", who,
+               first_block, block);
+  *m1 = block | (block - first_block) << 16;
+  return 0;
+}
+
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
 // BH (svgb200.h); every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) {

@@ -416,12 +416,8 @@ int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* ca
 
 // m1 of SVGB_MASK_BLOCK_CAUSAL from (block, first_block), and every parameter checked
 static int kv_block_m1(int sink, int window, int block, int first_block, int num_splits, int* m1, const char* who) {
-  SVGB_REQUIRE(block >= 1 && block < (1 << 16), "%s: block C = %d must lie in [1, 2^16) (it is packed in 16 bits)", who,
-               block);
-  SVGB_REQUIRE(first_block >= 1 && first_block <= block, "%s: first_block F = %d must lie in [1, C = %d]", who,
-               first_block, block);
+  if (block_causal_m1(block, first_block, m1, who)) return -1;
   SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
-  *m1 = block | (block - first_block) << 16;
   return block_causal_check(sink, *m1, window, who);
 }
 

@@ -49,6 +49,8 @@ _PROTOS = {
     "svgb_attn_plan_local_varlen_bytes": [_i, _i, _i, _psz],
     "svgb_attn_plan_local_varlen": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_plan_local_varlen_t": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_block_varlen": [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_block_varlen_t": [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_kvcache_append": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll, _pll,
                             _vp],
     "svgb_kvcache_append_e4m3": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll, _pll,

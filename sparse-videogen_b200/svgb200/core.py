@@ -17,7 +17,7 @@ MASK_PROF_HY_S, MASK_PROF_HY_T, MASK_PROF_WAN_S, MASK_PROF_WAN_T, MASK_PROF_COG_
 # local band with attention sinks (SVGB_MASK_LOCAL): m0 = sink, m1 = left, m2 = right; plan_local builds it
 MASK_LOCAL = 10
 # block-causal mask (SVGB_MASK_BLOCK_CAUSAL): m0 = sink, m1 = block | (block - first_block) << 16, m2 = window;
-# plan_block_causal and plan_kvcache(block=) build it
+# plan_block_causal, plan_local_varlen(block=) and plan_kvcache(block=) build it
 MASK_BLOCK_CAUSAL = 12
 # svgb_plan.kind (include/svgb200.h SVGB_PLAN_*)
 PLAN_VARBLOCK, PLAN_BAND, PLAN_GATHER, PLAN_BAND_T, PLAN_SEG, PLAN_SEG_T, PLAN_KVCACHE = 1, 2, 3, 4, 5, 6, 7
@@ -118,8 +118,13 @@ class AttnPlan:
                 # nseg for the host
                 (nseg,) = self.source
                 cu = self.ws.data_ptr() + SEG_BOUNDS_OFF + 4
-                self._key_major = _plan_local_varlen("svgb_attn_plan_local_varlen_t", cu, cu + 4 * (nseg + 1), nseg,
-                                                     d.S, d.BH, d.m0, d.m1, d.m2, self.ws.device)
+                if d.mask_mode == MASK_BLOCK_CAUSAL:  # (sink, W, C, F) from m0..m2 = sink, C | (C - F) << 16, W
+                    name, params = "svgb_attn_plan_block_varlen_t", (d.m0, d.m2, d.m1 & 0xffff,
+                                                                     (d.m1 & 0xffff) - (d.m1 >> 16))
+                else:
+                    name, params = "svgb_attn_plan_local_varlen_t", (d.m0, d.m1, d.m2)
+                self._key_major = _plan_local_varlen(name, cu, cu + 4 * (nseg + 1), nseg, d.S, d.BH, *params,
+                                                     self.ws.device)
             elif d.kind == PLAN_VARBLOCK and self.source is not None:
                 *ts, versions = self.source
                 if tuple(t._version for t in ts) != versions:
@@ -247,12 +252,15 @@ def plan_block_causal(BH: int, S: int, device, *, block: int, first_block: Optio
     return plan_band(MASK_BLOCK_CAUSAL, int(sink), m1, W, BH, S, device)
 
 
-def _plan_local_varlen(name, cu_q, cu_k, nseg, Sq, Skv, sink, left, right, device) -> AttnPlan:
+def _plan_local_varlen(name, cu_q, cu_k, nseg, Sq, Skv, *args) -> AttnPlan:
+    """args: the planner's mask parameters, (sink, left, right) or for the block entries (sink, W, C, F), then the
+    device."""
+    *params, device = args
     nbytes = C.c_size_t()
     check(lib().svgb_attn_plan_local_varlen_bytes(nseg, Sq, Skv, C.byref(nbytes)), "svgb_attn_plan_local_varlen_bytes")
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the bounds
     desc = Plan()
-    check(getattr(lib(), name)(cu_q, cu_k, nseg, Sq, Skv, sink, left, right, ws.data_ptr(), ws.numel(), C.byref(desc),
+    check(getattr(lib(), name)(cu_q, cu_k, nseg, Sq, Skv, *params, ws.data_ptr(), ws.numel(), C.byref(desc),
                                torch.cuda.current_stream(device).cuda_stream), name)
     _bump(2)
     return AttnPlan(desc, ws, (nseg,))
@@ -260,7 +268,7 @@ def _plan_local_varlen(name, cu_q, cu_k, nseg, Sq, Skv, sink, left, right, devic
 
 def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.Tensor] = None, *, total_q: int,
                       total_k: Optional[int] = None, causal: bool = False, window_size=(-1, -1),
-                      sink: int = 0, block: int = 0) -> AttnPlan:
+                      sink: int = 0, block: int = 0, first_block: Optional[int] = None) -> AttnPlan:
     """Causal or sliding-window attention with attention sinks inside packed variable-length segments, in
     FlashAttention's conventions (flash_attn_varlen_func): cu_seqlens_q / cu_seqlens_k are device int [nseg + 1]
     (cu_seqlens_k None: the same segments), query segment i attends key segment i only, and its queries are aligned to
@@ -271,11 +279,29 @@ def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.T
     [total, H, D] call: they are passed rather than read from cu_seqlens so that planning never waits on the device.
     One plan for every head (any H, batch, GQA group or view); attention() runs it forward and backward, in 'shd' and in
     'bhsd' (every batch element segmented alike).  Rows without an allowed key get o = 0 and lse = -inf.
-    block: only 0; block-causal masks inside packed segments are not supported (plan_block_causal is the square form)."""
+    block > 0: the block-causal rule of plan_block_causal inside every segment, its blocks anchored at the segment's key
+    0 (blocks of `block` keys, the first ending at `first_block`, default block): query position p of segment i sees its
+    key kj when kj < sink or e(p) - W <= kj < e(p), with W = window_size[0] counted back from the block end (-1:
+    unbounded) and window_size[1] = -1; causal=True is refused (the rule is causal).  Segments whose queries start
+    mid-block (Lq_i < Lk_i) round them inside the key segment's grid, as plan_kvcache(block=) does.  One clip per
+    segment of a packed batch is chunk-wise causal video training; block=0 is the token rule above."""
     if block:
-        raise SvgbError(f"plan_local_varlen: block={block}: block-causal masks inside packed segments are not "
-                        "supported; use plan_block_causal on a square sequence or plan_kvcache(block=) into a cache")
-    _need_cuda(cu_seqlens_q, cu_seqlens_k)
+        if causal:
+            raise SvgbError("plan_local_varlen: causal=True is redundant with block= (the block rule is causal); pass "
+                            "window_size=(W, -1)")
+        W, right = (int(w) for w in window_size)
+        if right != -1:
+            raise SvgbError(f"plan_local_varlen: with block=, window_size[1] = {right} must be -1 (no key past the "
+                            "block end)")
+        m1, W = _block_m1("plan_local_varlen", block, first_block, W, sink)
+    try:
+        _need_cuda(cu_seqlens_q, cu_seqlens_k)
+    except SvgbError as e:
+        if not block:
+            raise
+        # the block form plans on the device only: name the mask that was asked for, not just the missing device
+        raise SvgbError(f"plan_local_varlen: block-causal masks inside packed segments are not supported on CPU "
+                        f"tensors: {e}") from None
     cu_q = cu_seqlens_q.to(torch.int32).contiguous()
     cu_k = cu_q if cu_seqlens_k is None else cu_seqlens_k.to(torch.int32).contiguous()
     if cu_q.dim() != 1 or cu_k.shape != cu_q.shape or cu_q.numel() < 2:
@@ -283,6 +309,12 @@ def plan_local_varlen(cu_seqlens_q: torch.Tensor, cu_seqlens_k: Optional[torch.T
                         "be 1-D with the same nseg + 1 >= 2 entries")
     Sq = int(total_q)
     Skv = Sq if total_k is None else int(total_k)
+    if block:
+        C_ = m1 & 0xffff
+        if W == -1:  # no block end lies further than the longest segment + C past its key 0
+            W = min(max(Sq, Skv) + C_, 2**31 - 1)
+        return _plan_local_varlen("svgb_attn_plan_block_varlen", cu_q.data_ptr(), cu_k.data_ptr(), cu_q.numel() - 1,
+                                  Sq, Skv, int(sink), W, C_, C_ - (m1 >> 16), cu_q.device)
     left, right = (int(w) for w in window_size)
     if causal:
         if right > 0:
