@@ -81,6 +81,7 @@ typedef struct svgb_plan {
   int32_t max_items;     /* grid.x of the attention launch */
   int32_t items_stride;  /* 0 when one plan serves every head */
   int32_t mask_mode, m0, m1, m2;
+  int32_t varlen_items;  /* KV-cache plans of svgb_attn_plan_kvcache_varlen: items per split (> 0); 0 otherwise */
   int64_t counts_off, items_off, chunks_off; /* byte offsets inside the plan workspace */
   int64_t bytes;
 } svgb_plan;
@@ -292,6 +293,55 @@ int svgb_attn_plan_kvcache_block(const int32_t* cache_seqlens, const int32_t* ca
                                  const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
                                  int max_pages, int sink, int window, int block, int first_block, int num_splits,
                                  void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream);
+/* Variable-length queries and appends (FlashAttention 3's cu_seqlens_q / cu_seqlens_k_new): B streams, each with its own
+ * query count, in one plan.  cu_q: device int32 [B + 1], stream b's Lq_b = cu_q[b+1] - cu_q[b] queries are the packed
+ * rows [cu_q[b], cu_q[b+1]) of q [total_q, Hq, D] (Lq_b = 0 is legal).  cu_new: optional device int32 [B + 1], stream b
+ * appended Lnew_b = cu_new[b+1] - cu_new[b] rows before this attention (svgb_kvcache_append_varlen); NULL: none.  Stream
+ * b has L_b = min(cache_seqlens[b] + Lnew_b, capacity) keys and its query i sits at L_b - Lq_b + i (Lq_b > L_b puts
+ * queries at negative positions).  Mask: block = 0 is svgb_attn_plan_kvcache's local band (sink, left, right; window
+ * and first_block must be 0), block = C > 0 svgb_attn_plan_kvcache_block's (sink, window = W, block = C, first_block =
+ * F; left and right must be 0), one (C, F) for the batch.  With every Lq_b = Sq and Lnew_b = Snew the results are the
+ * uniform plan's, bit for bit.  A row without an allowed key gets o = 0 and lse = -inf.  Nothing is read on the host:
+ * the bounds are clamped to [0, total_q] on the device, and bounds out of order give an unspecified result that stays
+ * inside the tensors.  total_q >= 1 and max_q in [1, total_q] are host values: max_q bounds every Lq_b (pass total_q
+ * when unknown; a longer stream gives an unspecified result).
+ * One launch, one warp per item.  Items are 256 rows cut from each stream's first row, numbered stream after stream;
+ * their count is known on the device only, and the host bound per split is
+ *   I = min(B ceil(max_q / 256), (total_q + 255 B) / 256)
+ * (sum ceil(Lq_b / 256) <= (total_q + 255 B) / 256).  num_splits = n: n = 1 is a single plan (SVGB_PLAN_KVCACHE), n > 1
+ * a split plan (SVGB_PLAN_KVCACHE_SPLIT), split-major, item s I + i being split s of item i as in
+ * svgb_attn_plan_kvcache_split.  Items i past the streams' items have zero rows and an empty list: their CTAs write
+ * nothing.  plan->S = total_q, max_items = n I, varlen_items = I, every other field as the uniform plans'.  The
+ * workspace keeps the header int32 {B, -1, L_0 .. L_B-1, cq_0 .. cq_B} at SVGB_PLAN_SEG_BOUNDS_OFF (cq_b the clamped
+ * bounds; -1 in the Sq slot marks it), from which the forward finds a row's stream by binary search.
+ * Runs wherever the uniform plans run, on q [total_q, Hq, D] as B = 1 and Sq = total_q at the ABI:
+ * svgb_attn_fwd_strided (16-bit, GQA), svgb_attn_fwd_strided_e4m3 (per-head e4m3), svgb_attn_fwd_kvcache_e4m3_rows
+ * (per-row e4m3) and, split, svgb_attn_fwd_kvcache_split in every format, which takes I from plan->varlen_items.
+ * Workspace (integer division; slots as svgb_attn_plan_kvcache_bytes, with left = W - 1 and right = C - 1 for a
+ * block-causal plan):
+ *   bytes = 16 + align16(4 (2 B + 3)) + 32 n I + 8 n I ceil(slots / n)
+ * Refused by name: B < 1, total_q < 1, max_q outside [1, total_q], num_splits < 1, the mask arguments of the other form,
+ * and bad sink, left, right, W, C or F. */
+int svgb_attn_plan_kvcache_varlen_bytes(int B, int total_q, int max_q, int cap, int sink, int left, int right,
+                                        int window, int block, int first_block, int num_splits, size_t* bytes);
+int svgb_attn_plan_kvcache_varlen(const int32_t* cu_q, const int32_t* cache_seqlens, const int32_t* cu_new,
+                                  const int32_t* cache_batch_idx, const int32_t* block_table, int B, int total_q,
+                                  int max_q, int num_blocks, int block_rows, int max_pages, int sink, int left,
+                                  int right, int window, int block, int first_block, int num_splits, void* plan_ws,
+                                  size_t ws_bytes, svgb_plan* plan, void* stream);
+/* Variable-length append, every cache format in one entry: new rows k, v [total_new, Hkv, D] (strides {batch, head, row},
+ * the batch stride not stepped) where stream b's rows are [cu_new[b], cu_new[b+1]) (device int32 [B + 1]), written at
+ * its logical keys cache_seqlens[b] .. + Lnew_b - 1 under svgb_kvcache_append's skip rules; a row outside every stream
+ * is not written.  k_scale = v_scale = NULL: a 16-bit cache (svgb_kvcache_append); row_scales = 0 with k_scale, v_scale
+ * float [Hkv]: an e4m3 cache with per-head scales (svgb_kvcache_append_e4m3); row_scales = 1 with k_scale, v_scale float
+ * [num_blocks, Hkv, block_rows]: per-row scales the append writes (svgb_kvcache_append_e4m3_rows).  One launch;
+ * total_new > 0.  With every Lnew_b = Snew it writes what the uniform append writes. */
+int svgb_kvcache_append_varlen(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cu_new,
+                               const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                               const int32_t* block_table, int dtype, int B, int total_new, int Hkv, int D,
+                               int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                               const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                               float* k_scale, float* v_scale, int row_scales, void* stream);
 
 /* ---- attention -------------------------------------------------------------------------- */
 /* o = softmax(q k^T * sm_scale  [masked by plan]) v, per head.  Stands behind

@@ -191,6 +191,30 @@ __host__ __device__ inline SegOrigin kv_origin(const int* kv, int row, int sink)
   return o;
 }
 
+// Variable-length KV-cache plans (svgb_attn_plan_kvcache_varlen) keep kv = {B, kKvVarlen, L_0 .. L_B-1, cu_0 .. cu_B}:
+// stream b has its queries at packed rows [cu_b, cu_b+1) and query row q sits at logical position L_b - (cu_b+1 - q), so
+// the shift is cu_b+1 - L_b.  The marker in the Sq slot tells the header from a uniform one; the stream of a row is the
+// last one that starts at or before it (empty streams are skipped), found by binary search as seg_origin does.
+constexpr int kKvVarlen = -1;
+__host__ __device__ inline SegOrigin kv_origin_varlen(const int* kv, int row, int sink) {
+  const int B = kv[0];
+  const int* cu = kv + 2 + B;
+  int lo = 0, hi = B - 1;  // largest b < B with cu[b] <= row
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (cu[mid] <= row) lo = mid;
+    else hi = mid - 1;
+  }
+  SegOrigin o;
+  o.shift = cu[lo + 1] - kv[2 + lo];
+  o.sink_end = sink;
+  return o;
+}
+// the origin of the stream of `row` under either KV-cache header
+__host__ __device__ inline SegOrigin kv_stream_origin(const int* kv, int row, int sink) {
+  return kv[1] == kKvVarlen ? kv_origin_varlen(kv, row, sink) : kv_origin(kv, row, sink);
+}
+
 // Kind of a chunk of a segment plan, from the mask's interval form: 0 = omitted (no allowed pair), 1 = FULL (every pair
 // allowed), 2 = ELEM.  Query-major: rows r0..r1 are queries at positions p = q - shift, columns c0..c1 keys.  Key-major:
 // rows are keys, columns queries.  Pairs (p, kv) are allowed when kv < sink_end or p - left <= kv <= p + right; every
@@ -408,7 +432,8 @@ struct AttnArgs {
   const int* q_index = nullptr;  // optional [S]: query position used by the element mask (sampled rows)
   // segment plans: the plan's copy of the bounds {nseg, cq[0..nseg], ck[0..nseg]} (seg_origin); nullptr otherwise
   const int* segs = nullptr;
-  // KV-cache plans: segs is the plan's {B, Sq, L_b} (kv_origin) and element masks see each chunk's logical position
+  // KV-cache plans: segs is the plan's {B, Sq, L_b} (kv_origin) or its varlen header (kv_origin_varlen), and element
+  // masks see each chunk's logical position
   int kv_logical = 0;
   int out_f32 = 0;               // 1: o is fp32 (used for split-KV partials)
   // split KV-cache plans (SVGB_PLAN_KVCACHE_SPLIT): the plan's items per split, so that CTA x runs split

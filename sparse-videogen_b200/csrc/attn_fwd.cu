@@ -1124,7 +1124,8 @@ int svgb_attn_fwd_kvcache_split(const void* q, const void* k, const void* v, con
                "%s takes split KV-cache plans (svgb_attn_plan_kvcache_split) only (kind %d)", who, plan->kind);
   SVGB_REQUIRE(B > 0 && Sq > 0 && static_cast<long long>(B) * Sq == plan->S,
                "%s: the plan was built for %d query rows, called with B=%d streams of Sq=%d", who, plan->S, B, Sq);
-  const int items = B * ((Sq + kItemRows - 1) / kItemRows);  // items per split
+  // items per split: recorded by a varlen plan, whose item count depends on lengths only the device holds
+  const int items = plan->varlen_items > 0 ? plan->varlen_items : B * ((Sq + kItemRows - 1) / kItemRows);
   SVGB_REQUIRE(plan->max_items > 0 && plan->max_items % items == 0,
                "%s: the plan's %d items are no whole number of splits of %d items (B=%d, Sq=%d)", who, plan->max_items,
                items, B, Sq);

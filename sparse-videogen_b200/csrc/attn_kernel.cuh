@@ -446,7 +446,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant_
       // segment plans: the stream's segment shifts the query positions, moves the sink bound and anchors the block grid
       // (seg_origin); KV-cache plans: the stream's length shifts them to logical positions (kv_origin)
       SegOrigin so{0, m0};
-      if (args.segs) so = args.kv_logical ? kv_origin(args.segs, q0, m0) : seg_origin(args.segs, q0, false, m0);
+      if (args.segs) so = args.kv_logical ? kv_stream_origin(args.segs, q0, m0) : seg_origin(args.segs, q0, false, m0);
       int qm[2];
 #pragma unroll
       for (int v1 = 0; v1 < 2; ++v1) {

@@ -61,6 +61,19 @@ __device__ __forceinline__ uint2 kv_to_e4m3(uint4 x, float inv) {
 // vector of K and one of V per thread (e4m3 caches: 8 elements of each, written as 8 bytes).  Rows whose logical key
 // lies outside [0, capacity) or whose block lies outside the cache are not written.
 // =============================================================================================
+// Variable-length append (cu_new != NULL): the new rows are k, v [Snew = total_new, Hkv, D] and stream b's are rows
+// [cu_new[b], cu_new[b+1]) (the last stream that starts at or before a row holds it), written at keys cache_seqlens[b] ..
+// under the same skip rules; a row outside every stream is not written.
+__device__ __forceinline__ int kv_row_stream(const int* __restrict__ cu, int B, int row) {
+  int lo = 0, hi = B - 1;  // largest b < B with cu[b] <= row
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&cu[mid]) <= row) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
 template <int kStore, typename Cache = typename std::conditional<kStore == KV_COPY, uint16_t, uint8_t>::type>
 __global__ void __launch_bounds__(256)
 kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t* __restrict__ k,
@@ -68,15 +81,21 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
                  const int* __restrict__ table, int B, int Snew, int Hkv, int nvec, int nblocks, int block_rows,
                  int max_pages, int cap, Strides kcs, Strides vcs, Strides ks, Strides vs,
                  const float* __restrict__ k_scale, const float* __restrict__ v_scale, float* __restrict__ k_rows,
-                 float* __restrict__ v_rows) {
-  const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
+                 float* __restrict__ v_rows, const int* __restrict__ cu_new = nullptr) {
+  const long long total = static_cast<long long>(cu_new ? 1 : B) * Snew * Hkv * nvec;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(idx % nvec);
     long long r = idx / nvec;
     const int h = static_cast<int>(r % Hkv);
     r /= Hkv;
-    const int i = static_cast<int>(r % Snew), b = static_cast<int>(r / Snew);
+    int i = static_cast<int>(r % Snew), b = static_cast<int>(r / Snew);
+    const long long ko = b * ks.b + i * ks.r, vo = b * vs.b + i * vs.r;  // varlen: b = 0 and i = r, the packed row
+    if (cu_new) {  // the packed row's stream, and its index inside that stream
+      b = kv_row_stream(cu_new, B, i);
+      i -= __ldg(&cu_new[b]);
+      if (i < 0 || r >= __ldg(&cu_new[b + 1])) continue;
+    }
     const long long t = static_cast<long long>(__ldg(&seqlens[b])) + i;
     if (t < 0 || t >= cap) continue;
     const int tt = static_cast<int>(t);
@@ -90,8 +109,8 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
     }
     if (blk < 0 || blk >= nblocks) continue;
     const long long e = 8ll * c;
-    const uint4 kx = *reinterpret_cast<const uint4*>(k + b * ks.b + i * ks.r + h * ks.h + e);
-    const uint4 vx = *reinterpret_cast<const uint4*>(v + b * vs.b + i * vs.r + h * vs.h + e);
+    const uint4 kx = *reinterpret_cast<const uint4*>(k + ko + h * ks.h + e);
+    const uint4 vx = *reinterpret_cast<const uint4*>(v + vo + h * vs.h + e);
     if constexpr (kStore == KV_COPY) {
       *reinterpret_cast<uint4*>(kc + blk * kcs.b + row * kcs.r + h * kcs.h + e) = kx;
       *reinterpret_cast<uint4*>(vc + blk * vcs.b + row * vcs.r + h * vcs.h + e) = vx;
@@ -130,6 +149,49 @@ kv_append_kernel(Cache* __restrict__ kc, Cache* __restrict__ vc, const uint16_t*
 // Block-causal plans (block = m1 of SVGB_MASK_BLOCK_CAUSAL, left = W - 1, right = 0) round the item's first and last
 // positions to their block ends first: the visited window is [e(p0) - W, e(p1) - 1], and block = 0 is the token rule.
 // =============================================================================================
+// The list of one item (one warp): rows r0 .. r0 + nr - 1 of stream b, whose L keys sit at logical positions 0 .. L - 1
+// and whose query row q sits at position q - shift; split sp of nsplit.  Writes the kept chunks at `list` and returns
+// their count (at most slots).
+__device__ __forceinline__ int kv_item_list(const int* __restrict__ batch_idx, const int* __restrict__ table, int b,
+                                            int L, int shift, int r0, int nr, int sp, int nsplit, int nblocks,
+                                            int block_rows, int max_pages, int slots, int sink, int left, int right,
+                                            int block, int2* __restrict__ list) {
+  const int lane = threadIdx.x & 31;
+  SegOrigin o;
+  o.shift = shift;
+  o.sink_end = sink;
+  // chunks that can hold an allowed key: [0, ns) with sinks, [jlo, jhi] inside the window of positions p0 .. p1
+  const int nch = (L + kChunkCols - 1) / kChunkCols;
+  const int ns = (min(sink, L) + kChunkCols - 1) / kChunkCols;
+  // block-causal (block != 0): the rows' positions rounded to their block ends, where the mask is the local band
+  // (sink, W - 1, 0); rounding is monotone, so rows e0 .. e1 give the chunk kinds of the item's rows exactly
+  const int p0 = r0 - o.shift, p1 = p0 + nr - 1;
+  const int e0 = block ? block_last(p0, block) : p0, e1 = block ? block_last(p1, block) : p1;
+  const long long lo = std::max(static_cast<long long>(e0) - left, 0ll),
+                  hi = std::min(static_cast<long long>(e1) + right, static_cast<long long>(L) - 1);
+  const int jlo = max(ns, static_cast<int>(lo / kChunkCols));
+  const int jhi = hi < lo ? -1 : min(nch - 1, static_cast<int>(hi / kChunkCols));
+  const int nvis = ns + max(0, jhi - jlo + 1);
+  const int piece = (nvis + nsplit - 1) / nsplit;  // this split's visited chunks: [v_lo, v_hi)
+  const int v_lo = min(nvis, sp * piece), v_hi = min(nvis, v_lo + piece);
+  int n = 0;
+  for (int v0 = v_lo; v0 < v_hi; v0 += 32) {
+    const int vi = v0 + lane;
+    const int j = vi < ns ? vi : jlo + (vi - ns);
+    const int c0 = j * kChunkCols, valid = min(kChunkCols, L - c0);
+    const int kind = vi < v_hi ? seg_chunk_kind(false, e0 + o.shift, e1 + o.shift, c0, c0 + valid - 1, o, left, right) : 0;
+    const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
+    const int at = n + __popc(m & ((1u << lane) - 1u));
+    if (kind != 0 && at < slots) {
+      const int blk = kv_block(batch_idx, table, b, c0, nblocks, block_rows, max_pages);
+      const int row = blk * block_rows + (table ? c0 % block_rows : c0);
+      list[at] = make_int2(row, chunk_meta(valid, kind == 2) | (j << kChunkLogicalShift));
+    }
+    n += __popc(m);
+  }
+  return min(n, slots);
+}
+
 __global__ void __launch_bounds__(256)
 kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_idx, const int* __restrict__ table, int B,
                 int Sq, int Snew, int nblocks, int block_rows, int max_pages, int cap, int slots, int nsplit, int sink,
@@ -149,40 +211,80 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
   const int L = kv_len(__ldg(&seqlens[b]), Snew, cap);
   if (sp == 0 && k == 0 && lane == 0) kv[2 + b] = L;
   const int r0 = b * Sq + k * kItemRows, nr = min(kItemRows, Sq - k * kItemRows);
-  SegOrigin o;
-  o.shift = (b + 1) * Sq - L;
-  o.sink_end = sink;
-  // chunks that can hold an allowed key: [0, ns) with sinks, [jlo, jhi] inside the window of positions p0 .. p1
-  const int nch = (L + kChunkCols - 1) / kChunkCols;
-  const int ns = (min(sink, L) + kChunkCols - 1) / kChunkCols;
-  // block-causal (block != 0): the rows' positions rounded to their block ends, where the mask is the local band
-  // (sink, W - 1, 0); rounding is monotone, so rows e0 .. e1 give the chunk kinds of the item's rows exactly
-  const int p0 = r0 - o.shift, p1 = p0 + nr - 1;
-  const int e0 = block ? block_last(p0, block) : p0, e1 = block ? block_last(p1, block) : p1;
-  const long long lo = std::max(static_cast<long long>(e0) - left, 0ll),
-                  hi = std::min(static_cast<long long>(e1) + right, static_cast<long long>(L) - 1);
-  const int jlo = max(ns, static_cast<int>(lo / kChunkCols));
-  const int jhi = hi < lo ? -1 : min(nch - 1, static_cast<int>(hi / kChunkCols));
-  const int nvis = ns + max(0, jhi - jlo + 1);
-  const int piece = (nvis + nsplit - 1) / nsplit;  // this split's visited chunks: [v_lo, v_hi)
-  const int v_lo = min(nvis, sp * piece), v_hi = min(nvis, v_lo + piece);
   const int list = it * slots;
-  int n = 0;
-  for (int v0 = v_lo; v0 < v_hi; v0 += 32) {
-    const int vi = v0 + lane;
-    const int j = vi < ns ? vi : jlo + (vi - ns);
-    const int c0 = j * kChunkCols, valid = min(kChunkCols, L - c0);
-    const int kind = vi < v_hi ? seg_chunk_kind(false, e0 + o.shift, e1 + o.shift, c0, c0 + valid - 1, o, left, right) : 0;
-    const unsigned m = __ballot_sync(0xffffffffu, kind != 0);
-    const int at = n + __popc(m & ((1u << lane) - 1u));
-    if (kind != 0 && at < slots) {
-      const int blk = kv_block(batch_idx, table, b, c0, nblocks, block_rows, max_pages);
-      const int row = blk * block_rows + (table ? c0 % block_rows : c0);
-      chunks[list + at] = make_int2(row, chunk_meta(valid, kind == 2) | (j << kChunkLogicalShift));
+  const int n = kv_item_list(batch_idx, table, b, L, (b + 1) * Sq - L, r0, nr, sp, nsplit, nblocks, block_rows,
+                             max_pages, slots, sink, left, right, block, chunks + list);
+  if (lane == 0) put_item(items + 2 * it, r0, nr, list, n);
+}
+
+// Variable-length plans: stream b's queries are packed rows [cq_b, cq_b+1) with cq_b = cu_q[b] clamped to [0, total_q],
+// and its L_b = min(cache_seqlens[b] + cu_new[b+1] - cu_new[b], cap) keys (no cu_new: no rows appended).  Its rows are
+// cut into ceil(Lq_b / 256) items from its first row, numbered in stream order; item s I + i is split s of item i, and
+// items i past the streams' items get zero rows and an empty list, so they write nothing.  Block 0 writes the header
+// {B, kKvVarlen, L_b, cq_b}; each warp finds its item's stream from the scanned item counts, 32 streams at a time.
+__device__ __forceinline__ int kv_row_bound(const int* __restrict__ cu, int b, int total) {
+  return min(max(__ldg(&cu[b]), 0), total);
+}
+__device__ __forceinline__ int kv_new_rows(const int* __restrict__ cu_new, int b) {
+  return cu_new ? max(__ldg(&cu_new[b + 1]) - __ldg(&cu_new[b]), 0) : 0;
+}
+
+__global__ void __launch_bounds__(256)
+kv_varlen_lists_kernel(const int* __restrict__ cu_q, const int* __restrict__ seqlens, const int* __restrict__ cu_new,
+                       const int* __restrict__ batch_idx, const int* __restrict__ table, int B, int total_q, int I,
+                       int nblocks, int block_rows, int max_pages, int cap, int slots, int nsplit, int sink, int left,
+                       int right, int block, int* __restrict__ counts, int* __restrict__ kv, int2* __restrict__ chunks,
+                       int4* __restrict__ items) {
+  const int lane = threadIdx.x & 31;
+  const int it = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (blockIdx.x == 0) {
+    for (int b = threadIdx.x; b <= B; b += blockDim.x) {
+      kv[2 + B + b] = kv_row_bound(cu_q, b, total_q);
+      if (b < B) kv[2 + b] = kv_len(__ldg(&seqlens[b]), kv_new_rows(cu_new, b), cap);
     }
-    n += __popc(m);
+    if (threadIdx.x == 0) {
+      counts[0] = nsplit * I;
+      kv[0] = B;
+      kv[1] = kKvVarlen;
+    }
   }
-  if (lane == 0) put_item(items + 2 * it, r0, nr, list, min(n, slots));
+  if (it >= nsplit * I) return;
+  const int sp = it / I, i = it - sp * I;
+  int b = -1, k = 0;  // item i is item k of stream b
+  for (int b0 = 0, before = 0; b0 < B && b < 0; b0 += 32) {
+    const int bb = b0 + lane;
+    int lo = 0, nq = 0;
+    if (bb < B) {
+      lo = kv_row_bound(cu_q, bb, total_q);
+      nq = max(kv_row_bound(cu_q, bb + 1, total_q) - lo, 0);
+    }
+    const int n = (nq + kItemRows - 1) / kItemRows;
+    int incl = n;  // inclusive scan of the item counts over the lanes
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int x = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += x;
+    }
+    const int first = before + incl - n;
+    const unsigned hit = __ballot_sync(0xffffffffu, i >= first && i < first + n);
+    if (hit) {
+      const int src = __ffs(hit) - 1;
+      b = b0 + src;
+      k = i - __shfl_sync(0xffffffffu, first, src);
+    }
+    before += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  const int list = it * slots;
+  if (b < 0) {
+    if (lane == 0) put_item(items + 2 * it, 0, 0, list, 0);
+    return;
+  }
+  const int lo = kv_row_bound(cu_q, b, total_q), hi = max(kv_row_bound(cu_q, b + 1, total_q), lo);
+  const int L = kv_len(__ldg(&seqlens[b]), kv_new_rows(cu_new, b), cap);
+  const int r0 = lo + k * kItemRows, nr = min(kItemRows, hi - r0);
+  const int n = kv_item_list(batch_idx, table, b, L, hi - L, r0, nr, sp, nsplit, nblocks, block_rows, max_pages, slots,
+                             sink, left, right, block, chunks + list);
+  if (lane == 0) put_item(items + 2 * it, r0, nr, list, n);
 }
 
 // Workspace of a KV-cache plan, 16-byte aligned pieces:
@@ -192,18 +294,23 @@ kv_lists_kernel(const int* __restrict__ seqlens, const int* __restrict__ batch_i
 // ceil(slots / nsplit) slots each, the most a split's piece can hold.  A block-causal plan passes right = C - 1 here: its
 // rows' block ends lie up to C - 1 past them, so an item's window [e(p0) - W, e(p1) - 1] spans at most 255 + (W - 1) +
 // (C - 1) + 1 keys.
+// A variable-length plan (varlen_items = I > 0, its items per split) has nsplit I items, and its header
+// {B, kKvVarlen, L_0 .. L_B-1, cq_0 .. cq_B} holds B + 1 more ints.
 struct KvLayout {
   long long items, slots;
   size_t items_off, chunks_off, bytes;
 };
-static KvLayout kv_layout(int B, int Sq, int cap, int sink, int left, int right, int nsplit = 1) {
+static KvLayout kv_layout(int B, int Sq, int cap, int sink, int left, int right, int nsplit = 1,
+                          long long varlen_items = 0) {
   KvLayout L;
-  L.items = static_cast<long long>(nsplit) * B * ((Sq + kItemRows - 1) / kItemRows);
+  L.items = static_cast<long long>(nsplit) *
+            (varlen_items > 0 ? varlen_items : static_cast<long long>(B) * ((Sq + kItemRows - 1) / kItemRows));
   const long long win = (static_cast<long long>(sink) + kChunkCols - 1) / kChunkCols +
                         (kItemRows - 1 + static_cast<long long>(left) + right) / kChunkCols + 2;
   const long long slots = std::min<long long>((static_cast<long long>(cap) + kChunkCols - 1) / kChunkCols, win);
   L.slots = (slots + nsplit - 1) / nsplit;
-  L.items_off = SVGB_PLAN_SEG_BOUNDS_OFF + align_up(sizeof(int) * (2 + static_cast<size_t>(B)), 16);
+  L.items_off = SVGB_PLAN_SEG_BOUNDS_OFF +
+                align_up(sizeof(int) * (2 + static_cast<size_t>(B) + (varlen_items > 0 ? B + 1 : 0)), 16);
   L.chunks_off = L.items_off + 2 * sizeof(int4) * L.items;
   L.bytes = L.chunks_off + sizeof(int2) * L.items * L.slots;
   return L;
@@ -265,7 +372,7 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
                          int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                          const long long* vc_strides, const long long* k_strides, const long long* v_strides,
                          const float* k_scale, const float* v_scale, float* k_rows, float* v_rows, void* stream,
-                         const char* who) {
+                         const char* who, const int32_t* cu_new = nullptr) {
   const bool rows = k_rows != nullptr;
   const bool e4m3 = k_scale != nullptr || rows;
   SVGB_REQUIRE(cache_seqlens, "null pointer");
@@ -285,7 +392,7 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
   int cap = 0;
   if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
   const int nvec = D / 8;
-  const long long total = static_cast<long long>(B) * Snew * Hkv * nvec;
+  const long long total = static_cast<long long>(cu_new ? 1 : B) * Snew * Hkv * nvec;
   const unsigned blocks = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 1 << 20));
   cudaStream_t cs = static_cast<cudaStream_t>(stream);
   const uint16_t *kn = static_cast<const uint16_t*>(k), *vn = static_cast<const uint16_t*>(v);
@@ -293,19 +400,67 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
     kv_append_kernel<KV_COPY><<<blocks, 256, 0, cs>>>(
         static_cast<uint16_t*>(k_cache), static_cast<uint16_t*>(v_cache), kn, vn, cache_seqlens, cache_batch_idx,
         block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages, cap, st[0], st[1], st[2], st[3], nullptr,
-        nullptr, nullptr, nullptr);
+        nullptr, nullptr, nullptr, cu_new);
   } else if (rows) {
     auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_ROWS_BF16> : kv_append_kernel<KV_E4M3_ROWS_F16>;
     kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
                                  cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages,
-                                 cap, st[0], st[1], st[2], st[3], nullptr, nullptr, k_rows, v_rows);
+                                 cap, st[0], st[1], st[2], st[3], nullptr, nullptr, k_rows, v_rows, cu_new);
   } else {
     auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_BF16> : kv_append_kernel<KV_E4M3_F16>;
     kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
                                  cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages,
-                                 cap, st[0], st[1], st[2], st[3], k_scale, v_scale, nullptr, nullptr);
+                                 cap, st[0], st[1], st[2], st[3], k_scale, v_scale, nullptr, nullptr, cu_new);
   }
   SVGB_LAUNCH_OK();
+  return 0;
+}
+
+// Variable-length plans (svgb_attn_plan_kvcache_varlen): the item bound I per split, at most ceil(max_q / 256) items
+// per stream and at most (total_q + 255 B) / 256 in all, since sum ceil(Lq_b / 256) <= (sum Lq_b + 255 B) / 256
+static long long kv_varlen_items(int B, int total_q, int max_q) {
+  return std::min<long long>(static_cast<long long>(B) * ((max_q + kItemRows - 1) / kItemRows),
+                             (static_cast<long long>(total_q) + (kItemRows - 1) * static_cast<long long>(B)) / kItemRows);
+}
+
+// The arguments of the varlen pair, checked by name: block = 0 is the local band (sink, left, right) and takes no window
+// or first_block; block > 0 the block-causal mask (sink, W, C, F) and takes no left or right.  Gives the planner's m1
+// (0: local), left and right, and the layout's workspace.
+struct KvVarlen {
+  int m1, left, right;
+  long long I;
+  KvLayout L;
+};
+static int kv_varlen_args(int B, int total_q, int max_q, int cap, int sink, int left, int right, int window, int block,
+                          int first_block, int num_splits, KvVarlen* a, const char* who) {
+  SVGB_REQUIRE(B > 0 && total_q > 0 && cap > 0, "%s: bad arguments (B=%d, total_q=%d, capacity=%d)", who, B, total_q,
+               cap);
+  SVGB_REQUIRE(total_q < (1 << 30), "%s: total_q = %d query rows too many", who, total_q);
+  SVGB_REQUIRE(max_q >= 1 && max_q <= total_q, "%s: max_q (%d) must lie in [1, total_q = %d]", who, max_q, total_q);
+  SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
+  a->m1 = 0;
+  int widen = 0;  // the layout's right beyond the planner's: C - 1 for a block-causal plan
+  if (block) {
+    SVGB_REQUIRE(left == 0 && right == 0,
+                 "%s: a block-causal plan (block = %d) takes (window, block, first_block); left and right must be 0 "
+                 "(got %d, %d)", who, block, left, right);
+    if (block_causal_m1(block, first_block, &a->m1, who) || block_causal_check(sink, a->m1, window, who)) return -1;
+    a->left = window - 1;
+    a->right = 0;
+    widen = block - 1;
+  } else {
+    SVGB_REQUIRE(window == 0 && first_block == 0,
+                 "%s: a local plan (block = 0) takes (left, right); window and first_block must be 0 (got %d, %d)", who,
+                 window, first_block);
+    SVGB_REQUIRE(sink >= 0 && left >= 0 && right >= 0,
+                 "%s: sink (%d), left (%d) and right (%d) must be >= 0", who, sink, left, right);
+    a->left = left;
+    a->right = right;
+  }
+  a->I = kv_varlen_items(B, total_q, max_q);
+  a->L = kv_layout(B, total_q, cap, sink, a->left, a->right + widen, num_splits, a->I);
+  SVGB_REQUIRE(a->L.items * a->L.slots < (1ll << 31) && a->L.items < (1ll << 31),
+               "%s: plan too large for 32-bit chunk offsets", who);
   return 0;
 }
 
@@ -337,6 +492,7 @@ static int kv_plan_run(const int32_t* cache_seqlens, const int32_t* cache_batch_
   plan->m0 = sink;
   plan->m1 = block ? block : left;
   plan->m2 = block ? left + 1 : right;
+  plan->varlen_items = 0;
   plan->counts_off = 0;
   plan->items_off = static_cast<int64_t>(L.items_off);
   plan->chunks_off = static_cast<int64_t>(L.chunks_off);
@@ -437,6 +593,76 @@ int svgb_attn_plan_kvcache_block(const int32_t* cache_seqlens, const int32_t* ca
   if (kv_block_m1(sink, window, block, first_block, num_splits, &m1, who)) return -1;
   return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
                      window - 1, 0, num_splits, num_splits > 1, plan_ws, ws_bytes, plan, stream, who, m1);
+}
+
+int svgb_kvcache_append_varlen(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cu_new,
+                               const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                               const int32_t* block_table, int dtype, int B, int total_new, int Hkv, int D,
+                               int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
+                               const long long* vc_strides, const long long* k_strides, const long long* v_strides,
+                               float* k_scale, float* v_scale, int row_scales, void* stream) {
+  const char* who = "svgb_kvcache_append_varlen";
+  SVGB_REQUIRE(cu_new, "%s needs cu_new (device int32 [B + 1], the new rows of each stream)", who);
+  SVGB_REQUIRE(B > 0, "%s: bad stream count B=%d", who, B);
+  if (row_scales) {
+    if (kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
+    return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, total_new, Hkv,
+                         D, num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
+                         nullptr, k_scale, v_scale, stream, who, cu_new);
+  }
+  SVGB_REQUIRE(!k_scale == !v_scale, "%s: an e4m3 cache needs both scale vectors k_scale and v_scale (float [Hkv]); a "
+               "16-bit cache takes neither", who);
+  return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, total_new, Hkv, D,
+                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, k_scale, v_scale,
+                       nullptr, nullptr, stream, who, cu_new);
+}
+
+int svgb_attn_plan_kvcache_varlen_bytes(int B, int total_q, int max_q, int cap, int sink, int left, int right,
+                                        int window, int block, int first_block, int num_splits, size_t* bytes) {
+  const char* who = "svgb_attn_plan_kvcache_varlen_bytes";
+  SVGB_REQUIRE(bytes, "null pointer");
+  KvVarlen a;
+  if (kv_varlen_args(B, total_q, max_q, cap, sink, left, right, window, block, first_block, num_splits, &a, who))
+    return -1;
+  *bytes = a.L.bytes;
+  return 0;
+}
+
+int svgb_attn_plan_kvcache_varlen(const int32_t* cu_q, const int32_t* cache_seqlens, const int32_t* cu_new,
+                                  const int32_t* cache_batch_idx, const int32_t* block_table, int B, int total_q,
+                                  int max_q, int num_blocks, int block_rows, int max_pages, int sink, int left,
+                                  int right, int window, int block, int first_block, int num_splits, void* plan_ws,
+                                  size_t ws_bytes, svgb_plan* plan, void* stream) {
+  const char* who = "svgb_attn_plan_kvcache_varlen";
+  SVGB_REQUIRE(cu_q && cache_seqlens && plan_ws && plan, "null pointer");
+  int cap = 0;
+  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
+  KvVarlen a;
+  if (kv_varlen_args(B, total_q, max_q, cap, sink, left, right, window, block, first_block, num_splits, &a, who))
+    return -1;
+  SVGB_REQUIRE(ws_bytes >= a.L.bytes, "plan workspace too small: %zu < %zu", ws_bytes, a.L.bytes);
+  plan->kind = num_splits > 1 ? SVGB_PLAN_KVCACHE_SPLIT : SVGB_PLAN_KVCACHE;
+  plan->BH = num_blocks * block_rows;
+  plan->S = total_q;
+  plan->max_items = static_cast<int>(a.L.items);
+  plan->items_stride = 0;
+  plan->mask_mode = block ? MASK_BLOCK_CAUSAL : MASK_LOCAL;
+  plan->m0 = sink;
+  plan->m1 = block ? a.m1 : a.left;
+  plan->m2 = block ? window : a.right;
+  plan->varlen_items = static_cast<int>(a.I);
+  plan->counts_off = 0;
+  plan->items_off = static_cast<int64_t>(a.L.items_off);
+  plan->chunks_off = static_cast<int64_t>(a.L.chunks_off);
+  plan->bytes = static_cast<int64_t>(a.L.bytes);
+  char* ws = static_cast<char*>(plan_ws);
+  kv_varlen_lists_kernel<<<static_cast<unsigned>((a.L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      cu_q, cache_seqlens, cu_new, cache_batch_idx, block_table, B, total_q, static_cast<int>(a.I), num_blocks,
+      block_rows, max_pages, cap, static_cast<int>(a.L.slots), num_splits, sink, a.left, a.right, a.m1,
+      reinterpret_cast<int*>(ws), reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF),
+      reinterpret_cast<int2*>(ws + a.L.chunks_off), reinterpret_cast<int4*>(ws + a.L.items_off));
+  SVGB_LAUNCH_OK();
+  return 0;
 }
 
 }  // extern "C"

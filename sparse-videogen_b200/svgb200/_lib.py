@@ -23,6 +23,7 @@ class Plan(C.Structure):
         ("kind", C.c_int32), ("BH", C.c_int32), ("S", C.c_int32), ("max_items", C.c_int32),
         ("items_stride", C.c_int32),
         ("mask_mode", C.c_int32), ("m0", C.c_int32), ("m1", C.c_int32), ("m2", C.c_int32),
+        ("varlen_items", C.c_int32),
         ("counts_off", C.c_int64), ("items_off", C.c_int64), ("chunks_off", C.c_int64),
         ("bytes", C.c_int64),
     ]
@@ -63,6 +64,11 @@ _PROTOS = {
     "svgb_attn_plan_kvcache_split": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
     "svgb_attn_plan_kvcache_block_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _psz],
     "svgb_attn_plan_kvcache_block": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _pplan, _vp],
+    "svgb_attn_plan_kvcache_varlen_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _psz],
+    "svgb_attn_plan_kvcache_varlen": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp,
+                                      _sz, _pplan, _vp],
+    "svgb_kvcache_append_varlen": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _pll, _pll,
+                                   _pll, _pll, _vp, _vp, _i, _vp],
     "svgb_attn_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _f,
                       _pplan, _vp, _vp],
     "svgb_attn_fwd_kv": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _f, _pplan, _vp,

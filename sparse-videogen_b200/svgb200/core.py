@@ -359,7 +359,8 @@ def _cache_layout(B, block_table, cache_batch_idx):
 
 def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cache_seqlens, *,
                    block_table: Optional[torch.Tensor] = None, cache_batch_idx: Optional[torch.Tensor] = None,
-                   k_scale: Optional[torch.Tensor] = None, v_scale: Optional[torch.Tensor] = None):
+                   k_scale: Optional[torch.Tensor] = None, v_scale: Optional[torch.Tensor] = None,
+                   cu_seqlens: Optional[torch.Tensor] = None):
     """Write the new rows k, v [B, Snew, Hkv, D] into the cache in place, at keys cache_seqlens[b] .. + Snew - 1 of each
     stream b, in one launch.  The cache is contiguous, k_cache / v_cache [B_cache, S_cache, Hkv, D] with stream b in
     row cache_batch_idx[b] (default b), or paged, [num_pages, page_size, Hkv, D] with block_table int [B, max_pages]
@@ -370,7 +371,13 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     RN-satfinite(x * (1 / scale[h])), values past 448 * scale saturating (svgb_kvcache_append_e4m3).  [num_blocks, Hkv,
     block_rows] (contiguous, block_rows a multiple of 4, D = 128): one power-of-two scale per cache row, which the append
     computes from the row's absmax and writes there, so nothing saturates (svgb_kvcache_append_e4m3_rows).  16-bit
-    caches take no scales."""
+    caches take no scales.
+    cu_seqlens (device int [B + 1], FlashAttention 3's cu_seqlens_k_new): variable-length appends, k, v packed as
+    [total_new, Hkv, D] with stream b's rows at [cu_seqlens[b], cu_seqlens[b+1]), written at keys cache_seqlens[b] ..
+    under the same rules, in every cache format and one launch (svgb_kvcache_append_varlen)."""
+    if cu_seqlens is not None:
+        return _kvcache_append_varlen(k_cache, v_cache, k, v, cache_seqlens, block_table, cache_batch_idx, k_scale,
+                                      v_scale, cu_seqlens)
     _need_cuda(k_cache, v_cache, k, v)
     if k_cache.dim() != 4 or k.dim() != 4 or k_cache.shape != v_cache.shape or k.shape != v.shape:
         raise SvgbError(f"kvcache_append: k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] and "
@@ -416,6 +423,52 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     _bump()
 
 
+def _kvcache_append_varlen(k_cache, v_cache, k, v, cache_seqlens, block_table, cache_batch_idx, k_scale, v_scale,
+                           cu_seqlens):
+    """kvcache_append(cu_seqlens=): packed k, v [total_new, Hkv, D], svgb_kvcache_append_varlen."""
+    who = "kvcache_append"
+    _need_cuda(k_cache, v_cache, k, v)
+    if k_cache.dim() != 4 or k.dim() != 3 or k_cache.shape != v_cache.shape or k.shape != v.shape:
+        raise SvgbError(f"{who}: with cu_seqlens, k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] "
+                        f"and k, v {tuple(k.shape)} [total_new, Hkv, D], each pair of one shape")
+    if k.shape[1:] != k_cache.shape[2:]:
+        raise SvgbError(f"{who}: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
+    cu = _cu_seqlens(who, "cu_seqlens", cu_seqlens, None, k.device)
+    B = cu.numel() - 1
+    fp8 = k_cache.dtype == torch.float8_e4m3fn
+    rows = scales = None
+    if fp8:
+        if v_cache.dtype != k_cache.dtype or k.dtype != v.dtype:
+            raise SvgbError(f"{who}: an e4m3 k_cache needs an e4m3 v_cache, and k, v of one 16-bit dtype")
+        rows = _row_scales(who, k_scale, v_scale, k_cache)
+        scales = rows or _fp8_scales(who, k_scale, v_scale, k.shape[1])
+    else:
+        if k_scale is not None or v_scale is not None:
+            raise SvgbError(f"{who}: k_scale / v_scale are for float8_e4m3fn caches; a {k_cache.dtype} cache takes none")
+        if not (k_cache.dtype == v_cache.dtype == k.dtype == v.dtype):
+            raise SvgbError(f"{who}: the caches and the new rows must share one dtype")
+    dt = _dt(k)
+    T, Hkv, D = k.shape
+    if T == 0:
+        return
+    for c in (k_cache, v_cache):
+        if not _addressable(c.transpose(1, 2), "bhsd"):
+            raise SvgbError(f"{who}: the cache is written in place, so it must be 16-byte aligned with a last stride of 1 "
+                            "and other strides that are nonzero multiples of 8 elements")
+    k, v = (_addressed(t, "shd") for t in (k, v))
+    bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
+    lens = _seqlens(cache_seqlens, B, k.device)
+    fill = 16 if fp8 else 8
+    check(lib().svgb_kvcache_append_varlen(k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(),
+                                           cu.data_ptr(), lens.data_ptr(), _p(bi), _p(bt), dt, B, T, Hkv, D,
+                                           k_cache.shape[0], k_cache.shape[1], max_pages,
+                                           _st(k_cache.transpose(1, 2), "bhsd", fill),
+                                           _st(v_cache.transpose(1, 2), "bhsd", fill), _st(k, "shd"), _st(v, "shd"),
+                                           *((None, None) if scales is None else (t.data_ptr() for t in scales)),
+                                           1 if rows else 0, _stream(k)), "svgb_kvcache_append_varlen")
+    _bump()
+
+
 def _fp8_scales(who, k_scale, v_scale, Hkv):
     """The per-KV-head dequantisation scales of an e4m3 cache: both float32 device tensors [Hkv]."""
     if k_scale is None or v_scale is None:
@@ -451,11 +504,13 @@ def _row_scales(who, k_scale, v_scale, cache):
     return k_scale, v_scale
 
 
-def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0, cache_len: Optional[int] = None,
-                 block_table: Optional[torch.Tensor] = None, page_size: Optional[int] = None,
-                 cache_batch_idx: Optional[torch.Tensor] = None, causal: bool = False, window_size=(-1, -1),
-                 sink: int = 0, num_splits: int = 1, num_heads: Optional[int] = None, block: int = 0,
-                 first_block: Optional[int] = None) -> AttnPlan:
+def plan_kvcache(cache_seqlens, *, q_len: Optional[int] = None, num_blocks: int, new_len: int = 0,
+                 cache_len: Optional[int] = None, block_table: Optional[torch.Tensor] = None,
+                 page_size: Optional[int] = None, cache_batch_idx: Optional[torch.Tensor] = None, causal: bool = False,
+                 window_size=(-1, -1), sink: int = 0, num_splits: int = 1, num_heads: Optional[int] = None,
+                 block: int = 0, first_block: Optional[int] = None, cu_seqlens_q: Optional[torch.Tensor] = None,
+                 total_q: Optional[int] = None, max_seqlen_q: Optional[int] = None,
+                 cu_seqlens_new: Optional[torch.Tensor] = None) -> AttnPlan:
     """Attention of B streams of q_len queries into a KV cache, in FlashAttention's conventions
     (flash_attn_with_kvcache): stream b holds L_b = cache_seqlens[b] + new_len keys (new_len rows appended before this
     attention, e.g. by kvcache_append) and its query i sits at logical position L_b - q_len + i.  Query p sees key kv
@@ -473,8 +528,26 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
     `first_block`, default block): query p sees kv < sink and e(p) - W <= kv < e(p), with W = window_size[0] counted
     back from the block end (-1: unbounded) and window_size[1] = -1; causal=True is refused (the rule is causal).  When
     the q_len queries form one block, they all attend [L_b - W, L_b) plus the sinks.  A rolling cache that renumbers its
-    positions down by d keys keeps its blocks with first_block = ((F - d - 1) mod block) + 1 (INTEGRATION.md)."""
+    positions down by d keys keeps its blocks with first_block = ((F - d - 1) mod block) + 1 (INTEGRATION.md).
+    Variable-length queries (FlashAttention 3's cu_seqlens_q, in place of q_len): cu_seqlens_q device int [B + 1], stream
+    b's Lq_b = cu_seqlens_q[b+1] - cu_seqlens_q[b] queries are packed rows [cu_seqlens_q[b], cu_seqlens_q[b+1]) of q
+    [total_q, Hq, D], and its query i sits at L_b - Lq_b + i; total_q (q.shape[0]) is required and max_seqlen_q, the
+    longest Lq_b when known, tightens the plan's item bound (a stream longer than it gives an unspecified result).
+    cu_seqlens_new, device int [B + 1], gives the rows appended before this attention per stream (kvcache_append(...,
+    cu_seqlens=)) in place of new_len.  Every mask rule, num_splits and block= work as above, with one (block,
+    first_block) for the batch; Lq_b = 0 is legal.  attn_fwd then takes q [total_q, Hq, D] and returns o [total_q, Hq,
+    D] and lse [Hq, total_q].  Nothing is read on the host (svgb_attn_plan_kvcache_varlen)."""
+    if (q_len is None) == (cu_seqlens_q is None):
+        raise SvgbError("plan_kvcache: pass q_len (B streams of q_len queries) or cu_seqlens_q (variable-length "
+                        "queries), exactly one of them")
+    if cu_seqlens_new is not None and cu_seqlens_q is None:
+        raise SvgbError("plan_kvcache: cu_seqlens_new (variable-length appends) goes with cu_seqlens_q; uniform plans "
+                        "take new_len")
     blk = _kvcache_block_args(causal, window_size, sink, block, first_block) if block else None
+    if cu_seqlens_q is not None:
+        return _plan_kvcache_varlen(cache_seqlens, cu_seqlens_q, total_q, max_seqlen_q, cu_seqlens_new, new_len,
+                                    num_blocks, cache_len, block_table, page_size, cache_batch_idx, causal,
+                                    window_size, sink, num_splits, num_heads, blk)
     if block_table is not None:
         B = block_table.shape[0]
         if page_size is None:
@@ -525,6 +598,84 @@ def plan_kvcache(cache_seqlens, *, q_len: int, num_blocks: int, new_len: int = 0
                                                  C.byref(desc), stream), "svgb_attn_plan_kvcache_split")
     _bump()
     return AttnPlan(desc, ws, (B, Sq))
+
+
+def _cu_seqlens(who, name, cu, B, device) -> torch.Tensor:
+    """A cu_seqlens argument as device int32 [B + 1] (B None: any B >= 1), refused by name before any launch."""
+    if not isinstance(cu, torch.Tensor):
+        raise SvgbError(f"{who}: {name} must be a device int tensor [B + 1] (got {type(cu).__name__})")
+    if not cu.is_cuda:
+        raise SvgbError(f"{who}: {name} is on the CPU; variable-length KV-cache plans and appends read their bounds on "
+                        "the device only (no host read), so pass a CUDA tensor")
+    if cu.dim() != 1 or cu.numel() < 2 or (B is not None and cu.numel() != B + 1) or cu.is_floating_point():
+        want = "B + 1 >= 2" if B is None else f"B + 1 = {B + 1}"
+        raise SvgbError(f"{who}: {name} must be a 1-D int tensor of {want} entries (got {tuple(cu.shape)}, {cu.dtype})")
+    if device is not None and cu.device != device:
+        raise SvgbError(f"{who}: {name} is on {cu.device}, the other tensors on {device}")
+    return cu.to(torch.int32).contiguous()
+
+
+def _plan_kvcache_varlen(cache_seqlens, cu_seqlens_q, total_q, max_seqlen_q, cu_seqlens_new, new_len, num_blocks,
+                         cache_len, block_table, page_size, cache_batch_idx, causal, window_size, sink, num_splits,
+                         num_heads, blk):
+    """plan_kvcache(cu_seqlens_q=): svgb_attn_plan_kvcache_varlen, single (n = 1) or split, every argument checked
+    before the one launch."""
+    who = "plan_kvcache"
+    if total_q is None:
+        raise SvgbError(f"{who}: cu_seqlens_q needs total_q (q.shape[0], the packed query rows), which is passed rather "
+                        "than read from the device")
+    if cu_seqlens_new is not None and int(new_len):
+        raise SvgbError(f"{who}: cu_seqlens_new and new_len={new_len} both give the appended rows; pass one")
+    cu_q = _cu_seqlens(who, "cu_seqlens_q", cu_seqlens_q, None, None)
+    B = cu_q.numel() - 1
+    Tq = int(total_q)
+    if Tq < 1:
+        raise SvgbError(f"{who}: total_q={Tq} must be >= 1")
+    max_q = Tq if max_seqlen_q is None else int(max_seqlen_q)
+    if not 1 <= max_q <= Tq:
+        raise SvgbError(f"{who}: max_seqlen_q={max_q} must lie in [1, total_q={Tq}]")
+    cu_new = None if cu_seqlens_new is None else _cu_seqlens(who, "cu_seqlens_new", cu_seqlens_new, B, cu_q.device)
+    if block_table is not None:
+        if page_size is None:
+            raise SvgbError(f"{who}: a paged cache (block_table) needs page_size")
+        rows = int(page_size)
+        cap = block_table.shape[1] * rows
+    else:
+        if cache_len is None:
+            raise SvgbError(f"{who}: a contiguous cache needs cache_len (its rows per stream, k_cache.shape[1])")
+        rows = cap = int(cache_len)
+    bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
+    lens = _seqlens(cache_seqlens, B, cu_q.device)
+    if lens.device != cu_q.device:
+        raise SvgbError(f"{who}: cache_seqlens is on {lens.device}, cu_seqlens_q on {cu_q.device}")
+    if blk:
+        C_, F, W = blk
+        if W == -1:  # no query's block end lies further than cap + max_q + C from key 0
+            W = min(cap + max_q + C_, 2**31 - 1)
+        left, right, mask = W - 1, C_ - 1, (0, 0, W, C_, F)  # slot bound: left = W - 1, right = C - 1
+    else:
+        left, right = (int(w) for w in window_size)
+        if causal:
+            if right > 0:
+                raise SvgbError(f"{who}: causal=True looks no key ahead, but window_size[1] = {right}")
+            right = 0
+        # -1: no query position lies further than cap + max_q from a key
+        left, right = (min(cap + max_q, 2**31 - 1) if w == -1 else w for w in (left, right))
+        mask = (left, right, 0, 0, 0)
+    items = min(B * -(-max_q // 256), (Tq + 255 * B) // 256)  # the item bound I (svgb_attn_plan_kvcache_varlen_bytes)
+    n = _num_splits(num_splits, num_heads, items, 256, cap, sink, left, right)
+    nbytes = C.c_size_t()
+    check(lib().svgb_attn_plan_kvcache_varlen_bytes(B, Tq, max_q, cap, int(sink), *mask, n, C.byref(nbytes)),
+          "svgb_attn_plan_kvcache_varlen_bytes")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=cu_q.device)  # owned by the plan, with its header
+    desc = Plan()
+    check(lib().svgb_attn_plan_kvcache_varlen(cu_q.data_ptr(), lens.data_ptr(), _p(cu_new), _p(bi), _p(bt), B, Tq, max_q,
+                                              int(num_blocks), rows, max_pages, int(sink), *mask, n, ws.data_ptr(),
+                                              ws.numel(), C.byref(desc), torch.cuda.current_stream(cu_q.device).cuda_stream),
+          "svgb_attn_plan_kvcache_varlen")
+    _bump()
+    # attn_fwd runs the plan as one block of total_q packed rows
+    return AttnPlan(desc, ws, (1, Tq))
 
 
 def _num_splits(num_splits, num_heads, B, Sq, cap, sink, left, right):
@@ -746,6 +897,8 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     if plan.desc.kind in (PLAN_KVCACHE, PLAN_KVCACHE_SPLIT):
         if any(r is not None for r in (q_rows, kv_rows, o_rows)):
             raise SvgbError("a KV-cache plan (plan_kvcache) takes no row vectors (o_rows / q_rows / kv_rows)")
+        if plan.desc.varlen_items:
+            return _attn_kvcache_varlen(q, k, v, plan, return_lse, sm_scale, out, k_scale, v_scale)
         return _attn_kvcache(q, k, v, plan, return_lse, sm_scale, out, k_scale, v_scale)
     if k_scale is not None or v_scale is not None:
         raise SvgbError("k_scale / v_scale are for float8_e4m3fn caches under a KV-cache plan (plan_kvcache); other "
@@ -819,6 +972,25 @@ def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=
     return o, res[1].view(Hq, B, Sq).transpose(0, 1)
 
 
+def _attn_kvcache_varlen(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
+    """attn_fwd under a variable-length KV-cache plan (plan_kvcache(cu_seqlens_q=)): q [total_q, Hq, D] runs as one
+    block of total_q packed rows through _attn_kvcache, in every cache format, single pass or split; returns o
+    [total_q, Hq, D] (out itself when given) and lse [Hq, total_q], FlashAttention's varlen shapes."""
+    R = plan.S
+    if q.dim() != 3 or q.shape[0] != R:
+        raise SvgbError(f"a variable-length KV-cache plan for total_q={R} query rows takes q [total_q, Hq, D] (got "
+                        f"{tuple(q.shape)})")
+    if out is not None and (out.shape != q.shape or out.dim() != 3):
+        raise SvgbError(f"out {tuple(out.shape)} must have q's shape [total_q, Hq, D] {tuple(q.shape)}")
+    if needs_grad(q, k_cache, v_cache):
+        raise SvgbError("attention into a KV cache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
+    res = _attn_kvcache(q[None], k_cache, v_cache, plan, return_lse, sm_scale, None if out is None else out[None],
+                        k_scale, v_scale)
+    o = res[0] if return_lse else res
+    o = out if out is not None else o[0]
+    return (o, res[1][0]) if return_lse else o
+
+
 def _split_out(out, rows, Hq, D, dtype, device):
     """o [rows, Hq, D] of a split forward: out itself when it is contiguous (the merge writes it in place), else new."""
     if out is not None and out.is_contiguous():
@@ -833,7 +1005,7 @@ def _split_fwd(qf, q_strides, kf, vf, scales, o, plan, dtype, row_scales, cache_
     B, Sq = plan.source
     R, Hq, D = o.shape
     nb, rows, Hkv = cache_shape[:3]
-    n = plan.desc.max_items // (B * -(-Sq // 256))
+    n = plan.desc.max_items // (plan.desc.varlen_items or B * -(-Sq // 256))
     nbytes = C.c_size_t()
     check(lib().svgb_attn_fwd_kvcache_split_bytes(n, R, Hq, D, C.byref(nbytes)), "svgb_attn_fwd_kvcache_split_bytes")
     ws = workspace("kvcache_split", nbytes.value, o.device)

@@ -129,7 +129,8 @@ def _is_fp8(t) -> bool:
 def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None, rotary_sin=None, cache_seqlens=None,
                             cache_batch_idx=None, cache_leftpad=None, block_table=None, softmax_scale=None, causal=False,
                             window_size=(-1, -1), softcap=0.0, rotary_interleaved=True, alibi_slopes=None,
-                            num_splits=0, return_softmax_lse=False, *, q_descale=None, k_descale=None, v_descale=None):
+                            num_splits=0, return_softmax_lse=False, *, q_descale=None, k_descale=None, v_descale=None,
+                            cu_seqlens_q=None, cu_seqlens_k_new=None, max_seqlen_q=None):
     """flash_attn.flash_attn_with_kvcache (FlashAttention 2's signature and return convention), forward only.
     q [B, Sq, Hq, D]; k_cache, v_cache [B_cache, S_cache, Hkv, D] (stream b in row cache_batch_idx[b], default b) or
     paged [num_pages, page_size, Hkv, D] with block_table int32 [B, max_pages] (page_size a multiple of 128).  k, v
@@ -144,7 +145,12 @@ def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None
     FlashAttention 3, float32 [Hkv]: one dequantisation scale per key/value head for the whole cache (FlashAttention 3
     takes [B, Hkv], one per stream, which is refused by shape).  q stays bf16 and is quantised per query head inside the
     call; k, v stay 16-bit and are quantised by the append; out is bf16, D = 128.  An fp8 q, fp8 k / v and q_descale
-    are refused.  Without k_descale / v_descale the call makes exactly the 16-bit launches."""
+    are refused.  Without k_descale / v_descale the call makes exactly the 16-bit launches.
+    Variable-length streams (keyword-only, named as in FlashAttention 3): cu_seqlens_q device int [B + 1] packs stream
+    b's queries at rows [cu_seqlens_q[b], cu_seqlens_q[b+1]) of q [total_q, Hq, D]; cu_seqlens_k_new, device int
+    [B + 1], packs its new rows k, v [total_k_new, Hkv, D] likewise (required with k, v then), and max_seqlen_q, the
+    longest stream's queries, tightens the plan.  Returns out [total_q, Hq, D] and lse [Hq, total_q].  Still one
+    append, one plan and one forward (core.plan_kvcache(cu_seqlens_q=))."""
     import torch
 
     from . import core
@@ -177,6 +183,10 @@ def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None
         raise SvgbError("flash_attn_with_kvcache: k_descale and v_descale (float32 [Hkv]) go together with a "
                         "float8_e4m3fn cache, and only with one")
     scales = dict(k_scale=k_descale, v_scale=v_descale) if given else {}
+    if cu_seqlens_q is not None or cu_seqlens_k_new is not None or max_seqlen_q is not None:
+        return _with_kvcache_varlen(q, k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table,
+                                    softmax_scale, causal, window_size, return_softmax_lse, scales, cu_seqlens_q,
+                                    cu_seqlens_k_new, max_seqlen_q)
     B, Sq = q.shape[:2]
     if cache_seqlens is None:
         if block_table is not None:
@@ -188,6 +198,44 @@ def flash_attn_with_kvcache(q, k_cache, v_cache, k=None, v=None, rotary_cos=None
                             **scales)
     paged = block_table is not None
     plan = core.plan_kvcache(lens, q_len=Sq, num_blocks=k_cache.shape[0], new_len=0 if k is None else k.shape[1],
+                             cache_len=None if paged else k_cache.shape[1], block_table=block_table,
+                             page_size=k_cache.shape[1] if paged else None, cache_batch_idx=cache_batch_idx,
+                             causal=causal, window_size=window_size)
+    return core.attn_fwd(q, k_cache, v_cache, plan, return_lse=return_softmax_lse, sm_scale=softmax_scale, **scales)
+
+
+def _with_kvcache_varlen(q, k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, softmax_scale, causal,
+                        window_size, return_softmax_lse, scales, cu_seqlens_q, cu_seqlens_k_new, max_seqlen_q):
+    """flash_attn_with_kvcache with FlashAttention 3's variable-length keywords: core.kvcache_append(cu_seqlens=),
+    core.plan_kvcache(cu_seqlens_q=) and core.attn_fwd on q [total_q, Hq, D]."""
+    from . import core
+    from .core import SvgbError
+
+    if cu_seqlens_q is None:
+        raise SvgbError("flash_attn_with_kvcache: cu_seqlens_k_new and max_seqlen_q go with cu_seqlens_q (variable-length "
+                        "queries)")
+    if (k is None) != (cu_seqlens_k_new is None):
+        raise SvgbError("flash_attn_with_kvcache: with cu_seqlens_q, new rows k, v [total_k_new, Hkv, D] come with "
+                        "cu_seqlens_k_new, and cu_seqlens_k_new only with them")
+    if q.dim() != 3:
+        raise SvgbError(f"flash_attn_with_kvcache: with cu_seqlens_q, q must be [total_q, Hq, D] (got {tuple(q.shape)})")
+    cu_q = core._cu_seqlens("flash_attn_with_kvcache", "cu_seqlens_q", cu_seqlens_q, None, q.device)
+    B = cu_q.numel() - 1
+    if cu_seqlens_k_new is not None:  # refused here, before the append launches
+        cu_seqlens_k_new = core._cu_seqlens("flash_attn_with_kvcache", "cu_seqlens_k_new", cu_seqlens_k_new, B, q.device)
+    if max_seqlen_q is not None and not 1 <= int(max_seqlen_q) <= q.shape[0]:
+        raise SvgbError(f"flash_attn_with_kvcache: max_seqlen_q={max_seqlen_q} must lie in [1, total_q={q.shape[0]}]")
+    if cache_seqlens is None:
+        if block_table is not None:
+            raise SvgbError("flash_attn_with_kvcache: a paged cache (block_table) needs cache_seqlens")
+        cache_seqlens = k_cache.shape[1]
+    lens = core._seqlens(cache_seqlens, B, q.device)
+    if k is not None:
+        core.kvcache_append(k_cache, v_cache, k, v, lens, block_table=block_table, cache_batch_idx=cache_batch_idx,
+                            cu_seqlens=cu_seqlens_k_new, **scales)
+    paged = block_table is not None
+    plan = core.plan_kvcache(lens, cu_seqlens_q=cu_q, total_q=q.shape[0], max_seqlen_q=max_seqlen_q,
+                             cu_seqlens_new=cu_seqlens_k_new, num_blocks=k_cache.shape[0],
                              cache_len=None if paged else k_cache.shape[1], block_table=block_table,
                              page_size=k_cache.shape[1] if paged else None, cache_batch_idx=cache_batch_idx,
                              causal=causal, window_size=window_size)
