@@ -85,16 +85,18 @@ def key_inputs(S: int, D: int, enc: int, n_rows: torch.Tensor):
     return ex(q), ex(k), ex(torch.ones(S, D)), ex(o), ex(q), lse.contiguous()
 
 
-def key_expected(cnt: torch.Tensor, cnt_t: torch.Tensor, S: int, D: int, enc: int):
-    """Closed form of one head (fp64): cnt [S, D'] forward table and cnt_t [S, D'] transposed table of encoding enc
-    -> (dq, dk, dv) [S, D]."""
+def key_expected(cnt: torch.Tensor, cnt_t: torch.Tensor, S: int, D: int, enc: int, *, Skv: int | None = None):
+    """Closed form of one head (fp64): cnt [S, D'] forward table and cnt_t [Skv, D'] transposed table of encoding enc
+    (Skv None: S) -> dq [S, D], dk, dv [Skv, D]."""
     Dh = D // 2
+    K = S if Skv is None else Skv
     code = oc.key_codes(S, Dh, enc)
     d = torch.arange(Dh)
     f_row = 0.5 * torch.exp2(-code_L(code).double()) * (1 - code_delta(code)).double()
     f_k = 0.5 * torch.exp2(-code_L(d).double()) * (1 - code_delta(d)).double()
     f_v = torch.exp2(-code_L(d).double())
-    dq, dk, dv = (torch.zeros(S, D, dtype=torch.float64) for _ in range(3))
+    dq = torch.zeros(S, D, dtype=torch.float64)
+    dk, dv = (torch.zeros(K, D, dtype=torch.float64) for _ in range(2))
     dq[:, Dh:] = f_row[:, None] * cnt.cpu().double()
     dk[:, :Dh] = f_k[None] * cnt_t.cpu().double()
     dv[:, :Dh] = f_v[None] * cnt_t.cpu().double()
@@ -109,17 +111,21 @@ def key_counts_representable(max_count: int, dtype) -> bool:
     return bool((vals.to(dtype).double() == vals).all())
 
 
-def band_tables(mod, S: int, D: int, device):
-    """(cnt [2, S, D'], n [S], cnt_t [2, S, D']) of a band predicate mod(q_idx, kv_idx), D' = D / 2."""
-    cnt, n = oc.band_census(mod, S, D // 2, device)
-    cnt_t, _ = oc.band_census(lambda kk, qq: mod(qq, kk), S, D // 2, device)
+def band_tables(mod, S: int, D: int, device, *, Skv: int | None = None):
+    """(cnt [2, S, D'], n [S], cnt_t [2, Skv, D']) of a band predicate mod(q_idx, kv_idx) over S queries and Skv keys
+    (None: S), D' = D / 2.  The transposed table has a row per key and counts the queries by their codes over S."""
+    K = S if Skv is None else Skv
+    cnt, n = oc.band_census(mod, S, D // 2, device, Skv=K)
+    cnt_t, _ = oc.band_census(lambda kk, qq: mod(qq, kk), K, D // 2, device, Skv=S)
     return cnt.cpu(), n.cpu(), cnt_t.cpu()
 
 
-def blockmap_tables(bm, rows, cols, D: int):
-    """The same tables of one head's block map: the transposed table is the census of the transposed map."""
-    cnt, n = oc.blockmap_census(bm, rows, cols, D // 2)
-    cnt_t, _ = oc.blockmap_census(bm.T, cols, rows, D // 2)
+def blockmap_tables(bm, rows, cols, D: int, *, Skv: int | None = None):
+    """The same tables of one head's block map: the transposed table is the census of the transposed map.  Skv: the
+    column sizes sum to Skv and the row sizes to the query length (None: a square map)."""
+    Sq = None if Skv is None else int(rows.cpu().long().sum())
+    cnt, n = oc.blockmap_census(bm, rows, cols, D // 2, Skv=Skv)
+    cnt_t, _ = oc.blockmap_census(bm.T, cols, rows, D // 2, Skv=Sq)
     return cnt, n, cnt_t
 
 
@@ -319,10 +325,10 @@ class GradCase:
     H: int                       # heads (B * H of the call)
     c: float                     # c = fp32(sm_scale) * fp32(log2 e), an exact power of two
     q: torch.Tensor              # [H, S, D] float32 integers
-    k: torch.Tensor
-    v: torch.Tensor
-    o: torch.Tensor
-    do: torch.Tensor
+    k: torch.Tensor              # [H, Skv, D]
+    v: torch.Tensor              # [H, Skv, D]
+    o: torch.Tensor              # [H, S, D]
+    do: torch.Tensor             # [H, S, D]
     L: torch.Tensor              # [H, S] int, log2 of the lse of every row
     band: tuple | None = None    # (mode, m0, m1, m2)
     mod: object = None
@@ -330,16 +336,21 @@ class GradCase:
     rows: torch.Tensor | None = None
     cols: torch.Tensor | None = None
     notes: dict = field(default_factory=dict)
+    Skv: int | None = None       # keys (None: S)
+
+    @property
+    def Sk(self) -> int:
+        return self.S if self.Skv is None else self.Skv
 
     @property
     def sm_scale(self) -> float:
         return osm.scale_for(self.c)
 
     def mask(self, h: int, device="cpu") -> torch.Tensor:
-        """bool [S, S] element mask of head h."""
+        """bool [S, Skv] element mask of head h."""
         if self.mod is not None:
-            idx = torch.arange(self.S, device=device)
-            return self.mod(idx.view(-1, 1), idx.view(1, -1))
+            return self.mod(torch.arange(self.S, device=device).view(-1, 1),
+                            torch.arange(self.Sk, device=device).view(1, -1))
         from oracle.attention import block_mask_to_element_mask
 
         return block_mask_to_element_mask(self.bm[h], self.rows[h], self.cols[h]).to(device)
@@ -353,25 +364,27 @@ class GradCase:
         return out.to(device)
 
 
-def _grad_inputs(H, S, D, c, gen):
+def _grad_inputs(H, S, D, c, gen, *, Skv: int | None = None):
+    """q, k, v, o, do, L of the gradient census: q, o, do, L over S rows, k, v over Skv (None: S)."""
+    K = S if Skv is None else Skv
     a, b = osm.qk_ints(c)
     e = int(b * c)
     T = 2 // e                          # e t <= 2
     cols = torch.arange(D - 1)
     q = torch.zeros(H, S, D)
-    k = torch.zeros(H, S, D)
+    k = torch.zeros(H, K, D)
     for h in range(H):
         A = cols[(cols % 2) == h % 2]
         B = cols[(cols % 2) != h % 2]
         mag = torch.randint(1, 3, (S, D), generator=gen) * (torch.randint(0, 2, (S, D), generator=gen) * 2 - 1)
         keep = torch.rand(S, D, generator=gen) < 0.25
         q[h][:, A] = (mag * keep)[:, A].float()
-        mag = torch.randint(1, 3, (S, D), generator=gen) * (torch.randint(0, 2, (S, D), generator=gen) * 2 - 1)
-        keep = torch.rand(S, D, generator=gen) < 0.25
+        mag = torch.randint(1, 3, (K, D), generator=gen) * (torch.randint(0, 2, (K, D), generator=gen) * 2 - 1)
+        keep = torch.rand(K, D, generator=gen) < 0.25
         k[h][:, B] = (mag * keep)[:, B].float()
     q[:, :, D - 1] = float(b)
-    k[:, :, D - 1] = torch.randint(0, T + 1, (H, S), generator=gen).float()
-    v = torch.randint(-2, 3, (H, S, D), generator=gen).float()
+    k[:, :, D - 1] = torch.randint(0, T + 1, (H, K), generator=gen).float()
+    v = torch.randint(-2, 3, (H, K, D), generator=gen).float()
     do = torch.zeros(H, S, D)
     o = torch.zeros(H, S, D)
     two = torch.stack([torch.randperm(D, generator=gen)[:2] for _ in range(H * S)]).view(H, S, 2)
@@ -454,11 +467,18 @@ def grad_bsr_case(D=128, seed=3):
     return case
 
 
+def grad_rect_case(name, S, Skv, D=128, H=2, c=1.0, seed=7, **mask):
+    """A gradient-census case of S queries and Skv keys; `mask` holds mod= (a predicate over S x Skv, with band= its
+    plan parameters) or bm=, rows=, cols= (a rectangular block map)."""
+    g = torch.Generator().manual_seed(seed)
+    return GradCase(name, S, D, H, c, *_grad_inputs(H, S, D, c, g, Skv=Skv), Skv=Skv, **mask)
+
+
 MUTANTS = ("lse_next", "delta_next", "delta_64", "dk_no_scale", "dv_scale", "drop_pair")
 
 
 def grad_exact(case: GradCase, h: int, device="cpu", mutant: str | None = None):
-    """Exact fp64 accumulators (acc_q, acc_k, acc_v) [S, D] of head h before the epilogue, their budgets (largest
+    """Exact fp64 accumulators acc_q [S, D], (acc_k, acc_v) [Skv, D] of head h before the epilogue, their budgets (largest
     sum of |terms| over an element, in granules of 1/8) and statistics.  mutant: one of MUTANTS (an oracle restating
     a wrong kernel) or None."""
     dev = torch.device(device)
@@ -490,7 +510,7 @@ def grad_exact(case: GradCase, h: int, device="cpu", mutant: str | None = None):
 
 
 def grad_expected(case: GradCase, h: int, dtype, device="cpu", mutant: str | None = None):
-    """The stored gradients (dq, dk, dv) [S, D] in dtype: round16(fp32(acc) * fp32(sm_scale)) for dQ and dK,
+    """The stored gradients dq [S, D], (dk, dv) [Skv, D] in dtype: round16(fp32(acc) * fp32(sm_scale)) for dQ and dK,
     round16(acc) for dV (RNE at both roundings, as the kernel's fp32 multiply and cvt.rn)."""
     (aq, ak, av), _, _ = grad_exact(case, h, device, mutant)
     s = torch.tensor(case.sm_scale, dtype=torch.float32, device=aq.device)

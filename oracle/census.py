@@ -60,18 +60,20 @@ def _onehot_both(codes0: torch.Tensor, codes1: torch.Tensor, D: int, dtype) -> t
     return e
 
 
-def band_census(mod, S: int, D: int, device, row_chunk: int = 1024):
-    """Census tables of an element mask predicate mod(q_idx [R,1], kv_idx [1,S]) -> bool [R,S].
+def band_census(mod, S: int, D: int, device, row_chunk: int = 1024, *, Skv: int | None = None):
+    """Census tables of an element mask predicate mod(q_idx [R,1], kv_idx [1,Skv]) -> bool [R,Skv] over rows 0..S-1
+    and keys 0..Skv-1 (Skv None: S), the key codes taken over the Skv keys.
     Returns cnt int32 [2, S, D] (both encodings, row order) and n int64 [S] on `device`.
 
     The counts are formed by a 0/1 matmul; every partial sum is an integer no larger than the final count, which
     `column_bound` keeps below 2^11, so fp16 (GPU) or fp32 (CPU) arithmetic is exact."""
     dev = torch.device(device)
+    K = S if Skv is None else Skv
     mm_dtype = torch.float16 if dev.type == "cuda" else torch.float32
     for enc in ENCODINGS:
-        assert column_bound(S, D, enc) < 2048
-    e = _onehot_both(key_codes(S, D, 0, dev), key_codes(S, D, 1, dev), D, mm_dtype)
-    kv = torch.arange(S, device=dev, dtype=torch.int32).view(1, S)
+        assert column_bound(K, D, enc) < 2048
+    e = _onehot_both(key_codes(K, D, 0, dev), key_codes(K, D, 1, dev), D, mm_dtype)
+    kv = torch.arange(K, device=dev, dtype=torch.int32).view(1, K)
     cnt = torch.empty(2, S, D, dtype=torch.int32, device=dev)
     n = torch.empty(S, dtype=torch.int64, device=dev)
     for r0 in range(0, S, row_chunk):
@@ -85,15 +87,17 @@ def band_census(mod, S: int, D: int, device, row_chunk: int = 1024):
 
 
 def blockmap_census(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch.Tensor, D: int,
-                    key_ids: torch.Tensor | None = None):
+                    key_ids: torch.Tensor | None = None, *, Skv: int | None = None):
     """Census tables of a variable-block map (dynamic_block_sparse_fwd semantics, one head) in PLAN row order.
-    block_map [QC, KC], row_sz [QC], col_sz [KC]; key_ids [S] (optional): the key identity (the row of V) read at
+    block_map [QC, KC], row_sz [QC], col_sz [KC]; key_ids [Skv] (optional): the key identity (the row of V) read at
     each plan key position, e.g. the kv_rows gather or the k-cluster argsort.  Runs in fp64 on the CPU.
-    Returns cnt int64 [2, S, D], n int64 [S]."""
+    Skv None: a square map, the row and column sizes both sum to S; otherwise the row sizes sum to Sq and the column
+    sizes to Skv, and the key codes are taken over the Skv keys.
+    Returns cnt int64 [2, Sq, D], n int64 [Sq]."""
     bm = block_map.cpu().to(torch.float64)
     rs, cs = row_sz.cpu().long(), col_sz.cpu().long()
     S = int(cs.sum())
-    assert int(rs.sum()) == S
+    assert int(rs.sum()) == S if Skv is None else S == Skv
     ids = torch.arange(S) if key_ids is None else key_ids.cpu().long()
     e = _onehot_both(key_codes(S, D, 0)[ids], key_codes(S, D, 1)[ids], D, torch.float64)
     kb = torch.repeat_interleave(torch.arange(cs.numel()), cs)
@@ -103,6 +107,12 @@ def blockmap_census(block_map: torch.Tensor, row_sz: torch.Tensor, col_sz: torch
     qb = torch.repeat_interleave(torch.arange(rs.numel()), rs)
     c = cnt_qb[qb]
     return torch.stack([c[:, :D], c[:, D:]]), n_qb[qb]
+
+
+def rect_census(bm: torch.Tensor, rows: torch.Tensor, cols: torch.Tensor, D: int):
+    """blockmap_census of a rectangular map: cnt int64 [2, Sq, D] (keys of each query row with each code, both
+    encodings) and n int64 [Sq] of one head's map [QC, KC], row sizes [QC] (sum Sq), column sizes [KC] (sum Skv)."""
+    return blockmap_census(bm, rows, cols, D, Skv=int(cols.cpu().long().sum()))
 
 
 def scatter_rows(cnt: torch.Tensor, n: torch.Tensor, o_rows: torch.Tensor | None):

@@ -82,15 +82,15 @@ def qk_ints(c: float):
 @dataclass
 class Case:
     name: str
-    S: int
+    S: int                   # plan rows (queries)
     D: int
     H: int
     R: int
     c: list                  # effective c per head (fp32-exact powers of two)
-    kcls: torch.Tensor       # [H, S] key class per plan key position
-    kt: torch.Tensor         # [H, S] key level t per plan key position
+    kcls: torch.Tensor       # [H, Skv] key class per plan key position
+    kt: torch.Tensor         # [H, Skv] key level t per plan key position
     rcls: torch.Tensor       # [H, S] row class per plan row (D - 1, which no key has: a cold-only row)
-    v: torch.Tensor          # [H, S, D] int8, per plan key position
+    v: torch.Tensor          # [H, Skv, D] int8, per plan key position
     vs: list                 # v_scale per head (1.0 for 16-bit inputs)
     band: tuple | None = None            # (mode, m0, m1, m2) of plan_band
     mod: object = None                   # mask predicate of the band plan
@@ -102,11 +102,16 @@ class Case:
     kv_rows: torch.Tensor | None = None  # [H, S] gather: source row of plan key position p
     o_rows: torch.Tensor | None = None   # [H, S] output row of plan row r
     notes: dict = field(default_factory=dict)
+    Skv: int | None = None               # plan key positions (None: S); gather cases are square
+
+    @property
+    def Sk(self) -> int:
+        return self.S if self.Skv is None else self.Skv
 
     def qk_plan(self, dtype=torch.float32):
-        """Q, K [H, S, D] in plan order (integers, exact in every input format)."""
+        """Q [H, S, D] and K [H, Skv, D] in plan order (integers, exact in every input format)."""
         q = torch.zeros(self.H, self.S, self.D)
-        k = torch.zeros(self.H, self.S, self.D)
+        k = torch.zeros(self.H, self.Sk, self.D)
         C = self.D - 1
         for h in range(self.H):
             a, b = qk_ints(self.c[h])
@@ -114,12 +119,13 @@ class Case:
             live = self.rcls[h] < C
             q[h, r[live], self.rcls[h][live].long()] = float(a)
             q[h, :, C] = float(b)
-            k[h, r, self.kcls[h].long()] = 16.0
+            k[h, torch.arange(self.Sk), self.kcls[h].long()] = 16.0
             k[h, :, C] = self.kt[h].float()
         return q.to(dtype), k.to(dtype)
 
     def tensors(self, dtype=torch.float32):
-        """Q, K, V [H, S, D] as the kernel reads them: plan order, or scattered to source rows for gather plans."""
+        """Q [H, S, D], K, V [H, Skv, D] as the kernel reads them: plan order, or scattered to source rows for gather
+        plans."""
         q, k = self.qk_plan(dtype)
         v = self.v.to(dtype)
         if self.gather:
@@ -169,7 +175,7 @@ def _block_runs(bm_row, cols):
 def visit(case: Case, h: int, r: int):
     """(key positions, chunk ids) of plan row r of head h, in the kernel's visit order."""
     if case.mod is not None:
-        pos = torch.nonzero(case.mod(torch.tensor([[r]]), torch.arange(case.S).view(1, -1))[0]).flatten()
+        pos = torch.nonzero(case.mod(torch.tensor([[r]]), torch.arange(case.Sk).view(1, -1))[0]).flatten()
         return pos.numpy(), (pos // CHUNK).numpy()
     qb = int(torch.searchsorted(case.rows[h].long().cumsum(0), torch.tensor(r), right=True))
     runs = _block_runs(case.bm[h, qb], case.cols[h])
@@ -242,14 +248,14 @@ def simulate(case: Case, h: int, r: int, mutant: str | None = None):
 # closed form: per-row tables of (tier, level) sums
 # --------------------------------------------------------------------------------------------
 def _features(case: Case, h: int, device, dtype):
-    """[S, (R+1)(D+1)]: key p contributes [v_p, 1] in the column group of its level t(p)."""
+    """[Skv, (R+1)(D+1)]: key p contributes [v_p, 1] in the column group of its level t(p)."""
     R1, D1 = case.R + 1, case.D + 1
-    f = torch.zeros(case.S, R1, D1, dtype=dtype, device=device)
-    idx = torch.arange(case.S, device=device)
+    f = torch.zeros(case.Sk, R1, D1, dtype=dtype, device=device)
+    idx = torch.arange(case.Sk, device=device)
     t = case.kt[h].long().to(device)
     f[idx, t, : case.D] = case.v[h].to(device=device, dtype=dtype)
     f[idx, t, case.D] = 1
-    return f.view(case.S, R1 * D1)
+    return f.view(case.Sk, R1 * D1)
 
 
 def _reduce(case: Case, h: int, hot, allt):
@@ -297,7 +303,7 @@ def expected(case: Case, h: int, device="cpu", row_chunk: int = 1024, row_ids=No
         R1, D1 = case.R + 1, case.D + 1
         outs = []
         if case.mod is not None:
-            kv = torch.arange(case.S, device=dev).view(1, -1)
+            kv = torch.arange(case.Sk, device=dev).view(1, -1)
             ids = torch.arange(case.S, device=dev) if row_ids is None else torch.as_tensor(row_ids, device=dev)
             for r0 in range(0, ids.numel(), row_chunk):
                 rr = ids[r0:r0 + row_chunk]
@@ -413,9 +419,9 @@ def band_case(name, D=128, H=2, c=None, vs=None, seed=0):
                 rcls.expand(H, S).clone(), int_values(H, S, D, g), list(vs or [1.0] * H), band=band, mod=mod)
 
 
-def _anchor_classes(case: Case, L, C, frac):
+def _anchor_classes(case: Case, L, C, frac, offset=0):
     """Row classes of a block-map case: the class of the region holding the key at `frac` of the row's visit order,
-    so the row meets cold keys first and that region's rising t later."""
+    so the row meets cold keys first and that region's rising t later (regions as region_keys(..., offset))."""
     rcls = torch.full((case.H, case.S), case.D - 1, dtype=torch.long)
     for h in range(case.H):
         ends = case.rows[h].long().cumsum(0)
@@ -425,14 +431,14 @@ def _anchor_classes(case: Case, L, C, frac):
                 continue
             pos, _ = visit(case, h, int(ends[qb]) - n)
             if len(pos):
-                rcls[h, int(ends[qb]) - n: int(ends[qb])] = (int(pos[int(frac * len(pos))]) // L) % C
+                rcls[h, int(ends[qb]) - n: int(ends[qb])] = ((int(pos[int(frac * len(pos))]) + offset) // L) % C
     return with_cold_rows(rcls, case.D)
 
 
-def _finish_blocks(case: Case, L, R, C, frac):
-    kcls, kt = region_keys(case.S, L, C, R)
-    case.kcls, case.kt = kcls.expand(case.H, case.S).clone(), kt.expand(case.H, case.S).clone()
-    case.rcls = _anchor_classes(case, L, C, frac)
+def _finish_blocks(case: Case, L, R, C, frac, offset=0):
+    kcls, kt = region_keys(case.Sk, L, C, R, offset)
+    case.kcls, case.kt = kcls.expand(case.H, case.Sk).clone(), kt.expand(case.H, case.Sk).clone()
+    case.rcls = _anchor_classes(case, L, C, frac, offset)
     return case
 
 
@@ -477,6 +483,47 @@ def gather_case(D=128, c=None, vs=None, seed=2):
     case = Case("gather", S, D, H, 3, list(c or [1.0] * H), z, z, z, int_values(H, S, D, g), list(vs or [1.0] * H),
                 bm=bm, rows=rows, cols=cols, gather=True, q_rows=qperm, kv_rows=kperm, o_rows=qperm)
     return _finish_blocks(case, 2048, 3, 4, 0.5)
+
+
+def rect_blockmap_case(name, bm, rows, cols, D=128, c=None, vs=None, seed=5, L=512, R=3, C=4, frac=0.5, offset=0):
+    """A variable-block case of Sq = sum(rows) queries and Skv = sum(cols) keys: bm [H, QC, KC], rows [H, QC],
+    cols [H, KC].  Key classes and levels over the Skv keys (region_keys with `offset`), every q-block's class from its
+    own visit order (_anchor_classes), so its rows meet cold keys first, are wiped by their first hot chunk and rescale
+    afterwards."""
+    H = bm.shape[0]
+    Sq, Skv = int(rows[0].sum()), int(cols[0].sum())
+    g = torch.Generator().manual_seed(seed)
+    zq, zk = torch.zeros(H, Sq, dtype=torch.long), torch.zeros(H, Skv, dtype=torch.long)
+    case = Case(name, Sq, D, H, R, list(c or [1.0] * H), zk, zk, zq, int_values(H, Skv, D, g), list(vs or [1.0] * H),
+                bm=bm, rows=rows.int(), cols=cols.int(), Skv=Skv)
+    return _finish_blocks(case, L, R, C, frac, offset)
+
+
+def row_anchor_classes(mod, S, Skv, L, C, D, frac=0.5, device="cpu", row_chunk=512):
+    """Row classes [S] of a mask-predicate case over S x Skv: the class of the region holding the key at `frac` of each
+    row's own visit order (ascending keys), as _anchor_classes takes it per q-block; D - 1 for rows without keys."""
+    dev = torch.device(device)
+    rcls = torch.full((S,), D - 1, dtype=torch.long)
+    kv = torch.arange(Skv, device=dev).view(1, -1)
+    for r0 in range(0, S, row_chunk):
+        r1 = min(S, r0 + row_chunk)
+        m = mod(torch.arange(r0, r1, device=dev).view(-1, 1), kv)
+        n = m.sum(1)
+        idx = torch.floor(frac * n.double()).long()
+        pos = (m.long().cumsum(1) <= idx[:, None]).sum(1)  # the idx-th allowed key (0-based) of every row
+        rcls[r0:r1] = torch.where(n > 0, (pos // L) % C, torch.full_like(pos, D - 1)).cpu()
+    return rcls
+
+
+def mask_case(name, mod, S, Skv, D=128, H=2, L=384, R=3, C=8, c=None, vs=None, seed=6, frac=0.5, device="cpu"):
+    """A case of any mask predicate mod(q_idx, kv_idx) over S queries and Skv keys, in the visit order of band and
+    segment plans (128-key chunks in ascending key order): key regions of L keys over the Skv keys, each row's class
+    from its own visit order (row_anchor_classes), every 13th row cold-only."""
+    g = torch.Generator().manual_seed(seed)
+    kcls, kt = region_keys(Skv, L, C, R)
+    rcls = with_cold_rows(row_anchor_classes(mod, S, Skv, L, C, D, frac, device), D)
+    return Case(name, S, D, H, R, list(c or [1.0] * H), kcls.expand(H, Skv).clone(), kt.expand(H, Skv).clone(),
+                rcls.expand(H, S).clone(), int_values(H, Skv, D, g), list(vs or [1.0] * H), mod=mod, Skv=Skv)
 
 
 def bsr_case(D=128, seed=3):
@@ -546,7 +593,7 @@ def coverage(case: Case, stride: int = 1):
     see a wipe and then at least two partial rescales, cold-only rows with keys, rows without keys, and rows of a
     second 128-row stream (band plans: rows 128..255 of each 256-row item) with keys.  Also checks that the
     chunk-loop simulation reproduces the closed form on every visited row."""
-    st = dict(rows=0, keyed=0, covered=0, cold_only=0, keyless=0, stream1=0)
+    st = dict(rows=0, keyed=0, covered=0, wipes=0, cold_only=0, keyless=0, stream1=0)
     rows = list(range(0, case.S, stride))
     for h in range(case.H):
         if case.mod is not None:
@@ -563,6 +610,7 @@ def coverage(case: Case, stride: int = 1):
                 continue
             st["keyed"] += 1
             st["covered"] += int(s["wipe"] > 0 and s["partial"] >= 2)
+            st["wipes"] += int(s["wipe"] > 0)
             st["cold_only"] += int(int(case.rcls[h, r]) == case.D - 1)
             st["stream1"] += int(case.mod is not None and r % 256 >= 128)
     return st

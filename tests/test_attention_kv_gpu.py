@@ -16,24 +16,11 @@ import torch
 
 from oracle import bwd_census as obc
 from oracle import census as oc
+from oracle.census import rect_census
 
 pytestmark = pytest.mark.gpu
 
 TOL = {torch.bfloat16: 4e-2, torch.float16: 1e-2}
-
-
-def rect_census(bm, rows, cols, Dh):
-    """oracle.census.blockmap_census without its Sq == Skv premise: cnt int64 [2, Sq, Dh] (keys of each query row with
-    each code, both encodings) and n int64 [Sq] of one head's map [QC, KC], row sizes [QC], column sizes [KC]."""
-    rs, cs = rows.cpu().long(), cols.cpu().long()
-    Skv = int(cs.sum())
-    e = oc._onehot_both(oc.key_codes(Skv, Dh, 0), oc.key_codes(Skv, Dh, 1), Dh, torch.float64)
-    per_block = torch.zeros(cs.numel(), 2 * Dh, dtype=torch.float64).index_add_(
-        0, torch.repeat_interleave(torch.arange(cs.numel()), cs), e)
-    b = bm.cpu().double()
-    qb = torch.repeat_interleave(torch.arange(rs.numel()), rs)
-    c = (b @ per_block).round().long()[qb]
-    return torch.stack([c[:, :Dh], c[:, Dh:]]), (b @ cs.double()).round().long()[qb]
 
 
 def sizes(total, n, gen, zeros=()):
