@@ -375,98 +375,61 @@ def kvcache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k: torch.Tensor
     cu_seqlens (device int [B + 1], FlashAttention 3's cu_seqlens_k_new): variable-length appends, k, v packed as
     [total_new, Hkv, D] with stream b's rows at [cu_seqlens[b], cu_seqlens[b+1]), written at keys cache_seqlens[b] ..
     under the same rules, in every cache format and one launch (svgb_kvcache_append_varlen)."""
-    if cu_seqlens is not None:
-        return _kvcache_append_varlen(k_cache, v_cache, k, v, cache_seqlens, block_table, cache_batch_idx, k_scale,
-                                      v_scale, cu_seqlens)
+    who = "kvcache_append"
+    packed = cu_seqlens is not None
     _need_cuda(k_cache, v_cache, k, v)
-    if k_cache.dim() != 4 or k.dim() != 4 or k_cache.shape != v_cache.shape or k.shape != v.shape:
-        raise SvgbError(f"kvcache_append: k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] and "
-                        f"k, v {tuple(k.shape)} [B, Snew, Hkv, D], each pair of one shape")
-    if k.shape[2:] != k_cache.shape[2:]:
-        raise SvgbError(f"kvcache_append: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
-    fp8 = k_cache.dtype == torch.float8_e4m3fn
-    rows = None
-    if fp8:
-        if v_cache.dtype != k_cache.dtype or k.dtype != v.dtype:
-            raise SvgbError("kvcache_append: an e4m3 k_cache needs an e4m3 v_cache, and k, v of one 16-bit dtype")
-        rows = _row_scales("kvcache_append", k_scale, v_scale, k_cache)
-        scales = rows or _fp8_scales("kvcache_append", k_scale, v_scale, k.shape[2])
+    if k_cache.dim() != 4 or k.dim() != (3 if packed else 4) or k_cache.shape != v_cache.shape or k.shape != v.shape:
+        raise SvgbError(f"{who}: {'with cu_seqlens, ' if packed else ''}k_cache, v_cache {tuple(k_cache.shape)} must "
+                        f"be [blocks, rows, Hkv, D] and k, v {tuple(k.shape)} "
+                        f"{'[total_new, Hkv, D]' if packed else '[B, Snew, Hkv, D]'}, each pair of one shape")
+    if k.shape[-2:] != k_cache.shape[2:]:
+        raise SvgbError(f"{who}: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
+    if packed:
+        cu = _cu_seqlens(who, "cu_seqlens", cu_seqlens, None, k.device)
+        B = cu.numel() - 1
     else:
-        if k_scale is not None or v_scale is not None:
-            raise SvgbError("kvcache_append: k_scale / v_scale are for float8_e4m3fn caches; a "
-                            f"{k_cache.dtype} cache takes none")
-        if not (k_cache.dtype == v_cache.dtype == k.dtype == v.dtype):
-            raise SvgbError("kvcache_append: the caches and the new rows must share one dtype")
+        B = k.shape[0]
+    scales, per_row = _cache_format(who, k_cache, v_cache, k_scale, v_scale)
+    if k.dtype != v.dtype or (scales is None and k.dtype != k_cache.dtype):
+        raise SvgbError(f"{who}: the new rows k, v must share one dtype, and with a 16-bit cache the cache's")
     dt = _dt(k)
-    B, Snew, Hkv, D = k.shape
-    if Snew == 0:
+    N, Hkv, D = k.shape[-3:]  # new rows per stream, or packed rows
+    if N == 0:
         return
     for c in (k_cache, v_cache):
         if not _addressable(c.transpose(1, 2), "bhsd"):
-            raise SvgbError("kvcache_append: the cache is written in place, so it must be 16-byte aligned with a last "
+            raise SvgbError(f"{who}: the cache is written in place, so it must be 16-byte aligned with a last "
                             "stride of 1 and other strides that are nonzero multiples of 8 elements")
-    k, v = (_addressed(t.transpose(1, 2), "bhsd") for t in (k, v))
+    layout = "shd" if packed else "bhsd"
+    k, v = (_addressed(t if packed else t.transpose(1, 2), layout) for t in (k, v))
     bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
     lens = _seqlens(cache_seqlens, B, k.device)
-    fill = 16 if fp8 else 8  # e4m3 cache strides are multiples of 16 bytes
-    args = (k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(), lens.data_ptr(), _p(bi), _p(bt), dt, B,
-            Snew, Hkv, D, k_cache.shape[0], k_cache.shape[1], max_pages, _st(k_cache.transpose(1, 2), "bhsd", fill),
-            _st(v_cache.transpose(1, 2), "bhsd", fill), _st(k, "bhsd"), _st(v, "bhsd"))
-    if fp8 and rows:
-        check(lib().svgb_kvcache_append_e4m3_rows(*args, *(t.data_ptr() for t in scales), _stream(k)),
-              "svgb_kvcache_append_e4m3_rows")
-    elif fp8:
-        check(lib().svgb_kvcache_append_e4m3(*args, *(t.data_ptr() for t in scales), _stream(k)),
-              "svgb_kvcache_append_e4m3")
+    fill = 8 if scales is None else 16  # e4m3 cache strides are multiples of 16 bytes
+    sc = tuple(t.data_ptr() for t in scales or ())
+    if packed:  # one entry for every format: the scales (or none) and which format they are
+        name, bounds, sc = "svgb_kvcache_append_varlen", (cu.data_ptr(),), (sc or (None, None)) + (int(per_row),)
     else:
-        check(lib().svgb_kvcache_append(*args, _stream(k)), "svgb_kvcache_append")
+        name, bounds = "svgb_kvcache_append" + ("" if scales is None else "_e4m3_rows" if per_row else "_e4m3"), ()
+    check(getattr(lib(), name)(k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(), *bounds,
+                               lens.data_ptr(), _p(bi), _p(bt), dt, B, N, Hkv, D, k_cache.shape[0], k_cache.shape[1],
+                               max_pages, _st(k_cache.transpose(1, 2), "bhsd", fill),
+                               _st(v_cache.transpose(1, 2), "bhsd", fill), _st(k, layout), _st(v, layout), *sc,
+                               _stream(k)), name)
     _bump()
 
 
-def _kvcache_append_varlen(k_cache, v_cache, k, v, cache_seqlens, block_table, cache_batch_idx, k_scale, v_scale,
-                           cu_seqlens):
-    """kvcache_append(cu_seqlens=): packed k, v [total_new, Hkv, D], svgb_kvcache_append_varlen."""
-    who = "kvcache_append"
-    _need_cuda(k_cache, v_cache, k, v)
-    if k_cache.dim() != 4 or k.dim() != 3 or k_cache.shape != v_cache.shape or k.shape != v.shape:
-        raise SvgbError(f"{who}: with cu_seqlens, k_cache, v_cache {tuple(k_cache.shape)} must be [blocks, rows, Hkv, D] "
-                        f"and k, v {tuple(k.shape)} [total_new, Hkv, D], each pair of one shape")
-    if k.shape[1:] != k_cache.shape[2:]:
-        raise SvgbError(f"{who}: k {tuple(k.shape)} and k_cache {tuple(k_cache.shape)} differ in heads or D")
-    cu = _cu_seqlens(who, "cu_seqlens", cu_seqlens, None, k.device)
-    B = cu.numel() - 1
-    fp8 = k_cache.dtype == torch.float8_e4m3fn
-    rows = scales = None
-    if fp8:
-        if v_cache.dtype != k_cache.dtype or k.dtype != v.dtype:
-            raise SvgbError(f"{who}: an e4m3 k_cache needs an e4m3 v_cache, and k, v of one 16-bit dtype")
-        rows = _row_scales(who, k_scale, v_scale, k_cache)
-        scales = rows or _fp8_scales(who, k_scale, v_scale, k.shape[1])
-    else:
+def _cache_format(who, k_cache, v_cache, k_scale, v_scale):
+    """(scales, per_row) of a KV cache [num_blocks, block_rows, Hkv, D]: (None, False) for a 16-bit cache, which takes
+    no scales; for a float8_e4m3fn cache its (k_scale, v_scale), per cache row when either is 3-D (_row_scales, per_row
+    True), else per key/value head (_fp8_scales)."""
+    if v_cache.dtype != k_cache.dtype:
+        raise SvgbError(f"{who}: k_cache ({k_cache.dtype}) and v_cache ({v_cache.dtype}) must share one dtype")
+    if k_cache.dtype != torch.float8_e4m3fn:
         if k_scale is not None or v_scale is not None:
             raise SvgbError(f"{who}: k_scale / v_scale are for float8_e4m3fn caches; a {k_cache.dtype} cache takes none")
-        if not (k_cache.dtype == v_cache.dtype == k.dtype == v.dtype):
-            raise SvgbError(f"{who}: the caches and the new rows must share one dtype")
-    dt = _dt(k)
-    T, Hkv, D = k.shape
-    if T == 0:
-        return
-    for c in (k_cache, v_cache):
-        if not _addressable(c.transpose(1, 2), "bhsd"):
-            raise SvgbError(f"{who}: the cache is written in place, so it must be 16-byte aligned with a last stride of 1 "
-                            "and other strides that are nonzero multiples of 8 elements")
-    k, v = (_addressed(t, "shd") for t in (k, v))
-    bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
-    lens = _seqlens(cache_seqlens, B, k.device)
-    fill = 16 if fp8 else 8
-    check(lib().svgb_kvcache_append_varlen(k_cache.data_ptr(), v_cache.data_ptr(), k.data_ptr(), v.data_ptr(),
-                                           cu.data_ptr(), lens.data_ptr(), _p(bi), _p(bt), dt, B, T, Hkv, D,
-                                           k_cache.shape[0], k_cache.shape[1], max_pages,
-                                           _st(k_cache.transpose(1, 2), "bhsd", fill),
-                                           _st(v_cache.transpose(1, 2), "bhsd", fill), _st(k, "shd"), _st(v, "shd"),
-                                           *((None, None) if scales is None else (t.data_ptr() for t in scales)),
-                                           1 if rows else 0, _stream(k)), "svgb_kvcache_append_varlen")
-    _bump()
+        return None, False
+    rows = _row_scales(who, k_scale, v_scale, k_cache)
+    return rows or _fp8_scales(who, k_scale, v_scale, k_cache.shape[2]), rows is not None
 
 
 def _fp8_scales(who, k_scale, v_scale, Hkv):
@@ -537,67 +500,107 @@ def plan_kvcache(cache_seqlens, *, q_len: Optional[int] = None, num_blocks: int,
     cu_seqlens=)) in place of new_len.  Every mask rule, num_splits and block= work as above, with one (block,
     first_block) for the batch; Lq_b = 0 is legal.  attn_fwd then takes q [total_q, Hq, D] and returns o [total_q, Hq,
     D] and lse [Hq, total_q].  Nothing is read on the host (svgb_attn_plan_kvcache_varlen)."""
+    who = "plan_kvcache"
     if (q_len is None) == (cu_seqlens_q is None):
-        raise SvgbError("plan_kvcache: pass q_len (B streams of q_len queries) or cu_seqlens_q (variable-length "
-                        "queries), exactly one of them")
+        raise SvgbError(f"{who}: pass q_len (B streams of q_len queries) or cu_seqlens_q (variable-length queries), "
+                        "exactly one of them")
     if cu_seqlens_new is not None and cu_seqlens_q is None:
-        raise SvgbError("plan_kvcache: cu_seqlens_new (variable-length appends) goes with cu_seqlens_q; uniform plans "
-                        "take new_len")
-    blk = _kvcache_block_args(causal, window_size, sink, block, first_block) if block else None
-    if cu_seqlens_q is not None:
-        return _plan_kvcache_varlen(cache_seqlens, cu_seqlens_q, total_q, max_seqlen_q, cu_seqlens_new, new_len,
-                                    num_blocks, cache_len, block_table, page_size, cache_batch_idx, causal,
-                                    window_size, sink, num_splits, num_heads, blk)
+        raise SvgbError(f"{who}: cu_seqlens_new (variable-length appends) goes with cu_seqlens_q; uniform plans take "
+                        "new_len")
+    # geometry: rows per cache block and a stream's capacity, the streams B, the device, and the longest query run Qmax
+    # of a stream
     if block_table is not None:
-        B = block_table.shape[0]
         if page_size is None:
-            raise SvgbError("plan_kvcache: a paged cache (block_table) needs page_size")
+            raise SvgbError(f"{who}: a paged cache (block_table) needs page_size")
         rows = int(page_size)
         cap = block_table.shape[1] * rows
     else:
         if cache_len is None:
-            raise SvgbError("plan_kvcache: a contiguous cache needs cache_len (its rows per stream, k_cache.shape[1])")
-        B = cache_seqlens.numel() if isinstance(cache_seqlens, torch.Tensor) else None
-        if B is None:
-            if cache_batch_idx is None:
-                raise SvgbError("plan_kvcache: with an int cache_seqlens pass a tensor or cache_batch_idx for B")
-            B = cache_batch_idx.numel()
+            raise SvgbError(f"{who}: a contiguous cache needs cache_len (its rows per stream, k_cache.shape[1])")
         rows = cap = int(cache_len)
-    device = (cache_seqlens if isinstance(cache_seqlens, torch.Tensor) else
-              block_table if block_table is not None else cache_batch_idx).device
+    cu_q = cu_new = None
+    if cu_seqlens_q is not None:
+        if total_q is None:
+            raise SvgbError(f"{who}: cu_seqlens_q needs total_q (q.shape[0], the packed query rows), which is passed "
+                            "rather than read from the device")
+        if cu_seqlens_new is not None and int(new_len):
+            raise SvgbError(f"{who}: cu_seqlens_new and new_len={new_len} both give the appended rows; pass one")
+        cu_q = _cu_seqlens(who, "cu_seqlens_q", cu_seqlens_q, None, None)
+        B, device = cu_q.numel() - 1, cu_q.device
+        Sq = int(total_q)  # the plan runs as one block of total_q packed rows
+        if Sq < 1:
+            raise SvgbError(f"{who}: total_q={Sq} must be >= 1")
+        Qmax = Sq if max_seqlen_q is None else int(max_seqlen_q)
+        if not 1 <= Qmax <= Sq:
+            raise SvgbError(f"{who}: max_seqlen_q={Qmax} must lie in [1, total_q={Sq}]")
+        if cu_seqlens_new is not None:
+            cu_new = _cu_seqlens(who, "cu_seqlens_new", cu_seqlens_new, B, device)
+    else:
+        Sq = Qmax = int(q_len)
+        if block_table is not None:
+            B = block_table.shape[0]
+        elif isinstance(cache_seqlens, torch.Tensor):
+            B = cache_seqlens.numel()
+        elif cache_batch_idx is not None:
+            B = cache_batch_idx.numel()
+        else:
+            raise SvgbError(f"{who}: with an int cache_seqlens pass a tensor or cache_batch_idx for B")
+        device = (cache_seqlens if isinstance(cache_seqlens, torch.Tensor) else
+                  block_table if block_table is not None else cache_batch_idx).device
+    # mask: a local band (left, right), or block-causal (W, C, F) whose chunk slots are bounded as the band
+    # (left = W - 1, right = C - 1, svgb_attn_plan_kvcache_block); -1 is unbounded, no query position lying further than
+    # cap + Qmax from a key, nor a query's block end further than cap + Qmax + C from key 0
+    sink = int(sink)
+    if block:
+        if causal:
+            raise SvgbError(f"{who}: causal=True is redundant with block= (the block rule is causal); pass "
+                            "window_size=(W, -1)")
+        W, right = (int(w) for w in window_size)
+        if right != -1:
+            raise SvgbError(f"{who}: with block=, window_size[1] = {right} must be -1 (no key past the block end)")
+        m1, W = _block_m1(who, block, first_block, W, sink)
+        C_, F = m1 & 0xffff, (m1 & 0xffff) - (m1 >> 16)
+        if W == -1:
+            W = min(cap + Qmax + C_, 2**31 - 1)
+        left, right = W - 1, C_ - 1
+    else:
+        left, right = (int(w) for w in window_size)
+        if causal:
+            if right > 0:
+                raise SvgbError(f"{who}: causal=True looks no key ahead, but window_size[1] = {right}")
+            right = 0
+        left, right = (min(cap + Qmax, 2**31 - 1) if w == -1 else w for w in (left, right))
+    # the items of the single pass: B ceil(Sq / 256), or for packed queries the bound I of
+    # svgb_attn_plan_kvcache_varlen_bytes
+    items = B * -(-Sq // 256) if cu_q is None else min(B * -(-Qmax // 256), (Sq + 255 * B) // 256)
+    n = _num_splits(num_splits, num_heads, items, cap, sink, left, right)
     bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
     lens = _seqlens(cache_seqlens, B, device)
-    Sq = int(q_len)
-    if blk:
-        return _plan_kvcache_block(lens, bi, bt, B, Sq, int(new_len), int(num_blocks), rows, max_pages, cap, device,
-                                   sink, num_splits, num_heads, *blk)
-    left, right = (int(w) for w in window_size)
-    if causal:
-        if right > 0:
-            raise SvgbError(f"plan_kvcache: causal=True looks no key ahead, but window_size[1] = {right}")
-        right = 0
-    # -1: no query position lies further than cap + Sq from a key
-    left, right = (min(cap + Sq, 2**31 - 1) if w == -1 else w for w in (left, right))
-    n = _num_splits(num_splits, num_heads, B, Sq, cap, sink, left, right)
-    nbytes = C.c_size_t()
-    desc = Plan()
-    stream = torch.cuda.current_stream(device).cuda_stream
-    if n == 1:
-        check(lib().svgb_attn_plan_kvcache_bytes(B, Sq, cap, int(sink), left, right, C.byref(nbytes)),
-              "svgb_attn_plan_kvcache_bytes")
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the lengths
-        check(lib().svgb_attn_plan_kvcache(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks), rows,
-                                           max_pages, int(sink), left, right, ws.data_ptr(), ws.numel(), C.byref(desc),
-                                           stream), "svgb_attn_plan_kvcache")
+    if cu_q is not None and lens.device != device:
+        raise SvgbError(f"{who}: cache_seqlens is on {lens.device}, cu_seqlens_q on {device}")
+    # the planner pair: the _bytes query takes (sizes, cap, sink, mask), the planner (bounds, sizes, [Snew,] cache
+    # geometry, sink, mask), the mask ending in n on every entry but the single local one
+    if cu_q is not None:
+        name, bounds, sizes, new = "svgb_attn_plan_kvcache_varlen", (cu_q, lens, cu_new), (B, Sq, Qmax), ()
+        mask = (0, 0, W, C_, F, n) if block else (left, right, 0, 0, 0, n)
     else:
-        check(lib().svgb_attn_plan_kvcache_split_bytes(B, Sq, cap, int(sink), left, right, n, C.byref(nbytes)),
-              "svgb_attn_plan_kvcache_split_bytes")
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
-        check(lib().svgb_attn_plan_kvcache_split(lens.data_ptr(), _p(bi), _p(bt), B, Sq, int(new_len), int(num_blocks),
-                                                 rows, max_pages, int(sink), left, right, n, ws.data_ptr(), ws.numel(),
-                                                 C.byref(desc), stream), "svgb_attn_plan_kvcache_split")
+        bounds, sizes, new = (lens,), (B, Sq), (int(new_len),)
+        if block:
+            name, mask = "svgb_attn_plan_kvcache_block", (W, C_, F, n)
+        elif n == 1:
+            name, mask = "svgb_attn_plan_kvcache", (left, right)
+        else:
+            name, mask = "svgb_attn_plan_kvcache_split", (left, right, n)
+    nbytes = C.c_size_t()
+    check(getattr(lib(), name + "_bytes")(*sizes, cap, sink, *mask, C.byref(nbytes)), name + "_bytes")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)  # owned by the plan, with its copy of the lengths
+    desc = Plan()
+    check(getattr(lib(), name)(*(_p(t) for t in bounds), _p(bi), _p(bt), *sizes, *new, int(num_blocks), rows,
+                               max_pages, sink, *mask, ws.data_ptr(), ws.numel(), C.byref(desc),
+                               torch.cuda.current_stream(device).cuda_stream), name)
     _bump()
-    return AttnPlan(desc, ws, (B, Sq))
+    # attn_fwd runs a variable-length plan as one block of total_q packed rows
+    return AttnPlan(desc, ws, (B, Sq) if cu_q is None else (1, Sq))
 
 
 def _cu_seqlens(who, name, cu, B, device) -> torch.Tensor:
@@ -615,70 +618,8 @@ def _cu_seqlens(who, name, cu, B, device) -> torch.Tensor:
     return cu.to(torch.int32).contiguous()
 
 
-def _plan_kvcache_varlen(cache_seqlens, cu_seqlens_q, total_q, max_seqlen_q, cu_seqlens_new, new_len, num_blocks,
-                         cache_len, block_table, page_size, cache_batch_idx, causal, window_size, sink, num_splits,
-                         num_heads, blk):
-    """plan_kvcache(cu_seqlens_q=): svgb_attn_plan_kvcache_varlen, single (n = 1) or split, every argument checked
-    before the one launch."""
-    who = "plan_kvcache"
-    if total_q is None:
-        raise SvgbError(f"{who}: cu_seqlens_q needs total_q (q.shape[0], the packed query rows), which is passed rather "
-                        "than read from the device")
-    if cu_seqlens_new is not None and int(new_len):
-        raise SvgbError(f"{who}: cu_seqlens_new and new_len={new_len} both give the appended rows; pass one")
-    cu_q = _cu_seqlens(who, "cu_seqlens_q", cu_seqlens_q, None, None)
-    B = cu_q.numel() - 1
-    Tq = int(total_q)
-    if Tq < 1:
-        raise SvgbError(f"{who}: total_q={Tq} must be >= 1")
-    max_q = Tq if max_seqlen_q is None else int(max_seqlen_q)
-    if not 1 <= max_q <= Tq:
-        raise SvgbError(f"{who}: max_seqlen_q={max_q} must lie in [1, total_q={Tq}]")
-    cu_new = None if cu_seqlens_new is None else _cu_seqlens(who, "cu_seqlens_new", cu_seqlens_new, B, cu_q.device)
-    if block_table is not None:
-        if page_size is None:
-            raise SvgbError(f"{who}: a paged cache (block_table) needs page_size")
-        rows = int(page_size)
-        cap = block_table.shape[1] * rows
-    else:
-        if cache_len is None:
-            raise SvgbError(f"{who}: a contiguous cache needs cache_len (its rows per stream, k_cache.shape[1])")
-        rows = cap = int(cache_len)
-    bt, bi, max_pages = _cache_layout(B, block_table, cache_batch_idx)
-    lens = _seqlens(cache_seqlens, B, cu_q.device)
-    if lens.device != cu_q.device:
-        raise SvgbError(f"{who}: cache_seqlens is on {lens.device}, cu_seqlens_q on {cu_q.device}")
-    if blk:
-        C_, F, W = blk
-        if W == -1:  # no query's block end lies further than cap + max_q + C from key 0
-            W = min(cap + max_q + C_, 2**31 - 1)
-        left, right, mask = W - 1, C_ - 1, (0, 0, W, C_, F)  # slot bound: left = W - 1, right = C - 1
-    else:
-        left, right = (int(w) for w in window_size)
-        if causal:
-            if right > 0:
-                raise SvgbError(f"{who}: causal=True looks no key ahead, but window_size[1] = {right}")
-            right = 0
-        # -1: no query position lies further than cap + max_q from a key
-        left, right = (min(cap + max_q, 2**31 - 1) if w == -1 else w for w in (left, right))
-        mask = (left, right, 0, 0, 0)
-    items = min(B * -(-max_q // 256), (Tq + 255 * B) // 256)  # the item bound I (svgb_attn_plan_kvcache_varlen_bytes)
-    n = _num_splits(num_splits, num_heads, items, 256, cap, sink, left, right)
-    nbytes = C.c_size_t()
-    check(lib().svgb_attn_plan_kvcache_varlen_bytes(B, Tq, max_q, cap, int(sink), *mask, n, C.byref(nbytes)),
-          "svgb_attn_plan_kvcache_varlen_bytes")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=cu_q.device)  # owned by the plan, with its header
-    desc = Plan()
-    check(lib().svgb_attn_plan_kvcache_varlen(cu_q.data_ptr(), lens.data_ptr(), _p(cu_new), _p(bi), _p(bt), B, Tq, max_q,
-                                              int(num_blocks), rows, max_pages, int(sink), *mask, n, ws.data_ptr(),
-                                              ws.numel(), C.byref(desc), torch.cuda.current_stream(cu_q.device).cuda_stream),
-          "svgb_attn_plan_kvcache_varlen")
-    _bump()
-    # attn_fwd runs the plan as one block of total_q packed rows
-    return AttnPlan(desc, ws, (1, Tq))
-
-
-def _num_splits(num_splits, num_heads, B, Sq, cap, sink, left, right):
+def _num_splits(num_splits, num_heads, items, cap, sink, left, right):
+    """The split count n of a plan whose single pass has `items` 256-query items per head (num_splits=0: automatic)."""
     n = int(num_splits)
     if n < 0:
         raise SvgbError(f"plan_kvcache: num_splits={n} must be >= 0 (0: automatic, 1: no split)")
@@ -686,41 +627,8 @@ def _num_splits(num_splits, num_heads, B, Sq, cap, sink, left, right):
         if num_heads is None:
             raise SvgbError("plan_kvcache: num_splits=0 picks the split count from the grid, so it needs num_heads (q's "
                             "query heads)")
-        n = kvcache_num_splits(B * -(-Sq // 256) * int(num_heads), _kvcache_slots(cap, int(sink), left, right),
-                               _sm_count())
+        n = kvcache_num_splits(items * int(num_heads), _kvcache_slots(cap, sink, left, right), _sm_count())
     return n
-
-
-def _kvcache_block_args(causal, window_size, sink, block, first_block):
-    """(block C, first_block F, window W or -1) of plan_kvcache(block=), checked before any device work."""
-    if causal:
-        raise SvgbError("plan_kvcache: causal=True is redundant with block= (the block rule is causal); pass "
-                        "window_size=(W, -1)")
-    W, right = (int(w) for w in window_size)
-    if right != -1:
-        raise SvgbError(f"plan_kvcache: with block=, window_size[1] = {right} must be -1 (no key past the block end)")
-    m1, W = _block_m1("plan_kvcache", block, first_block, W, sink)
-    return m1 & 0xffff, (m1 & 0xffff) - (m1 >> 16), W
-
-
-def _plan_kvcache_block(lens, bi, bt, B, Sq, new_len, num_blocks, rows, max_pages, cap, device, sink, num_splits,
-                        num_heads, C_, F, W):
-    """plan_kvcache(block=): svgb_attn_plan_kvcache_block, single (n = 1) or split."""
-    if W == -1:  # no query's block end lies further than cap + Sq + C from key 0
-        W = min(cap + Sq + C_, 2**31 - 1)
-    # the slot bound of a block plan: left = W - 1, right = C - 1 (svgb_attn_plan_kvcache_block)
-    n = _num_splits(num_splits, num_heads, B, Sq, cap, sink, W - 1, C_ - 1)
-    nbytes = C.c_size_t()
-    check(lib().svgb_attn_plan_kvcache_block_bytes(B, Sq, cap, int(sink), W, C_, F, n, C.byref(nbytes)),
-          "svgb_attn_plan_kvcache_block_bytes")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
-    desc = Plan()
-    check(lib().svgb_attn_plan_kvcache_block(lens.data_ptr(), _p(bi), _p(bt), B, Sq, new_len, num_blocks, rows,
-                                             max_pages, int(sink), W, C_, F, n, ws.data_ptr(), ws.numel(),
-                                             C.byref(desc), torch.cuda.current_stream(device).cuda_stream),
-          "svgb_attn_plan_kvcache_block")
-    _bump()
-    return AttnPlan(desc, ws, (B, Sq))
 
 
 # The automatic split count of plan_kvcache(num_splits=0), from tools/kvcache_perf.py on the H100 (DESIGN.md): split only
@@ -838,7 +746,7 @@ def _attn(q, k, v, o, plan, layout, dtype, scales, rows, return_lse, sm_scale):
         _gqa_check(dtype, plan, rows)
     lse = torch.empty(BH, Sq, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    if plan.desc.kind == PLAN_KVCACHE or not all(t.is_contiguous() for t in (q, k, v, o)):
+    if not all(t.is_contiguous() for t in (q, k, v, o)):
         B = q.shape[0] if layout == "bhsd" else 1
         check(lib().svgb_attn_fwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _p(lse), dtype, B,
                                           q.shape[1], k.shape[1], Sq, Skv, D, *(_st(t, layout) for t in (q, k, v, o)),
@@ -897,8 +805,6 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
     if plan.desc.kind in (PLAN_KVCACHE, PLAN_KVCACHE_SPLIT):
         if any(r is not None for r in (q_rows, kv_rows, o_rows)):
             raise SvgbError("a KV-cache plan (plan_kvcache) takes no row vectors (o_rows / q_rows / kv_rows)")
-        if plan.desc.varlen_items:
-            return _attn_kvcache_varlen(q, k, v, plan, return_lse, sm_scale, out, k_scale, v_scale)
         return _attn_kvcache(q, k, v, plan, return_lse, sm_scale, out, k_scale, v_scale)
     if k_scale is not None or v_scale is not None:
         raise SvgbError("k_scale / v_scale are for float8_e4m3fn caches under a KV-cache plan (plan_kvcache); other "
@@ -927,157 +833,104 @@ def attn_fwd(q, k, v, plan: AttnPlan, *, layout: str = "bhsd", o_rows: Optional[
 
 
 def _attn_kvcache(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale=None, v_scale=None):
-    """attn_fwd under a KV-cache plan: q [B, Sq, Hq, D] as B * Sq packed rows, the cache [blocks, rows, Hkv, D] as
-    blocks * rows rows (both views), o [B, Sq, Hq, D] and lse [B, Hq, Sq] (flash_attn_with_kvcache's shapes).
-    float8_e4m3fn caches (FP8 KV cache) take bf16 q, D = 128 and k_scale, v_scale float32 [Hkv]: q is quantised per
-    query head over the call's B * Sq rows (quantize_e4m3 on a transposed [Hq, B * Sq, D] copy) and o is bf16.  With
-    per-row scales [num_blocks, Hkv, block_rows] each q row is quantised on its own (_attn_kvcache_fp8_rows)."""
-    B, Sq = plan.source
-    if q.dim() != 4 or q.shape[:2] != (B, Sq) or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
-        raise SvgbError(f"a KV-cache plan for B={B} streams of Sq={Sq} queries takes q [B, Sq, Hq, D] (got "
-                        f"{tuple(q.shape)}) and k_cache, v_cache [blocks, rows, Hkv, D] of one shape (got "
-                        f"{tuple(k_cache.shape)}, {tuple(v_cache.shape)})")
-    if k_cache.shape[0] * k_cache.shape[1] != plan.S_kv:
+    """attn_fwd under a KV-cache plan: q [B, Sq, Hq, D] (variable-length plans: [total_q, Hq, D]) as R = B * Sq
+    (total_q) packed rows, the cache [blocks, rows, Hkv, D] as blocks * rows rows (both views); returns o of q's shape
+    (out itself when given) and lse [B, Hq, Sq] ([Hq, total_q]), flash_attn_with_kvcache's shapes.  A split plan runs as
+    two launches, the attention into fp32 partials in a cached workspace and their merge into o.
+    float8_e4m3fn caches (FP8 KV cache) take bf16 q, D = 128 and k_scale, v_scale, and o is bf16.  With per-head scales
+    [Hkv] q is quantised per query head over the call's R rows (quantize_e4m3 on a transposed [Hq, R, D] copy), with
+    per-row scales [num_blocks, Hkv, block_rows] each q row on its own (quantize_e4m3_rows, read in place)."""
+    if q.dim() not in (3, 4) or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
+        raise SvgbError(f"a KV-cache plan takes q [B, Sq, Hq, D] or [total_q, Hq, D] (got {tuple(q.shape)}) and "
+                        f"k_cache, v_cache [blocks, rows, Hkv, D] of one shape (got {tuple(k_cache.shape)}, "
+                        f"{tuple(v_cache.shape)})")
+    nb, rows, Hkv, Dc = k_cache.shape
+    if nb * rows != plan.S_kv:
         raise SvgbError(f"the KV-cache plan was built for {plan.S_kv} cache rows, the cache {tuple(k_cache.shape)} has "
-                        f"{k_cache.shape[0] * k_cache.shape[1]}")
-    if k_cache.dtype == torch.float8_e4m3fn:
-        rows = _row_scales("attn_fwd on an FP8 KV cache", k_scale, v_scale, k_cache)
-        if rows:
-            return _attn_kvcache_fp8_rows(q, k_cache, v_cache, plan, return_lse, sm_scale, out, *rows)
-        return _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale)
-    if k_scale is not None or v_scale is not None:
-        raise SvgbError(f"k_scale / v_scale are for float8_e4m3fn caches; a {k_cache.dtype} cache takes none")
-    if not (q.dtype == k_cache.dtype == v_cache.dtype):
+                        f"{nb * rows}")
+    fp8 = k_cache.dtype == torch.float8_e4m3fn
+    Hq, D = q.shape[-2:]
+    if fp8:
+        if q.dtype != torch.bfloat16:
+            raise SvgbError(f"an FP8 KV cache takes bf16 q (got {q.dtype}); it is quantised here, and the output is "
+                            "bf16")
+        if D != 128 or Dc != 128:
+            raise SvgbError(f"an FP8 KV cache needs head_dim 128 (got q {D}, cache {Dc}): 64-byte e4m3 rows have no "
+                            "128-byte swizzle")
+    elif q.dtype != k_cache.dtype:
         raise SvgbError("q and the caches must share one dtype")
-    if out is not None and (out.shape != q.shape or out.dtype != q.dtype):
-        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype")
-    Hq, D = q.shape[2:]
-    qf = _addressed(q.reshape(B * Sq, Hq, D), "shd")
-    kf, vf = (_addressed(c.flatten(0, 1), "shd") for c in (k_cache, v_cache))
-    if plan.desc.kind == PLAN_KVCACHE_SPLIT:
-        if q.shape[3] != k_cache.shape[3] or Hq % k_cache.shape[2]:
-            raise SvgbError(f"q {tuple(q.shape)} and the cache {tuple(k_cache.shape)} differ in D, or q's heads are no "
-                            "multiple of the cache's")
-        o = _split_out(out, B * Sq, Hq, D, q.dtype, q.device)
-        lse = _split_fwd(qf, _st(qf, "shd"), kf, vf, None, o, plan, _dt(q), 0, k_cache.shape, return_lse, sm_scale)
-        return _split_result(o, lse, out, B, Sq, return_lse)
-    of = torch.empty_like(qf)
-    res = _attn(qf, kf, vf, of, plan, "shd", _dt(q), (None, None, None), (None, None, None), return_lse, sm_scale)
-    o = of.view(B, Sq, Hq, D)
-    if out is not None:
-        out.copy_(o)
-        o = out
-    if not return_lse:
-        return o
-    return o, res[1].view(Hq, B, Sq).transpose(0, 1)
-
-
-def _attn_kvcache_varlen(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
-    """attn_fwd under a variable-length KV-cache plan (plan_kvcache(cu_seqlens_q=)): q [total_q, Hq, D] runs as one
-    block of total_q packed rows through _attn_kvcache, in every cache format, single pass or split; returns o
-    [total_q, Hq, D] (out itself when given) and lse [Hq, total_q], FlashAttention's varlen shapes."""
-    R = plan.S
-    if q.dim() != 3 or q.shape[0] != R:
-        raise SvgbError(f"a variable-length KV-cache plan for total_q={R} query rows takes q [total_q, Hq, D] (got "
-                        f"{tuple(q.shape)})")
-    if out is not None and (out.shape != q.shape or out.dim() != 3):
-        raise SvgbError(f"out {tuple(out.shape)} must have q's shape [total_q, Hq, D] {tuple(q.shape)}")
+    if D != Dc or not Hkv or Hq % Hkv:
+        raise SvgbError(f"q {tuple(q.shape)} and the cache {tuple(k_cache.shape)} differ in D, or q's {Hq} heads are "
+                        f"not a multiple of the cache's {Hkv} key/value heads")
+    o_dtype = torch.bfloat16 if fp8 else q.dtype
+    if out is not None and (out.shape != q.shape or out.dtype != o_dtype):
+        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype{' bf16' if fp8 else ''}")
+    scales, per_row = _cache_format("attn_fwd on a KV cache", k_cache, v_cache, k_scale, v_scale)
     if needs_grad(q, k_cache, v_cache):
         raise SvgbError("attention into a KV cache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
-    res = _attn_kvcache(q[None], k_cache, v_cache, plan, return_lse, sm_scale, None if out is None else out[None],
-                        k_scale, v_scale)
-    o = res[0] if return_lse else res
-    o = out if out is not None else o[0]
-    return (o, res[1][0]) if return_lse else o
-
-
-def _split_out(out, rows, Hq, D, dtype, device):
-    """o [rows, Hq, D] of a split forward: out itself when it is contiguous (the merge writes it in place), else new."""
-    if out is not None and out.is_contiguous():
-        return out.view(rows, Hq, D)
-    return torch.empty(rows, Hq, D, dtype=dtype, device=device)
-
-
-def _split_fwd(qf, q_strides, kf, vf, scales, o, plan, dtype, row_scales, cache_shape, return_lse, sm_scale):
-    """svgb_attn_fwd_kvcache_split under a split KV-cache plan: the attention into fp32 partials in a cached workspace,
-    then the merge into o [B Sq, Hq, D]; returns the lse [Hq, B Sq] or None.  Two launches.  scales: None (16-bit) or
-    (q_scale, k_scale, v_scale) of an e4m3 cache, per head (row_scales = 0) or per row (1)."""
     B, Sq = plan.source
-    R, Hq, D = o.shape
-    nb, rows, Hkv = cache_shape[:3]
-    n = plan.desc.max_items // (plan.desc.varlen_items or B * -(-Sq // 256))
-    nbytes = C.c_size_t()
-    check(lib().svgb_attn_fwd_kvcache_split_bytes(n, R, Hq, D, C.byref(nbytes)), "svgb_attn_fwd_kvcache_split_bytes")
-    ws = workspace("kvcache_split", nbytes.value, o.device)
-    lse = torch.empty(Hq, R, dtype=torch.float32, device=o.device) if return_lse else None
+    varlen = plan.desc.varlen_items > 0
+    if varlen and (q.dim() != 3 or q.shape[0] != Sq):
+        raise SvgbError(f"a variable-length KV-cache plan for total_q={Sq} query rows takes q [total_q, Hq, D] (got "
+                        f"{tuple(q.shape)})")
+    if not varlen and (q.dim() != 4 or q.shape[:2] != (B, Sq)):
+        raise SvgbError(f"a KV-cache plan for B={B} streams of Sq={Sq} queries takes q [B, Sq, Hq, D] (got "
+                        f"{tuple(q.shape)})")
+    R = B * Sq
+    # the q operand and its (batch, head, row) strides; the cache as [nb * rows, Hkv, D] views, e4m3 read in place
+    if scales is None:
+        dt, fill = _dt(q), 8
+        qa = _addressed(q.reshape(R, Hq, D), "shd")
+        q_st = _st(qa, "shd")
+        kf, vf = (_addressed(c.flatten(0, 1), "shd") for c in (k_cache, v_cache))
+    else:
+        dt, fill = _E4M3, 16
+        if per_row:
+            qa, q_scale = quantize_e4m3_rows(q.reshape(R, Hq, D))
+            q_st = _st(qa, "shd", 16)
+        else:  # [Hq, R, D]: one batch element of the scale kernel's [heads, rows, D]
+            qa, q_scale = quantize_e4m3(q.reshape(R, Hq, D).transpose(0, 1).contiguous())
+            q_st = _st(qa[None], "bhsd", 16)
+        scales = (q_scale, *scales)
+        kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))
+    lse = torch.empty(Hq, R, dtype=torch.float32, device=q.device) if return_lse else None
     scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    fill = 16 if dtype == _E4M3 else 8
-    check(lib().svgb_attn_fwd_kvcache_split(qf.data_ptr(), kf.data_ptr(), vf.data_ptr(), *map(_p, scales or (None,) * 3),
-                                            o.data_ptr(), _p(lse), dtype, row_scales, B, Hq, Hkv, Sq, nb, rows, D,
-                                            q_strides, _st(kf, "shd", fill), _st(vf, "shd", fill), _st(o, "shd"), scale,
-                                            C.byref(plan.desc), plan.ws.data_ptr(), ws.data_ptr(), ws.numel(),
-                                            _stream(o)), "svgb_attn_fwd_kvcache_split")
-    _bump(2)
-    return lse
-
-
-def _split_result(o, lse, out, B, Sq, return_lse):
-    """o [B, Sq, Hq, D] (copied into an out= the merge could not write) and lse [B, Hq, Sq], as _attn_kvcache returns
-    them."""
-    Hq, D = o.shape[1:]
-    o = o.view(B, Sq, Hq, D)
-    if out is not None:
+    split = plan.desc.kind == PLAN_KVCACHE_SPLIT
+    if split:  # the merge writes a contiguous out= in place
+        o = (out.view(R, Hq, D) if out is not None and out.is_contiguous() else
+             torch.empty(R, Hq, D, dtype=o_dtype, device=q.device))
+        n = plan.desc.max_items // (plan.desc.varlen_items or B * -(-Sq // 256))
+        nbytes = C.c_size_t()
+        check(lib().svgb_attn_fwd_kvcache_split_bytes(n, R, Hq, D, C.byref(nbytes)),
+              "svgb_attn_fwd_kvcache_split_bytes")
+        buf = workspace("kvcache_split", nbytes.value, q.device)
+        name = "svgb_attn_fwd_kvcache_split"
+        args = (*map(_p, scales or (None,) * 3), o.data_ptr(), _p(lse), dt, int(per_row), B, Hq, Hkv, Sq, nb, rows, D)
+        ws = (buf.data_ptr(), buf.numel())
+    else:
+        o = torch.empty_like(qa) if scales is None else torch.empty(R, Hq, D, dtype=o_dtype, device=q.device)
+        ws = ()
+        if scales is None:  # q, o as one batch element, each at its own strides
+            name, args = "svgb_attn_fwd_strided", (o.data_ptr(), _p(lse), dt, 1, Hq, Hkv, R, nb * rows, D)
+        elif per_row:
+            name, args = "svgb_attn_fwd_kvcache_e4m3_rows", (*map(_p, scales), o.data_ptr(), _p(lse), Hq, Hkv, R, nb,
+                                                              rows, D)
+        else:
+            name, args = "svgb_attn_fwd_strided_e4m3", (*map(_p, scales), o.data_ptr(), _p(lse), 1, Hq, Hkv, R,
+                                                         nb * rows, D)
+    check(getattr(lib(), name)(qa.data_ptr(), kf.data_ptr(), vf.data_ptr(), *args, q_st, _st(kf, "shd", fill),
+                               _st(vf, "shd", fill), _st(o, "shd"), scale, C.byref(plan.desc), plan.ws.data_ptr(), *ws,
+                               _stream(q)), name)
+    _bump(2 if split else 1)
+    if out is None:
+        o = o.view(q.shape)
+    else:
         if o.data_ptr() != out.data_ptr():
-            out.copy_(o)
+            out.copy_(o.view(out.shape))  # an out= the kernels did not write
         o = out
     if not return_lse:
         return o
-    return o, lse.view(Hq, B, Sq).transpose(0, 1)
-
-
-def _attn_kvcache_fp8(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
-    """_attn_kvcache on float8_e4m3fn caches: svgb_attn_fwd_strided_e4m3 with the cache read in place."""
-    B, Sq = plan.source
-    Hq, D = q.shape[2:]
-    Hkv = k_cache.shape[2]
-    if v_cache.dtype != torch.float8_e4m3fn:
-        raise SvgbError("an e4m3 k_cache needs an e4m3 v_cache")
-    if q.dtype != torch.bfloat16:
-        raise SvgbError(f"an FP8 KV cache takes bf16 q (got {q.dtype}); it is quantised per query head here, and the "
-                        "output is bf16")
-    if D != 128 or k_cache.shape[3] != 128:
-        raise SvgbError(f"an FP8 KV cache needs head_dim 128 (got q {D}, cache {k_cache.shape[3]}): 64-byte e4m3 rows "
-                        "have no 128-byte swizzle")
-    if Hq % Hkv:
-        raise SvgbError(f"q's {Hq} heads must be a multiple of the cache's {Hkv} key/value heads")
-    if out is not None and (out.shape != q.shape or out.dtype != torch.bfloat16):
-        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype bf16")
-    ks, vs = _fp8_scales("attn_fwd on an FP8 KV cache", k_scale, v_scale, Hkv)
-    # per query head over the B * Sq rows of this call: the scale kernel takes [heads, rows, D]
-    q8, q_scale = quantize_e4m3(q.reshape(B * Sq, Hq, D).transpose(0, 1).contiguous())
-    kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))  # [rows, Hkv, D] views, read in place
-    if plan.desc.kind == PLAN_KVCACHE_SPLIT:
-        o = _split_out(out, B * Sq, Hq, D, torch.bfloat16, q.device)
-        lse = _split_fwd(q8, _st(q8[None], "bhsd", 16), kf, vf, (q_scale, ks, vs), o, plan, _E4M3, 0, k_cache.shape,
-                         return_lse, sm_scale)
-        return _split_result(o, lse, out, B, Sq, return_lse)
-    o = torch.empty(B * Sq, Hq, D, dtype=torch.bfloat16, device=q.device)
-    lse = torch.empty(Hq, B * Sq, dtype=torch.float32, device=q.device) if return_lse else None
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    # q8 [Hq, B Sq, D] is one batch element; the cache and o are "shd" views, each at its own strides
-    check(lib().svgb_attn_fwd_strided_e4m3(q8.data_ptr(), kf.data_ptr(), vf.data_ptr(), q_scale.data_ptr(),
-                                           ks.data_ptr(), vs.data_ptr(), o.data_ptr(), _p(lse), 1, Hq, Hkv, B * Sq,
-                                           plan.S_kv, D, _st(q8[None], "bhsd", 16), _st(kf, "shd", 16), _st(vf, "shd", 16),
-                                           _st(o, "shd"), scale, C.byref(plan.desc), plan.ws.data_ptr(), _stream(q)),
-          "svgb_attn_fwd_strided_e4m3")
-    _bump()
-    o = o.view(B, Sq, Hq, D)
-    if out is not None:
-        out.copy_(o)
-        o = out
-    if not return_lse:
-        return o
-    return o, lse.view(Hq, B, Sq).transpose(0, 1)
+    return o, lse if varlen else lse.view(Hq, B, Sq).transpose(0, 1)
 
 
 def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, *, layout: str = "bhsd", sm_scale: Optional[float] = None,
@@ -1230,50 +1083,6 @@ class _Permute(torch.autograd.Function):
     def backward(ctx, g):
         perm, = ctx.saved_tensors
         return (permute_gather if ctx.scatter else permute_scatter)(g, perm), None, None
-
-
-def _attn_kvcache_fp8_rows(q, k_cache, v_cache, plan, return_lse, sm_scale, out, k_scale, v_scale):
-    """_attn_kvcache on an e4m3 cache with per-row scales: q quantised per row (quantize_e4m3_rows, read in place), then
-    svgb_attn_fwd_kvcache_e4m3_rows on the cache in place.  Each stream's o and lse depend on that stream alone."""
-    B, Sq = plan.source
-    Hq, D = q.shape[2:]
-    nb, rows, Hkv, _ = k_cache.shape
-    if v_cache.dtype != torch.float8_e4m3fn:
-        raise SvgbError("an e4m3 k_cache needs an e4m3 v_cache")
-    if q.dtype != torch.bfloat16:
-        raise SvgbError(f"an FP8 KV cache takes bf16 q (got {q.dtype}); it is quantised per row here, and the output is "
-                        "bf16")
-    if D != 128:
-        raise SvgbError(f"an FP8 KV cache needs head_dim 128 (got q {D})")
-    if Hq % Hkv:
-        raise SvgbError(f"q's {Hq} heads must be a multiple of the cache's {Hkv} key/value heads")
-    if out is not None and (out.shape != q.shape or out.dtype != torch.bfloat16):
-        raise SvgbError(f"out {tuple(out.shape)} {out.dtype} must have q's shape and dtype bf16")
-    if needs_grad(q, k_cache, v_cache):
-        raise SvgbError("attention into a KV cache has no backward: the KV-cache plan (plan_kvcache) runs forward only")
-    q8, q_scale = quantize_e4m3_rows(q.reshape(B * Sq, Hq, D))
-    kf, vf = (c.flatten(0, 1).view(torch.uint8) for c in (k_cache, v_cache))  # [rows, Hkv, D] views, read in place
-    if plan.desc.kind == PLAN_KVCACHE_SPLIT:
-        o = _split_out(out, B * Sq, Hq, D, torch.bfloat16, q.device)
-        lse = _split_fwd(q8, _st(q8, "shd", 16), kf, vf, (q_scale, k_scale, v_scale), o, plan, _E4M3, 1, k_cache.shape,
-                         return_lse, sm_scale)
-        return _split_result(o, lse, out, B, Sq, return_lse)
-    o = torch.empty(B * Sq, Hq, D, dtype=torch.bfloat16, device=q.device)
-    lse = torch.empty(Hq, B * Sq, dtype=torch.float32, device=q.device) if return_lse else None
-    scale = float(D) ** -0.5 if sm_scale is None else float(sm_scale)
-    check(lib().svgb_attn_fwd_kvcache_e4m3_rows(q8.data_ptr(), kf.data_ptr(), vf.data_ptr(), q_scale.data_ptr(),
-                                                k_scale.data_ptr(), v_scale.data_ptr(), o.data_ptr(), _p(lse), Hq, Hkv,
-                                                B * Sq, nb, rows, D, _st(q8, "shd", 16), _st(kf, "shd", 16),
-                                                _st(vf, "shd", 16), _st(o, "shd"), scale, C.byref(plan.desc),
-                                                plan.ws.data_ptr(), _stream(q)), "svgb_attn_fwd_kvcache_e4m3_rows")
-    _bump()
-    o = o.view(B, Sq, Hq, D)
-    if out is not None:
-        out.copy_(o)
-        o = out
-    if not return_lse:
-        return o
-    return o, lse.view(Hq, B, Sq).transpose(0, 1)
 
 
 def quantize_e4m3_rows(x: torch.Tensor):
