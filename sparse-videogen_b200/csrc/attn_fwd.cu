@@ -663,19 +663,9 @@ static int plan_varblock_impl(const uint8_t* map, const int32_t* row_sz, const i
                "plan too large for 32-bit chunk offsets");
   const int max_items = varblock_max_items(Sq, QC);
   const int cap = varblock_chunk_cap(Skv, KC);
-  plan->kind = gather ? SVGB_PLAN_GATHER : SVGB_PLAN_VARBLOCK;
-  plan->BH = BH;
-  plan->S = Sq;
-  plan->max_items = max_items;
-  plan->items_stride = max_items;
-  plan->mask_mode = MASK_NONE;
-  plan->m0 = rect ? Skv : 0;
-  plan->m1 = 0;
-  plan->m2 = 0;
-  plan->counts_off = 0;
-  plan->items_off = align_up(sizeof(int) * BH, 256);
-  plan->chunks_off = plan->items_off + align_up(2 * sizeof(int4) * BH * max_items, 256);
-  plan->bytes = need;
+  const int64_t items_off = align_up(sizeof(int) * BH, 256);
+  write_plan(plan, gather ? SVGB_PLAN_GATHER : SVGB_PLAN_VARBLOCK, BH, Sq, max_items, max_items, MASK_NONE,
+             rect ? Skv : 0, 0, 0, 0, items_off, items_off + align_up(2 * sizeof(int4) * BH * max_items, 256), need);
   char* ws = static_cast<char*>(plan_ws);
   // per q-block list lengths: scratch of the two plan kernels, after the lists
   const size_t lens_off = plan->chunks_off + align_up(sizeof(int2) * static_cast<size_t>(BH) * QC * cap, 256);
@@ -742,19 +732,10 @@ static int plan_local_varlen_impl(const int32_t* cu_q, const int32_t* cu_k, int 
   SVGB_REQUIRE(L.max_chunks < (1ll << 31) && nseg < (1 << 29), "plan too large for 32-bit chunk offsets");
   const int rows = transposed ? Skv : Sq, cols = transposed ? Sq : Skv;
   const int max_items = static_cast<int>(std::min<long long>(rows, (rows + 510ll * nseg) / 256));
-  plan->kind = transposed ? SVGB_PLAN_SEG_T : SVGB_PLAN_SEG;
-  plan->BH = cols;  // a segment plan serves every head: BH holds its key/value length (svgb200.h)
-  plan->S = rows;
-  plan->max_items = max_items;
-  plan->items_stride = 0;
-  plan->mask_mode = block ? MASK_BLOCK_CAUSAL : MASK_LOCAL;
-  plan->m0 = sink;
-  plan->m1 = block ? block : left;
-  plan->m2 = block ? left + 1 : right;
-  plan->counts_off = 0;
-  plan->items_off = static_cast<int64_t>(L.items_off);
-  plan->chunks_off = static_cast<int64_t>(L.chunks_off);
-  plan->bytes = static_cast<int64_t>(need);
+  // a segment plan serves every head: BH holds its key/value length (svgb200.h)
+  write_plan(plan, transposed ? SVGB_PLAN_SEG_T : SVGB_PLAN_SEG, cols, rows, max_items, 0,
+             block ? MASK_BLOCK_CAUSAL : MASK_LOCAL, sink, block ? block : left, block ? left + 1 : right, 0,
+             static_cast<int64_t>(L.items_off), static_cast<int64_t>(L.chunks_off), static_cast<int64_t>(need));
   char* ws = static_cast<char*>(plan_ws);
   int* counts = reinterpret_cast<int*>(ws);
   int* segs = reinterpret_cast<int*>(ws + L.segs_off);
@@ -769,56 +750,199 @@ static int plan_local_varlen_impl(const int32_t* cu_q, const int32_t* cu_k, int 
   return 0;
 }
 
-// Every forward entry: q / o over Sq rows and BH heads in B batch elements, k / v over Skv rows and BH / kv_group
-// heads, each tensor with its own strides.
-static int attn_fwd_run(const void* q, const void* k, const void* v, const float* q_scale, const float* k_scale,
-                        const float* v_scale, void* o, float* lse, const int32_t* q_rows, const int32_t* kv_rows,
-                        const int32_t* o_rows, int dtype, int B, int BH, int kv_group, int Sq, int Skv, int D,
-                        Strides qs, Strides ks, Strides vs, Strides os, float sm_scale, const svgb_plan* plan,
-                        const void* plan_ws, void* stream, int scale_block_rows = 0, int split_items = 0) {
-  SVGB_REQUIRE(q && k && v && o && plan && plan_ws, "null pointer");
-  SVGB_REQUIRE((plan->kind == SVGB_PLAN_KVCACHE_SPLIT) == (split_items > 0),
-               "internal: a split KV-cache plan runs with its split count, and only it");
-  SVGB_REQUIRE(dtype != SVGB_E4M3 || (q_scale && k_scale && v_scale),
-               "fp8 attention needs the three per-head scale vectors");
-  SVGB_REQUIRE(dtype == SVGB_E4M3 || (!q_scale && !k_scale && !v_scale),
-               "per-head scale vectors are for e4m3 inputs only (dtype %d)", dtype);
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND_T,
-               "a key-major band plan (svgb_attn_plan_band_t) is for svgb_attn_bwd; the forward takes svgb_attn_plan_band");
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG_T,
-               "a key-major segment plan (svgb_attn_plan_local_varlen_t) is for the backward; the forward takes "
-               "svgb_attn_plan_local_varlen");
-  const bool kvc = plan->kind == SVGB_PLAN_KVCACHE || plan->kind == SVGB_PLAN_KVCACHE_SPLIT;
-  SVGB_REQUIRE(!kvc || (!q_rows && !kv_rows && !o_rows),
+// One forward call, as every entry hands it over: q / o over Sq rows and Hq heads in B batch elements, k / v over Skv
+// rows and Hkv heads, each tensor with its own strides.  A split plan's call has B streams of Sq rows each, run as
+// B * Sq packed rows; a KV-cache entry's Skv is its num_blocks x block_rows cache rows.
+struct AttnFwdCall {
+  const void *q, *k, *v;
+  const float *q_scale, *k_scale, *v_scale;
+  void* o;
+  float* lse;
+  const int32_t *q_rows, *kv_rows, *o_rows;
+  int dtype, row_scales;  // row_scales: e4m3 with per-row k / v scales beside the cache rows
+  int B, Hq, Hkv, Sq, Skv, D;
+  Strides qs, ks, vs, os;
+  float sm_scale;
+  const svgb_plan* plan;
+  const void* plan_ws;
+  int num_blocks, block_rows;  // KV-cache entries: the cache geometry (0: none)
+  void* ws;                    // split plans: the fp32 partials
+  size_t ws_bytes;
+  void* stream;
+};
+
+// input formats
+enum { FMT_16BIT = 1, FMT_E4M3 = 2, FMT_E4M3_ROWS = 4 };
+// addressing: one stride pair for q, k, v and one for o; a q and a k / v pair; or per-tensor strides
+enum { ADDR_FLAT, ADDR_FLAT_KV, ADDR_STRIDED };
+// bit k: plan kind k; bit 0: kinds outside 1 .. 8, which svgb_attn_fwd runs as variable-block plans
+constexpr unsigned kind_bit(int kind) { return kind >= 1 && kind <= 8 ? 1u << kind : 1u; }
+constexpr unsigned K_VARBLOCK = 1u << SVGB_PLAN_VARBLOCK, K_BAND = 1u << SVGB_PLAN_BAND, K_GATHER = 1u << SVGB_PLAN_GATHER,
+                   K_SEG = 1u << SVGB_PLAN_SEG, K_KVCACHE = 1u << SVGB_PLAN_KVCACHE,
+                   K_SPLIT = 1u << SVGB_PLAN_KVCACHE_SPLIT;
+
+// what one forward entry accepts
+struct AttnFwdRule {
+  const char* who;
+  unsigned kinds;
+  const char* kinds_text;  // the accepted kinds, for the refusal
+  unsigned formats;
+  int addr;
+  bool row_vectors;  // q_rows / kv_rows / o_rows
+  bool split;        // split KV-cache plans, with a partials workspace
+};
+enum { FWD, FWD_KV, FWD_GQA, FWD_STRIDED, FWD_STRIDED_E4M3, FWD_KVCACHE_E4M3_ROWS, FWD_KVCACHE_SPLIT };
+static constexpr AttnFwdRule kFwdRules[] = {
+    {"svgb_attn_fwd", K_VARBLOCK | K_BAND | K_GATHER | K_SEG | K_KVCACHE | 1u,
+     "variable-block, band, gather, segment or KV-cache plans", FMT_16BIT | FMT_E4M3, ADDR_FLAT, true, false},
+    {"svgb_attn_fwd_kv", K_VARBLOCK | K_SEG, "segment plans and variable-block plans", FMT_16BIT, ADDR_FLAT_KV, false,
+     false},
+    {"svgb_attn_fwd_gqa", K_VARBLOCK | K_BAND | K_SEG | K_KVCACHE, "variable-block, band, segment or KV-cache plans",
+     FMT_16BIT, ADDR_FLAT_KV, false, false},
+    {"svgb_attn_fwd_strided", K_VARBLOCK | K_BAND | K_SEG | K_KVCACHE, "variable-block, band, segment or KV-cache plans",
+     FMT_16BIT, ADDR_STRIDED, false, false},
+    {"svgb_attn_fwd_strided_e4m3", K_VARBLOCK | K_BAND | K_KVCACHE, "variable-block, band or KV-cache plans", FMT_E4M3,
+     ADDR_STRIDED, false, false},
+    {"svgb_attn_fwd_kvcache_e4m3_rows", K_KVCACHE, "KV-cache plans (svgb_attn_plan_kvcache)", FMT_E4M3_ROWS,
+     ADDR_STRIDED, false, false},
+    {"svgb_attn_fwd_kvcache_split", K_SPLIT, "split KV-cache plans (svgb_attn_plan_kvcache_split)",
+     FMT_16BIT | FMT_E4M3 | FMT_E4M3_ROWS, ADDR_STRIDED, false, true},
+};
+
+static bool e4m3_strides(Strides s) { return s.b % 16 == 0 && s.h % 16 == 0 && s.r % 16 == 0; }
+
+// items per split of a split plan: recorded by a varlen plan, whose item count depends on lengths only the device holds
+static int split_items(const AttnFwdCall& c) {
+  return c.plan->varlen_items > 0 ? c.plan->varlen_items : c.B * ((c.Sq + kItemRows - 1) / kItemRows);
+}
+
+// Every rule of the forward, in one order, before any device work.
+static int attn_fwd_check(const AttnFwdCall& c, const AttnFwdRule& r) {
+  const char* who = r.who;
+  const svgb_plan* plan = c.plan;
+  SVGB_REQUIRE(c.q && c.k && c.v && c.o && plan && c.plan_ws && (!r.split || c.ws), "null pointer");
+  const int kind = plan->kind;
+  // plan kinds
+  const char* hint = kind == SVGB_PLAN_KVCACHE_SPLIT
+                         ? "; a split KV-cache plan (svgb_attn_plan_kvcache_split) runs on svgb_attn_fwd_kvcache_split only"
+                     : kind == SVGB_PLAN_BAND_T || kind == SVGB_PLAN_SEG_T
+                         ? "; a key-major plan (svgb_attn_plan_band_t or svgb_attn_plan_local_varlen_t) is for the "
+                           "backward: key-major plans have no GQA, strided or forward path"
+                     : kind == SVGB_PLAN_GATHER
+                         ? "; gather plans (svgb_attn_plan_varblock_gather) and row vectors run on svgb_attn_fwd only"
+                     : kind == SVGB_PLAN_SEG ? "; segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs"
+                                             : "";
+  SVGB_REQUIRE(r.kinds & kind_bit(kind), "%s takes %s only (kind %d)%s", who, r.kinds_text, kind, hint);
+  // input format: 16-bit, or e4m3 with per-head or per-row scales
+  const bool e4m3 = c.dtype == SVGB_E4M3;
+  SVGB_REQUIRE(e4m3 || c.dtype == SVGB_BF16 || c.dtype == SVGB_F16, "%s: dtype %d unsupported", who, c.dtype);
+  SVGB_REQUIRE(r.formats & (!e4m3 ? FMT_16BIT : c.row_scales ? FMT_E4M3_ROWS : FMT_E4M3),
+               "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no path here)", who, c.dtype);
+  SVGB_REQUIRE(!e4m3 || (kind != SVGB_PLAN_SEG && kind != SVGB_PLAN_SEG_T),
+               "%s: segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs, not e4m3", who);
+  // the flat entry's scales are [BH] by query head: an e4m3 cache, whose scales are by key/value head, is strided
+  SVGB_REQUIRE(!e4m3 || r.addr != ADDR_FLAT || kind != SVGB_PLAN_KVCACHE,
+               "KV-cache plans (svgb_attn_plan_kvcache) take bf16 or fp16 inputs here; an e4m3 cache takes "
+               "svgb_attn_fwd_strided_e4m3");
+  if (e4m3) {
+    SVGB_REQUIRE(c.D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
+                 who, c.D);
+    if (c.row_scales) {
+      SVGB_REQUIRE(c.q_scale, "%s needs the three scale tensors: the query row scales q_scale (float [Hq, Sq]), then "
+                   "k_scale and v_scale", who);
+      if (kv_scale_rows_check(c.k_scale, c.v_scale, c.block_rows, who)) return -1;
+    } else {
+      SVGB_REQUIRE(c.q_scale && c.k_scale && c.v_scale,
+                   "%s needs the three scale vectors q_scale [B*Hq], k_scale and v_scale [B*Hkv]; an e4m3 cache needs "
+                   "the three scale tensors", who);
+    }
+    for (Strides s : {c.qs, c.ks, c.vs})
+      SVGB_REQUIRE(e4m3_strides(s),
+                   "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
+                   s.b, s.h, s.r);
+  } else {
+    SVGB_REQUIRE(!c.q_scale && !c.k_scale && !c.v_scale && !c.row_scales,
+                 "%s: 16-bit inputs (dtype %d) take no scales; scales are for e4m3 inputs", who, c.dtype);
+  }
+  // row vectors
+  const bool kvc = kind == SVGB_PLAN_KVCACHE || kind == SVGB_PLAN_KVCACHE_SPLIT;
+  SVGB_REQUIRE(!kvc || (!c.q_rows && !c.kv_rows && !c.o_rows),
                "KV-cache plans (svgb_attn_plan_kvcache) take no row vectors or gathers (q_rows / kv_rows / o_rows)");
-  const bool seg = plan->kind == SVGB_PLAN_SEG;
-  SVGB_REQUIRE(!seg || dtype != SVGB_E4M3, "segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs, not e4m3");
-  SVGB_REQUIRE(!seg || (!q_rows && !kv_rows && !o_rows),
+  SVGB_REQUIRE(kind != SVGB_PLAN_SEG || (!c.q_rows && !c.kv_rows && !c.o_rows),
                "segment plans (svgb_attn_plan_local_varlen) take no row vectors (q_rows / kv_rows / o_rows)");
-  const bool gather = plan->kind == SVGB_PLAN_GATHER;
-  SVGB_REQUIRE(gather || (!q_rows && !kv_rows),
+  SVGB_REQUIRE(kind == SVGB_PLAN_GATHER || (!c.q_rows && !c.kv_rows),
                "row gathers (q_rows / kv_rows) need a gather plan from svgb_attn_plan_varblock_gather");
-  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == Skv && (plan->items_stride == 0 || plan->BH == BH / kv_group),
-               "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
-               plan_kv_len(plan), BH / kv_group, Sq, Skv);
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0 && os.r % 8 == 0 && os.h % 8 == 0 && os.b % 8 == 0,
+  // heads, addressing and the cache
+  SVGB_REQUIRE(c.B > 0 && c.Hq > 0 && c.Hkv > 0 && c.Hq % c.Hkv == 0,
+               "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d (B=%d)", who, c.Hq, c.Hkv, c.B);
+  SVGB_REQUIRE(c.D == 64 || c.D == 128, "head_dim %d unsupported (64 or 128)", c.D);
+  if (r.addr == ADDR_FLAT_KV) {
+    for (const void* p : {c.q, c.k, c.v})
+      SVGB_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
+    for (Strides s : {c.qs, c.ks})
+      SVGB_REQUIRE(s.r % 8 == 0 && s.h % 8 == 0, "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
+  }
+  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(c.o) & 15) == 0 && c.os.r % 8 == 0 && c.os.h % 8 == 0 && c.os.b % 8 == 0,
                "output must be 16-byte aligned with strides multiple of 8 elements");
-  const char* ws = static_cast<const char*>(plan_ws);
+  if (c.block_rows || c.num_blocks)
+    SVGB_REQUIRE(c.num_blocks > 0 && c.block_rows > 0 && static_cast<long long>(c.num_blocks) * c.block_rows < (1ll << 31),
+                 "%s: bad cache geometry (num_blocks=%d, block_rows=%d)", who, c.num_blocks, c.block_rows);
+  // the plan's lengths and heads; a split plan serves B streams of Sq rows as B * Sq packed rows
+  int Sq = c.Sq;
+  if (r.split) {
+    SVGB_REQUIRE(c.Sq > 0 && static_cast<long long>(c.B) * c.Sq == plan->S,
+                 "%s: the plan was built for %d query rows, called with B=%d streams of Sq=%d", who, plan->S, c.B, c.Sq);
+    Sq = plan->S;
+  }
+  const int BHkv = (r.split ? 1 : c.B) * c.Hkv;
+  SVGB_REQUIRE(kind != SVGB_PLAN_BAND || Sq == c.Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, c.Skv);
+  SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
+               "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
+  SVGB_REQUIRE(plan->S == Sq && plan_kv_len(plan) == c.Skv,
+               "plan was built for BH=%d Sq=%d Skv=%d, called with BH=%d Sq=%d Skv=%d", plan->BH, plan->S,
+               plan_kv_len(plan), BHkv, Sq, c.Skv);
+  if (r.split) {
+    const int items = split_items(c);
+    SVGB_REQUIRE(plan->max_items > 0 && plan->max_items % items == 0,
+                 "%s: the plan's %d items are no whole number of splits of %d items (B=%d, Sq=%d)", who, plan->max_items,
+                 items, c.B, c.Sq);
+    size_t need = 0;
+    if (svgb_attn_fwd_kvcache_split_bytes(plan->max_items / items, Sq, c.Hq, c.D, &need)) return -1;
+    SVGB_REQUIRE(c.ws_bytes >= need, "%s: workspace too small: %zu < %zu", who, c.ws_bytes, need);
+    SVGB_REQUIRE((reinterpret_cast<uintptr_t>(c.ws) & 15) == 0, "%s: the workspace must be 16-byte aligned", who);
+  }
+  return 0;
+}
+
+// A checked call: one launch, and for a split plan the LSE merge of its fp32 partials.
+static int attn_fwd_run(const AttnFwdCall& c) {
+  const svgb_plan* plan = c.plan;
+  const int kind = plan->kind;
+  const bool seg = kind == SVGB_PLAN_SEG, split = kind == SVGB_PLAN_KVCACHE_SPLIT;
+  const bool kvc = kind == SVGB_PLAN_KVCACHE || split;
+  const int B = split ? 1 : c.B, Sq = split ? plan->S : c.Sq, BH = B * c.Hq;
+  const int items = split ? split_items(c) : 0, nsplit = split ? plan->max_items / items : 0;
+  // split: o is the fp32 partials o [n, R, Hq, D] (the split as its batch dimension), then lse [n, Hq, R]
+  float* o_part = static_cast<float*>(c.ws);
+  float* lse_part = split ? o_part + static_cast<size_t>(nsplit) * Sq * c.Hq * c.D : nullptr;
+  const Strides os = split ? Strides{static_cast<long long>(Sq) * c.Hq * c.D, c.D, static_cast<long long>(c.Hq) * c.D}
+                           : c.os;
+  const char* ws = static_cast<const char*>(c.plan_ws);
   AttnArgs a;
   a.items = reinterpret_cast<const int4*>(ws + plan->items_off);
   a.item_count = reinterpret_cast<const int*>(ws + plan->counts_off);
   a.chunks = reinterpret_cast<const int2*>(ws + plan->chunks_off);
   a.items_stride = plan->items_stride;
-  a.kv_group = kv_group;
-  a.o = o;
+  a.kv_group = c.Hq / c.Hkv;
+  a.o = split ? static_cast<void*>(o_part) : c.o;
   a.o_row_stride = os.r;
   a.o_head_stride = os.h;
   a.o_batch_stride = os.b;
-  a.o_rows = o_rows;
-  a.lse = lse;
-  a.scale_log2 = sm_scale * 1.4426950408889634f;
+  a.o_rows = c.o_rows;
+  a.lse = split ? lse_part : c.lse;
+  a.scale_log2 = c.sm_scale * 1.4426950408889634f;
   a.S = Sq;
-  if (plan->kind == SVGB_PLAN_BAND || seg || kvc) {  // a variable-block plan's m0 is its Skv, not a mask parameter
+  if (kind == SVGB_PLAN_BAND || seg || kvc) {  // a variable-block plan's m0 is its Skv, not a mask parameter
     a.mask_mode = plan->mask_mode;
     a.m0 = plan->m0;
     a.m1 = plan->m1;
@@ -826,24 +950,40 @@ static int attn_fwd_run(const void* q, const void* k, const void* v, const float
   }
   if (seg || kvc) a.segs = reinterpret_cast<const int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF);
   a.kv_logical = kvc ? 1 : 0;
-  a.q_scale = q_scale;
-  a.k_scale = k_scale;
-  a.v_scale = v_scale;
-  a.q_rows = q_rows;
-  a.kv_rows = kv_rows;
-  a.q_ptr = q;
-  a.k_ptr = k;
-  a.v_ptr = v;
-  a.in_row_stride = qs.r;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
-  a.in_head_stride = qs.h;
-  a.scale_block_rows = scale_block_rows;
-  if (split_items > 0) {  // o: the fp32 partials, one batch-stride apart per split (svgb_attn_fwd_kvcache_split)
+  a.q_scale = c.q_scale;
+  a.k_scale = c.k_scale;
+  a.v_scale = c.v_scale;
+  a.q_rows = c.q_rows;
+  a.kv_rows = c.kv_rows;
+  a.q_ptr = c.q;
+  a.k_ptr = c.k;
+  a.v_ptr = c.v;
+  a.in_row_stride = c.qs.r;  // gather plans: q, k and v share one stride pair (svgb_attn_fwd)
+  a.in_head_stride = c.qs.h;
+  a.scale_block_rows = c.dtype == SVGB_E4M3 && c.row_scales ? c.block_rows : 0;
+  if (split) {
     a.out_f32 = 1;
-    a.split_items = split_items;
+    a.split_items = items;
     a.o_split_stride = os.b;
   }
-  return attn_fwd_impl(q, qs, Sq, k, ks, v, vs, Skv, dtype, B, BH, D, a, gather, plan->max_items,
-                       static_cast<cudaStream_t>(stream));
+  cudaStream_t st = static_cast<cudaStream_t>(c.stream);
+  if (attn_fwd_impl(c.q, c.qs, Sq, c.k, c.ks, c.v, c.vs, c.Skv, c.dtype, B, BH, c.D, a, kind == SVGB_PLAN_GATHER,
+                    plan->max_items, st))
+    return -1;
+  if (!split) return 0;
+  const bool bf16 = c.dtype != SVGB_F16;  // e4m3 caches give bf16 o
+  auto merge = c.D == 128 ? (bf16 ? kv_split_merge_kernel<128, true> : kv_split_merge_kernel<128, false>)
+                          : (bf16 ? kv_split_merge_kernel<64, true> : kv_split_merge_kernel<64, false>);
+  const long long warps = static_cast<long long>(Sq) * c.Hq;
+  merge<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, st>>>(o_part, lse_part, nsplit, Sq, c.Hq,
+                                                                 static_cast<uint16_t*>(c.o), c.os.r, c.os.h, c.lse);
+  SVGB_LAUNCH_OK();
+  return 0;
+}
+
+static int attn_fwd(const AttnFwdCall& c, int row) {
+  if (attn_fwd_check(c, kFwdRules[row])) return -1;
+  return attn_fwd_run(c);
 }
 
 }  // namespace svgb
@@ -905,19 +1045,8 @@ static int plan_band_impl(int mask_mode, int m0, int m1, int m2, int BH, int S, 
   const int n_chunks = (S + kChunkCols - 1) / kChunkCols;
   SVGB_REQUIRE(n_items <= n_items_cap, "internal: item count");
   SVGB_REQUIRE(static_cast<size_t>(n_items_cap) * n_chunks < (1ull << 31), "plan too large");
-  plan->kind = transposed ? SVGB_PLAN_BAND_T : SVGB_PLAN_BAND;
-  plan->BH = BH;
-  plan->S = S;
-  plan->max_items = n_items;
-  plan->items_stride = 0;
-  plan->mask_mode = mask_mode;
-  plan->m0 = m0;
-  plan->m1 = m1;
-  plan->m2 = m2;
-  plan->counts_off = 0;
-  plan->items_off = 256;
-  plan->chunks_off = 256 + align_up(2 * sizeof(int4) * n_items_cap, 256);
-  plan->bytes = need;
+  write_plan(plan, transposed ? SVGB_PLAN_BAND_T : SVGB_PLAN_BAND, BH, S, n_items, 0, mask_mode, m0, m1, m2, 0, 256,
+             256 + align_up(2 * sizeof(int4) * n_items_cap, 256), need);
   char* ws = static_cast<char*>(plan_ws);
   plan_band_kernel<<<n_items, kItemRows, 0, static_cast<cudaStream_t>(stream)>>>(
       mask_mode, m0, m1, m2, S, n_chunks, sg, transposed ? 1 : 0, reinterpret_cast<int*>(ws + plan->counts_off),
@@ -981,66 +1110,46 @@ int svgb_attn_fwd(const void* q, const void* k, const void* v, const float* q_sc
                   const int32_t* o_rows, int dtype, int BH, int S, int D, long long row_stride,
                   long long head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                   const svgb_plan* plan, const void* plan_ws, void* stream) {
-  if (no_split_plan(plan, "svgb_attn_fwd")) return -1;
-  // its scales are [BH] by query head: an e4m3 cache, whose scales are by key/value head, takes the strided e4m3 entry
-  SVGB_REQUIRE(!plan || plan->kind != SVGB_PLAN_KVCACHE || dtype != SVGB_E4M3,
-               "KV-cache plans (svgb_attn_plan_kvcache) take bf16 or fp16 inputs here; an e4m3 cache takes "
-               "svgb_attn_fwd_strided_e4m3");
   const Strides in = flat_strides(row_stride, head_stride, BH);
-  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, 1, BH, 1, S, S, D,
-                      in, in, in, flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, stream);
+  return attn_fwd({q, k, v, q_scale, k_scale, v_scale, o, lse, q_rows, kv_rows, o_rows, dtype, 0, 1, BH, BH, S, S, D,
+                   in, in, in, flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, 0, 0, nullptr,
+                   0, stream},
+                  FWD);
 }
 
 int svgb_attn_fwd_kv(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BH, int Sq,
                      int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                      long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                      const svgb_plan* plan, const void* plan_ws, void* stream) {
-  SVGB_REQUIRE(plan, "null pointer");
-  if (no_split_plan(plan, "svgb_attn_fwd_kv")) return -1;
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
-               "svgb_attn_fwd_kv takes bf16 or fp16 inputs (dtype %d; e4m3 attention needs Sq == Skv, svgb_attn_fwd)",
-               dtype);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_SEG,
-               "svgb_attn_fwd_kv takes segment plans and variable-block plans only (kind %d; band, gather and "
-               "profiling plans need Sq == Skv, svgb_attn_fwd)", plan->kind);
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
-                   (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
-                   kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
-               "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
   const Strides kv = flat_strides(kv_row_stride, kv_head_stride, BH);
-  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 1, BH, 1, Sq, Skv,
-                      D, flat_strides(q_row_stride, q_head_stride, BH), kv, kv,
-                      flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, stream);
+  return attn_fwd({q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 0, 1, BH, BH, Sq, Skv,
+                   D, flat_strides(q_row_stride, q_head_stride, BH), kv, kv,
+                   flat_strides(o_row_stride, o_head_stride, BH), sm_scale, plan, plan_ws, 0, 0, nullptr, 0, stream},
+                  FWD_KV);
 }
 
 int svgb_attn_fwd_gqa(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int BHq, int BHkv,
                       int Sq, int Skv, int D, long long q_row_stride, long long q_head_stride, long long kv_row_stride,
                       long long kv_head_stride, long long o_row_stride, long long o_head_stride, float sm_scale,
                       const svgb_plan* plan, const void* plan_ws, void* stream) {
-  if (no_split_plan(plan, "svgb_attn_fwd_gqa")) return -1;
-  if (attn_gqa_check(dtype, BHq, BHkv, Sq, Skv, plan, "svgb_attn_fwd_gqa")) return -1;
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
-                   (reinterpret_cast<uintptr_t>(v) & 15) == 0 && q_row_stride % 8 == 0 && q_head_stride % 8 == 0 &&
-                   kv_row_stride % 8 == 0 && kv_head_stride % 8 == 0,
-               "q, k, v must be 16-byte aligned with strides multiple of 8 elements");
   const Strides kv = flat_strides(kv_row_stride, kv_head_stride, BHkv);
-  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 1, BHq, BHq / BHkv,
-                      Sq, Skv, D, flat_strides(q_row_stride, q_head_stride, BHq), kv, kv,
-                      flat_strides(o_row_stride, o_head_stride, BHq), sm_scale, plan, plan_ws, stream);
+  return attn_fwd({q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 0, 1, BHq, BHkv, Sq,
+                   Skv, D, flat_strides(q_row_stride, q_head_stride, BHq), kv, kv,
+                   flat_strides(o_row_stride, o_head_stride, BHq), sm_scale, plan, plan_ws, 0, 0, nullptr, 0, stream},
+                  FWD_GQA);
 }
 
 int svgb_attn_fwd_strided(const void* q, const void* k, const void* v, void* o, float* lse, int dtype, int B, int Hq,
                           int Hkv, int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
                           const long long* v_strides, const long long* o_strides, float sm_scale,
                           const svgb_plan* plan, const void* plan_ws, void* stream) {
-  if (no_split_plan(plan, "svgb_attn_fwd_strided")) return -1;
   Strides st[4];
   if (attn_strided_check(B, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st,
-                         "svgb_attn_fwd_strided"))
+                         kFwdRules[FWD_STRIDED].who))
     return -1;
-  if (attn_gqa_check(dtype, B * Hq, B * Hkv, Sq, Skv, plan, "svgb_attn_fwd_strided")) return -1;
-  return attn_fwd_run(q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, B, B * Hq,
-                      Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, stream);
+  return attn_fwd({q, k, v, nullptr, nullptr, nullptr, o, lse, nullptr, nullptr, nullptr, dtype, 0, B, Hq, Hkv, Sq, Skv,
+                   D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, 0, 0, nullptr, 0, stream},
+                  FWD_STRIDED);
 }
 
 int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, const float* q_scale,
@@ -1048,30 +1157,13 @@ int svgb_attn_fwd_strided_e4m3(const void* q, const void* k, const void* v, cons
                                int Sq, int Skv, int D, const long long* q_strides, const long long* k_strides,
                                const long long* v_strides, const long long* o_strides, float sm_scale,
                                const svgb_plan* plan, const void* plan_ws, void* stream) {
-  const char* who = "svgb_attn_fwd_strided_e4m3";
-  if (no_split_plan(plan, who)) return -1;
-  SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
-               who, D);
-  SVGB_REQUIRE(q_scale && k_scale && v_scale,
-               "%s needs the three scale vectors: q_scale [B*Hq], k_scale and v_scale [B*Hkv]", who);
-  SVGB_REQUIRE(plan, "null pointer");
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_SEG && plan->kind != SVGB_PLAN_SEG_T,
-               "%s: segment plans (svgb_attn_plan_local_varlen) take bf16 or fp16 inputs, not e4m3", who);
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_GATHER,
-               "%s: gather plans (svgb_attn_plan_varblock_gather) and row vectors run on svgb_attn_fwd only", who);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_KVCACHE,
-               "%s takes variable-block, band or KV-cache plans (kind %d)", who, plan->kind);
   Strides st[4];
-  if (attn_strided_check(B, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st, who)) return -1;
-  for (int i = 0; i < 3; ++i)
-    SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
-                 "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
-                 st[i].b, st[i].h, st[i].r);
-  SVGB_REQUIRE(Hq % Hkv == 0, "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d", who, Hq,
-               Hkv);
-  if (attn_group_plan_check(B * Hkv, Sq, Skv, plan, who)) return -1;
-  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, B, B * Hq,
-                      Hq / Hkv, Sq, Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, stream);
+  if (attn_strided_check(B, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st,
+                         kFwdRules[FWD_STRIDED_E4M3].who))
+    return -1;
+  return attn_fwd({q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, 0, B, Hq, Hkv, Sq,
+                   Skv, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws, 0, 0, nullptr, 0, stream},
+                  FWD_STRIDED_E4M3);
 }
 
 int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v, const float* q_scale,
@@ -1079,29 +1171,14 @@ int svgb_attn_fwd_kvcache_e4m3_rows(const void* q, const void* k, const void* v,
                                     int Sq, int num_blocks, int block_rows, int D, const long long* q_strides,
                                     const long long* k_strides, const long long* v_strides, const long long* o_strides,
                                     float sm_scale, const svgb_plan* plan, const void* plan_ws, void* stream) {
-  const char* who = "svgb_attn_fwd_kvcache_e4m3_rows";
-  SVGB_REQUIRE(plan, "null pointer");
-  if (no_split_plan(plan, who)) return -1;
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_KVCACHE,
-               "%s takes KV-cache plans (svgb_attn_plan_kvcache) only (kind %d): per-row scales live beside the cache "
-               "rows", who, plan->kind);
-  SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
-               who, D);
-  SVGB_REQUIRE(q_scale, "%s needs the query row scales q_scale (float [Hq, Sq])", who);
-  if (kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
-  SVGB_REQUIRE(num_blocks > 0 && block_rows > 0 && static_cast<long long>(num_blocks) * block_rows < (1ll << 31),
-               "%s: bad cache geometry (num_blocks=%d, block_rows=%d)", who, num_blocks, block_rows);
   Strides st[4];
-  if (attn_strided_check(1, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st, who)) return -1;
-  for (int i = 0; i < 3; ++i)
-    SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
-                 "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
-                 st[i].b, st[i].h, st[i].r);
-  SVGB_REQUIRE(Hq % Hkv == 0, "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d", who, Hq,
-               Hkv);
-  return attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, 1, Hq,
-                      Hq / Hkv, Sq, num_blocks * block_rows, D, st[0], st[1], st[2], st[3], sm_scale, plan, plan_ws,
-                      stream, block_rows);
+  if (attn_strided_check(1, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st,
+                         kFwdRules[FWD_KVCACHE_E4M3_ROWS].who))
+    return -1;
+  return attn_fwd({q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, SVGB_E4M3, 1, 1, Hq, Hkv, Sq,
+                   static_cast<int>(static_cast<long long>(num_blocks) * block_rows), D, st[0], st[1], st[2], st[3],
+                   sm_scale, plan, plan_ws, num_blocks, block_rows, nullptr, 0, stream},
+                  FWD_KVCACHE_E4M3_ROWS);
 }
 
 int svgb_attn_fwd_kvcache_split_bytes(int num_splits, int rows, int Hq, int D, size_t* bytes) {
@@ -1118,62 +1195,14 @@ int svgb_attn_fwd_kvcache_split(const void* q, const void* k, const void* v, con
                                 const long long* k_strides, const long long* v_strides, const long long* o_strides,
                                 float sm_scale, const svgb_plan* plan, const void* plan_ws, void* ws, size_t ws_bytes,
                                 void* stream) {
-  const char* who = "svgb_attn_fwd_kvcache_split";
-  SVGB_REQUIRE(plan && ws, "null pointer");
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_KVCACHE_SPLIT,
-               "%s takes split KV-cache plans (svgb_attn_plan_kvcache_split) only (kind %d)", who, plan->kind);
-  SVGB_REQUIRE(B > 0 && Sq > 0 && static_cast<long long>(B) * Sq == plan->S,
-               "%s: the plan was built for %d query rows, called with B=%d streams of Sq=%d", who, plan->S, B, Sq);
-  // items per split: recorded by a varlen plan, whose item count depends on lengths only the device holds
-  const int items = plan->varlen_items > 0 ? plan->varlen_items : B * ((Sq + kItemRows - 1) / kItemRows);
-  SVGB_REQUIRE(plan->max_items > 0 && plan->max_items % items == 0,
-               "%s: the plan's %d items are no whole number of splits of %d items (B=%d, Sq=%d)", who, plan->max_items,
-               items, B, Sq);
-  const int nsplit = plan->max_items / items;
-  const bool e4m3 = dtype == SVGB_E4M3;
-  SVGB_REQUIRE(e4m3 || dtype == SVGB_BF16 || dtype == SVGB_F16, "%s: dtype %d unsupported", who, dtype);
-  if (e4m3) {
-    SVGB_REQUIRE(D == 128, "%s: the e4m3 path needs head_dim 128 (got %d): 64-byte e4m3 rows have no 128-byte swizzle",
-                 who, D);
-    SVGB_REQUIRE(q_scale && k_scale && v_scale, "%s: an e4m3 cache needs the three scale tensors q_scale, k_scale and "
-                 "v_scale", who);
-    if (row_scales && kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
-  } else {
-    SVGB_REQUIRE(!q_scale && !k_scale && !v_scale && !row_scales,
-                 "%s: 16-bit inputs (dtype %d) take no scales; scales are for e4m3 caches", who, dtype);
-  }
-  SVGB_REQUIRE(num_blocks > 0 && block_rows > 0 && static_cast<long long>(num_blocks) * block_rows < (1ll << 31),
-               "%s: bad cache geometry (num_blocks=%d, block_rows=%d)", who, num_blocks, block_rows);
   Strides st[4];
-  if (attn_strided_check(1, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st, who)) return -1;
-  if (e4m3)
-    for (int i = 0; i < 3; ++i)
-      SVGB_REQUIRE(st[i].b % 16 == 0 && st[i].h % 16 == 0 && st[i].r % 16 == 0,
-                   "%s: every e4m3 (batch, head, row) stride must be a multiple of 16 bytes (got %lld, %lld, %lld)", who,
-                   st[i].b, st[i].h, st[i].r);
-  SVGB_REQUIRE(Hq % Hkv == 0, "%s: the query heads Hq=%d must be a multiple of the key/value heads Hkv=%d", who, Hq,
-               Hkv);
-  const int R = plan->S;
-  size_t need = 0;
-  if (svgb_attn_fwd_kvcache_split_bytes(nsplit, R, Hq, D, &need)) return -1;
-  SVGB_REQUIRE(ws_bytes >= need, "%s: workspace too small: %zu < %zu", who, ws_bytes, need);
-  SVGB_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "%s: the workspace must be 16-byte aligned", who);
-  // partials: o [n, R, Hq, D] (the split as its batch dimension), then lse [n, Hq, R]
-  float* o_part = static_cast<float*>(ws);
-  float* lse_part = o_part + static_cast<size_t>(nsplit) * R * Hq * D;
-  const Strides ps{static_cast<long long>(R) * Hq * D, D, static_cast<long long>(Hq) * D};
-  if (attn_fwd_run(q, k, v, q_scale, k_scale, v_scale, o_part, lse_part, nullptr, nullptr, nullptr,
-                   e4m3 ? SVGB_E4M3 : dtype, 1, Hq, Hq / Hkv, R, num_blocks * block_rows, D, st[0], st[1], st[2], ps,
-                   sm_scale, plan, plan_ws, stream, e4m3 && row_scales ? block_rows : 0, items))
+  if (attn_strided_check(1, Hq, Hkv, {q, k, v, o}, {q_strides, k_strides, v_strides, o_strides}, st,
+                         kFwdRules[FWD_KVCACHE_SPLIT].who))
     return -1;
-  const bool bf16 = dtype != SVGB_F16;  // e4m3 caches give bf16 o
-  auto merge = D == 128 ? (bf16 ? kv_split_merge_kernel<128, true> : kv_split_merge_kernel<128, false>)
-                        : (bf16 ? kv_split_merge_kernel<64, true> : kv_split_merge_kernel<64, false>);
-  const long long warps = static_cast<long long>(R) * Hq;
-  merge<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      o_part, lse_part, nsplit, R, Hq, static_cast<uint16_t*>(o), st[3].r, st[3].h, lse);
-  SVGB_LAUNCH_OK();
-  return 0;
+  return attn_fwd({q, k, v, q_scale, k_scale, v_scale, o, lse, nullptr, nullptr, nullptr, dtype, row_scales, B, Hq, Hkv,
+                   Sq, static_cast<int>(static_cast<long long>(num_blocks) * block_rows), D, st[0], st[1], st[2], st[3],
+                   sm_scale, plan, plan_ws, num_blocks, block_rows, ws, ws_bytes, stream},
+                  FWD_KVCACHE_SPLIT);
 }
 
 int svgb_density(const uint8_t* map, const int32_t* row_sz, const int32_t* col_sz, int BH, int QC,

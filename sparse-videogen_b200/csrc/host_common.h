@@ -93,6 +93,14 @@ inline int block_causal_m1(int block, int first_block, int* m1, const char* who)
   return 0;
 }
 
+// every field of a plan descriptor, so that no planner leaves one indeterminate; varlen_items is 0 outside the
+// variable-length KV-cache planner
+inline void write_plan(svgb_plan* p, int kind, int BH, int S, int max_items, int items_stride, int mask_mode, int m0,
+                       int m1, int m2, int varlen_items, int64_t items_off, int64_t chunks_off, int64_t bytes) {
+  *p = svgb_plan{kind, BH, S, max_items, items_stride, mask_mode, m0, m1, m2, varlen_items, 0, items_off, chunks_off,
+                 bytes};
+}
+
 // key/value rows of a plan: a variable-block plan of svgb_attn_plan_varblock_kv records them in m0, a segment plan in
 // BH (svgb200.h); every other plan has Skv = S
 inline int plan_kv_len(const svgb_plan* p) {
@@ -100,49 +108,6 @@ inline int plan_kv_len(const svgb_plan* p) {
       p->kind == SVGB_PLAN_KVCACHE_SPLIT)
     return p->BH;
   return p->kind == SVGB_PLAN_VARBLOCK && p->m0 > 0 ? p->m0 : p->S;
-}
-
-// what a plan of an accepted kind needs to be shared by the groups of query heads: band plans Sq == Skv, per-head
-// plans built over the BHkv key/value heads
-inline int attn_group_plan_check(int BHkv, int Sq, int Skv, const svgb_plan* plan, const char* who) {
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_BAND || Sq == Skv, "%s: band plans need Sq == Skv (got %d, %d)", who, Sq, Skv);
-  SVGB_REQUIRE(plan->items_stride == 0 || plan->BH == BHkv,
-               "%s: a per-head plan is built over the BHkv=%d key/value heads (plan BH=%d)", who, BHkv, plan->BH);
-  return 0;
-}
-
-// the checks the grouped-query and strided entries (svgb_attn_{fwd,bwd}_{gqa,strided}) share, before any device
-// work: BHq query heads in groups over BHkv key/value heads, 16-bit inputs, and a variable-block plan over the
-// key/value heads, a band plan (one work list for every head, Sq == Skv) or a segment plan (one work list for every head)
-inline int attn_gqa_check(int dtype, int BHq, int BHkv, int Sq, int Skv, const svgb_plan* plan, const char* who) {
-  SVGB_REQUIRE(plan, "null pointer");
-  SVGB_REQUIRE(BHq > 0 && BHkv > 0 && BHq % BHkv == 0,
-               "%s: the query heads BHq=%d must be a multiple of the key/value heads BHkv=%d", who, BHq, BHkv);
-  SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16,
-               "%s takes bf16 or fp16 inputs (dtype %d; e4m3 attention has no GQA or strided path)", who, dtype);
-  SVGB_REQUIRE(plan->kind == SVGB_PLAN_VARBLOCK || plan->kind == SVGB_PLAN_BAND || plan->kind == SVGB_PLAN_SEG ||
-                   plan->kind == SVGB_PLAN_KVCACHE,
-               "%s takes variable-block, band, segment or KV-cache plans (kind %d; gather and key-major plans have no "
-               "GQA or strided path)", who, plan->kind);
-  return attn_group_plan_check(BHkv, Sq, Skv, plan, who);
-}
-
-// KV-cache plans (svgb_attn_plan_kvcache) run forward only, as FlashAttention's flash_attn_with_kvcache
-inline int no_kvcache_backward(const svgb_plan* plan, const char* who) {
-  SVGB_REQUIRE(plan, "null pointer");
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_KVCACHE,
-               "%s: a KV-cache plan (svgb_attn_plan_kvcache) has no backward; it runs forward only", who);
-  SVGB_REQUIRE(plan->kind != SVGB_PLAN_KVCACHE_SPLIT,
-               "%s: a split KV-cache plan (svgb_attn_plan_kvcache_split) has no backward; it runs forward only, on "
-               "svgb_attn_fwd_kvcache_split", who);
-  return 0;
-}
-
-// a split KV-cache plan writes fp32 partials that a merge combines: only svgb_attn_fwd_kvcache_split runs it
-inline int no_split_plan(const svgb_plan* plan, const char* who) {
-  SVGB_REQUIRE(!plan || plan->kind != SVGB_PLAN_KVCACHE_SPLIT,
-               "%s: a split KV-cache plan (svgb_attn_plan_kvcache_split) runs on svgb_attn_fwd_kvcache_split only", who);
-  return 0;
 }
 
 // the operands of a strided entry (svgb_attn_fwd_strided, svgb_attn_bwd_strided), before any device work: B batch

@@ -316,15 +316,6 @@ static KvLayout kv_layout(int B, int Sq, int cap, int sink, int left, int right,
   return L;
 }
 
-static int kv_plan_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes, int nsplit = 1) {
-  SVGB_REQUIRE(B > 0 && Sq > 0 && cap > 0 && bytes, "bad arguments (B=%d, Sq=%d, capacity=%d)", B, Sq, cap);
-  SVGB_REQUIRE(sink >= 0 && left >= 0 && right >= 0,
-               "KV-cache plan: sink (%d), left (%d) and right (%d) must be >= 0", sink, left, right);
-  SVGB_REQUIRE(nsplit >= 1, "split KV-cache plan: num_splits (%d) must be >= 1", nsplit);
-  *bytes = kv_layout(B, Sq, cap, sink, left, right, nsplit).bytes;
-  return 0;
-}
-
 // the cache geometry both entries take: num_blocks blocks of block_rows rows, paged when block_table is given; returns
 // the capacity of a stream in *cap
 static int kv_geometry(const int32_t* cache_batch_idx, const int32_t* block_table, int num_blocks, int block_rows,
@@ -365,21 +356,27 @@ int svgb::kv_scale_rows_check(const float* k_scale, const float* v_scale, int bl
   return 0;
 }
 
-// every append: 16-bit new rows (dtype) into a 16-bit cache of that dtype, or into an e4m3 cache with the per-head
-// scales k_scale, v_scale, or (k_rows, v_rows given) with per-row scales the append writes
+// every append: 16-bit new rows (dtype) into a 16-bit cache of that dtype (no scales), into an e4m3 cache with the
+// per-head scales k_scale, v_scale, or (row_scales) into an e4m3 cache with per-row scales k_scale, v_scale that the
+// append writes; `formats` are those the entry takes (FMT_*)
+enum { FMT_16BIT = 1, FMT_E4M3 = 2, FMT_E4M3_ROWS = 4 };
 static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
                          const int32_t* cache_batch_idx, const int32_t* block_table, int dtype, int B, int Snew,
                          int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                          const long long* vc_strides, const long long* k_strides, const long long* v_strides,
-                         const float* k_scale, const float* v_scale, float* k_rows, float* v_rows, void* stream,
+                         float* k_scale, float* v_scale, bool row_scales, unsigned formats, void* stream,
                          const char* who, const int32_t* cu_new = nullptr) {
-  const bool rows = k_rows != nullptr;
-  const bool e4m3 = k_scale != nullptr || rows;
+  const int fmt = row_scales ? FMT_E4M3_ROWS : k_scale || v_scale ? FMT_E4M3 : FMT_16BIT;
+  const bool e4m3 = fmt != FMT_16BIT;
+  SVGB_REQUIRE(formats & fmt, "%s needs both scale vectors k_scale and v_scale (float [Hkv])", who);
+  if (fmt == FMT_E4M3_ROWS && kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
+  SVGB_REQUIRE(fmt != FMT_E4M3 || (k_scale && v_scale), "%s: an e4m3 cache needs both scale vectors k_scale and "
+               "v_scale (float [Hkv]); a 16-bit cache takes neither", who);
   SVGB_REQUIRE(cache_seqlens, "null pointer");
   SVGB_REQUIRE(dtype == SVGB_BF16 || dtype == SVGB_F16, "%s takes bf16 or fp16 %s (dtype %d)", who,
                e4m3 ? "new rows" : "caches", dtype);
   SVGB_REQUIRE(D == 64 || D == 128, "%s: head_dim %d unsupported (64 or 128)", who, D);
-  SVGB_REQUIRE(!rows || D == 128, "%s: per-row scales need head_dim 128 (got %d)", who, D);
+  SVGB_REQUIRE(fmt != FMT_E4M3_ROWS || D == 128, "%s: per-row scales need head_dim 128 (got %d)", who, D);
   SVGB_REQUIRE(Snew > 0, "%s: no new rows (Snew=%d)", who, Snew);
   Strides st[4];
   if (attn_strided_check(B, Hkv, Hkv, {k_cache, v_cache, k, v}, {kc_strides, vc_strides, k_strides, v_strides}, st, who))
@@ -401,11 +398,11 @@ static int kv_append_run(void* k_cache, void* v_cache, const void* k, const void
         static_cast<uint16_t*>(k_cache), static_cast<uint16_t*>(v_cache), kn, vn, cache_seqlens, cache_batch_idx,
         block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages, cap, st[0], st[1], st[2], st[3], nullptr,
         nullptr, nullptr, nullptr, cu_new);
-  } else if (rows) {
+  } else if (row_scales) {
     auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_ROWS_BF16> : kv_append_kernel<KV_E4M3_ROWS_F16>;
     kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
                                  cache_batch_idx, block_table, B, Snew, Hkv, nvec, num_blocks, block_rows, max_pages,
-                                 cap, st[0], st[1], st[2], st[3], nullptr, nullptr, k_rows, v_rows, cu_new);
+                                 cap, st[0], st[1], st[2], st[3], nullptr, nullptr, k_scale, v_scale, cu_new);
   } else {
     auto kern = dtype == SVGB_BF16 ? kv_append_kernel<KV_E4M3_BF16> : kv_append_kernel<KV_E4M3_F16>;
     kern<<<blocks, 256, 0, cs>>>(static_cast<uint8_t*>(k_cache), static_cast<uint8_t*>(v_cache), kn, vn, cache_seqlens,
@@ -423,86 +420,102 @@ static long long kv_varlen_items(int B, int total_q, int max_q) {
                              (static_cast<long long>(total_q) + (kItemRows - 1) * static_cast<long long>(B)) / kItemRows);
 }
 
-// The arguments of the varlen pair, checked by name: block = 0 is the local band (sink, left, right) and takes no window
-// or first_block; block > 0 the block-causal mask (sink, W, C, F) and takes no left or right.  Gives the planner's m1
-// (0: local), left and right, and the layout's workspace.
-struct KvVarlen {
+// What one KV-cache plan is: B streams of Sq query rows each (uniform), or total_q = Sq packed rows of which a stream
+// holds at most max_q (varlen); the local band (sink, left, right) or the block-causal mask (sink, window, block,
+// first_block); n splits, and whether it is a split plan (SVGB_PLAN_KVCACHE_SPLIT).
+struct KvPlanSpec {
+  int B, Sq, max_q;
+  bool varlen;
+  int sink, left, right;
+  bool block_causal;
+  int window, block, first_block;
+  int nsplit;
+  bool split;
+};
+// the checked plan: its mask (m1 = 0, or m1 of SVGB_MASK_BLOCK_CAUSAL), the planner's left and right, I and the layout
+struct KvPlanArgs {
   int m1, left, right;
   long long I;
   KvLayout L;
 };
-static int kv_varlen_args(int B, int total_q, int max_q, int cap, int sink, int left, int right, int window, int block,
-                          int first_block, int num_splits, KvVarlen* a, const char* who) {
-  SVGB_REQUIRE(B > 0 && total_q > 0 && cap > 0, "%s: bad arguments (B=%d, total_q=%d, capacity=%d)", who, B, total_q,
-               cap);
-  SVGB_REQUIRE(total_q < (1 << 30), "%s: total_q = %d query rows too many", who, total_q);
-  SVGB_REQUIRE(max_q >= 1 && max_q <= total_q, "%s: max_q (%d) must lie in [1, total_q = %d]", who, max_q, total_q);
-  SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
+
+// Every argument rule of the KV-cache planners and their _bytes twins, against the capacity cap of a stream.
+static int kv_plan_check(const KvPlanSpec& s, int cap, KvPlanArgs* a, const char* who) {
+  SVGB_REQUIRE(s.B > 0 && s.Sq > 0 && cap > 0, "%s: bad arguments (B=%d, rows=%d, capacity=%d)", who, s.B, s.Sq, cap);
+  const long long rows = s.varlen ? s.Sq : static_cast<long long>(s.B) * s.Sq;
+  SVGB_REQUIRE(rows < (1ll << 30), "%s: %lld query rows too many", who, rows);
+  SVGB_REQUIRE(!s.varlen || (s.max_q >= 1 && s.max_q <= s.Sq), "%s: max_q (%d) must lie in [1, total_q = %d]", who,
+               s.max_q, s.Sq);
+  SVGB_REQUIRE(s.nsplit >= 1, "%s: num_splits (%d) must be >= 1", who, s.nsplit);
   a->m1 = 0;
   int widen = 0;  // the layout's right beyond the planner's: C - 1 for a block-causal plan
-  if (block) {
-    SVGB_REQUIRE(left == 0 && right == 0,
+  if (s.block_causal) {
+    SVGB_REQUIRE(s.left == 0 && s.right == 0,
                  "%s: a block-causal plan (block = %d) takes (window, block, first_block); left and right must be 0 "
-                 "(got %d, %d)", who, block, left, right);
-    if (block_causal_m1(block, first_block, &a->m1, who) || block_causal_check(sink, a->m1, window, who)) return -1;
-    a->left = window - 1;
+                 "(got %d, %d)", who, s.block, s.left, s.right);
+    if (block_causal_m1(s.block, s.first_block, &a->m1, who) || block_causal_check(s.sink, a->m1, s.window, who))
+      return -1;
+    a->left = s.window - 1;
     a->right = 0;
-    widen = block - 1;
+    widen = s.block - 1;
   } else {
-    SVGB_REQUIRE(window == 0 && first_block == 0,
+    SVGB_REQUIRE(s.window == 0 && s.first_block == 0,
                  "%s: a local plan (block = 0) takes (left, right); window and first_block must be 0 (got %d, %d)", who,
-                 window, first_block);
-    SVGB_REQUIRE(sink >= 0 && left >= 0 && right >= 0,
-                 "%s: sink (%d), left (%d) and right (%d) must be >= 0", who, sink, left, right);
-    a->left = left;
-    a->right = right;
+                 s.window, s.first_block);
+    SVGB_REQUIRE(s.sink >= 0 && s.left >= 0 && s.right >= 0, "%s: sink (%d), left (%d) and right (%d) must be >= 0",
+                 who, s.sink, s.left, s.right);
+    a->left = s.left;
+    a->right = s.right;
   }
-  a->I = kv_varlen_items(B, total_q, max_q);
-  a->L = kv_layout(B, total_q, cap, sink, a->left, a->right + widen, num_splits, a->I);
+  a->I = s.varlen ? kv_varlen_items(s.B, s.Sq, s.max_q) : 0;
+  a->L = kv_layout(s.B, s.Sq, cap, s.sink, a->left, a->right + widen, s.nsplit, a->I);
   SVGB_REQUIRE(a->L.items * a->L.slots < (1ll << 31) && a->L.items < (1ll << 31),
                "%s: plan too large for 32-bit chunk offsets", who);
   return 0;
 }
 
-// both planners: svgb_attn_plan_kvcache's plan (nsplit = 1, split = false: SVGB_PLAN_KVCACHE) and the split plan of
-// svgb_attn_plan_kvcache_split (SVGB_PLAN_KVCACHE_SPLIT)
-// the block-causal planner (block = m1 != 0, left = W - 1, right = 0) of svgb_attn_plan_kvcache_block
-static int kv_plan_run(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table, int B,
-                       int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left, int right,
-                       int nsplit, bool split, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream,
-                       const char* who, int block = 0) {
-  const int widen = block ? (block & 0xffff) - 1 : 0;  // kv_layout's right for a block-causal plan
-  SVGB_REQUIRE(cache_seqlens && plan_ws && plan, "null pointer");
+static int kv_plan_bytes(const KvPlanSpec& s, int cap, size_t* bytes, const char* who) {
+  SVGB_REQUIRE(bytes, "null pointer");
+  KvPlanArgs a;
+  if (kv_plan_check(s, cap, &a, who)) return -1;
+  *bytes = a.L.bytes;
+  return 0;
+}
+
+// Every KV-cache planner: the checks, the descriptor and one launch of the uniform or the variable-length list kernel.
+// Uniform plans take Snew new rows per stream, variable-length plans cu_q and the optional cu_new.
+static int kv_plan(const KvPlanSpec& s, const int32_t* cu_q, const int32_t* cache_seqlens, const int32_t* cu_new,
+                   int Snew, const int32_t* cache_batch_idx, const int32_t* block_table, int num_blocks, int block_rows,
+                   int max_pages, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream, const char* who) {
+  SVGB_REQUIRE((cu_q || !s.varlen) && cache_seqlens && plan_ws && plan, "null pointer");
   SVGB_REQUIRE(Snew >= 0, "%s: Snew=%d < 0", who, Snew);
   int cap = 0;
   if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
-  size_t need = 0;
-  if (kv_plan_bytes(B, Sq, cap, sink, left, right + widen, &need, nsplit)) return -1;
-  SVGB_REQUIRE(ws_bytes >= need, "plan workspace too small: %zu < %zu", ws_bytes, need);
-  SVGB_REQUIRE(static_cast<long long>(B) * Sq < (1ll << 30), "%s: B * Sq = %lld query rows too many", who,
-               static_cast<long long>(B) * Sq);
-  const KvLayout L = kv_layout(B, Sq, cap, sink, left, right + widen, nsplit);
-  SVGB_REQUIRE(L.items * L.slots < (1ll << 31) && L.items < (1ll << 31), "plan too large for 32-bit chunk offsets");
-  plan->kind = split ? SVGB_PLAN_KVCACHE_SPLIT : SVGB_PLAN_KVCACHE;
-  plan->BH = num_blocks * block_rows;  // a KV-cache plan serves every head: BH holds the cache rows (svgb200.h)
-  plan->S = B * Sq;
-  plan->max_items = static_cast<int>(L.items);
-  plan->items_stride = 0;
-  plan->mask_mode = block ? MASK_BLOCK_CAUSAL : MASK_LOCAL;
-  plan->m0 = sink;
-  plan->m1 = block ? block : left;
-  plan->m2 = block ? left + 1 : right;
-  plan->varlen_items = 0;
-  plan->counts_off = 0;
-  plan->items_off = static_cast<int64_t>(L.items_off);
-  plan->chunks_off = static_cast<int64_t>(L.chunks_off);
-  plan->bytes = static_cast<int64_t>(need);
+  KvPlanArgs a;
+  if (kv_plan_check(s, cap, &a, who)) return -1;
+  const KvLayout& L = a.L;
+  SVGB_REQUIRE(ws_bytes >= L.bytes, "plan workspace too small: %zu < %zu", ws_bytes, L.bytes);
+  // a KV-cache plan serves every head: BH holds the cache rows (svgb200.h)
+  write_plan(plan, s.split ? SVGB_PLAN_KVCACHE_SPLIT : SVGB_PLAN_KVCACHE, num_blocks * block_rows,
+             s.varlen ? s.Sq : s.B * s.Sq, static_cast<int>(L.items), 0, s.block_causal ? MASK_BLOCK_CAUSAL : MASK_LOCAL,
+             s.sink, s.block_causal ? a.m1 : a.left, s.block_causal ? s.window : a.right, static_cast<int>(a.I),
+             static_cast<int64_t>(L.items_off), static_cast<int64_t>(L.chunks_off), static_cast<int64_t>(L.bytes));
   char* ws = static_cast<char*>(plan_ws);
-  kv_lists_kernel<<<static_cast<unsigned>((L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, cap,
-      static_cast<int>(L.slots), nsplit, sink, left, right, block, reinterpret_cast<int*>(ws),
-      reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF), reinterpret_cast<int2*>(ws + L.chunks_off),
-      reinterpret_cast<int4*>(ws + L.items_off));
+  int* counts = reinterpret_cast<int*>(ws);
+  int* kv = reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF);
+  int2* chunks = reinterpret_cast<int2*>(ws + L.chunks_off);
+  int4* items = reinterpret_cast<int4*>(ws + L.items_off);
+  const unsigned grid = static_cast<unsigned>((L.items + 7) / 8);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (s.varlen)
+    kv_varlen_lists_kernel<<<grid, 256, 0, st>>>(cu_q, cache_seqlens, cu_new, cache_batch_idx, block_table, s.B, s.Sq,
+                                                 static_cast<int>(a.I), num_blocks, block_rows, max_pages, cap,
+                                                 static_cast<int>(L.slots), s.nsplit, s.sink, a.left, a.right, a.m1,
+                                                 counts, kv, chunks, items);
+  else
+    kv_lists_kernel<<<grid, 256, 0, st>>>(cache_seqlens, cache_batch_idx, block_table, s.B, s.Sq, Snew, num_blocks,
+                                          block_rows, max_pages, cap, static_cast<int>(L.slots), s.nsplit, s.sink,
+                                          a.left, a.right, a.m1, counts, kv, chunks, items);
   SVGB_LAUNCH_OK();
   return 0;
 }
@@ -516,7 +529,7 @@ int svgb_kvcache_append(void* k_cache, void* v_cache, const void* k, const void*
                         void* stream) {
   return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
                        num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
-                       nullptr, nullptr, nullptr, stream, "svgb_kvcache_append");
+                       nullptr, false, FMT_16BIT, stream, "svgb_kvcache_append");
 }
 
 int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cache_seqlens,
@@ -524,11 +537,11 @@ int svgb_kvcache_append_e4m3(void* k_cache, void* v_cache, const void* k, const 
                              int Hkv, int D, int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                              const long long* vc_strides, const long long* k_strides, const long long* v_strides,
                              const float* k_scale, const float* v_scale, void* stream) {
-  const char* who = "svgb_kvcache_append_e4m3";
-  SVGB_REQUIRE(k_scale && v_scale, "%s needs both scale vectors k_scale and v_scale (float [Hkv])", who);
+  // the per-head scales are only read
   return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
-                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, k_scale,
-                       v_scale, nullptr, nullptr, stream, who);
+                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides,
+                       const_cast<float*>(k_scale), const_cast<float*>(v_scale), false, FMT_E4M3, stream,
+                       "svgb_kvcache_append_e4m3");
 }
 
 int svgb_kvcache_append_e4m3_rows(void* k_cache, void* v_cache, const void* k, const void* v,
@@ -537,62 +550,9 @@ int svgb_kvcache_append_e4m3_rows(void* k_cache, void* v_cache, const void* k, c
                                   int num_blocks, int block_rows, int max_pages, const long long* kc_strides,
                                   const long long* vc_strides, const long long* k_strides, const long long* v_strides,
                                   float* k_scale, float* v_scale, void* stream) {
-  const char* who = "svgb_kvcache_append_e4m3_rows";
-  if (kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
   return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, Snew, Hkv, D,
-                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
-                       nullptr, k_scale, v_scale, stream, who);
-}
-
-int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {
-  return kv_plan_bytes(B, Sq, cap, sink, left, right, bytes);
-}
-
-int svgb_attn_plan_kvcache(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table,
-                           int B, int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left,
-                           int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
-  return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
-                     left, right, 1, false, plan_ws, ws_bytes, plan, stream, "svgb_attn_plan_kvcache");
-}
-
-int svgb_attn_plan_kvcache_split_bytes(int B, int Sq, int cap, int sink, int left, int right, int num_splits,
-                                       size_t* bytes) {
-  return kv_plan_bytes(B, Sq, cap, sink, left, right, bytes, num_splits);
-}
-
-int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
-                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
-                                 int max_pages, int sink, int left, int right, int num_splits, void* plan_ws,
-                                 size_t ws_bytes, svgb_plan* plan, void* stream) {
-  const char* who = "svgb_attn_plan_kvcache_split";
-  SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
-  return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
-                     left, right, num_splits, true, plan_ws, ws_bytes, plan, stream, who);
-}
-
-// m1 of SVGB_MASK_BLOCK_CAUSAL from (block, first_block), and every parameter checked
-static int kv_block_m1(int sink, int window, int block, int first_block, int num_splits, int* m1, const char* who) {
-  if (block_causal_m1(block, first_block, m1, who)) return -1;
-  SVGB_REQUIRE(num_splits >= 1, "%s: num_splits (%d) must be >= 1", who, num_splits);
-  return block_causal_check(sink, *m1, window, who);
-}
-
-int svgb_attn_plan_kvcache_block_bytes(int B, int Sq, int cap, int sink, int window, int block, int first_block,
-                                       int num_splits, size_t* bytes) {
-  int m1 = 0;
-  if (kv_block_m1(sink, window, block, first_block, num_splits, &m1, "svgb_attn_plan_kvcache_block_bytes")) return -1;
-  return kv_plan_bytes(B, Sq, cap, sink, window - 1, block - 1, bytes, num_splits);
-}
-
-int svgb_attn_plan_kvcache_block(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
-                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
-                                 int max_pages, int sink, int window, int block, int first_block, int num_splits,
-                                 void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
-  const char* who = "svgb_attn_plan_kvcache_block";
-  int m1 = 0;
-  if (kv_block_m1(sink, window, block, first_block, num_splits, &m1, who)) return -1;
-  return kv_plan_run(cache_seqlens, cache_batch_idx, block_table, B, Sq, Snew, num_blocks, block_rows, max_pages, sink,
-                     window - 1, 0, num_splits, num_splits > 1, plan_ws, ws_bytes, plan, stream, who, m1);
+                       num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, k_scale,
+                       v_scale, true, FMT_E4M3_ROWS, stream, "svgb_kvcache_append_e4m3_rows");
 }
 
 int svgb_kvcache_append_varlen(void* k_cache, void* v_cache, const void* k, const void* v, const int32_t* cu_new,
@@ -604,28 +564,61 @@ int svgb_kvcache_append_varlen(void* k_cache, void* v_cache, const void* k, cons
   const char* who = "svgb_kvcache_append_varlen";
   SVGB_REQUIRE(cu_new, "%s needs cu_new (device int32 [B + 1], the new rows of each stream)", who);
   SVGB_REQUIRE(B > 0, "%s: bad stream count B=%d", who, B);
-  if (row_scales) {
-    if (kv_scale_rows_check(k_scale, v_scale, block_rows, who)) return -1;
-    return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, total_new, Hkv,
-                         D, num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, nullptr,
-                         nullptr, k_scale, v_scale, stream, who, cu_new);
-  }
-  SVGB_REQUIRE(!k_scale == !v_scale, "%s: an e4m3 cache needs both scale vectors k_scale and v_scale (float [Hkv]); a "
-               "16-bit cache takes neither", who);
   return kv_append_run(k_cache, v_cache, k, v, cache_seqlens, cache_batch_idx, block_table, dtype, B, total_new, Hkv, D,
                        num_blocks, block_rows, max_pages, kc_strides, vc_strides, k_strides, v_strides, k_scale, v_scale,
-                       nullptr, nullptr, stream, who, cu_new);
+                       row_scales != 0, FMT_16BIT | FMT_E4M3 | FMT_E4M3_ROWS, stream, who, cu_new);
+}
+
+// the spec of each planner: B, Sq, max_q, varlen, sink, left, right, block_causal, window, block, first_block, nsplit,
+// split
+int svgb_attn_plan_kvcache_bytes(int B, int Sq, int cap, int sink, int left, int right, size_t* bytes) {
+  return kv_plan_bytes({B, Sq, 0, false, sink, left, right, false, 0, 0, 0, 1, false}, cap, bytes,
+                       "svgb_attn_plan_kvcache_bytes");
+}
+
+int svgb_attn_plan_kvcache(const int32_t* cache_seqlens, const int32_t* cache_batch_idx, const int32_t* block_table,
+                           int B, int Sq, int Snew, int num_blocks, int block_rows, int max_pages, int sink, int left,
+                           int right, void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
+  return kv_plan({B, Sq, 0, false, sink, left, right, false, 0, 0, 0, 1, false}, nullptr, cache_seqlens, nullptr, Snew,
+                 cache_batch_idx, block_table, num_blocks, block_rows, max_pages, plan_ws, ws_bytes, plan, stream,
+                 "svgb_attn_plan_kvcache");
+}
+
+int svgb_attn_plan_kvcache_split_bytes(int B, int Sq, int cap, int sink, int left, int right, int num_splits,
+                                       size_t* bytes) {
+  return kv_plan_bytes({B, Sq, 0, false, sink, left, right, false, 0, 0, 0, num_splits, true}, cap, bytes,
+                       "svgb_attn_plan_kvcache_split_bytes");
+}
+
+int svgb_attn_plan_kvcache_split(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
+                                 int max_pages, int sink, int left, int right, int num_splits, void* plan_ws,
+                                 size_t ws_bytes, svgb_plan* plan, void* stream) {
+  return kv_plan({B, Sq, 0, false, sink, left, right, false, 0, 0, 0, num_splits, true}, nullptr, cache_seqlens, nullptr,
+                 Snew, cache_batch_idx, block_table, num_blocks, block_rows, max_pages, plan_ws, ws_bytes, plan, stream,
+                 "svgb_attn_plan_kvcache_split");
+}
+
+int svgb_attn_plan_kvcache_block_bytes(int B, int Sq, int cap, int sink, int window, int block, int first_block,
+                                       int num_splits, size_t* bytes) {
+  return kv_plan_bytes({B, Sq, 0, false, sink, 0, 0, true, window, block, first_block, num_splits, num_splits > 1}, cap,
+                       bytes, "svgb_attn_plan_kvcache_block_bytes");
+}
+
+int svgb_attn_plan_kvcache_block(const int32_t* cache_seqlens, const int32_t* cache_batch_idx,
+                                 const int32_t* block_table, int B, int Sq, int Snew, int num_blocks, int block_rows,
+                                 int max_pages, int sink, int window, int block, int first_block, int num_splits,
+                                 void* plan_ws, size_t ws_bytes, svgb_plan* plan, void* stream) {
+  return kv_plan({B, Sq, 0, false, sink, 0, 0, true, window, block, first_block, num_splits, num_splits > 1}, nullptr,
+                 cache_seqlens, nullptr, Snew, cache_batch_idx, block_table, num_blocks, block_rows, max_pages, plan_ws,
+                 ws_bytes, plan, stream, "svgb_attn_plan_kvcache_block");
 }
 
 int svgb_attn_plan_kvcache_varlen_bytes(int B, int total_q, int max_q, int cap, int sink, int left, int right,
                                         int window, int block, int first_block, int num_splits, size_t* bytes) {
-  const char* who = "svgb_attn_plan_kvcache_varlen_bytes";
-  SVGB_REQUIRE(bytes, "null pointer");
-  KvVarlen a;
-  if (kv_varlen_args(B, total_q, max_q, cap, sink, left, right, window, block, first_block, num_splits, &a, who))
-    return -1;
-  *bytes = a.L.bytes;
-  return 0;
+  return kv_plan_bytes({B, total_q, max_q, true, sink, left, right, block != 0, window, block, first_block, num_splits,
+                        num_splits > 1},
+                       cap, bytes, "svgb_attn_plan_kvcache_varlen_bytes");
 }
 
 int svgb_attn_plan_kvcache_varlen(const int32_t* cu_q, const int32_t* cache_seqlens, const int32_t* cu_new,
@@ -633,36 +626,10 @@ int svgb_attn_plan_kvcache_varlen(const int32_t* cu_q, const int32_t* cache_seql
                                   int max_q, int num_blocks, int block_rows, int max_pages, int sink, int left,
                                   int right, int window, int block, int first_block, int num_splits, void* plan_ws,
                                   size_t ws_bytes, svgb_plan* plan, void* stream) {
-  const char* who = "svgb_attn_plan_kvcache_varlen";
-  SVGB_REQUIRE(cu_q && cache_seqlens && plan_ws && plan, "null pointer");
-  int cap = 0;
-  if (kv_geometry(cache_batch_idx, block_table, num_blocks, block_rows, max_pages, &cap, who)) return -1;
-  KvVarlen a;
-  if (kv_varlen_args(B, total_q, max_q, cap, sink, left, right, window, block, first_block, num_splits, &a, who))
-    return -1;
-  SVGB_REQUIRE(ws_bytes >= a.L.bytes, "plan workspace too small: %zu < %zu", ws_bytes, a.L.bytes);
-  plan->kind = num_splits > 1 ? SVGB_PLAN_KVCACHE_SPLIT : SVGB_PLAN_KVCACHE;
-  plan->BH = num_blocks * block_rows;
-  plan->S = total_q;
-  plan->max_items = static_cast<int>(a.L.items);
-  plan->items_stride = 0;
-  plan->mask_mode = block ? MASK_BLOCK_CAUSAL : MASK_LOCAL;
-  plan->m0 = sink;
-  plan->m1 = block ? a.m1 : a.left;
-  plan->m2 = block ? window : a.right;
-  plan->varlen_items = static_cast<int>(a.I);
-  plan->counts_off = 0;
-  plan->items_off = static_cast<int64_t>(a.L.items_off);
-  plan->chunks_off = static_cast<int64_t>(a.L.chunks_off);
-  plan->bytes = static_cast<int64_t>(a.L.bytes);
-  char* ws = static_cast<char*>(plan_ws);
-  kv_varlen_lists_kernel<<<static_cast<unsigned>((a.L.items + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      cu_q, cache_seqlens, cu_new, cache_batch_idx, block_table, B, total_q, static_cast<int>(a.I), num_blocks,
-      block_rows, max_pages, cap, static_cast<int>(a.L.slots), num_splits, sink, a.left, a.right, a.m1,
-      reinterpret_cast<int*>(ws), reinterpret_cast<int*>(ws + SVGB_PLAN_SEG_BOUNDS_OFF),
-      reinterpret_cast<int2*>(ws + a.L.chunks_off), reinterpret_cast<int4*>(ws + a.L.items_off));
-  SVGB_LAUNCH_OK();
-  return 0;
+  return kv_plan({B, total_q, max_q, true, sink, left, right, block != 0, window, block, first_block, num_splits,
+                  num_splits > 1},
+                 cu_q, cache_seqlens, cu_new, 0, cache_batch_idx, block_table, num_blocks, block_rows, max_pages,
+                 plan_ws, ws_bytes, plan, stream, "svgb_attn_plan_kvcache_varlen");
 }
 
 }  // extern "C"
